@@ -1,6 +1,7 @@
 """Benchmark of the Marigold denoising hot path (BASELINE.json metric: denoise-steps/sec @768 px).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config c2|c3|c4|c5]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 --config selects the BASELINE.json configuration (default c2 = configs[1], the headline; the others are the
@@ -14,9 +15,15 @@ loop; SURVEY.md §8e) and `value` = N * K / max-over-ranks device time.
 
 Weights are random-init tensors of the SD-2 UNet / SD VAE architecture (no checkpoints offline) and the
 image / noise are synthetic: "data": "synthetic". Inputs exceed L2: every step streams the 1.73 GB bf16
-UNet weights from HBM (L2 is 126 MB), so no explicit flush is needed between iterations.
+UNet weights from HBM (an H100's L2 is 50 MB), so no explicit flush is needed between iterations.
 
 One JSON line is printed by rank 0; see DESIGN.md §Measurement for every field.
+
+--dump-outputs DIR (rank 0) writes, after the timed steps, what the timed path returned in its last step: the denoised
+latents of this rank's members (latent.npy, float32 [B, 4, res/8, res/8]), and the prediction of the last end-to-end
+pipeline call (prediction.npy, float32). With --impl reference it writes the reference arm's latent after its last timed
+step (latent.npy, float32 [1, 4, res/8, res/8] at the resolution the arm ran). Weights, image and noise are seeded, so two builds run with the same arguments
+can be compared output for output.
 """
 from __future__ import annotations
 
@@ -97,12 +104,32 @@ def synthetic_image(S: int, seed: int = 1234):
 
 
 def _peaks():
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        d = json.loads(p.read_text())
-        return {"tflops_sustained": d.get("bf16_tflops_sustained"), "tflops_burst": d.get("bf16_tflops"),
-                "hbm_gbs": d.get("hbm_gbs"), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"tflops_sustained": 1400.0, "tflops_burst": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    """Data-sheet peaks of the H100 SXM (700 W): dense bf16 tensor throughput and HBM3 bandwidth. Not reached in
+    practice, and lower on a card with a lower power limit (the JSON line records the card's name and limit)."""
+    return {"tflops_sustained": 989.0, "tflops_burst": 989.0, "hbm_gbs": 3350.0,
+            "source": "NVIDIA H100 SXM data sheet (dense bf16, not measured)"}
+
+
+def smi_id(index: int) -> str:
+    """nvidia-smi's id of CUDA device `index`. nvidia-smi ignores CUDA_VISIBLE_DEVICES, so the CUDA ordinal can name
+    another card; the UUID cannot."""
+    import torch
+
+    u = str(torch.cuda.get_device_properties(index).uuid)
+    return u if u.startswith("GPU-") else "GPU-" + u
+
+
+def gpu_identity(index: int) -> dict:
+    """Name, power limit and maximum SM clock of the card, read in the same run as the measurement."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={smi_id(index)}", "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout
+        name, pl, mx = [c.strip() for c in out.strip().split(",")]
+        return {"name": name, "power_limit_w": float(pl), "sm_max_mhz": float(mx)}
+    except Exception:  # noqa: BLE001
+        import torch
+
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "sm_max_mhz": None}
 
 
 class ClockSampler:
@@ -116,7 +143,7 @@ class ClockSampler:
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
              "clocks_event_reasons.sw_power_cap")
         try:
-            self.proc = subprocess.Popen(["nvidia-smi", f"--id={self.index}", f"--query-gpu={q}",
+            self.proc = subprocess.Popen(["nvidia-smi", f"--id={smi_id(self.index)}", f"--query-gpu={q}",
                                           "--format=csv,noheader,nounits", "-lms", "100"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             threading.Thread(target=self._read, daemon=True).start()
@@ -259,6 +286,7 @@ def run_b200(args):
     sync_all()
     launches = int(lib.mgb_launch_count() - l0)
     clocks = sampler.stop()
+    timed_latent = target.float().cpu().numpy() if (args.dump_outputs and rank == 0 and B) else None
     ms_local = e0.elapsed_time(e1)
     ms = parallel.barrier_max_ms(ms_local, dev)
     if B:
@@ -293,6 +321,14 @@ def run_b200(args):
     h2d = img_pinned.numel() * img_pinned.element_size() + len(mine) * 4 * lh * lw * 4
     res_np = out.normals_np if cfg["task"] == "normals" else out.depth_np
     d2h = res_np.size * 4
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        dump = Path(args.dump_outputs)
+        dump.mkdir(parents=True, exist_ok=True)
+        if timed_latent is not None:
+            np.save(dump / "latent.npy", timed_latent.astype(np.float32))
+        np.save(dump / "prediction.npy", np.asarray(res_np, dtype=np.float32))
 
     # ---- dominant kernels alone (CUDA-graph replay => pure device time) ---------------------------
     kern = None
@@ -323,6 +359,7 @@ def run_b200(args):
                        "parallelism": f"members-dp{world}",
                        "l2": "inputs > L2: 1.73 GB of bf16 weights stream from HBM every step",
                        "weights": "random init (torch default init, seed 0)"},
+            "gpu": gpu_identity(local_rank),
             "clocks": clocks,
             "gpu_launches": launches,
             "cpu_enqueue_ms_per_step": t_enqueue * 1e3 / K,
@@ -335,7 +372,7 @@ def run_b200(args):
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
                          "frac": achieved / peak, "traffic": None,
                          "what": f"whole fused UNet step (all kernels), algorithmic FLOP {F_UNET[res]:.4g} per member-step",
-                         "peak_source": pk["source"] + ", bf16_tflops_sustained x n_gpus",
+                         "peak_source": pk["source"] + " x n_gpus",
                          "dominant_kernel": kern[0] if kern else None,
                          "kernels": kern},
             "gpu_library_baseline": libbase,
@@ -372,7 +409,7 @@ def _graph_time_us(torch, launch, n=20, reps=5):
 
 def _library_baseline(unet, text, res, steps):
     """Informational GPU yardstick (SURVEY.md 2.3 / 8d): the oracle graph of one UNet + DDIM step run by torch in bf16 on
-    the same B200 — cuDNN convolutions, cuBLAS linears, SDPA attention, eager launches — i.e. what the reference pipeline
+    the same GPU — cuDNN convolutions, cuBLAS linears, SDPA attention, eager launches — i.e. what the reference pipeline
     executes with torch_dtype=bfloat16. Not part of the product path."""
     import copy
 
@@ -415,7 +452,7 @@ def _library_baseline(unet, text, res, steps):
 
 def _dominant_kernel_roofline(torch):
     """The two kernels that dominate a 768-px UNet step BY TIME, each timed alone from a CUDA graph of 20 launches
-    against the burst peak: (1) flash self-attention over the 9216 latent tokens (5 launches x ~0.2 ms per step),
+    against the data-sheet peak: (1) flash self-attention over the 9216 latent tokens (5 launches per step),
     (2) the top-level 3x3 conv 320 -> 320 @ 96x96 (16 launches per step)."""
     from marigold_b200 import _lib, ops
     from marigold_b200._lib import check, ptr, stream_ptr
@@ -432,8 +469,7 @@ def _dominant_kernel_roofline(torch):
     out.append({"kernel": "flash_attn64_kernel + attn_combine_kernel (self-attention, T=9216, 5 heads x 64)",
                 "us_per_launch": us, "achieved": ach, "peak": pk["tflops_burst"], "unit": "TFLOP/s",
                 "frac": ach / pk["tflops_burst"], "share_of_step": "5 launches/step",
-                "peak_source": pk["source"] + ", bf16_tflops (burst: kernel timed alone)",
-                "traffic": None, "traffic_source": "profiles/r02_kernel_table.md (ncu --set full, dram read+write)"})
+                "peak_source": pk["source"] + " (kernel timed alone)", "traffic": None})
     # (2) conv
     NB, H, W_, Cc = 1, 96, 96, 320
     x = torch.randn(NB, H, W_, Cc, device="cuda").to(torch.bfloat16)
@@ -448,14 +484,10 @@ def _dominant_kernel_roofline(torch):
     us = _graph_time_us(torch, launch)
     flop = 2.0 * NB * H * W_ * Cc * Cc * 9
     ach = flop / (us * 1e-6) / 1e12
-    out.append({"kernel": "gemm_tc_kernel<160> (implicit-GEMM conv3x3 320->320 @96x96)", "us_per_launch": us,
+    out.append({"kernel": "gemm_tc_kernel (implicit-GEMM conv3x3 320->320 @96x96)", "us_per_launch": us,
                 "achieved": ach, "peak": pk["tflops_burst"], "unit": "TFLOP/s", "frac": ach / pk["tflops_burst"],
                 "share_of_step": "16 launches/step",
-                "peak_source": pk["source"] + ", bf16_tflops (burst: kernel timed alone)",
-                # one `ncu --set full` capture of this launch: dram__bytes_read.sum + dram__bytes_write.sum. Algorithmic
-                # bytes are 19.5e6 (A 5.9e6 bf16, weights 1.8e6, fp32 output 11.8e6): operands and output stay in the
-                # 126 MB L2 between kernels, so DRAM sees less than the algorithm moves.
-                "traffic": 7791872, "traffic_source": "ncu r01f, dram read+write bytes per launch"})
+                "peak_source": pk["source"] + " (kernel timed alone)", "traffic": None})
     return out
 
 
@@ -536,6 +568,11 @@ def run_reference(args):
                        "note": "reference pipeline needs diffusers (absent offline): oracle port on host cores"},
             "cpu_baseline": cpu,
             "e2e": {"value": value, "unit": "denoise-steps/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
+    if args.dump_outputs:
+        import numpy as np
+
+        Path(args.dump_outputs).mkdir(parents=True, exist_ok=True)
+        np.save(Path(args.dump_outputs) / "latent.npy", x.numpy().astype(np.float32))
     print(json.dumps(line), flush=True)
 
 
@@ -549,6 +586,8 @@ if __name__ == "__main__":
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-library-baseline", action="store_true")
     ap.add_argument("--no-kernel-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed path's outputs of its last step as float32 .npy files into DIR")
     a = ap.parse_args()
     if a.warmup < 3 and a.impl == "b200":
         a.warmup = 3

@@ -1,4 +1,4 @@
-/* libmarigold_b200 — C ABI of the B200-native Marigold denoising hot path.
+/* libmarigold_b200 — C ABI of the H100-native (sm_90a) Marigold denoising hot path.
  *
  * The reference (prs-eth/Marigold) has no FFI: its hot path is the Python object protocol
  *   vae.encoder / vae.quant_conv            marigold/marigold_depth_pipeline.py:491-492
@@ -62,7 +62,7 @@ typedef struct {
 int mgb_create(const mgb_config* cfg, mgb_handle** out);
 void mgb_destroy(mgb_handle* h);
 const char* mgb_last_error(void);
-/* library build info: "sm_100a;tcgen05;..." */
+/* library build info: "libmarigold_b200 sm_90a: wgmma ..." */
 const char* mgb_build_info(void);
 
 /* ---- weights (replaces DiffusionPipeline.from_pretrained state-dict loading) ---------------- */

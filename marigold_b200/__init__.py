@@ -1,4 +1,4 @@
-"""marigold_b200 — B200-native (sm_100a) implementation of Marigold's denoising hot path.
+"""marigold_b200 — H100-native (sm_90a) implementation of Marigold's denoising hot path.
 
 Public surface mirrors the reference package (marigold/__init__.py:30-41) for the path in scope:
 pipelines + output dataclasses + ensembling, plus the Engine that stands in for unet/vae/scheduler.

@@ -1,4 +1,4 @@
-"""Build libmarigold_b200.so in-tree with nvcc for sm_100a (no torch extension machinery).
+"""Build libmarigold_b200.so in-tree with nvcc for sm_90a (no torch extension machinery).
 
     python -m marigold_b200.build [--force] [--verbose]
 
@@ -20,7 +20,7 @@ BUILD = PKG / "_build"
 LIB = PKG / "libmarigold_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -71,7 +71,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             list(ex.map(lambda s: _compile(s, verbose), todo))
     objs = [BUILD / (s.stem + ".o") for s in srcs]
     if todo or not LIB.exists() or any(o.stat().st_mtime > LIB.stat().st_mtime for o in objs):
-        cmd = [_nvcc(), "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [_nvcc(), "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a",
                "-Xcompiler", "-fPIC"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

@@ -23,8 +23,8 @@ extern "C" {
 
 const char* mgb_last_error(void) { return get_error(); }
 const char* mgb_build_info(void) {
-  return "libmarigold_b200 sm_100a: tcgen05.mma kind::f16 (bf16->fp32 TMEM), cp.async.bulk.tensor (TMA) SWIZZLE_128B, "
-         "mbarrier pipelines; no CPU fallback";
+  return "libmarigold_b200 sm_90a: wgmma.mma_async bf16 (fp32 register accumulators), cp.async.bulk.tensor (TMA) "
+         "SWIZZLE_128B, mbarrier pipelines; no CPU fallback";
 }
 int64_t mgb_launch_count(void) { return launch_count(); }
 /* debug hook (not in the public header): per-CTA clock64 phase stamps of subsequent GEMM launches */

@@ -1,4 +1,4 @@
-// Flash self-attention for head_dim 64 on sm_100a (tcgen05 + TMEM + TMA).
+// Flash self-attention for head_dim 64 on sm_90a (wgmma + TMA).
 //
 // Replaces F.scaled_dot_product_attention under diffusers' Attention (attn1 of every
 // BasicTransformerBlock) reached from reference marigold/marigold_depth_pipeline.py:461-463.
@@ -6,24 +6,17 @@
 //   qkv : bf16 [NB * T, 3C]   (Q | K | V column blocks; head h owns columns h*64 .. h*64+63)
 //   out : bf16 [NB * T, C]
 //
-// One CTA = 128 queries of one (image, head), KV processed in blocks of 64 tokens; 192 threads:
-//   warp 0     TMA producer: Q tile (128 x 64) once, K / V tiles (64 x 64) through 3-stage rings
-//   warp 1     TMEM allocator + MMA issuer
-//                S_b = Q K_j^T          M128 N64 K64, both operands K-major, b = j & 1 (double-buffered)
-//                O  += P_b V_j          M128 N64 K64, A = P (bf16, K-major, written by the softmax warps
-//                                       into a SWIZZLE_128B smem tile), B = V in its natural [token, d]
-//                                       layout = MN-major operand (no transpose pass); O stays in TMEM
-//   warps 2-9  softmax. A query row is shared by TWO threads (warps w and w+4 own the same TMEM lane quarter):
-//                each handles 32 of the block's 64 scores, ONE TMEM read of S per block; the row max is
-//                exchanged through shared memory (named barrier per lane quarter). Halving the per-thread
-//                dependent chain and doubling the warps per scheduler is worth more than the exchange costs:
-//                the loop is bound by one warp's LDTM -> max -> exp2 -> STTM latency chain, not by a pipe.
-//                Lazy rescaling: the row keeps a reference max m_ref; P = exp2(S*c - m_ref). Only when
-//                a block's max exceeds m_ref by more than 8 (P could exceed 2^8) is O in TMEM
-//                rescaled (tcgen05.ld / st), which after the first blocks is rare; otherwise the
-//                softmax warps never wait on the PV MMA.
-// TMEM: S0 [0,64) S1 [64,128) O [128,192) -> 256 columns, two CTAs per SM (smem ~98 KB each) so the
-// exp (MUFU) phase of one CTA overlaps the load/convert/store phase of the other.
+// One CTA = 128 queries of one (image, head), KV processed in blocks of 64 tokens; 288 threads:
+//   warps 0-7  two consumer warpgroups, 64 query rows each:
+//                S  = Q K_j^T    wgmma m64n64k16 x 4, both operands K-major in shared memory, S in registers
+//                softmax         online, in registers: a row lives in the four lanes of a quad (two shuffles per
+//                                max / sum), O and l rescaled when the row max grows
+//                O += P V_j      wgmma m64n64k16 x 4, A = P (bf16) straight from the S registers (the accumulator
+//                                fragment of 16 columns is the A fragment of one k16 step), B = V in its natural
+//                                [token, d] layout as an MN-major (transposed) operand: no transpose pass
+//   warp 8     TMA producer: Q tile (128 x 64) once, K / V tiles (64 x 64) through 3-stage rings
+// Two CTAs per SM (~66 KB of shared memory and <= 113 registers per thread each): the softmax of one warpgroup
+// overlaps the MMAs of the others.
 #include <cstdlib>
 #include "common.cuh"
 #include "kernels.h"
@@ -31,64 +24,38 @@
 
 namespace mgb {
 
-constexpr int attn_threads(int rt) { return 64 + 128 * rt; }   // producer + MMA warps, 4 RT softmax warps
+constexpr int kAttnConsumers = 256;
+constexpr int kAttnThreads = kAttnConsumers + 32;
 constexpr int kQBytes = 128 * 128;       // 128 rows x 64 bf16
 constexpr int kKvBytes = 64 * 128;       // 64 rows x 64 bf16
-constexpr int kPBytes = 128 * 128;       // 128 rows x 64 bf16
 constexpr int kKvStages = 3;
-constexpr float kRescaleThreshold = 8.0f;  // log2 units
-constexpr int kAttnDefaultRT = 2;
-// P (bf16) goes back to tensor memory and feeds the PV MMA as a TMEM A-operand: no smem round trip and no
-// generic->async proxy fence in the softmax loop.
-// RT = softmax threads per query row (2 or 4: warps w, w+4, .. own the same TMEM lane quarter and split a block's 64
-// scores). The loop is a per-warp dependent chain (LDTM -> max -> exchange -> exp2 -> STTM), not a saturated pipe: ncu
-// reads the XU pipe (MUFU.EX2 + F2FP) at 102 %, yet converting on the integer ALU and evaluating 25-50 % of the
-// exponentials as an FMA-pipe polynomial made the kernel 7-18 % SLOWER (r01 and r02). More, shorter chains per row are
-// the lever: RT = 4 halves every thread's share and doubles the warps per scheduler.
 struct AttnParams {
   CUtensorMap tmap_q;   // 3D {3C, T, NB}, box {64, 128, 1}
   CUtensorMap tmap_kv;  // 3D {3C, T, NB}, box {64, 64, 1}
   bf16* out;
   int T, C;
   float scale_log2;
-  // split-KV (balances the last wave: 72 x 5 = 360 tiles on 296 CTA slots is 2 rounds of full tiles, but 1.25 rounds
-  // of quarter tiles): blockIdx.z = img * splits + split; split s covers KV blocks [s * nkv / splits, (s+1) * ...).
-  // With splits > 1 the CTA writes un-normalised fp32 O plus (m, l) per row; attn_combine_kernel merges them.
+  // split-KV (balances the last wave of CTAs): blockIdx.z = img * splits + split; split s covers KV blocks
+  // [s * nkv / splits, (s+1) * ...). With splits > 1 the CTA writes un-normalised fp32 O plus (m, l) per row;
+  // attn_combine_kernel merges them.
   int splits;
   float* part_o;    // [splits][NB][C/64][T][64]
   float* part_ml;   // [splits][NB][C/64][T][2]   (m in log2 units incl. the softmax scale, l)
 };
 
-// 64-thread named barrier of one TMEM lane quarter (constant ids: a register id makes ptxas reserve all 16)
-template <int N>
-__device__ __forceinline__ void quarter_barrier(int q) {
-  switch (q) {
-    case 0: asm volatile("bar.sync 1, %0;" ::"n"(N) : "memory"); break;
-    case 1: asm volatile("bar.sync 2, %0;" ::"n"(N) : "memory"); break;
-    case 2: asm volatile("bar.sync 3, %0;" ::"n"(N) : "memory"); break;
-    default: asm volatile("bar.sync 4, %0;" ::"n"(N) : "memory"); break;
-  }
-}
-
-template <int RT>
-__global__ void __launch_bounds__(attn_threads(RT), 2) flash_attn64_kernel(const __grid_constant__ AttnParams p) {
+__global__ void __launch_bounds__(kAttnThreads, 2) flash_attn64_kernel(const __grid_constant__ AttnParams p) {
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + kQBytes;
   uint8_t* sV = sK + kKvStages * kKvBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kKvStages * kKvBytes);
   uint64_t* q_full = bars;                   // 1
   uint64_t* k_full = bars + 1;               // [3]
-  uint64_t* k_empty = bars + 4;              // [3]
+  uint64_t* k_empty = bars + 4;              // [3]  one arrival per consumer warpgroup
   uint64_t* v_full = bars + 7;               // [3]
   uint64_t* v_empty = bars + 10;             // [3]
-  uint64_t* s_full = bars + 13;              // [2]
-  uint64_t* p_full = bars + 15;              // [2]  (128 arrivals)
-  uint64_t* p_empty = bars + 17;             // [2]  PV(j) complete: P buffer free, O updated
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 19);
-  float* s_xch = reinterpret_cast<float*>(bars + 20);   // [2 slots][4 quarters][2 halves][32 lanes] row-max exchange (+ final l)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128, head = blockIdx.y, img = blockIdx.z / p.splits, split = blockIdx.z % p.splits;
@@ -96,38 +63,23 @@ __global__ void __launch_bounds__(attn_threads(RT), 2) flash_attn64_kernel(const
   const int jb0 = split * nkv_all / p.splits;                 // first KV block of this CTA
   const int nkv = (split + 1) * nkv_all / p.splits - jb0;     // its number of KV blocks (>= 1: host keeps splits <= nkv_all)
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&p.tmap_q);
     tma_prefetch_desc(&p.tmap_kv);
     mbar_init(q_full, 1);
     for (int s = 0; s < kKvStages; ++s) {
-      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1);
-      mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&s_full[b], 1);
-      mbar_init(&p_full[b], 128 * RT);
-      mbar_init(&p_empty[b], 1);
+      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 2);
+      mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 2);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_ptr_smem, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t tmem_o = tmem_base + 128;
   pdl_wait();
 
-  // Producer and MMA issuer are single-thread latency chains (see gemm_tc.cu): whole loop inside one elected
-  // thread, shared-window addresses and descriptor words precomputed, counters instead of % and /. The first
-  // version (elect + warp sync + generic addressing per phase) took ~1300 cycles per KV block and bounded the
-  // whole kernel (384k cycles for T = 9216 = 2 waves x 144 blocks x 1333).
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
+    // One thread running a latency chain: whole loop inside one elected thread, shared-window addresses
+    // precomputed, counters instead of % and /.
     if (elect_one()) {
       const uint32_t kfull = smem_u32(k_full), kempty = smem_u32(k_empty), vfull = smem_u32(v_full),
                      vempty = smem_u32(v_empty);
@@ -137,189 +89,131 @@ __global__ void __launch_bounds__(attn_threads(RT), 2) flash_attn64_kernel(const
       const int ck = p.C + head * 64, cv = 2 * p.C + head * 64;
       uint32_t s = 0, ph = 0;
       for (int j = 0; j < nkv; ++j) {
-        mbar_wait_a(kempty + s * 8, ph ^ 1);
+        mbar_wait_wg(kempty + s * 8, ph ^ 1);
         mbar_expect_tx_a(kfull + s * 8, kKvBytes);
         tma_load_3d_a(sK_a + s * kKvBytes, &p.tmap_kv, kfull + s * 8, ck, (jb0 + j) * 64, img);
-        mbar_wait_a(vempty + s * 8, ph ^ 1);
+        mbar_wait_wg(vempty + s * 8, ph ^ 1);
         mbar_expect_tx_a(vfull + s * 8, kKvBytes);
         tma_load_3d_a(sV_a + s * kKvBytes, &p.tmap_kv, vfull + s * 8, cv, (jb0 + j) * 64, img);
         if (++s == kKvStages) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 64, false);
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(128, 64, true);
-      constexpr uint32_t kHi = uint32_t(kDescSw128Hi >> 32), kLbo = 1u << 16;
-      const uint32_t kfull = smem_u32(k_full), kempty = smem_u32(k_empty), vfull = smem_u32(v_full),
-                     vempty = smem_u32(v_empty), sfull = smem_u32(s_full), pfull = smem_u32(p_full),
-                     pempty = smem_u32(p_empty);
-      const uint32_t dq_lo = (smem_u32(sQ) >> 4) | kLbo, dk_lo0 = (smem_u32(sK) >> 4) | kLbo,
-                     dv_lo0 = (smem_u32(sV) >> 4) | kLbo;
-      uint32_t ks = 0, kph = 0, vs = 0, vph = 0;
-      auto issue_s = [&](int j) {
-        mbar_wait_a(kfull + ks * 8, kph);
-        const uint32_t dk_lo = dk_lo0 + ks * uint32_t(kKvBytes >> 4);
-        const uint32_t ts = tmem_base + uint32_t(j & 1) * 64;
-        umma_bf16(ts, make_u64(dq_lo, kHi), make_u64(dk_lo, kHi), idesc_s, 0u);
-        umma_bf16(ts, make_u64(dq_lo + 2, kHi), make_u64(dk_lo + 2, kHi), idesc_s, 1u);
-        umma_bf16(ts, make_u64(dq_lo + 4, kHi), make_u64(dk_lo + 4, kHi), idesc_s, 1u);
-        umma_bf16(ts, make_u64(dq_lo + 6, kHi), make_u64(dk_lo + 6, kHi), idesc_s, 1u);
-        umma_commit_a(kempty + ks * 8);
-        umma_commit_a(sfull + uint32_t(j & 1) * 8);
-        if (++ks == kKvStages) { ks = 0; kph ^= 1; }
-      };
-      mbar_wait_a(smem_u32(q_full), 0);
-      issue_s(0);
-      for (int j = 0; j < nkv; ++j) {
-        // S(j+1) goes into the other S buffer: free because softmax(j-1) signalled p_full(j-1), which
-        // this thread waited for before PV(j-1)
-        if (j + 1 < nkv) issue_s(j + 1);
-        const uint32_t b = uint32_t(j & 1);
-        mbar_wait_a(pfull + b * 8, uint32_t(j >> 1) & 1u);
-        mbar_wait_a(vfull + vs * 8, vph);
-        tc_fence_after();
-        // A: P (bf16) in TMEM, 16 bf16 = 8 columns per K=16 step; B: V [kv, d] d-contiguous (MN-major):
-        // 16 kv rows = 2048 B per K=16 step
-        const uint32_t tp = tmem_base + 192 + b * 32;
-        const uint32_t dv_lo = dv_lo0 + vs * uint32_t(kKvBytes >> 4);
-        umma_bf16_ts(tmem_o, tp, make_u64(dv_lo, kHi), idesc_pv, j > 0 ? 1u : 0u);
-        umma_bf16_ts(tmem_o, tp + 8, make_u64(dv_lo + 128, kHi), idesc_pv, 1u);
-        umma_bf16_ts(tmem_o, tp + 16, make_u64(dv_lo + 256, kHi), idesc_pv, 1u);
-        umma_bf16_ts(tmem_o, tp + 24, make_u64(dv_lo + 384, kHi), idesc_pv, 1u);
-        umma_commit_a(vempty + vs * 8);
-        umma_commit_a(pempty + b * 8);
-        if (++vs == kKvStages) { vs = 0; vph ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== softmax =====================
-    constexpr int NS = 64 / RT;             // scores (and O columns) per thread
-    const int q = warp & 3;                 // TMEM lane quarter
-    const int h = (warp - 2) >> 2;          // which part of the block's 64 scores / of O's 64 columns
-    const int row = q * 32 + lane;
-    const uint32_t lane_off = uint32_t(q * 32) << 16;
-    float m_ref = 0.f, l_run = 0.f;
-    for (int j = 0; j < nkv; ++j) {
-      const int b = j & 1, u = j >> 1;
-      mbar_wait(&s_full[b], u & 1);
-      tc_fence_after();
-      uint32_t r[NS];
-      TmemIO<NS>::ld(tmem_base + lane_off + b * 64 + h * NS, r);
-      tmem_wait_ld();
-      const int kv_valid = p.T - (jb0 + j) * 64 - h * NS;   // >= NS except possibly in the last block
-      if (kv_valid < NS) {                          // ragged tail (T % 64 != 0): mask once, then share the fast path
-#pragma unroll
-        for (int i = 0; i < NS; ++i)
-          if (i >= kv_valid) r[i] = 0xff800000u;    // -inf
-      }
-      // partial row max with 4 independent chains, then the exchange with the warps owning the other scores of the row
-      float mxa = __uint_as_float(r[0]), mxb = __uint_as_float(r[1]), mxc = __uint_as_float(r[2]),
-            mxd = __uint_as_float(r[3]);
-#pragma unroll
-      for (int i = 4; i < NS; i += 4) {
-        mxa = fmaxf(mxa, __uint_as_float(r[i]));
-        mxb = fmaxf(mxb, __uint_as_float(r[i + 1]));
-        mxc = fmaxf(mxc, __uint_as_float(r[i + 2]));
-        mxd = fmaxf(mxd, __uint_as_float(r[i + 3]));
-      }
-      float mx = fmaxf(fmaxf(mxa, mxb), fmaxf(mxc, mxd));
-      float* xs = s_xch + ((b * 4 + q) * RT) * 32;
-      xs[h * 32 + lane] = mx;
-      quarter_barrier<32 * RT>(q);
-#pragma unroll
-      for (int k = 1; k < RT; ++k) mx = fmaxf(mx, xs[((h + k) % RT) * 32 + lane]);
-      const float m_blk = mx * p.scale_log2;
-      if (j == 0) {
-        m_ref = m_blk;
-      } else {
-        const bool need = m_blk > m_ref + kRescaleThreshold;
-        if (__any_sync(0xffffffffu, need)) {      // identical decision in every warp of the quarter
-          // rescale O (and l) of the rows that need it; other rows multiply by 1
-          const float m_new = need ? m_blk : m_ref;
-          const float alpha = ex2_approx(m_ref - m_new);
-          m_ref = m_new;
-          l_run *= alpha;
-          mbar_wait(&p_empty[(j - 1) & 1], ((j - 1) >> 1) & 1);   // every PV issued so far has completed
-          tc_fence_after();
-          uint32_t o[NS];
-          TmemIO<NS>::ld(tmem_o + lane_off + h * NS, o);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < NS; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          TmemIO<NS>::st(tmem_o + lane_off + h * NS, o);
-          tmem_wait_st();
-        }
-      }
-      // P = exp2(S * c - m_ref) (exp2(-inf) = 0 masks the tail); bf16 pairs; 4 partial row sums
-      // (the scale-and-shift and the row sums go through FFMA2 / FADD2: two scores per instruction)
-      uint32_t pk[NS / 2];
-      f2 ls01 = f2_splat(0.f), ls23 = ls01;
-      const f2 sc2 = f2_splat(p.scale_log2), nm2 = f2_splat(-m_ref);
-#pragma unroll
-      for (int i = 0; i < NS / 4; ++i) {
-        float t0, t1, t2, t3;
-        f2_split(f2_fma(f2_make(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1])), sc2, nm2), t0, t1);
-        f2_split(f2_fma(f2_make(__uint_as_float(r[4 * i + 2]), __uint_as_float(r[4 * i + 3])), sc2, nm2), t2, t3);
-        const float a0 = ex2_approx(t0), a1 = ex2_approx(t1), a2 = ex2_approx(t2), a3 = ex2_approx(t3);
-        ls01 = f2_add(ls01, f2_make(a0, a1));
-        ls23 = f2_add(ls23, f2_make(a2, a3));
-        pk[2 * i] = pack_bf16x2(a0, a1);
-        pk[2 * i + 1] = pack_bf16x2(a2, a3);
-      }
-      {
-        float ls0, ls1, ls2, ls3;
-        f2_split(ls01, ls0, ls1);
-        f2_split(ls23, ls2, ls3);
-        l_run += (ls0 + ls1) + (ls2 + ls3);
-      }
-      // P buffer b was last read by PV(j-2)
-      mbar_wait(&p_empty[b], (u & 1) ^ 1);
-      TmemIO<NS / 2>::st(tmem_base + 192 + b * 32 + h * (NS / 2) + lane_off, pk);
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(&p_full[b]);
-    }
-    // epilogue: O / l. The parts of a row add their partial sums through the exchange buffer
-    // (slot (nkv & 1): not the one the last block's max exchange used).
-    float* xl = s_xch + (((nkv & 1) * 4 + q) * RT) * 32;
-    xl[h * 32 + lane] = l_run;
-    quarter_barrier<32 * RT>(q);
-    float l_tot = 0.f;
-#pragma unroll
-    for (int k = 0; k < RT; ++k) l_tot += xl[k * 32 + lane];      // same order in every part: identical l_tot
-    mbar_wait(&p_empty[(nkv - 1) & 1], ((nkv - 1) >> 1) & 1);
-    tc_fence_after();
-    const int qrow = q0 + row;
-    uint32_t o0[NS];
-    TmemIO<NS>::ld(tmem_o + lane_off + h * NS, o0);
-    tmem_wait_ld();
-    if (qrow < p.T) {
-      if (p.splits == 1) {
-        const float inv = 1.f / l_tot;
-        uint4* dst = reinterpret_cast<uint4*>(p.out + ((size_t)img * p.T + qrow) * p.C + head * 64 + h * NS);
-#pragma unroll
-        for (int i = 0; i < NS / 8; ++i)
-          dst[i] = make_uint4(pack_bf16x2(__uint_as_float(o0[8 * i]) * inv, __uint_as_float(o0[8 * i + 1]) * inv),
-                              pack_bf16x2(__uint_as_float(o0[8 * i + 2]) * inv, __uint_as_float(o0[8 * i + 3]) * inv),
-                              pack_bf16x2(__uint_as_float(o0[8 * i + 4]) * inv, __uint_as_float(o0[8 * i + 5]) * inv),
-                              pack_bf16x2(__uint_as_float(o0[8 * i + 6]) * inv, __uint_as_float(o0[8 * i + 7]) * inv));
-      } else {
-        const size_t prow = ((size_t(split) * gridDim.z / p.splits + img) * gridDim.y + head) * p.T + qrow;
-        uint4* dst = reinterpret_cast<uint4*>(p.part_o + prow * 64 + h * NS);
-#pragma unroll
-        for (int i = 0; i < NS / 4; ++i) dst[i] = make_uint4(o0[4 * i], o0[4 * i + 1], o0[4 * i + 2], o0[4 * i + 3]);
-        if (h == 0) *reinterpret_cast<float2*>(p.part_ml + prow * 2) = make_float2(m_ref, l_tot);
-      }
-    }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+
+  // ===================== consumers =====================
+  const int wg = warp >> 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  // this thread's two query rows (accumulator fragment rows l/4 and l/4 + 8 of its warp's 16) and column pairs
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cpair = (lane & 3) * 2;
+  constexpr uint32_t kHi = uint32_t(kDescSw128Hi >> 32), kLbo = 1u << 16;
+  const uint32_t dq_lo = ((smem_u32(sQ) + uint32_t(wg) * 64u * 128u) >> 4) | kLbo;
+  const uint32_t dk_lo0 = (smem_u32(sK) >> 4) | kLbo, dv_lo0 = (smem_u32(sV) >> 4) | kLbo;
+  const uint32_t kfull = smem_u32(k_full), vfull = smem_u32(v_full);
+
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running max (log2 units) and partial sums, rows lo / hi
+  mbar_wait_wg(smem_u32(q_full), 0);
+  uint32_t s = 0, ph = 0;
+  for (int j = 0; j < nkv; ++j) {
+    // ---- S = Q K^T
+    float sc[32];
+    mbar_wait_wg(kfull + s * 8, ph);
+    const uint32_t dk_lo = dk_lo0 + s * uint32_t(kKvBytes >> 4);
+    wgmma_fence();
+    Wgmma<64>::ss(sc, make_u64(dq_lo, kHi), make_u64(dk_lo, kHi), 0u);
+    Wgmma<64>::ss(sc, make_u64(dq_lo + 2, kHi), make_u64(dk_lo + 2, kHi), 1u);
+    Wgmma<64>::ss(sc, make_u64(dq_lo + 4, kHi), make_u64(dk_lo + 4, kHi), 1u);
+    Wgmma<64>::ss(sc, make_u64(dq_lo + 6, kHi), make_u64(dk_lo + 6, kHi), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+    if (wg_leader) mbar_arrive(&k_empty[s]);
+
+    // ---- online softmax (exp2 domain: the softmax scale folded into scale_log2)
+    const int kv_valid = p.T - (jb0 + j) * 64;     // >= 64 except possibly in the last block
+    if (kv_valid < 64) {                           // ragged tail (T % 64 != 0)
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const int c = 8 * jj + cpair;
+        if (c >= kv_valid) { sc[4 * jj] = -INFINITY; sc[4 * jj + 2] = -INFINITY; }
+        if (c + 1 >= kv_valid) { sc[4 * jj + 1] = -INFINITY; sc[4 * jj + 3] = -INFINITY; }
+      }
+    }
+    float mx0 = sc[0], mx1 = sc[2];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      mx0 = fmaxf(mx0, fmaxf(sc[4 * jj], sc[4 * jj + 1]));
+      mx1 = fmaxf(mx1, fmaxf(sc[4 * jj + 2], sc[4 * jj + 3]));
+    }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float mn0 = fmaxf(m0, mx0 * p.scale_log2), mn1 = fmaxf(m1, mx1 * p.scale_log2);
+    const float a0 = ex2_approx(m0 - mn0), a1 = ex2_approx(m1 - mn1);   // 0 on the first block (m = -inf)
+    m0 = mn0; m1 = mn1;
+    l0 *= a0; l1 *= a1;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      o[4 * jj] *= a0; o[4 * jj + 1] *= a0;
+      o[4 * jj + 2] *= a1; o[4 * jj + 3] *= a1;
+    }
+    // P = exp2(S * c - m) (exp2(-inf) = 0 masks the tail), packed to bf16 pairs in the wgmma A-fragment order:
+    // k16 step kk takes accumulator column groups 2 kk and 2 kk + 1
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const float e0 = ex2_approx(fmaf(sc[4 * jj], p.scale_log2, -m0));
+      const float e1 = ex2_approx(fmaf(sc[4 * jj + 1], p.scale_log2, -m0));
+      const float e2 = ex2_approx(fmaf(sc[4 * jj + 2], p.scale_log2, -m1));
+      const float e3 = ex2_approx(fmaf(sc[4 * jj + 3], p.scale_log2, -m1));
+      l0 += e0 + e1;
+      l1 += e2 + e3;
+      pa[jj >> 1][(jj & 1) * 2] = pack_bf16x2(e0, e1);
+      pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16x2(e2, e3);
+    }
+
+    // ---- O += P V: V [kv, d] d-contiguous (MN-major B): 16 kv rows = 2048 B per k16 step
+    mbar_wait_wg(vfull + s * 8, ph);
+    const uint32_t dv_lo = dv_lo0 + s * uint32_t(kKvBytes >> 4);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) Wgmma<64>::rs_tb(o, pa[kk], make_u64(dv_lo + 128 * kk, kHi), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if (wg_leader) mbar_arrive(&v_empty[s]);
+    if (++s == kKvStages) { s = 0; ph ^= 1; }
+  }
+
+  // ---- epilogue: the quad's partial sums give the row sums; O / l
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int qrow = q0 + r_lo + 8 * h;
+    if (qrow >= p.T) continue;
+    const float m = h ? m1 : m0, l = h ? l1 : l0;
+    if (p.splits == 1) {
+      const float inv = 1.f / l;
+      bf16* dst = p.out + ((size_t)img * p.T + qrow) * p.C + head * 64 + cpair;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+    } else {
+      const size_t prow = ((size_t(split) * gridDim.z / p.splits + img) * gridDim.y + head) * p.T + qrow;
+      float* dst = p.part_o + prow * 64 + cpair;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(o[4 * jj + 2 * h], o[4 * jj + 2 * h + 1]);
+      if ((lane & 3) == 0) *reinterpret_cast<float2*>(p.part_ml + prow * 2) = make_float2(m, l);
+    }
   }
 }
 
@@ -356,14 +250,14 @@ __global__ void __launch_bounds__(256) attn_combine_kernel(const float* __restri
 
 // KV splits that minimise the number of CTA rounds (2 CTAs per SM) weighted by the split's length
 int flash_attn64_splits(int NB, int T, int C) {
-  const int units = ((T + 127) / 128) * (C / 64) * NB, nkv = (T + 63) / 64, slots = 148 * 2;
+  const int units = ((T + 127) / 128) * (C / 64) * NB, nkv = (T + 63) / 64, slots = kNumSMs * 2;
   int best = 1;
   double best_t = 1e30;
   for (int s = 1; s <= 8; ++s) {
     if (s > 1 && nkv / s < 6) break;
     const double rounds = double((units * s + slots - 1) / slots);
-    // measured (r01, T = 9216): a CTA's fixed cost (prologue, Q load, first S, epilogue) is worth ~15 KV blocks,
-    // the combine pass ~8
+    // cost model: a CTA's fixed cost (prologue, Q load, first S, epilogue) is worth ~15 KV blocks, the combine
+    // pass ~8 (estimates, not measured on the H100)
     const double t = rounds * (double(nkv) / s + 15.0) + (s > 1 ? 8.0 : 0.0);
     if (t < best_t - 1e-9) { best_t = t; best = s; }
   }
@@ -400,11 +294,8 @@ int launch_flash_attn64(const bf16* qkv, bf16* out, int NB, int T, int C, float 
       p.part_ml = ws + size_t(sp) * NB * (C / 64) * T * 64;
     }
   }
-  static const size_t dbg_pad = getenv("MGB_ATTN_SMEM_PAD") ? size_t(atoi(getenv("MGB_ATTN_SMEM_PAD"))) : 0;   // debug: force 1 CTA/SM
-  const size_t smem = 1024 + kQBytes + 2 * kKvStages * kKvBytes + 256 + 4096 + dbg_pad;
-  // softmax threads per row: MGB_ATTN_RT = 2 | 4
-  static const int rt = getenv("MGB_ATTN_RT") ? atoi(getenv("MGB_ATTN_RT")) : kAttnDefaultRT;
-  void (*kern)(AttnParams) = rt == 4 ? flash_attn64_kernel<4> : flash_attn64_kernel<2>;
+  const size_t smem = 1024 + kQBytes + 2 * kKvStages * kKvBytes + 256;
+  void (*kern)(AttnParams) = flash_attn64_kernel;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
@@ -412,7 +303,7 @@ int launch_flash_attn64(const bf16* qkv, bf16* out, int NB, int T, int C, float 
     attr_set = true;
   }
   dim3 grid((T + 127) / 128, C / 64, NB * p.splits);
-  cudaError_t e = launch_k(kern, grid, attn_threads(rt == 4 ? 4 : 2), smem, stream, p);
+  cudaError_t e = launch_k(kern, grid, kAttnThreads, smem, stream, p);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { set_error("flash_attn64 launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   if (p.splits > 1) {

@@ -9,7 +9,7 @@ namespace mgb {
 
 static inline int grid_for(size_t n, int threads) {
   size_t b = (n + threads - 1) / threads;
-  const size_t cap = 148 * 16;
+  const size_t cap = size_t(kNumSMs) * 16;
   return int(b < cap ? (b ? b : 1) : cap);
 }
 #define MGB_LAUNCH_CHECK(name)                                       \

@@ -21,8 +21,8 @@
 namespace mgb {
 
 constexpr int kEnsThreads = 256;
-constexpr int kEnsMaxBlocks = 148 * 4;     // reduce / normals kernels
-constexpr int kEnsCostBlocks = 148 * 2;    // cost kernels: blocks per parameter set
+constexpr int kEnsMaxBlocks = kNumSMs * 4;    // reduce / normals kernels
+constexpr int kEnsCostBlocks = kNumSMs * 2;   // cost kernels: blocks per parameter set
 constexpr int kEnsMaxE = 16;               // register-resident (templated) kernels; larger ensembles take the *_dyn path
 constexpr int kEnsDynMaxE = 64;
 constexpr int kEnsMaxP = 2 * kEnsDynMaxE + 1;   // parameter sets per batch call (one forward-difference gradient)

@@ -14,7 +14,7 @@
 namespace mgb {
 
 constexpr int kEvThreads = 256;
-constexpr int kEvBlocks = 148 * 2;
+constexpr int kEvBlocks = kNumSMs * 2;
 constexpr int kEvSums = 12;
 
 __device__ __forceinline__ void block_reduce_store(double (&v)[kEvSums], int n, double* __restrict__ out) {
@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(kEvThreads)
 
 // scale, shift of min || [p 1] [s t]^T - g ||^2 over the valid pixels (np.linalg.lstsq in alignment.py:66-69)
 // Sum of quantity k over the blocks' partials by one warp: lane l takes blocks l, l + 32, ... (independent loads), xor tree.
-// (A single thread walking 296 x 12 dependent loads took 100 us.)
+// (A single thread would walk blocks x 12 dependent loads.)
 __device__ __forceinline__ double warp_sum_partials(const double* __restrict__ part, int nblocks, int k) {
   double t = 0.0;
   for (int b = threadIdx.x & 31; b < nblocks; b += 32) t += part[(size_t)b * kEvSums + k];

@@ -1,16 +1,14 @@
-// tcgen05 GEMM / implicit-GEMM convolution for sm_100a.
+// Warpgroup-MMA (wgmma) GEMM / implicit-GEMM convolution for sm_90a.
 //
-//   D[M, N] = A[M, K] * B[N, K]^T,  bf16 operands, fp32 accumulation in TMEM.
+//   D[M, N] = A[M, K] * B[N, K]^T,  bf16 operands, fp32 accumulation in registers.
 //
-// One 128 x BLOCK_N output tile per CTA. Warp roles (192 threads):
-//   warp 0      TMA producer: A tile (128 rows x 64 K, SWIZZLE_128B) + B tile (BLOCK_N x 64 K)
+// One 128 x BLOCK_N output tile per CTA. Warp roles (288 threads):
+//   warps 0..7  two consumer warpgroups. Warpgroup g issues 4 x wgmma m64 n BLOCK_N k16 per pipeline stage on rows
+//               [64 g, 64 g + 64) of the A tile and the whole B tile, keeps one stage of MMAs in flight
+//               (wgmma.wait_group 1) and releases a stage once its MMAs have completed. Then the fused epilogue
+//               (bias / activation / GEGLU / residual / scheduler step / output cast) from its accumulator registers.
+//   warp 8      TMA producer: A tile (128 rows x 64 K, SWIZZLE_128B) + B tile (BLOCK_N x 64 K)
 //               per pipeline stage, completion signalled on an mbarrier (complete_tx).
-//   warp 1      TMEM allocator + MMA issuer: one elected lane issues 4 x tcgen05.mma (K = 16 each)
-//               per stage and releases the stage with tcgen05.commit.
-//   warps 2..9  epilogue: tcgen05.ld the fp32 accumulator (one row per thread), apply the fused
-//               epilogue (bias / activation / GEGLU / residual / scheduler step / output cast), store.
-//               Two warps per TMEM lane quarter (w and w+4) take alternate 32-column chunks: the epilogue
-//               is bound by per-warp load/store latency chains, not by SM store bandwidth.
 //
 // A operand addressing:
 //   mode 0  rows: 2D tensor map {K, M}; tile m covers rows [128 m, 128 m + 128).
@@ -20,10 +18,10 @@
 //           padding costs nothing and no im2col buffer exists.
 //   mode 2  3x3 stride-1 conv with operand reuse: per channel block the producer loads the tile's HALO
 //           ((tile_h+2) x (tile_w+2) pixels x 64 channels, one 128 B swizzle row per pixel) ONCE, and the 9 taps
-//           are 9 UMMA descriptors into it: tile_w == 8, so an 8-row core-matrix group is one image row of the
+//           are 9 wgmma descriptors into it: tile_w == 8, so an 8-row core-matrix group is one image row of the
 //           tile and the stride between groups (SBO) is the halo row pitch. A traffic per channel block drops
 //           from 9 x 16 KB to 23 KB; the B (weight) tiles keep their own ring, one tile per tap. K order is
-//           (channel block, tap). The kernel is L2->SM bandwidth bound, so this is a direct speed-up.
+//           (channel block, tap). Off by default (MGB_CONV_HALO); bit-compatible with mode 1.
 // Replaces (behaviourally) the cuDNN/cuBLAS calls under torch.nn.Conv2d / Linear reached from
 // reference marigold/marigold_depth_pipeline.py:461-463,491-492,512-513.
 #include <algorithm>
@@ -35,13 +33,16 @@ namespace mgb {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
-constexpr int kEpiWarps = 8;                          // two warps per TMEM lane quarter, alternating column chunks
-constexpr int kGemmThreads = 64 + 32 * kEpiWarps;
+constexpr int kConsumerThreads = 256;                 // two warpgroups of 64 tile rows each
+constexpr int kProducerWarp = kConsumerThreads / 32;
+constexpr int kGemmThreads = kConsumerThreads + 32;
 
 __host__ __device__ constexpr int a_stage_bytes() { return BLOCK_M * BLOCK_K * 2; }
 __host__ __device__ constexpr int b_stage_bytes(int block_n) { return block_n * BLOCK_K * 2; }
-__host__ __device__ constexpr int tmem_cols_for(int n) { return n <= 32 ? 32 : n <= 64 ? 64 : n <= 128 ? 128 : 256; }
+// Epilogue scratch: every consumer warp stages its 16 accumulator rows in fp32 at this pitch (floats). The 8-float pad
+// makes the fragment's 64-bit stores and the row-contiguous 128-bit reloads bank-conflict free.
+__host__ __device__ constexpr int epi_pitch(int block_n) { return block_n + 8; }
+size_t gemm_epi_scratch_bytes(int block_n) { return size_t(kConsumerThreads / 32) * 16 * epi_pitch(block_n) * sizeof(float); }
 
 size_t gemm_smem_bytes(int block_n, int stages, int a_ring_bytes) {
   // 1024 B alignment slack + A ring + B ring + barriers
@@ -146,16 +147,11 @@ __device__ __forceinline__ void epilogue_special(const GemmEpilogue& e, const Ro
 }
 
 // -------------------------------------------------------------------------------------------------
-// Coalesced epilogue. After tcgen05.ld a lane holds ONE row x 32 columns. The 32 x 32 fp32 chunk is
-// transposed through a per-warp smem scratch (pitch 36 floats: conflict-free for 128-bit accesses) so that
-// 8 lanes cover one row's 128 contiguous bytes and a warp instruction moves four full lines; bias,
-// activation, residual and the casts are applied AFTER the transpose, where a lane owns 4 fixed columns.
-// The code is deliberately rolled and small: it runs once per CTA, i.e. always from a cold instruction
-// cache (the first, unrolled version was 60 KB of SASS and spent ~20k cycles per CTA fetching itself).
+// Coalesced epilogue. A warp's accumulator fragment (16 rows; a lane holds pairs of columns of two rows) is staged
+// through shared memory so that 8 lanes cover one row's 128 contiguous bytes and a warp instruction moves four full
+// lines; bias, activation, residual and the casts are applied after the reload, where a lane owns 4 fixed columns.
+// The store loop is deliberately rolled and small: it runs once per CTA, i.e. from a cold instruction cache.
 // -------------------------------------------------------------------------------------------------
-constexpr int kEpiPitch = 36;
-constexpr int kEpiPitchB = kEpiPitch * 4;
-
 struct TileGeom {
   int mode;
   long long m_base;
@@ -186,21 +182,13 @@ static __device__ __noinline__ void store_tail(float4 x, int nv, const float* re
   }
 }
 
-// Row-owner phase: 32 accumulator columns of this lane's row -> scratch row `lane`.
-__device__ __forceinline__ void scratch_put(float* s_wr, const uint32_t (&r)[32]) {
-  uint4* d = reinterpret_cast<uint4*>(s_wr);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) d[i] = make_uint4(r[4 * i], r[4 * i + 1], r[4 * i + 2], r[4 * i + 3]);
-}
-
 // -------------------------------------------------------------------------------------------------
 // The kernel
 // -------------------------------------------------------------------------------------------------
-// MINB = CTAs per SM the kernel is compiled for. 1: up to 156 registers per thread, deep operand ring (one output tile
-// per SM at a time; single-wave grids). 2: <= 96 registers and <= 113 KB of shared memory, so TWO CTAs share an SM and
-// the epilogue of one tile (TMEM -> registers -> global, latency-bound) runs under the K loop of the other — the
-// overlap a persistent kernel gets from a double-buffered accumulator, obtained from the hardware scheduler instead
-// (2 x 256 TMEM columns = the whole tensor memory). Used for multi-wave grids (GEGLU feed-forward, QKV, VAE convs).
+// MINB = CTAs per SM the kernel is compiled for. 1: the register file of an SM for one CTA (accumulators of up to
+// 128 x 256), deep operand ring, one output tile per SM at a time. 2: <= 113 registers per thread and <= 113 KB of
+// shared memory, so TWO CTAs share an SM and the epilogue of one tile runs under the K loop of the other. Used for
+// multi-wave grids with block_n <= 128 (GEGLU feed-forward, QKV, VAE convs).
 template <int BLOCK_N, int MINB>
 __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   pdl_launch_dependents();
@@ -217,10 +205,8 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
   uint8_t* smem_b = smem + (halo ? size_t(p.halo_slots) * p.halo_slot_bytes : size_t(stages) * kABytes);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + size_t(stages) * kBBytes);
   uint64_t* empty_bar = full_bar + stages;
-  uint64_t* tmem_full_bar = empty_bar + stages;
-  uint64_t* a_full = tmem_full_bar + 1;     // mode 2: halo ring barriers (up to 4 slots)
+  uint64_t* a_full = empty_bar + stages;     // mode 2: halo ring barriers (up to 4 slots)
   uint64_t* a_empty = a_full + 4;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(a_empty + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -238,36 +224,27 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
     tx = r - ty * p.tiles_x;
   }
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&p.tmap_a);
     tma_prefetch_desc(&p.tmap_b);
     if (p.num_kb1 < p.num_kb) tma_prefetch_desc(&p.tmap_a2);
 #pragma unroll 1
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);          // one arrival per consumer warpgroup
     }
-    mbar_init(tmem_full_bar, 1);
 #pragma unroll 1
     for (int s = 0; s < 4; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 2);
     }
     fence_mbar_init();
   }
-  constexpr uint32_t kTmemCols = tmem_cols_for(BLOCK_N);
-  if (warp == 1) {
-    tmem_alloc(tmem_ptr_smem, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   // Weights never depend on a predecessor kernel: start streaming the first B tiles of the pipeline
   // before waiting on it (the A operand and residuals are read only after pdl_wait()).
   const int n_pre = min(stages, kb1 - kb0);
-  if (warp == 0 && !((p.epi.flags >> 22) & 1) && elect_one()) {
+  if (warp == kProducerWarp && !((p.epi.flags >> 22) & 1) && elect_one()) {
     for (int i = 0; i < n_pre; ++i) {
       mbar_arrive_expect_tx(&full_bar[i], halo ? kBBytes : kABytes + kBBytes);
       int kc = kb0 + i;
@@ -280,19 +257,15 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
   long long* dbg = p.dbg ? p.dbg + ((size_t(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 8 : nullptr;
   if (dbg && threadIdx.x == 0) { dbg[0] = t_entry; dbg[1] = clock64(); }
 
-  // The producer and the MMA issuer are each ONE thread running a latency chain per K block; measured
-  // (tools/conv_phases.py, profiles/r01_gemm_issue_loop.txt): the tensor core retires a 128 x 160 x 16 MMA in 78
-  // cycles when fed back to back, but the first version of these loops took ~650 cycles per K block (elect + warp
-  // sync + generic->shared conversions + 64-bit descriptor arithmetic + integer divisions), i.e. the tensor pipe
-  // idled half of the time. Hence: whole loop inside one elected thread, shared-window addresses and descriptor
-  // words precomputed, counters instead of divisions.
+  // The producer is ONE thread running a latency chain per K block: whole loop inside one elected thread,
+  // shared-window addresses precomputed, counters instead of divisions.
 #ifdef MGB_GEMM_DEBUG_LOOPS
   const bool dbg_no_tma = (p.epi.flags >> 22) & 1, dbg_no_mma = (p.epi.flags >> 23) & 1;
 #else
   constexpr bool dbg_no_tma = false, dbg_no_mma = false;
 #endif
   const uint32_t full_a = smem_u32(full_bar), empty_a = smem_u32(empty_bar);
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
     if (!dbg_no_tma && elect_one()) {
       uint32_t stage = 0, phase = 0;
@@ -303,7 +276,7 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
         const int mrow = m_tile * BLOCK_M;
         int kc = kb0 * BLOCK_K;
         for (int kb = kb0; kb < kb1; ++kb, kc += BLOCK_K) {
-          mbar_wait_a(empty_a + stage * 8, phase ^ 1);
+          mbar_wait_wg(empty_a + stage * 8, phase ^ 1);
           const uint32_t fb = full_a + stage * 8;
           if (kb - kb0 >= n_pre) {        // (the first n_pre weight tiles were issued before pdl_wait)
             mbar_expect_tx_a(fb, kABytes + kBBytes);
@@ -319,7 +292,7 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
         int tap = kb0 / cblocks, cb = kb0 - tap * cblocks;
         int kc = kb0 * BLOCK_K;
         for (int kb = kb0; kb < kb1; ++kb, kc += BLOCK_K) {
-          mbar_wait_a(empty_a + stage * 8, phase ^ 1);
+          mbar_wait_wg(empty_a + stage * 8, phase ^ 1);
           const uint32_t fb = full_a + stage * 8;
           if (kb - kb0 >= n_pre) {
             mbar_expect_tx_a(fb, kABytes + kBBytes);
@@ -346,7 +319,7 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
         int cb = kb0 / 9, tap = 0, bk = cb * BLOCK_K;
         for (int kb = kb0; kb < kb1; ++kb) {
           if (tap == 0) {
-            mbar_wait_a(aempty_a + aslot * 8, aphase ^ 1);
+            mbar_wait_wg(aempty_a + aslot * 8, aphase ^ 1);
             const uint32_t fa = afull_a + aslot * 8, sa = sa0 + aslot * slot_bytes;
             mbar_expect_tx_a(fa, copy_tx * uint32_t(copies));
             if (copies == 1) {
@@ -358,11 +331,11 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
             }
             if (++aslot == slots) { aslot = 0; aphase ^= 1; }
           }
-          // The first n_pre B tiles were issued before pdl_wait and need no slot wait. (They MUST NOT wait: the MMA
-          // thread may already have consumed and released such a stage, and a first-pass parity wait on a barrier
+          // The first n_pre B tiles were issued before pdl_wait and need no slot wait. (They MUST NOT wait: the
+          // consumers may already have consumed and released such a stage, and a first-pass parity wait on a barrier
           // that has completed a phase blocks forever.)
           if (kb - kb0 >= n_pre) {
-            mbar_wait_a(empty_a + stage * 8, phase ^ 1);
+            mbar_wait_wg(empty_a + stage * 8, phase ^ 1);
             const uint32_t fb = full_a + stage * 8;
             mbar_expect_tx_a(fb, kBBytes);
             tma_load_2d_a(sb0 + stage * kBBytes, &p.tmap_b, fb, bk, ncol);
@@ -373,101 +346,133 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BLOCK_M, BLOCK_N);
-      constexpr uint32_t kDescHi = uint32_t(kDescSw128Hi >> 32);       // SBO 1024, version 1, SWIZZLE_128B
-      constexpr uint32_t kLbo = 1u << 16;
-      const uint32_t ustages = uint32_t(stages);
-      const uint32_t a_lo0 = (smem_u32(smem_a) >> 4) | kLbo, b_lo0 = (smem_u32(smem_b) >> 4) | kLbo;
-      uint32_t stage = 0, phase = 0;
-      if (!halo) {
-        for (int kb = kb0; kb < kb1; ++kb) {
-          if (!dbg_no_tma) mbar_wait_a(full_a + stage * 8, phase);
-          if (dbg && kb == kb0) dbg[2] = clock64();
-          const uint32_t al = a_lo0 + stage * uint32_t(kABytes >> 4), bl = b_lo0 + stage * uint32_t(kBBytes >> 4);
-          if (!dbg_no_mma) {
-            // K advance: +32 B (2 descriptor units) inside the 128 B swizzle atom
-            umma_bf16(tmem_base, make_u64(al, kDescHi), make_u64(bl, kDescHi), idesc, kb > kb0 ? 1u : 0u);
-            umma_bf16(tmem_base, make_u64(al + 2, kDescHi), make_u64(bl + 2, kDescHi), idesc, 1u);
-            umma_bf16(tmem_base, make_u64(al + 4, kDescHi), make_u64(bl + 4, kDescHi), idesc, 1u);
-            umma_bf16(tmem_base, make_u64(al + 6, kDescHi), make_u64(bl + 6, kDescHi), idesc, 1u);
-          }
-          umma_commit_a(empty_a + stage * 8);
-          if (++stage == ustages) { stage = 0; phase ^= 1; }
-        }
-      } else {
-        const uint32_t afull_a = smem_u32(a_full), aempty_a = smem_u32(a_empty);
-        const uint32_t slots = uint32_t(p.halo_slots), slot_u = uint32_t(p.halo_slot_bytes) >> 4;
-        const uint32_t off_dy = uint32_t(p.halo_w) * 128u >> 4;
-        const uint32_t off_dx = (p.halo_copies == 1 ? 128u : uint32_t(p.halo_copy_bytes)) >> 4;
-        // 8-row groups are image rows of the halo box: SBO = halo row pitch
-        const uint32_t hiA = off_dy | (1u << 14) | (2u << 29);
-        uint32_t aslot = 0, aphase = 0, dx = 0, dy = 0, a_off = 0;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          if ((dx | dy) == 0 && !dbg_no_tma) mbar_wait_a(afull_a + aslot * 8, aphase);
-          if (!dbg_no_tma) mbar_wait_a(full_a + stage * 8, phase);
-          if (dbg && kb == kb0) dbg[2] = clock64();
-          const uint32_t al = a_lo0 + aslot * slot_u + a_off, bl = b_lo0 + stage * uint32_t(kBBytes >> 4);
-          if (!dbg_no_mma) {
-            umma_bf16(tmem_base, make_u64(al, hiA), make_u64(bl, kDescHi), idesc, kb > kb0 ? 1u : 0u);
-            umma_bf16(tmem_base, make_u64(al + 2, hiA), make_u64(bl + 2, kDescHi), idesc, 1u);
-            umma_bf16(tmem_base, make_u64(al + 4, hiA), make_u64(bl + 4, kDescHi), idesc, 1u);
-            umma_bf16(tmem_base, make_u64(al + 6, hiA), make_u64(bl + 6, kDescHi), idesc, 1u);
-          }
-          umma_commit_a(empty_a + stage * 8);
-          a_off += off_dx;
-          if (++dx == 3) {
-            dx = 0;
-            a_off += off_dy - 3 * off_dx;
-            if (++dy == 3) {
-              dy = 0; a_off = 0;
-              umma_commit_a(aempty_a + aslot * 8);
-              if (++aslot == slots) { aslot = 0; aphase ^= 1; }
-            }
-          }
-          if (++stage == ustages) { stage = 0; phase ^= 1; }
-        }
-      }
-      umma_commit_a(smem_u32(tmem_full_bar));
-    }
-    __syncwarp();
-  } else {
-    // ===================== epilogue =====================
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;
-    TileGeom tg;
-    tg.mode = p.mode; tg.m_base = (long long)m_tile * BLOCK_M; tg.M = p.M;
-    tg.img = img; tg.ty = ty; tg.tx = tx; tg.H = p.H; tg.W = p.W;
-    tg.tile_w_shift = p.tile_w_shift; tg.tile_w_mask = p.tile_w - 1; tg.tile_h = p.tile_h;
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    if (dbg && threadIdx.x == 64) dbg[3] = clock64();
-    const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16);
-    const GemmEpilogue& e = p.epi;
-    const int n0 = n_tile * BLOCK_N;
+    return;
+  }
 
-    const int ehalf = (warp - 2) >> 2;   // which of the two warps of this lane quarter
-    if constexpr (BLOCK_N == 16) {
-      if (ehalf == 0) {
+  // ===================== consumers: MMA =====================
+  const int wg = warp >> 2;                          // rows [64 wg, 64 wg + 64) of the tile
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  float acc[BLOCK_N / 2];
+#pragma unroll
+  for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+  {
+    constexpr uint32_t kDescHi = uint32_t(kDescSw128Hi >> 32);       // SBO 1024, SWIZZLE_128B
+    constexpr uint32_t kLbo = 1u << 16;
+    const uint32_t ustages = uint32_t(stages);
+    const uint32_t b_lo0 = (smem_u32(smem_b) >> 4) | kLbo;
+    uint32_t stage = 0, phase = 0;
+    int prev = -1;         // stage of the previous K block: released once wgmma.wait_group 1 shows its MMAs complete
+    if (!halo) {
+      // the A tile's rows are 128 B apart (conv tiles: pixels in TMA box order), so rows 64.. start 8 KB in
+      const uint32_t a_lo0 = ((smem_u32(smem_a) + uint32_t(wg) * 64u * 128u) >> 4) | kLbo;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        if (!dbg_no_tma) mbar_wait_wg(full_a + stage * 8, phase);
+        if (dbg && kb == kb0 && threadIdx.x == 0) dbg[2] = clock64();
+        const uint32_t al = a_lo0 + stage * uint32_t(kABytes >> 4), bl = b_lo0 + stage * uint32_t(kBBytes >> 4);
+        if (!dbg_no_mma) {
+          wgmma_fence();
+          // K advance: +32 B (2 descriptor units) inside the 128 B swizzle atom
+          Wgmma<BLOCK_N>::ss(acc, make_u64(al, kDescHi), make_u64(bl, kDescHi), 1u);
+          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 2, kDescHi), make_u64(bl + 2, kDescHi), 1u);
+          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 4, kDescHi), make_u64(bl + 4, kDescHi), 1u);
+          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 6, kDescHi), make_u64(bl + 6, kDescHi), 1u);
+          wgmma_commit();
+          wgmma_wait<1>();
+        }
+        if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+        prev = int(stage);
+        if (++stage == ustages) { stage = 0; phase ^= 1; }
+      }
+    } else {
+      const uint32_t afull_a = smem_u32(a_full);
+      const uint32_t slots = uint32_t(p.halo_slots), slot_u = uint32_t(p.halo_slot_bytes) >> 4;
+      const uint32_t off_dy = uint32_t(p.halo_w) * 128u >> 4;
+      const uint32_t off_dx = (p.halo_copies == 1 ? 128u : uint32_t(p.halo_copy_bytes)) >> 4;
+      // 8-row groups are image rows of the halo box: SBO = halo row pitch; warpgroup 1 starts 8 image rows down
+      const uint32_t hiA = off_dy | (1u << 30);
+      const uint32_t a_lo0 = ((smem_u32(smem_a) >> 4) + uint32_t(wg) * 8u * off_dy) | kLbo;
+      uint32_t aslot = 0, aphase = 0, dx = 0, dy = 0, a_off = 0;
+      int prev_slot = -1;  // halo slot whose last tap was the previous K block
+      for (int kb = kb0; kb < kb1; ++kb) {
+        if ((dx | dy) == 0 && !dbg_no_tma) mbar_wait_wg(afull_a + aslot * 8, aphase);
+        if (!dbg_no_tma) mbar_wait_wg(full_a + stage * 8, phase);
+        if (dbg && kb == kb0 && threadIdx.x == 0) dbg[2] = clock64();
+        const uint32_t al = a_lo0 + aslot * slot_u + a_off, bl = b_lo0 + stage * uint32_t(kBBytes >> 4);
+        if (!dbg_no_mma) {
+          constexpr uint32_t kDescHiB = uint32_t(kDescSw128Hi >> 32);
+          wgmma_fence();
+          Wgmma<BLOCK_N>::ss(acc, make_u64(al, hiA), make_u64(bl, kDescHiB), 1u);
+          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 2, hiA), make_u64(bl + 2, kDescHiB), 1u);
+          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 4, hiA), make_u64(bl + 4, kDescHiB), 1u);
+          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 6, hiA), make_u64(bl + 6, kDescHiB), 1u);
+          wgmma_commit();
+          wgmma_wait<1>();
+        }
+        if (prev >= 0 && wg_leader) {
+          mbar_arrive(&empty_bar[prev]);
+          if (prev_slot >= 0) mbar_arrive(&a_empty[prev_slot]);
+        }
+        prev = int(stage);
+        prev_slot = -1;
+        a_off += off_dx;
+        if (++dx == 3) {
+          dx = 0;
+          a_off += off_dy - 3 * off_dx;
+          if (++dy == 3) {
+            dy = 0; a_off = 0;
+            prev_slot = int(aslot);
+            if (++aslot == slots) { aslot = 0; aphase ^= 1; }
+          }
+        }
+        if (++stage == ustages) { stage = 0; phase ^= 1; }
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+  }
+
+  // ===================== consumers: epilogue =====================
+  // Every MMA of both warpgroups has completed and every issued stage was consumed: the operand ring is free and
+  // becomes the staging scratch, 16 rows x epi_pitch floats per warp (the host sizes the ring to hold it).
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+  if (dbg && threadIdx.x == 0) dbg[3] = clock64();
+  constexpr int kPitch = epi_pitch(BLOCK_N);
+  const int row0 = wg * 64 + (warp & 3) * 16;       // first tile row of this warp
+  float* s_base = reinterpret_cast<float*>(smem_a) + warp * 16 * kPitch;
+  {
+    const int r = lane >> 2, c2 = (lane & 3) * 2;
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      *reinterpret_cast<float2*>(s_base + r * kPitch + 8 * j + c2) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(s_base + (r + 8) * kPitch + 8 * j + c2) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+  __syncwarp();
+  TileGeom tg;
+  tg.mode = p.mode; tg.m_base = (long long)m_tile * BLOCK_M; tg.M = p.M;
+  tg.img = img; tg.ty = ty; tg.tx = tx; tg.H = p.H; tg.W = p.W;
+  tg.tile_w_shift = p.tile_w_shift; tg.tile_w_mask = p.tile_w - 1; tg.tile_h = p.tile_h;
+  const GemmEpilogue& e = p.epi;
+  const int n0 = n_tile * BLOCK_N;
+
+  if constexpr (BLOCK_N == 16) {
+    // one lane per row: the whole row (<= 16 accumulator columns) in registers
+    if (lane < 16) {
       RowCtx rc;
-      rc.valid = tile_row_index(tg, row, &rc.m);
-      uint32_t r[16];
-      tmem_ld16(taddr, r);
-      tmem_wait_ld();
+      rc.valid = tile_row_index(tg, row0 + lane, &rc.m);
+      const float* src = s_base + lane * kPitch;
       if (p.partial != nullptr) {
         float* dst = p.partial + ((long long)split * p.M + rc.m) * p.N + n0;
         if (rc.valid) {
 #pragma unroll
           for (int i = 0; i < 16; ++i)
-            if (n0 + i < p.N) dst[i] = __uint_as_float(r[i]);
+            if (n0 + i < p.N) dst[i] = src[i];
         }
       } else {
         float v[16];
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
-          v[i] = __uint_as_float(r[i]);
+          v[i] = src[i];
           if (e.flags & EPI_SCALE) v[i] *= e.scale;
           if (e.bias && (n0 + i) < p.N) v[i] += __ldg(e.bias + n0 + i);
         }
@@ -477,171 +482,118 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
           epilogue_chunk<16>(e, rc, v, n0, p.N - n0);
         }
       }
-      }
-    } else {
-      // the operand pipeline is drained (every issued stage was consumed): its smem is the transpose
-      // scratch, one 32 x 36 fp32 tile per warp (two for GEGLU: value + gate chunk); the host checks the ring size
-      const int s_stride = ((p.partial == nullptr) && (e.flags & EPI_GEGLU)) ? 2 * 32 * kEpiPitch : 32 * kEpiPitch;
-      float* s_base = reinterpret_cast<float*>(smem_a) + (warp - 2) * s_stride;
-      float* s_wr = s_base + lane * kEpiPitch;
-      const int sub = lane >> 3, c4 = (lane & 7) * 4;
-      const float* s_rd = s_base + sub * kEpiPitch + c4;
-      const bool raw = p.partial != nullptr;                 // split-K: raw accumulators, epilogue deferred
-      const bool geglu = !raw && (e.flags & EPI_GEGLU);
-      float* out_f32 = raw ? p.partial + (long long)split * p.M * p.N : e.out_f32;
-      bf16* out_bf16 = raw ? nullptr : e.out_bf16;
-      const float* residual = raw ? nullptr : e.residual;
-      const float* bias = raw ? nullptr : e.bias;
-      const int ldo = raw ? p.N : e.ldo;
-      const int n_out = geglu ? p.N / 2 : p.N;               // output columns
-      const int half = BLOCK_N / 2;
-      const int chunks = geglu ? half / 32 : BLOCK_N / 32;
-      const float scale = (!raw && (e.flags & EPI_SCALE)) ? e.scale : 1.0f;
-      const bool silu = !raw && (e.flags & EPI_SILU);
-      const bool ld_vec = (ldo & 3) == 0;
-      // row addressing: after the transpose this lane stores rows R = it * 4 + (lane >> 3), it = 0..7, of its warp's
-      // 32-row slab. MINB == 1: hoisted out of the chunk loop (8 offsets live); MINB == 2: recomputed per batch of 4 rows
-      constexpr int RB = MINB == 2 ? 4 : 8;   // rows in flight per lane
-      long long off[MINB == 2 ? 1 : 8];
-      uint32_t vmask = 0;
-      if constexpr (MINB == 1) {
+    }
+  } else {
+    // after the reload this lane owns columns c4 .. c4 + 3 of a 32-column chunk in rows it * 4 + (lane >> 3), it = 0..3
+    const int sub = lane >> 3, c4 = (lane & 7) * 4;
+    const float* s_rd = s_base + sub * kPitch + c4;
+    const bool raw = p.partial != nullptr;                 // split-K: raw accumulators, epilogue deferred
+    const bool geglu = !raw && (e.flags & EPI_GEGLU);
+    float* out_f32 = raw ? p.partial + (long long)split * p.M * p.N : e.out_f32;
+    bf16* out_bf16 = raw ? nullptr : e.out_bf16;
+    const float* residual = raw ? nullptr : e.residual;
+    const float* bias = raw ? nullptr : e.bias;
+    const int ldo = raw ? p.N : e.ldo;
+    const int n_out = geglu ? p.N / 2 : p.N;               // output columns
+    const int half = BLOCK_N / 2;
+    const int chunks = geglu ? half / 32 : BLOCK_N / 32;
+    const float scale = (!raw && (e.flags & EPI_SCALE)) ? e.scale : 1.0f;
+    const bool silu = !raw && (e.flags & EPI_SILU);
+    const bool ld_vec = (ldo & 3) == 0;
+    long long off[4];
+    uint32_t vmask = 0;
 #pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          long long m;
-          const bool ok = tile_row_index(tg, q * 32 + it * 4 + sub, &m);
-          off[it] = m * (long long)ldo;
-          vmask |= uint32_t(ok) << it;
-        }
-      }
+    for (int it = 0; it < 4; ++it) {
+      long long m;
+      const bool ok = tile_row_index(tg, row0 + it * 4 + sub, &m);
+      off[it] = m * (long long)ldo;
+      vmask |= uint32_t(ok) << it;
+    }
 #pragma unroll 1
-      for (int j = ehalf; j < chunks; j += 2) {
-        const long long c0 = (dbg && j < 2) ? clock64() : 0;
-        {
-          uint32_t r[32];
-          tmem_ld32(taddr + j * 32, r);
-          tmem_wait_ld();
-          scratch_put(s_wr, r);
+    for (int j = 0; j < chunks; ++j) {
+      const int acc_col = n0 + j * 32 + c4;                                   // accumulator column (bias index)
+      const int col = geglu ? n_tile * half + j * 32 + c4 : acc_col;          // output column
+      const int nv = n_out - col;
+      float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f), g4 = b4;
+      if (bias && nv >= 4) {
+        b4 = __ldg(reinterpret_cast<const float4*>(bias + acc_col));
+        if (geglu) g4 = __ldg(reinterpret_cast<const float4*>(bias + acc_col + half));
+      } else if (bias && nv > 0) {
+        b4.x = __ldg(bias + acc_col);
+        if (nv > 1) b4.y = __ldg(bias + acc_col + 1);
+        if (nv > 2) b4.z = __ldg(bias + acc_col + 2);
+      }
+      // warp-uniform: the whole 32-column chunk is inside the matrix
+      const int chunk_nv = n_out - (col - c4);
+      if (chunk_nv <= 0) break;
+      const float* s_chunk = s_rd + j * 32;
+      const bool vec = ld_vec && nv >= 4;
+      if (!geglu && !silu && ld_vec && chunk_nv >= 32) {
+        // fast path: all scratch and residual loads of the lane's 4 rows are issued before anything is consumed
+        float4 x[4], rr[4];
+#pragma unroll
+        for (int it = 0; it < 4; ++it) x[it] = *reinterpret_cast<const float4*>(s_chunk + it * (4 * kPitch));
+        if (residual) {
+#pragma unroll
+          for (int it = 0; it < 4; ++it)
+            rr[it] = ((vmask >> it) & 1u) ? __ldg(reinterpret_cast<const float4*>(residual + off[it] + col))
+                                          : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int it = 0; it < 4; ++it) {
+          f2 v01 = f2_fma(f2_make(x[it].x, x[it].y), f2_splat(scale), f2_make(b4.x, b4.y));
+          f2 v23 = f2_fma(f2_make(x[it].z, x[it].w), f2_splat(scale), f2_make(b4.z, b4.w));
+          if (residual) {
+            v01 = f2_add(v01, f2_make(rr[it].x, rr[it].y));
+            v23 = f2_add(v23, f2_make(rr[it].z, rr[it].w));
+          }
+          float4 v;
+          f2_split(v01, v.x, v.y);
+          f2_split(v23, v.z, v.w);
+          if ((vmask >> it) & 1u) {
+            const long long o = off[it] + col;
+            if (out_f32) *reinterpret_cast<float4*>(out_f32 + o) = v;
+            if (out_bf16)
+              *reinterpret_cast<uint2*>(out_bf16 + o) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
+          }
+        }
+      } else {
+        // general path (GEGLU's erf polynomial, SiLU, ragged / unaligned tails): rolled to stay small
+#pragma unroll 1
+        for (int it = 0; it < 4; ++it) {
+          float4 x = *reinterpret_cast<const float4*>(s_chunk + it * (4 * kPitch));
           if (geglu) {
-            tmem_ld32(taddr + half + j * 32, r);
-            tmem_wait_ld();
-            scratch_put(s_wr + 32 * kEpiPitch, r);
+            const float4 g = *reinterpret_cast<const float4*>(s_chunk + half + it * (4 * kPitch));
+            // (value + bias) * gelu(gate + bias), in pairs
+            const f2 y01 = f2_mul(f2_add(f2_make(x.x, x.y), f2_make(b4.x, b4.y)),
+                                  gelu_erf_f2(f2_add(f2_make(g.x, g.y), f2_make(g4.x, g4.y))));
+            const f2 y23 = f2_mul(f2_add(f2_make(x.z, x.w), f2_make(b4.z, b4.w)),
+                                  gelu_erf_f2(f2_add(f2_make(g.z, g.w), f2_make(g4.z, g4.w))));
+            f2_split(y01, x.x, x.y);
+            f2_split(y23, x.z, x.w);
+          } else {
+            x.x = fmaf(x.x, scale, b4.x); x.y = fmaf(x.y, scale, b4.y);
+            x.z = fmaf(x.z, scale, b4.z); x.w = fmaf(x.w, scale, b4.w);
+            if (silu) { x.x = silu_f(x.x); x.y = silu_f(x.y); x.z = silu_f(x.z); x.w = silu_f(x.w); }
           }
-        }
-        __syncwarp();
-        const long long c1 = (dbg && j < 2) ? clock64() : 0;
-        const int acc_col = n0 + j * 32 + c4;                                   // accumulator column (bias index)
-        const int col = geglu ? n_tile * half + j * 32 + c4 : acc_col;          // output column
-        const int nv = n_out - col;
-        float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f), g4 = b4;
-        if (bias && nv >= 4) {
-          b4 = __ldg(reinterpret_cast<const float4*>(bias + acc_col));
-          if (geglu) g4 = __ldg(reinterpret_cast<const float4*>(bias + acc_col + half));
-        } else if (bias && nv > 0) {
-          b4.x = __ldg(bias + acc_col);
-          if (nv > 1) b4.y = __ldg(bias + acc_col + 1);
-          if (nv > 2) b4.z = __ldg(bias + acc_col + 2);
-        }
-        // warp-uniform: the whole 32-column chunk is inside the matrix (the fast path uses full-mask shuffles)
-        const int chunk_nv = n_out - (col - c4);
-        if (chunk_nv <= 0) { __syncwarp(); continue; }
-        const bool vec = ld_vec && nv >= 4;
-        if (!geglu && !silu && ld_vec && chunk_nv >= 32) {
-          // fast path. All scratch loads and residual loads of a batch of RB rows are issued BEFORE anything is consumed
-          // (tried and rejected, r01: requesting the next TMEM chunk / the residual rows one phase earlier made the
-          // epilogue 15% slower)
-#pragma unroll
-          for (int r0 = 0; r0 < 8; r0 += RB) {
-            float4 x[RB], rr[RB];
-            long long ob[RB];
-            uint32_t vm = 0;
-#pragma unroll
-            for (int it = 0; it < RB; ++it) {
-              if constexpr (MINB == 1) {
-                ob[it] = off[r0 + it];
-                vm |= ((vmask >> (r0 + it)) & 1u) << it;
-              } else {
-                long long m;
-                const bool ok = tile_row_index(tg, q * 32 + (r0 + it) * 4 + sub, &m);
-                ob[it] = m * (long long)ldo;
-                vm |= uint32_t(ok) << it;
-              }
-              x[it] = *reinterpret_cast<const float4*>(s_rd + (r0 + it) * (4 * kEpiPitch));
-            }
+          if (!((vmask >> it) & 1u) || nv <= 0) continue;
+          const long long o = off[it] + col;
+          if (vec) {
             if (residual) {
-#pragma unroll
-              for (int it = 0; it < RB; ++it)
-                rr[it] = ((vm >> it) & 1u) ? __ldg(reinterpret_cast<const float4*>(residual + ob[it] + col))
-                                           : make_float4(0.f, 0.f, 0.f, 0.f);
+              const float4 rr = __ldg(reinterpret_cast<const float4*>(residual + o));
+              x.x += rr.x; x.y += rr.y; x.z += rr.z; x.w += rr.w;
             }
-#pragma unroll
-            for (int it = 0; it < RB; ++it) {
-              f2 v01 = f2_fma(f2_make(x[it].x, x[it].y), f2_splat(scale), f2_make(b4.x, b4.y));
-              f2 v23 = f2_fma(f2_make(x[it].z, x[it].w), f2_splat(scale), f2_make(b4.z, b4.w));
-              if (residual) {
-                v01 = f2_add(v01, f2_make(rr[it].x, rr[it].y));
-                v23 = f2_add(v23, f2_make(rr[it].z, rr[it].w));
-              }
-              float4 v;
-              f2_split(v01, v.x, v.y);
-              f2_split(v23, v.z, v.w);
-              if ((vm >> it) & 1u) {
-                const long long o = ob[it] + col;
-                if (out_f32) *reinterpret_cast<float4*>(out_f32 + o) = v;
-                if (out_bf16)
-                  *reinterpret_cast<uint2*>(out_bf16 + o) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
-              }
-            }
-          }
-        } else {
-          // general path (GEGLU's erf polynomial, SiLU, ragged / unaligned tails): rolled to stay small
-#pragma unroll 1
-          for (int it = 0; it < 8; ++it) {
-            long long m;
-            const bool valid = tile_row_index(tg, q * 32 + it * 4 + sub, &m);
-            float4 x = *reinterpret_cast<const float4*>(s_rd + it * (4 * kEpiPitch));
-            if (geglu) {
-              const float4 g = *reinterpret_cast<const float4*>(s_rd + 32 * kEpiPitch + it * (4 * kEpiPitch));
-              // (value + bias) * gelu(gate + bias), packed pairs (FFMA2 / FADD2 / FMUL2)
-              const f2 y01 = f2_mul(f2_add(f2_make(x.x, x.y), f2_make(b4.x, b4.y)),
-                                    gelu_erf_f2(f2_add(f2_make(g.x, g.y), f2_make(g4.x, g4.y))));
-              const f2 y23 = f2_mul(f2_add(f2_make(x.z, x.w), f2_make(b4.z, b4.w)),
-                                    gelu_erf_f2(f2_add(f2_make(g.z, g.w), f2_make(g4.z, g4.w))));
-              f2_split(y01, x.x, x.y);
-              f2_split(y23, x.z, x.w);
-            } else {
-              x.x = fmaf(x.x, scale, b4.x); x.y = fmaf(x.y, scale, b4.y);
-              x.z = fmaf(x.z, scale, b4.z); x.w = fmaf(x.w, scale, b4.w);
-              if (silu) { x.x = silu_f(x.x); x.y = silu_f(x.y); x.z = silu_f(x.z); x.w = silu_f(x.w); }
-            }
-            if (!valid || nv <= 0) continue;
-            const long long o = m * (long long)ldo + col;
-            if (vec) {
-              if (residual) {
-                const float4 rr = __ldg(reinterpret_cast<const float4*>(residual + o));
-                x.x += rr.x; x.y += rr.y; x.z += rr.z; x.w += rr.w;
-              }
-              if (out_f32) *reinterpret_cast<float4*>(out_f32 + o) = x;
-              if (out_bf16)
-                *reinterpret_cast<uint2*>(out_bf16 + o) = make_uint2(pack_bf16x2(x.x, x.y), pack_bf16x2(x.z, x.w));
-            } else {
-              store_tail(x, nv, residual, out_f32, out_bf16, o);
-            }
+            if (out_f32) *reinterpret_cast<float4*>(out_f32 + o) = x;
+            if (out_bf16)
+              *reinterpret_cast<uint2*>(out_bf16 + o) = make_uint2(pack_bf16x2(x.x, x.y), pack_bf16x2(x.z, x.w));
+          } else {
+            store_tail(x, nv, residual, out_f32, out_bf16, o);
           }
         }
-        __syncwarp();
-        if (dbg && j < 2 && threadIdx.x == 64) { dbg[6 + j] = ((c1 - c0) << 32) | (clock64() - c1); }
       }
     }
-    if (dbg && threadIdx.x == 64) dbg[4] = clock64();
-    tc_fence_before();
   }
-
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
-  if (dbg && threadIdx.x == 0) dbg[5] = clock64();
+  if (dbg && threadIdx.x == 0) { dbg[4] = clock64(); dbg[5] = clock64(); }
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -725,8 +677,6 @@ int launch_gemm_tc(const GemmParams& p, int block_n, int splits, int ctas_per_sm
     switch (block_n) {
       case 64: return launch_one<64, 2>(p, splits, stream);
       case 128: return launch_one<128, 2>(p, splits, stream);
-      case 160: return launch_one<160, 2>(p, splits, stream);
-      case 256: return launch_one<256, 2>(p, splits, stream);
       default: break;
     }
   }
@@ -751,7 +701,7 @@ int launch_splitk_epilogue(const GemmParams& p_in, int block_n, int splits, cuda
   // blocks never straddle images (rows_per_img = hw when known, else the whole M)
   const int rows_per_img = (p.epi.hw > 0 && p.M % p.epi.hw == 0) ? p.epi.hw : p.M;
   const int imgs = p.M / rows_per_img;
-  int blocks_per_img = std::max(1, std::min(rows_per_img, (148 * 2) / imgs));
+  int blocks_per_img = std::max(1, std::min(rows_per_img, (kNumSMs * 2) / imgs));
   const int rows_per_block = (rows_per_img + blocks_per_img - 1) / blocks_per_img;
   blocks_per_img = (rows_per_img + rows_per_block - 1) / rows_per_block;
   cudaError_t e = launch_k(splitk_epilogue_kernel, imgs * blocks_per_img, kSkThreads, 0, stream, p, splits,

@@ -68,7 +68,7 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-static inline int grid_of(long long n) { return int(std::min<long long>((n + 255) / 256, 148 * 16)); }
+static inline int grid_of(long long n) { return int(std::min<long long>((n + 255) / 256, kNumSMs * 16)); }
 
 // src [NC, H, W] (u8 or f32) -> dst f32 [NC, h, w]; tmp: NC * H * w floats. mode: 0 bilinear-aa, 1 bicubic-aa, 2 nearest-exact.
 // post: 0 none, 1 round + clamp to [0, 255], 2 round + clamp, then x / 255 * 2 - 1.

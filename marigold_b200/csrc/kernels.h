@@ -12,13 +12,17 @@ namespace mgb {
 
 typedef __nv_bfloat16 bf16;
 
+// Streaming multiprocessors of the target GPU (H100 SXM). Sizes grids and waves in the launch heuristics only; the
+// GroupNorm grid barrier, whose correctness depends on co-residency, queries the device instead (norm.cu).
+constexpr int kNumSMs = 132;
+
 // error plumbing (api.cu)
 void set_error(const char* fmt, ...);
 const char* get_error();
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 GEMM / implicit-GEMM convolution
-//   D[M, N] = A[M, K] * B[N, K]^T   (A, B bf16 K-major; fp32 accumulation in TMEM)
+// wgmma GEMM / implicit-GEMM convolution (gemm_tc.cu)
+//   D[M, N] = A[M, K] * B[N, K]^T   (A, B bf16 K-major; fp32 accumulation in registers)
 // ---------------------------------------------------------------------------------------------
 enum : int {
   EPI_GEGLU = 1,        // acc tile = [value | gate] halves; out = (v + bv) * gelu_erf(g + bg)
@@ -77,12 +81,14 @@ struct GemmParams {
 };
 
 // Launch. block_n in {16, 32, 64, 128, 160, 256}; ctas_per_sm 1 or 2 (2: p.stages must keep gemm_smem_bytes <= 113 KB,
-// block_n >= 64). Returns cudaError_t as int.
+// block_n 64 or 128). Returns cudaError_t as int.
 int launch_gemm_tc(const GemmParams& p, int block_n, int splits, int ctas_per_sm, cudaStream_t stream);
 void set_gemm_debug_buffer(long long* dev_ptr);  // debug hook: phase timestamps of subsequent launches
 // Deferred epilogue for split-K: sums `splits` partials and applies p.epi.
 int launch_splitk_epilogue(const GemmParams& p, int block_n, int splits, cudaStream_t stream);
 size_t gemm_smem_bytes(int block_n, int stages, int a_ring_bytes = -1 /* -1: stages x 16 KB A tiles */);
+// Bytes of the operand ring the epilogue reuses as its staging scratch (block_n > 16); the ring must be at least this.
+size_t gemm_epi_scratch_bytes(int block_n);
 
 // Tensor-map helpers (driver entry point fetched through the runtime; no -lcuda needed).
 int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,

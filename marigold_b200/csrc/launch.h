@@ -1,5 +1,5 @@
 // Kernel launch helper: every kernel of the library is launched with programmatic dependent launch
-// (PDL) allowed, so the next kernel's launch latency and prologue (barrier init, TMEM allocation,
+// (PDL) allowed, so the next kernel's launch latency and prologue (barrier init,
 // tensor-map prefetch) overlap the tail of the previous one. Every kernel therefore executes
 // pdl_launch_dependents() at its top and pdl_wait() before its first access to global memory that a
 // predecessor may have written (common.cuh). Under stream capture the attribute becomes a programmatic

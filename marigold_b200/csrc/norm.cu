@@ -371,8 +371,8 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 // a_out bf16 [M, C] = LN3(y) (operand of the feed-forward GEMM).
 // -------------------------------------------------------------------------------------------------
 // Persistent blocks with the folded tables in shared memory (G, U as bf16 [H][C]; c1 and the two LayerNorm affines fp32):
-// the first versions re-read G and U from L1 / L2 for every token (13-205 KB per token against 1-5 KB of activations)
-// and ran at 28-60 us per launch; from shared memory the tables cost one conflict-free LDS.64 per quad and head.
+// re-reading G and U from L1 / L2 for every token would move 13-205 KB per token against 1-5 KB of activations; from
+// shared memory the tables cost one conflict-free LDS.64 per quad and head.
 // One warp per token, tokens strided over the grid.
 __device__ __forceinline__ float4 bf16x4_to_f4(uint2 v) {
   const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162*>(&v.x), b = *reinterpret_cast<const __nv_bfloat162*>(&v.y);
@@ -395,7 +395,7 @@ __global__ void __launch_bounds__(256, QL <= 3 ? 4 : QL <= 5 ? 3 : 1)
   float4* sP = reinterpret_cast<float4*>(sU + (size_t)H * Q);         // [5][Q]: c1, g2, b2, g3, b3
   {
     // static weights (may be read before the predecessor kernel has finished): six 1-D bulk copies (TMA) issued by one
-    // thread, completion counted on an mbarrier. (A per-thread copy loop serialised ~50 L2 round trips: 50 us per launch.)
+    // thread, completion counted on an mbarrier. (A per-thread copy loop would serialise ~50 L2 round trips.)
     __shared__ __align__(8) uint64_t bar;
     if (threadIdx.x == 0) {
       mbar_init(&bar, 1);
@@ -526,7 +526,7 @@ __global__ void __launch_bounds__(256, QL <= 3 ? 4 : QL <= 5 ? 3 : 1)
 
 // Wide rows (C = 1280, few tokens): FOUR warps per token, each owning a contiguous quarter of the channels; LayerNorm
 // sums and the per-head partial dot products meet in shared memory behind a 128-thread named barrier per token group.
-// (One warp per token left these levels at 28 us per launch: 576 tokens x a 20-head serial chain on 8 warps per SM.)
+// (One warp per token leaves 576 tokens x a 20-head serial chain on few warps per SM.)
 constexpr int kXwMaxH = 32;
 __device__ __forceinline__ void xw_barrier(int g) {
   if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
@@ -689,8 +689,8 @@ int launch_xattn2_fused(const float* x, bf16* y, bf16* a_out, const float* g2, c
   if (C % 4 != 0 || C / 4 > 32 * kLnMaxQ || H < 1) { set_error("xattn2: unsupported C=%d H=%d", C, H); return MGB_ERR_INVALID; }
   const size_t smem = size_t(2) * H * C * 2 + size_t(5) * C * 4;
   if (smem > 200 * 1024) { set_error("xattn2: C=%d H=%d needs %zu B of shared memory", C, H, smem); return MGB_ERR_INVALID; }
-  // Four warps per token pay while the launch is latency-bound (few tokens: one member's 24^2 / 12^2 levels, 25 vs 28 us);
-  // with many tokens (batched members) one warp per token has the higher throughput (c3, 8 members: 312 vs 316 steps/s).
+  // Four warps per token pay while the launch is latency-bound (few tokens: one member's 24^2 / 12^2 levels); with many
+  // tokens (batched members) one warp per token has the higher throughput.
   // MGB_XATTN_WIDE_MAXM overrides the token count up to which the wide kernel is used.
   static const int wide_max_m = getenv("MGB_XATTN_WIDE_MAXM") ? atoi(getenv("MGB_XATTN_WIDE_MAXM")) : 1024;
   if (C % 16 == 0 && C / 16 > 40 && C / 16 <= 96 && H <= kXwMaxH && M <= wide_max_m) {
@@ -701,7 +701,7 @@ int launch_xattn2_fused(const float* x, bf16* y, bf16* a_out, const float* g2, c
       if (e != cudaSuccess) { set_error("xattn2 attr: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
       wide_attr = true;
     }
-    const int blocks = std::max(1, std::min((M + 1) / 2, 148));
+    const int blocks = std::max(1, std::min((M + 1) / 2, kNumSMs));
     cudaError_t e = launch_k(xattn2_wide_kernel, blocks, 256, smem, stream, x, y, a_out, g2, b2, g3, b3, GU, c1, M, C, H, scale, eps);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("xattn2 launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
@@ -722,7 +722,7 @@ int launch_xattn2_fused(const float* x, bf16* y, bf16* a_out, const float* g2, c
   // one wave of resident blocks, each loading the tables once
   const int by_regs = ql <= 3 ? 4 : ql <= 5 ? 3 : 1;
   const int per_sm = std::max(1, std::min<int>(by_regs, int((220 * 1024) / (smem + 1024))));
-  const int blocks = std::max(1, std::min((M + warps_per_block - 1) / warps_per_block, 148 * per_sm));
+  const int blocks = std::max(1, std::min((M + warps_per_block - 1) / warps_per_block, kNumSMs * per_sm));
   cudaError_t e = launch_k(kern, blocks, 256, smem, stream, x, y, a_out, g2, b2, g3, b3, GU, c1, M, C, H, scale, eps);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { set_error("xattn2 launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }

@@ -5,12 +5,12 @@ namespace mgb {
 
 constexpr int kGnThreads = 256;
 constexpr int kGnLoads = 8;          // float4 loads in flight per thread and round
-constexpr int kGnMaxChunks = 1184;   // CTAs per image (8 per SM)
+constexpr int kGnMaxChunks = 1056;   // CTAs per image (8 per SM of an H100 SXM)
 
 // Thread geometry: Tq lanes along channel quads x Tp lanes along pixels; a thread owns Kq quads (Kq in {1, 2, 4}) and
 // R = 8 / Kq pixels per round, so that ALL of a round's loads are issued before anything is consumed. These kernels
 // run between two GEMMs on tensors that mostly sit in L2: they are bound by dependent load latency, not bandwidth
-// (the first version walked pixels with 2-3 dependent round trips per quad and took 9-15 us on 0.7-12 MB).
+// (walking pixels with 2-3 dependent round trips per quad would serialise them).
 struct GnGeom {
   int Q;          // C / 4
   int Tq, Tp;     // Tq * Tp <= 256

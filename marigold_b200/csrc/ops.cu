@@ -18,7 +18,7 @@ int conv_halo_variant() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("MGB_CONV_HALO");
-    v = e ? atoi(e) : 0;   // measured r01: no gain once the MMA issue loop runs at the tcgen05 floor (6.71 vs 6.54 ms/step)
+    v = e ? atoi(e) : 0;   // off by default: an experiment switch
     if (v == 2) v = 1;     // (variant 2, descriptor base offset set, is numerically WRONG: the swizzle is address based)
     if (v < 0 || v > 3) v = 0;
   }
@@ -195,28 +195,25 @@ int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) 
     return MGB_ERR_INVALID;
   }
   // Multi-wave grids run two CTAs per SM (gemm_tc.cu, MINB = 2): shallow operand rings of <= 113 KB, the epilogue of
-  // one tile under the K loop of its neighbour. Single-wave grids keep one CTA per SM with a deep ring.
+  // one tile under the K loop of its neighbour. Single-wave grids, and tiles whose accumulators do not fit half the
+  // register file (block_n > 128), keep one CTA per SM with a deep ring.
   static const int two_cta_env = getenv("MGB_GEMM_2CTA") ? atoi(getenv("MGB_GEMM_2CTA")) : 1;
+  // the drained operand ring doubles as the epilogue's staging scratch: it must hold gemm_epi_scratch_bytes()
+  const int need = block_n > 16 ? int(gemm_epi_scratch_bytes(block_n)) : 0;
   int ctas_per_sm = 1;
   {
     const long long m_tiles = p.mode == 0 ? (p.M + 127) / 128 : (long long)(p.M / (p.H * p.W)) * p.tiles_x * p.tiles_y;
     const long long ctas = m_tiles * ((p.N + block_n - 1) / block_n) * splits;
-    if (two_cta_env && block_n >= 64 && p.mode != 2 && ctas > 148) {
+    if (two_cta_env && block_n >= 64 && block_n <= 128 && p.mode != 2 && ctas > kNumSMs) {
       const int stage_bytes = 16384 + block_n * 128;
-      const int st2 = std::min(p.stages, (113 * 1024 - 1280) / stage_bytes);
-      const int need = 8 * ((p.epi.flags & EPI_GEGLU) ? 9216 : 4608);
-      if (st2 >= 2 && st2 * stage_bytes >= need) { p.stages = st2; ctas_per_sm = 2; }
+      const int max_st = (113 * 1024 - 1280) / stage_bytes;
+      const int st = std::min(max_st, std::max(p.stages, (need + stage_bytes - 1) / stage_bytes));
+      if (st >= 2 && st * stage_bytes >= need) { p.stages = st; ctas_per_sm = 2; }
     }
-    // experiment switch (MGB_GEMM_2CTA=2): single-wave grids keep their deep ring but run the 96-register binary, so that
-    // small successor kernels launched early (PDL) can become resident beside the tail of this one
-    if (two_cta_env == 2 && ctas_per_sm == 1 && block_n >= 64 && p.mode != 2) ctas_per_sm = -2;
   }
   const int kernel_minb = ctas_per_sm == 1 ? 1 : 2;
-  if (ctas_per_sm == -2) ctas_per_sm = 1;
   if (block_n > 16 && ctas_per_sm == 1) {
-    // the drained operand ring doubles as the epilogue's transpose scratch (8 warps x 4.5 KB, x2 for GEGLU): deepen
-    // the pipeline until that fits
-    const int need = 8 * ((p.epi.flags & EPI_GEGLU) ? 9216 : 4608);
+    // deepen the pipeline until the ring holds the epilogue scratch
     for (;;) {
       const int ring = (p.mode == 2 ? p.halo_slots * p.halo_slot_bytes : p.stages * 16384) + p.stages * block_n * 128;
       if (ring >= need || p.stages >= 16) break;
@@ -264,8 +261,9 @@ static int tile_model() {
   return v;
 }
 
-// Tile-shape heuristic. Cost model (cycles): per CTA  num_kb * 2*BN (tcgen05 floor at M=128)
-// + epilogue ~ 6*BN + fixed 3000; CTAs run in waves of 148 (1 CTA/SM).
+// Tile-shape heuristic. Cost model (SM cycles): per CTA  num_kb * K-block time + epilogue + prologue; CTAs run in waves
+// of kNumSMs (1 CTA/SM). The H100's dense bf16 rate is 2048 MAC per cycle and SM, so a 128 x BN x 64 K block cannot take
+// less than 4*BN cycles (the tensor-core floor).
 void choose_tile(int m_tiles, int N, int num_kb, bool geglu, bool allow_split, int* block_n, int* splits,
                  int* stages, int a_ring_bytes) {
   const int cands[6] = {256, 160, 128, 64, 32, 16};
@@ -282,24 +280,26 @@ void choose_tile(int m_tiles, int N, int num_kb, bool geglu, bool allow_split, i
       if (sp > 1 && num_kb / sp < 4) break;
       if (a_ring_bytes > 0 && sp > num_kb / 9) break;
       const long long ctas = (long long)m_tiles * n_tiles * sp;
-      const long long waves = (ctas + 147) / 148;
+      const long long waves = (ctas + kNumSMs - 1) / kNumSMs;
       const int kb = a_ring_bytes > 0 ? 9 * ((num_kb / 9 + sp - 1) / sp) : (num_kb + sp - 1) / sp;
       double t;
       if (tile_model() == 0) {
-        double cta_cycles = double(kb) * 2.0 * bn + 6.0 * bn + 3000.0;
-        // small tiles are smem-bandwidth bound: A (16 KB) + B per k-block at 128 B/cycle
-        const double smem_cycles = double(kb) * ((a_ring_bytes > 0 ? 2560.0 : 16384.0) + bn * 128.0) / 128.0 + 6.0 * bn + 3000.0;
+        // alternative model (MGB_TILE_MODEL=0); its epilogue / fixed / reduce constants are estimates, not measurements
+        double cta_cycles = double(kb) * 4.0 * bn + 6.0 * bn + 3000.0;
+        // small tiles are smem-bandwidth bound: A (16 KB) + B per k-block, B read by both warpgroups, at 128 B/cycle
+        const double smem_cycles = double(kb) * ((a_ring_bytes > 0 ? 2560.0 : 16384.0) + 2.0 * bn * 128.0) / 128.0 + 6.0 * bn + 3000.0;
         cta_cycles = std::max(cta_cycles, smem_cycles);
         t = waves * cta_cycles;
-        if (sp > 1) t += 4000.0 + double(m_tiles) * 128.0 * N * sp * 4.0 / (148.0 * 64.0);  // reduce pass
+        if (sp > 1) t += 4000.0 + double(m_tiles) * 128.0 * N * sp * 4.0 / (double(kNumSMs) * 64.0);  // reduce pass
       } else {
-        // constants measured with tools/conv_phases.py (r01): K block = max(tcgen05 floor 2*BN + 40, issue / smem floor
-        // ~260) cycles; epilogue = ceil(BN / 64) * 2000 (8 warps, 2000 cycles per 32-column chunk per warp);
-        // prologue + first operand latency 3300; a split-K reduce launch costs ~9000 cycles + its traffic
-        const double per_kb = std::max(2.0 * bn + 40.0, 260.0);
-        const double cta_cycles = double(kb) * per_kb + double((bn + 63) / 64) * 2000.0 + 3300.0;
+        // Measured on an H100 SXM (400 W) with the clock stamps of tools/gemm_phases.py, K = 2880, one CTA per SM:
+        // K block 1030 cycles at BN = 256 (floor 1024), 814 at BN = 160 (floor 640), i.e. max(4*BN + 40, ~800);
+        // epilogue 6.1 k cycles at BN = 128 / 160 and 9.8 k at BN = 256, ~2.5 k per 64 columns; prologue + first
+        // operand ~3.6 k. The split-K reduce launch (~9000 cycles + its traffic) is an estimate, not measured.
+        const double per_kb = std::max(4.0 * bn + 40.0, 800.0);
+        const double cta_cycles = double(kb) * per_kb + double((bn + 63) / 64) * 2500.0 + 3600.0;
         t = waves * cta_cycles;
-        if (sp > 1) t += 9000.0 + double(m_tiles) * 128.0 * N * sp * 4.0 / (148.0 * 64.0);
+        if (sp > 1) t += 9000.0 + double(m_tiles) * 128.0 * N * sp * 4.0 / (double(kNumSMs) * 64.0);
       }
       if (t < best) { best = t; bbn = bn; bsp = sp; }
     }

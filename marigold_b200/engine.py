@@ -52,7 +52,7 @@ _DT = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 class Engine:
     def __init__(self, cfg: EngineConfig = EngineConfig(), device: Optional[torch.device] = None):
         if not torch.cuda.is_available():
-            raise _lib.MgbError("marigold_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.MgbError("marigold_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _lib.load()
         self.cfg = cfg
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())

@@ -133,8 +133,8 @@ def _check_ensemble_size(engine, ensemble_size: int) -> None:
 
 
 def find_batch_size(ensemble_size: int, input_res: int, dtype: torch.dtype) -> int:
-    """reference batchsize.py:60-90 is a VRAM table for A100/3090/1080Ti; on a 180 GB B200 every
-    supported configuration fits, so all members go in one batch (capped to bound the arena)."""
+    """reference batchsize.py:60-90 is a VRAM table for A100/3090/1080Ti; on an 80 GB H100 every supported
+    configuration fits in batches of 16 members up to 768 px and 8 above, so that is the cap (it bounds the arena)."""
     return max(1, min(ensemble_size, 16 if input_res <= 768 else 8))
 
 

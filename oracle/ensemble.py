@@ -6,7 +6,7 @@ CPU restatement of the reference's test-time ensembling, marigold/util/ensemble.
   ensemble_normals  :199-249
 
 PARITY PINNED: tests/golden/ensemble_*.npz were produced by running the reference's own functions in
-the build container (tests/golden/make_golden.py imports /root/reference/marigold/util/ensemble.py
+tests/golden/make_golden.py (it imports the reference checkout's marigold/util/ensemble.py
 through a package shim); tests/test_oracle.py checks this restatement against them, including the
 member index picked by the lower median / argmax.
 """

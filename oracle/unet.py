@@ -5,7 +5,7 @@ configuration Marigold uses (reference call site: marigold/marigold_depth_pipeli
 `in_channels=8` pinned by src/trainer/marigold_depth_trainer.py:189-204).
 
 PARITY UNPINNED: `diffusers` (requirements.txt:2, `>=0.25.0`, no lockfile) is neither vendored in
-/root/reference nor installed, and no checkpoint is on disk, so this restatement follows the
+the reference repository nor installed, and no checkpoint is on disk, so this restatement follows the
 published architecture (SURVEY.md App. A.1) and is cross-checked only by its parameter count
 (865.9 M for the SD-2 config, tests/test_oracle.py). Module/parameter names are diffusers'
 state-dict names so that a real checkpoint would load unchanged.

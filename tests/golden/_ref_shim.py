@@ -1,17 +1,18 @@
-"""Import the reference's own util modules from /root/reference WITHOUT importing `marigold/__init__`
-(which needs diffusers). Only usable in the build container; used by make_golden.py to produce the
-committed fixtures. matplotlib is stubbed (only colorize_depth_maps uses it)."""
+"""Import the reference's own util modules from a checkout of the original Marigold repository (path in
+$MARIGOLD_REFERENCE) WITHOUT importing `marigold/__init__` (which needs diffusers). Used by make_golden.py to produce
+the committed fixtures; the tests never need it. matplotlib is stubbed (only colorize_depth_maps uses it)."""
 import importlib.util
+import os
 import sys
 import types
 from pathlib import Path
 
-REF = Path("/root/reference")
+REF = Path(os.environ.get("MARIGOLD_REFERENCE", "reference"))
 
 
 def load_reference_utils():
-    if not REF.exists():
-        raise RuntimeError("/root/reference is not available (fixtures are generated in the build container only)")
+    if not (REF / "marigold" / "util").is_dir():
+        raise RuntimeError(f"no Marigold checkout at {REF} (set MARIGOLD_REFERENCE to regenerate the fixtures)")
     if "matplotlib" not in sys.modules:
         sys.modules["matplotlib"] = types.ModuleType("matplotlib")
     pkg = types.ModuleType("refmarigold")

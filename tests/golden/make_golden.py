@@ -1,5 +1,5 @@
-"""Generate tests/golden/*.npz by running the REFERENCE's own functions (build container only:
-needs /root/reference). Inputs are regenerated from seeds by tests/golden/cases.py, so only the
+"""Generate tests/golden/*.npz by running the REFERENCE's own functions (needs a checkout of the original
+Marigold repository, path in $MARIGOLD_REFERENCE). Inputs are regenerated from seeds by tests/golden/cases.py, so only the
 reference outputs are stored.
 
     python tests/golden/make_golden.py

@@ -43,7 +43,7 @@ def test_unet_step_matches_oracle(tiny, B, lh, lw):
         out = eng.unet_step(rgb.cuda(), tgt, step, want_model_out=True)
         torch.cuda.synchronize()
         e = record(f"tiny/unet_step{step}/B{B}", rel_err(out, ref))
-        assert e < 1.6e-2, f"unet step {step}: rel err {e}"   # bf16 operands through ~60 GEMM layers; measured <= 1.05e-2
+        assert e < 1.6e-2, f"unet step {step}: rel err {e}"   # bf16 operands through ~60 GEMM layers; measured <= 1.07e-2 (H100)
         upd = kx[step] * x + kv[step] * out.cpu()
         assert rel_err(tgt, upd) < 1e-5                     # fused scheduler epilogue is fp32-exact
 
@@ -60,7 +60,7 @@ def test_vae_encode_matches_oracle(tiny, B, H, W):
     out = eng.encode(rgb.cuda())
     torch.cuda.synchronize()
     assert out.shape == ref.shape == (B, 4, H // 8, W // 8)
-    assert record(f"tiny/encode_{H}x{W}", rel_err(out, ref)) < 2e-2    # measured <= 1.5e-2
+    assert record(f"tiny/encode_{H}x{W}", rel_err(out, ref)) < 2e-2    # measured <= 1.5e-2 (H100)
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
@@ -89,9 +89,9 @@ def test_vae_decode_matches_oracle(tiny, mode):
         assert record("tiny/decode_normals_min_cos", cos.min()) > 0.995, f"min cosine {cos.min()}"
         # channel order and sign everywhere the vector is not tiny: max component error
         strong3 = strong[:, None].expand_as(o)
-        assert record("tiny/decode_normals_max_abs", (o - ref).abs()[strong3].max()) < 8e-2   # ~ decode error 1.5e-2 / |raw| 0.3; measured 5.2e-2
+        assert record("tiny/decode_normals_max_abs", (o - ref).abs()[strong3].max()) < 8e-2   # ~ decode error 1.5e-2 / |raw| 0.3; measured 5.6e-2 (H100)
     else:
-        assert record(f"tiny/decode_mode{mode}", rel_err(out, ref)) < 2e-2    # measured <= 1.5e-2
+        assert record(f"tiny/decode_mode{mode}", rel_err(out, ref)) < 2e-2    # measured <= 1.5e-2 (H100)
 
 
 def test_denoise_trajectory_ddim_and_lcm(tiny):
@@ -121,4 +121,4 @@ def test_denoise_trajectory_ddim_and_lcm(tiny):
                 x = o.step(v, t, x, noise=zs[i] if (kind == "lcm" and i < n - 1) else None)
         out = eng.denoise(rgb.cuda(), x0.cuda(), zs.cuda() if kind == "lcm" else None)
         torch.cuda.synchronize()
-        assert record(f"tiny/trajectory_{kind}", rel_err(out, x)) < 1e-2, kind   # measured 4.9e-3
+        assert record(f"tiny/trajectory_{kind}", rel_err(out, x)) < 1e-2, kind   # measured 4.9e-3 (H100)

@@ -38,8 +38,8 @@ def test_depth_pipeline_single_member_matches_oracle(setup):
     ref, _, _ = ora(img, ensemble_size=1, noise=z0)
     assert out.depth_np.shape == (128, 128) and out.uncertainty is None and out.depth_colored is not None
     # bf16 operand tolerance for a 4-step trajectory + decoder (the map lives in [0,1])
-    assert record("tiny/pipe_depth_max", np.abs(out.depth_np - ref).max()) < 1.5e-2      # measured 1.0e-2
-    assert record("tiny/pipe_depth_mean", np.abs(out.depth_np - ref).mean()) < 2e-3   # measured 8.6e-4
+    assert record("tiny/pipe_depth_max", np.abs(out.depth_np - ref).max()) < 1.5e-2      # measured 8.2e-3 (H100)
+    assert record("tiny/pipe_depth_mean", np.abs(out.depth_np - ref).mean()) < 2e-3   # measured 8.6e-4 (H100)
     # run-to-run reproducibility: every kernel sums in a fixed order (no data atomics anywhere on the path)
     out2 = pipe(img, ensemble_size=1, noise=z0, show_progress_bar=False)
     np.testing.assert_array_equal(out.depth_np, out2.depth_np)
@@ -63,7 +63,7 @@ def test_depth_pipeline_ensemble_and_resize(setup):
     ora100 = OracleDepthPipeline(unet, vae, DDIMSchedulerOracle(), text, 2, 100)
     ref100, _, _ = ora100(img, ensemble_size=1, noise=z1)
     assert odd.depth_np.shape == ref100.shape == (128, 256)
-    assert record("tiny/pipe_depth_50x100_max", np.abs(odd.depth_np - ref100).max()) < 1.5e-2   # measured 8.3e-3
+    assert record("tiny/pipe_depth_50x100_max", np.abs(odd.depth_np - ref100).max()) < 1.5e-2   # measured 8.2e-3 (H100)
     out = pipe(img, ensemble_size=3, noise=z0, batch_size=2, show_progress_bar=False,
                ensemble_kwargs=dict(output_uncertainty=True))
     ora = OracleDepthPipeline(unet, vae, DDIMSchedulerOracle(), text, 2, 128)
@@ -76,7 +76,7 @@ def test_depth_pipeline_ensemble_and_resize(setup):
     rgb_norm, _ = pipe._preprocess(img, 128, "bilinear")
     members = pipe._infer_members(rgb_norm, 3, 2, 2, None, z0, None, 0)
     assert members.shape == ref_members.shape == (3, 1, 64, 128)
-    assert record("tiny/pipe_members_max", (members.cpu() - ref_members).abs().max()) < 2e-2   # measured 1.4e-2
+    assert record("tiny/pipe_members_max", (members.cpu() - ref_members).abs().max()) < 2e-2   # measured 1.3e-2 (H100)
     # ... and the ensemble of IDENTICAL members matches the oracle's ensemble when given the same alignment
     # (the BFGS trajectory itself is rounding-chaotic on such near-flat random-weight maps; test_ensemble_gpu)
     from marigold_b200.ensemble import ensemble_depth
@@ -101,7 +101,7 @@ def test_depth_pipeline_lcm(setup):
     out = pipe(img, ensemble_size=1, noise=z0[:1], step_noise=zs[:, :1], show_progress_bar=False)
     ora = OracleDepthPipeline(unet, vae, LCMSchedulerOracle(), text, 4, 128)
     ref, _, _ = ora(img, ensemble_size=1, noise=z0[:1], step_noise=zs[:, :1])
-    assert record("tiny/pipe_lcm_max", np.abs(out.depth_np - ref).max()) < 2e-2   # measured 1.2e-2
+    assert record("tiny/pipe_lcm_max", np.abs(out.depth_np - ref).max()) < 2e-2   # measured 1.4e-2 (H100)
 
 
 def test_normals_pipeline_and_errors(setup):

@@ -40,14 +40,13 @@ def run(M, N, K, bn, stages, out_dtype="f32", flags=0):
     ph = {"prologue": (d[:, 1] - d[:, 0]), "first_stage": (d[:, 2] - d[:, 1]), "mainloop": (d[:, 3] - d[:, 2]),
           "epilogue": (d[:, 4] - d[:, 3]), "teardown": (d[:, 5] - d[:, 4]), "total": (d[:, 5] - d[:, 0])}
     s = " ".join(f"{k}={v.median().item():.0f}/{v.max().item():.0f}" for k, v in ph.items())
-    di = dbg.cpu()
-    for j in (0, 1):
-        v = int(di[:, 6 + j].median().item())
-        s += f" chunk{j}[ld+sts={v >> 32} loop={v & 0xffffffff}]"
+    s += f" mainloop/kb={ph['mainloop'].median().item() / (K // 64):.0f}"
     print(f"M{M} N{N} K{K} bn{bn} st{stages} {out_dtype} flags={flags:#x}: event_us={e0.elapsed_time(e1)*1e3:.1f} ctas={ctas} cycles(median/max): {s}", flush=True)
 
 
 if __name__ == "__main__":
+    for bn in (64, 128, 160, 256):                       # K-loop cycles per 64-deep K block vs the tile width
+        run(9216, 1280, 2880, bn, 4)
     run(128, 160, 64, 160, 2)
     run(9216, 320, 320, 160, 5)
     run(9216, 320, 320, 160, 5, "bf16")

@@ -2,7 +2,7 @@
 fp32 and under torch's bf16 autocast / pure-bf16 weights on the CPU, on the tiny seeded configuration of the parity
 tests. This is what `torch_dtype=torch.bfloat16` does to the reference itself and makes north_star's 1e-3 bar
 interpretable: our GPU path (bf16 operands, fp32 accumulate / trunk / statistics) is compared with the same fp32
-oracle in tests/test_net_gpu.py. CPU only; writes profiles/r01_ref_bf16_gap.json.
+oracle in tests/test_net_gpu.py. CPU only; writes out/ref_bf16_gap.json.
 """
 import json
 import sys
@@ -57,4 +57,5 @@ res["ddim4_depth_pure_bf16_vs_fp32"] = rel_err(db, dr)
 res["note"] = ("rel_err = max|a-b| / max|b| (tests/helpers.py). The product's figures against the same fp32 oracle: UNet step "
                "~0.9e-2, final depth (smoke) ~0.9e-2 with bf16 operands and fp32 accumulation/trunk.")
 print(json.dumps(res, indent=1))
-(ROOT / "profiles" / "r01_ref_bf16_gap.json").write_text(json.dumps(res, indent=1))
+(ROOT / "out").mkdir(exist_ok=True)
+(ROOT / "out" / "ref_bf16_gap.json").write_text(json.dumps(res, indent=1))
