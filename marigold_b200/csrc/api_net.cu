@@ -727,8 +727,7 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
   count_launch(2);
   const bool any_noise = step_noise != nullptr;
   if (!any_noise) CUDA_TRY(cudaMemsetAsync(nz, 0, n * 4, c.stream));   // kz * 0 must stay finite
-  static const bool env_no_graph = getenv("MGB_NO_GRAPH") != nullptr;
-  const bool graphs = h->use_graph && !env_no_graph;
+  static const bool graphs = getenv("MGB_NO_GRAPH") == nullptr;
   mgb_handle::StepGraph& G = h->step_graph;
   for (int i = first_step; i < first_step + num_steps; ++i) {
     if (h->kz_host[i] != 0.f) {

@@ -65,10 +65,10 @@ int mgb_op_conv2d(const void* x, const void* w, const float* bias, const float* 
   const int taps = kind == 1 ? 1 : 9;
   if (block_n <= 0) {
     int tw, th;
-    conv_tile_shape(Hout, Wout, &tw, &th, kind);
+    conv_tile_shape(Hout, Wout, &tw, &th);
     const int m_tiles = NB * ((Wout + tw - 1) / tw) * ((Hout + th - 1) / th);
     int bn, sp, st;
-    choose_tile(m_tiles, Cout, taps * Cin / 64, false, splitk_ws != nullptr, &bn, &sp, &st, conv_halo_ring_bytes(kind));
+    choose_tile(m_tiles, Cout, taps * Cin / 64, false, splitk_ws != nullptr, &bn, &sp, &st);
     block_n = bn; if (splits <= 0) splits = sp; if (stages <= 0) stages = st;
   }
   if (splits <= 0) splits = 1;

@@ -18,7 +18,6 @@ namespace mgb {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
@@ -127,22 +126,6 @@ __device__ __forceinline__ void bulk_copy_g2s(void* dst_smem, const void* src_gm
                : "memory");
 }
 
-// explicit shared-space 128-bit accesses (pointer arithmetic on the aligned dynamic-smem base decays to
-// generic addressing otherwise)
-__device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ float4 lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-
-// generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads)
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-
 // ------------------------------------------------------------------------------------------------
 // TMA
 // ------------------------------------------------------------------------------------------------
@@ -162,15 +145,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                            int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, "
-      "%7}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3), "r"(c4)
-      : "memory");
-}
 
 // ------------------------------------------------------------------------------------------------
 // wgmma: descriptors
@@ -185,9 +159,6 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
 // MN-major, SWIZZLE_128B, 64 bf16 contiguous along MN: successive K rows 128 B apart, 8-row K
 // groups 1024 B apart (SBO); LBO = distance between 64-element MN groups (unused when MN <= 64).
 constexpr uint64_t kDescSw128Hi = (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
-__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16) {
-  return kDescSw128Hi | (uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16) | uint64_t((smem_addr >> 4) & 0x3FFF);
-}
 __device__ __forceinline__ uint64_t make_u64(uint32_t lo, uint32_t hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
@@ -363,20 +334,9 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
-// Pairs of fp32 values: two independent lanes of arithmetic. Every operation rounds like its scalar form (the _rn
-// intrinsics keep the compiler from contracting a separate multiply and add into one FMA).
-struct f2 {
-  float lo, hi;
-};
-__device__ __forceinline__ f2 f2_make(float lo, float hi) { return f2{lo, hi}; }
-__device__ __forceinline__ f2 f2_splat(float v) { return f2{v, v}; }
-__device__ __forceinline__ void f2_split(f2 v, float& lo, float& hi) { lo = v.lo; hi = v.hi; }
-__device__ __forceinline__ f2 f2_fma(f2 a, f2 b, f2 c) { return f2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
-__device__ __forceinline__ f2 f2_add(f2 a, f2 b) { return f2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
-__device__ __forceinline__ f2 f2_sub(f2 a, f2 b) { return f2{__fsub_rn(a.lo, b.lo), __fsub_rn(a.hi, b.hi)}; }
-__device__ __forceinline__ f2 f2_mul(f2 a, f2 b) { return f2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
 
-// Exact-erf GELU (diffusers GEGLU: F.gelu(gate), default approximate="none"), two values per call.
+// Exact-erf GELU (diffusers GEGLU: F.gelu(gate), default approximate="none"). The _rn intrinsics keep the compiler
+// from contracting a separate multiply and add into one FMA, so the rounding is exactly the one written here.
 //   gelu(x) = x/2 (1 + erf(x / sqrt 2)) = (h + |h|) - |h| erfc(|x| / sqrt 2),  h = x / 2
 //   erfc(a / sqrt 2) = 2^-Q(a), Q a degree-8 polynomial without constant term, weighted minimax fit on [0, 6]
 //   (monotone beyond, so large |x| just underflows to 0): |erf error| <= 8.4e-8, |gelu error| <= 2.6e-7 in fp32 Horner
@@ -392,27 +352,18 @@ constexpr float kGeluK5 = 4.850499795e-03f;
 constexpr float kGeluK6 = -1.144385853e-02f;
 constexpr float kGeluK7 = -4.803082033e-03f;
 constexpr float kGeluK8 = -6.790186621e-04f;
-__device__ __forceinline__ f2 gelu_erf_f2(f2 x) {
-  const f2 h = f2_mul(x, f2_splat(0.5f));
-  float h0, h1;
-  f2_split(h, h0, h1);
-  const f2 n = f2_make(-fabsf(h0), -fabsf(h1));
-  f2 p = f2_fma(f2_splat(kGeluK8), n, f2_splat(kGeluK7));
-  p = f2_fma(p, n, f2_splat(kGeluK6));
-  p = f2_fma(p, n, f2_splat(kGeluK5));
-  p = f2_fma(p, n, f2_splat(kGeluK4));
-  p = f2_fma(p, n, f2_splat(kGeluK3));
-  p = f2_fma(p, n, f2_splat(kGeluK2));
-  p = f2_fma(p, n, f2_splat(kGeluK1));
-  float q0, q1;
-  f2_split(f2_mul(p, n), q0, q1);                               // -Q(|x|)
-  const f2 e = f2_make(ex2_approx(q0), ex2_approx(q1));         // erfc(|x| / sqrt 2)
-  return f2_fma(n, e, f2_sub(h, n));
-}
-__device__ __forceinline__ float gelu_erf_f(float x) {
-  float lo, hi;
-  f2_split(gelu_erf_f2(f2_make(x, x)), lo, hi);
-  return lo;
+__device__ __forceinline__ float gelu_erf(float x) {
+  const float h = __fmul_rn(x, 0.5f);
+  const float n = -fabsf(h);
+  float p = __fmaf_rn(kGeluK8, n, kGeluK7);
+  p = __fmaf_rn(p, n, kGeluK6);
+  p = __fmaf_rn(p, n, kGeluK5);
+  p = __fmaf_rn(p, n, kGeluK4);
+  p = __fmaf_rn(p, n, kGeluK3);
+  p = __fmaf_rn(p, n, kGeluK2);
+  p = __fmaf_rn(p, n, kGeluK1);
+  const float e = ex2_approx(__fmul_rn(p, n));   // 2^-Q(|x|) = erfc(|x| / sqrt 2)
+  return __fmaf_rn(n, e, __fsub_rn(h, n));
 }
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);

@@ -1,5 +1,5 @@
 // Streaming (HBM-bound) helpers around the tensor-core kernels: layout changes that feed TMA
-// (space-to-depth parity planes for stride-2 convs, nearest x2 upsampling, channel concat, latent
+// (space-to-depth parity planes for stride-2 convs, nearest x2 upsampling, latent
 // packing), the ABI's NCHW<->NHWC conversions, the tiny dense layers (time MLP, text K/V) and a row softmax. All use 128-bit accesses where the layout allows.
 #include "common.cuh"
 #include "kernels.h"
@@ -78,40 +78,6 @@ int launch_upsample2x(const float* x, bf16* y, int NB, int H, int W, int C, int 
   launch_k(upsample2x_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const float4*>(x),
            reinterpret_cast<uint2*>(y), NB, H, W, Ho, Wo, C / 4);
   MGB_LAUNCH_CHECK("upsample2x");
-}
-
-// out[M, Ca + Cb] = [a | b]  (torch.cat(dim=1) in NHWC)
-__global__ void concat_kernel(const float4* __restrict__ a, const float4* __restrict__ b, float4* __restrict__ out,
-                              size_t M, int Qa, int Qb) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int Qo = Qa + Qb;
-  const size_t total = M * Qo;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const size_t m = i / Qo;
-    const int q = int(i - m * Qo);
-    out[i] = q < Qa ? __ldg(a + m * Qa + q) : __ldg(b + m * Qb + (q - Qa));
-  }
-}
-int launch_concat(const float* a, const float* b, float* out, int M, int Ca, int Cb, cudaStream_t stream) {
-  if ((Ca | Cb) % 4) { set_error("concat: channels %% 4 != 0"); return MGB_ERR_INVALID; }
-  const size_t n = (size_t)M * ((Ca + Cb) / 4);
-  launch_k(concat_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const float4*>(a),
-           reinterpret_cast<const float4*>(b), reinterpret_cast<float4*>(out), size_t(M), Ca / 4, Cb / 4);
-  MGB_LAUNCH_CHECK("concat");
-}
-
-__global__ void cast_bf16_kernel(const float4* __restrict__ x, uint2* __restrict__ y, size_t n4) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    const float4 v = __ldg(x + i);
-    y[i] = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
-  }
-}
-int launch_cast_bf16(const float* x, bf16* y, size_t n, cudaStream_t stream) {
-  if (n % 4) { set_error("cast_bf16: n %% 4 != 0"); return MGB_ERR_INVALID; }
-  cast_bf16_kernel<<<grid_for(n / 4, 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(x),
-                                                             reinterpret_cast<uint2*>(y), n / 4);
-  MGB_LAUNCH_CHECK("cast_bf16");
 }
 
 // UNet conv_in operand (reference marigold_depth_pipeline.py:456-458, marigold_iid_pipeline.py:538-540: rgb latent FIRST):

@@ -16,12 +16,6 @@
 //           stride-1). A CTA's 128 rows are a tile_h x tile_w pixel rectangle; K block kb maps to
 //           (tap, channel block); the tap shifts the box by (dy, dx) and TMA zero-fills the halo, so
 //           padding costs nothing and no im2col buffer exists.
-//   mode 2  3x3 stride-1 conv with operand reuse: per channel block the producer loads the tile's HALO
-//           ((tile_h+2) x (tile_w+2) pixels x 64 channels, one 128 B swizzle row per pixel) ONCE, and the 9 taps
-//           are 9 wgmma descriptors into it: tile_w == 8, so an 8-row core-matrix group is one image row of the
-//           tile and the stride between groups (SBO) is the halo row pitch. A traffic per channel block drops
-//           from 9 x 16 KB to 23 KB; the B (weight) tiles keep their own ring, one tile per tap. K order is
-//           (channel block, tap). Off by default (MGB_CONV_HALO); bit-compatible with mode 1.
 // Replaces (behaviourally) the cuDNN/cuBLAS calls under torch.nn.Conv2d / Linear reached from
 // reference marigold/marigold_depth_pipeline.py:461-463,491-492,512-513.
 #include <algorithm>
@@ -44,10 +38,9 @@ __host__ __device__ constexpr int b_stage_bytes(int block_n) { return block_n * 
 __host__ __device__ constexpr int epi_pitch(int block_n) { return block_n + 8; }
 size_t gemm_epi_scratch_bytes(int block_n) { return size_t(kConsumerThreads / 32) * 16 * epi_pitch(block_n) * sizeof(float); }
 
-size_t gemm_smem_bytes(int block_n, int stages, int a_ring_bytes) {
+size_t gemm_smem_bytes(int block_n, int stages) {
   // 1024 B alignment slack + A ring + B ring + barriers
-  const size_t a = a_ring_bytes >= 0 ? size_t(a_ring_bytes) : size_t(stages) * a_stage_bytes();
-  return 1024 + a + size_t(stages) * b_stage_bytes(block_n) + 256;
+  return 1024 + size_t(stages) * (a_stage_bytes() + b_stage_bytes(block_n)) + 256;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -200,13 +193,10 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
   const int stages = p.stages;
   constexpr int kABytes = a_stage_bytes();
   constexpr int kBBytes = b_stage_bytes(BLOCK_N);
-  const bool halo = p.mode == 2;
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + (halo ? size_t(p.halo_slots) * p.halo_slot_bytes : size_t(stages) * kABytes);
+  uint8_t* smem_b = smem + size_t(stages) * kABytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + size_t(stages) * kBBytes);
   uint64_t* empty_bar = full_bar + stages;
-  uint64_t* a_full = empty_bar + stages;     // mode 2: halo ring barriers (up to 4 slots)
-  uint64_t* a_empty = a_full + 4;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -233,23 +223,16 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);          // one arrival per consumer warpgroup
     }
-#pragma unroll 1
-    for (int s = 0; s < 4; ++s) {
-      mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 2);
-    }
     fence_mbar_init();
   }
   __syncthreads();
   // Weights never depend on a predecessor kernel: start streaming the first B tiles of the pipeline
   // before waiting on it (the A operand and residuals are read only after pdl_wait()).
   const int n_pre = min(stages, kb1 - kb0);
-  if (warp == kProducerWarp && !((p.epi.flags >> 22) & 1) && elect_one()) {
+  if (warp == kProducerWarp && elect_one()) {
     for (int i = 0; i < n_pre; ++i) {
-      mbar_arrive_expect_tx(&full_bar[i], halo ? kBBytes : kABytes + kBBytes);
-      int kc = kb0 + i;
-      if (halo) { const int cb = kc / 9; kc = (kc - cb * 9) * p.cblocks + cb; }   // K order (cb, tap) -> weight column block
-      tma_load_2d(smem_b + size_t(i) * kBBytes, &p.tmap_b, &full_bar[i], kc * BLOCK_K, n_tile * BLOCK_N);
+      mbar_arrive_expect_tx(&full_bar[i], kABytes + kBBytes);
+      tma_load_2d(smem_b + size_t(i) * kBBytes, &p.tmap_b, &full_bar[i], (kb0 + i) * BLOCK_K, n_tile * BLOCK_N);
     }
   }
   // everything above overlapped the previous kernel's tail; operands / residuals are read below
@@ -259,15 +242,10 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
 
   // The producer is ONE thread running a latency chain per K block: whole loop inside one elected thread,
   // shared-window addresses precomputed, counters instead of divisions.
-#ifdef MGB_GEMM_DEBUG_LOOPS
-  const bool dbg_no_tma = (p.epi.flags >> 22) & 1, dbg_no_mma = (p.epi.flags >> 23) & 1;
-#else
-  constexpr bool dbg_no_tma = false, dbg_no_mma = false;
-#endif
   const uint32_t full_a = smem_u32(full_bar), empty_a = smem_u32(empty_bar);
   if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
-    if (!dbg_no_tma && elect_one()) {
+    if (elect_one()) {
       uint32_t stage = 0, phase = 0;
       const uint32_t sa0 = smem_u32(smem_a), sb0 = smem_u32(smem_b);
       const int ncol = n_tile * BLOCK_N;
@@ -287,7 +265,7 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
           else tma_load_2d_a(sa0 + stage * kABytes, &p.tmap_a2, fb, (kb - p.num_kb1) * BLOCK_K, mrow);
           if (++stage == ustages) { stage = 0; phase ^= 1; }
         }
-      } else if (p.mode == 1) {
+      } else {
         const int cblocks = p.cblocks, x0 = tx * p.tile_w, y0 = ty * p.tile_h;
         int tap = kb0 / cblocks, cb = kb0 - tap * cblocks;
         int kc = kb0 * BLOCK_K;
@@ -308,42 +286,6 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
           }
           if (++stage == ustages) { stage = 0; phase ^= 1; }
         }
-      } else {
-        // halo conv: K order (channel block, tap); splits are whole channel blocks
-        const uint32_t afull_a = smem_u32(a_full), aempty_a = smem_u32(a_empty);
-        const uint32_t copy_tx = uint32_t(p.halo_w) * uint32_t(p.tile_h + 2) * 128u;
-        const uint32_t slots = uint32_t(p.halo_slots), slot_bytes = uint32_t(p.halo_slot_bytes);
-        const int copies = p.halo_copies, cstep = p.cblocks * BLOCK_K;
-        const int x0 = tx * p.tile_w - 1, y0 = ty * p.tile_h - 1;
-        uint32_t aslot = 0, aphase = 0;
-        int cb = kb0 / 9, tap = 0, bk = cb * BLOCK_K;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          if (tap == 0) {
-            mbar_wait_wg(aempty_a + aslot * 8, aphase ^ 1);
-            const uint32_t fa = afull_a + aslot * 8, sa = sa0 + aslot * slot_bytes;
-            mbar_expect_tx_a(fa, copy_tx * uint32_t(copies));
-            if (copies == 1) {
-              tma_load_5d_a(sa, &p.tmap_a, fa, cb * BLOCK_K, x0, y0, 0, img);
-            } else {
-              for (int d = 0; d < 3; ++d)
-                tma_load_5d_a(sa + uint32_t(d) * uint32_t(p.halo_copy_bytes), &p.tmap_a, fa, cb * BLOCK_K, x0 + d,
-                              y0, 0, img);
-            }
-            if (++aslot == slots) { aslot = 0; aphase ^= 1; }
-          }
-          // The first n_pre B tiles were issued before pdl_wait and need no slot wait. (They MUST NOT wait: the
-          // consumers may already have consumed and released such a stage, and a first-pass parity wait on a barrier
-          // that has completed a phase blocks forever.)
-          if (kb - kb0 >= n_pre) {
-            mbar_wait_wg(empty_a + stage * 8, phase ^ 1);
-            const uint32_t fb = full_a + stage * 8;
-            mbar_expect_tx_a(fb, kBBytes);
-            tma_load_2d_a(sb0 + stage * kBBytes, &p.tmap_b, fb, bk, ncol);
-          }
-          bk += cstep;
-          if (++tap == 9) { tap = 0; ++cb; bk = cb * BLOCK_K; }
-          if (++stage == ustages) { stage = 0; phase ^= 1; }
-        }
       }
     }
     return;
@@ -362,70 +304,23 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
     const uint32_t b_lo0 = (smem_u32(smem_b) >> 4) | kLbo;
     uint32_t stage = 0, phase = 0;
     int prev = -1;         // stage of the previous K block: released once wgmma.wait_group 1 shows its MMAs complete
-    if (!halo) {
-      // the A tile's rows are 128 B apart (conv tiles: pixels in TMA box order), so rows 64.. start 8 KB in
-      const uint32_t a_lo0 = ((smem_u32(smem_a) + uint32_t(wg) * 64u * 128u) >> 4) | kLbo;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        if (!dbg_no_tma) mbar_wait_wg(full_a + stage * 8, phase);
-        if (dbg && kb == kb0 && threadIdx.x == 0) dbg[2] = clock64();
-        const uint32_t al = a_lo0 + stage * uint32_t(kABytes >> 4), bl = b_lo0 + stage * uint32_t(kBBytes >> 4);
-        if (!dbg_no_mma) {
-          wgmma_fence();
-          // K advance: +32 B (2 descriptor units) inside the 128 B swizzle atom
-          Wgmma<BLOCK_N>::ss(acc, make_u64(al, kDescHi), make_u64(bl, kDescHi), 1u);
-          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 2, kDescHi), make_u64(bl + 2, kDescHi), 1u);
-          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 4, kDescHi), make_u64(bl + 4, kDescHi), 1u);
-          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 6, kDescHi), make_u64(bl + 6, kDescHi), 1u);
-          wgmma_commit();
-          wgmma_wait<1>();
-        }
-        if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
-        prev = int(stage);
-        if (++stage == ustages) { stage = 0; phase ^= 1; }
-      }
-    } else {
-      const uint32_t afull_a = smem_u32(a_full);
-      const uint32_t slots = uint32_t(p.halo_slots), slot_u = uint32_t(p.halo_slot_bytes) >> 4;
-      const uint32_t off_dy = uint32_t(p.halo_w) * 128u >> 4;
-      const uint32_t off_dx = (p.halo_copies == 1 ? 128u : uint32_t(p.halo_copy_bytes)) >> 4;
-      // 8-row groups are image rows of the halo box: SBO = halo row pitch; warpgroup 1 starts 8 image rows down
-      const uint32_t hiA = off_dy | (1u << 30);
-      const uint32_t a_lo0 = ((smem_u32(smem_a) >> 4) + uint32_t(wg) * 8u * off_dy) | kLbo;
-      uint32_t aslot = 0, aphase = 0, dx = 0, dy = 0, a_off = 0;
-      int prev_slot = -1;  // halo slot whose last tap was the previous K block
-      for (int kb = kb0; kb < kb1; ++kb) {
-        if ((dx | dy) == 0 && !dbg_no_tma) mbar_wait_wg(afull_a + aslot * 8, aphase);
-        if (!dbg_no_tma) mbar_wait_wg(full_a + stage * 8, phase);
-        if (dbg && kb == kb0 && threadIdx.x == 0) dbg[2] = clock64();
-        const uint32_t al = a_lo0 + aslot * slot_u + a_off, bl = b_lo0 + stage * uint32_t(kBBytes >> 4);
-        if (!dbg_no_mma) {
-          constexpr uint32_t kDescHiB = uint32_t(kDescSw128Hi >> 32);
-          wgmma_fence();
-          Wgmma<BLOCK_N>::ss(acc, make_u64(al, hiA), make_u64(bl, kDescHiB), 1u);
-          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 2, hiA), make_u64(bl + 2, kDescHiB), 1u);
-          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 4, hiA), make_u64(bl + 4, kDescHiB), 1u);
-          Wgmma<BLOCK_N>::ss(acc, make_u64(al + 6, hiA), make_u64(bl + 6, kDescHiB), 1u);
-          wgmma_commit();
-          wgmma_wait<1>();
-        }
-        if (prev >= 0 && wg_leader) {
-          mbar_arrive(&empty_bar[prev]);
-          if (prev_slot >= 0) mbar_arrive(&a_empty[prev_slot]);
-        }
-        prev = int(stage);
-        prev_slot = -1;
-        a_off += off_dx;
-        if (++dx == 3) {
-          dx = 0;
-          a_off += off_dy - 3 * off_dx;
-          if (++dy == 3) {
-            dy = 0; a_off = 0;
-            prev_slot = int(aslot);
-            if (++aslot == slots) { aslot = 0; aphase ^= 1; }
-          }
-        }
-        if (++stage == ustages) { stage = 0; phase ^= 1; }
-      }
+    // the A tile's rows are 128 B apart (conv tiles: pixels in TMA box order), so rows 64.. start 8 KB in
+    const uint32_t a_lo0 = ((smem_u32(smem_a) + uint32_t(wg) * 64u * 128u) >> 4) | kLbo;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait_wg(full_a + stage * 8, phase);
+      if (dbg && kb == kb0 && threadIdx.x == 0) dbg[2] = clock64();
+      const uint32_t al = a_lo0 + stage * uint32_t(kABytes >> 4), bl = b_lo0 + stage * uint32_t(kBBytes >> 4);
+      wgmma_fence();
+      // K advance: +32 B (2 descriptor units) inside the 128 B swizzle atom
+      Wgmma<BLOCK_N>::ss(acc, make_u64(al, kDescHi), make_u64(bl, kDescHi), 1u);
+      Wgmma<BLOCK_N>::ss(acc, make_u64(al + 2, kDescHi), make_u64(bl + 2, kDescHi), 1u);
+      Wgmma<BLOCK_N>::ss(acc, make_u64(al + 4, kDescHi), make_u64(bl + 4, kDescHi), 1u);
+      Wgmma<BLOCK_N>::ss(acc, make_u64(al + 6, kDescHi), make_u64(bl + 6, kDescHi), 1u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+      prev = int(stage);
+      if (++stage == ustages) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
@@ -541,15 +436,12 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
         }
 #pragma unroll
         for (int it = 0; it < 4; ++it) {
-          f2 v01 = f2_fma(f2_make(x[it].x, x[it].y), f2_splat(scale), f2_make(b4.x, b4.y));
-          f2 v23 = f2_fma(f2_make(x[it].z, x[it].w), f2_splat(scale), f2_make(b4.z, b4.w));
+          float4 v = make_float4(__fmaf_rn(x[it].x, scale, b4.x), __fmaf_rn(x[it].y, scale, b4.y),
+                                 __fmaf_rn(x[it].z, scale, b4.z), __fmaf_rn(x[it].w, scale, b4.w));
           if (residual) {
-            v01 = f2_add(v01, f2_make(rr[it].x, rr[it].y));
-            v23 = f2_add(v23, f2_make(rr[it].z, rr[it].w));
+            v.x = __fadd_rn(v.x, rr[it].x); v.y = __fadd_rn(v.y, rr[it].y);
+            v.z = __fadd_rn(v.z, rr[it].z); v.w = __fadd_rn(v.w, rr[it].w);
           }
-          float4 v;
-          f2_split(v01, v.x, v.y);
-          f2_split(v23, v.z, v.w);
           if ((vmask >> it) & 1u) {
             const long long o = off[it] + col;
             if (out_f32) *reinterpret_cast<float4*>(out_f32 + o) = v;
@@ -564,13 +456,11 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
           float4 x = *reinterpret_cast<const float4*>(s_chunk + it * (4 * kPitch));
           if (geglu) {
             const float4 g = *reinterpret_cast<const float4*>(s_chunk + half + it * (4 * kPitch));
-            // (value + bias) * gelu(gate + bias), in pairs
-            const f2 y01 = f2_mul(f2_add(f2_make(x.x, x.y), f2_make(b4.x, b4.y)),
-                                  gelu_erf_f2(f2_add(f2_make(g.x, g.y), f2_make(g4.x, g4.y))));
-            const f2 y23 = f2_mul(f2_add(f2_make(x.z, x.w), f2_make(b4.z, b4.w)),
-                                  gelu_erf_f2(f2_add(f2_make(g.z, g.w), f2_make(g4.z, g4.w))));
-            f2_split(y01, x.x, x.y);
-            f2_split(y23, x.z, x.w);
+            // (value + bias) * gelu(gate + bias)
+            x.x = __fmul_rn(__fadd_rn(x.x, b4.x), gelu_erf(__fadd_rn(g.x, g4.x)));
+            x.y = __fmul_rn(__fadd_rn(x.y, b4.y), gelu_erf(__fadd_rn(g.y, g4.y)));
+            x.z = __fmul_rn(__fadd_rn(x.z, b4.z), gelu_erf(__fadd_rn(g.z, g4.z)));
+            x.w = __fmul_rn(__fadd_rn(x.w, b4.w), gelu_erf(__fadd_rn(g.w, g4.w)));
           } else {
             x.x = fmaf(x.x, scale, b4.x); x.y = fmaf(x.y, scale, b4.y);
             x.z = fmaf(x.z, scale, b4.z); x.w = fmaf(x.w, scale, b4.w);
@@ -653,7 +543,7 @@ template <int BN, int MINB>
 static int launch_one(const GemmParams& p_in, int splits, cudaStream_t stream) {
   GemmParams p = p_in;
   p.dbg = g_gemm_dbg;
-  const size_t smem = gemm_smem_bytes(BN, p.stages, p.mode == 2 ? p.halo_slots * p.halo_slot_bytes : -1);
+  const size_t smem = gemm_smem_bytes(BN, p.stages);
   static bool attr_set = false;  // per template instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);

@@ -56,8 +56,7 @@ struct GemmParams {
   CUtensorMap tmap_a2; // mode 0, optional: 2D {K2, M}, A = [A1 | A2] along K. Mode 1, optional second A operand: 5D {C2, W, H, 1, NB} of a 1x1 convolution over the same output
                        // pixels whose K blocks follow the 3x3 taps (K concatenation: a ResnetBlock's conv2 + conv_shortcut
                        // as ONE implicit GEMM with weights [W2 | Wsc])
-  int mode;            // 0 = row-major activations, 1 = implicit conv (one A tile per tap), 2 = implicit 3x3 conv
-                       // whose 9 taps read ONE shared-memory halo per channel block (see gemm_tc.cu)
+  int mode;            // 0 = row-major activations, 1 = implicit conv (one A tile per tap)
   int M, N;            // logical GEMM rows / accumulator columns
   int num_kb;          // total K blocks of 64
   int num_kb1;         // K blocks of the first A operand (== num_kb without tmap_a2)
@@ -71,10 +70,6 @@ struct GemmParams {
   int cblocks;         // Cin / 64
   int ntaps;
   int8_t tap_p[12], tap_dy[12], tap_dx[12];
-  // mode 2: halo geometry. halo_copies == 1: one (tile_h+2) x (tile_w+2) pixel box, taps address it at a
-  // 128 B-granular offset; halo_copies == 3: three (tile_h+2) x tile_w boxes (dx = -1, 0, +1), taps only shift
-  // by whole rows (1024 B-aligned operand starts).
-  int halo_w, halo_copies, halo_copy_bytes, halo_slot_bytes, halo_slots, halo_base_off;
   float* partial;      // split-K: fp32 [splits, M, N] raw accumulators (epilogue deferred)
   long long* dbg;      // optional per-CTA phase timestamps [ctas][8] (tools/gemm_phases.py), else nullptr
   GemmEpilogue epi;
@@ -86,7 +81,7 @@ int launch_gemm_tc(const GemmParams& p, int block_n, int splits, int ctas_per_sm
 void set_gemm_debug_buffer(long long* dev_ptr);  // debug hook: phase timestamps of subsequent launches
 // Deferred epilogue for split-K: sums `splits` partials and applies p.epi.
 int launch_splitk_epilogue(const GemmParams& p, int block_n, int splits, cudaStream_t stream);
-size_t gemm_smem_bytes(int block_n, int stages, int a_ring_bytes = -1 /* -1: stages x 16 KB A tiles */);
+size_t gemm_smem_bytes(int block_n, int stages);
 // Bytes of the operand ring the epilogue reuses as its staging scratch (block_n > 16); the ring must be at least this.
 size_t gemm_epi_scratch_bytes(int block_n);
 
@@ -139,10 +134,6 @@ int launch_xattn2_fold(const float* wq, const float* wo, const float* bo, const 
 int launch_space_to_depth(const float* x, bf16* y, int NB, int H, int W, int C, cudaStream_t stream);
 // nearest upsampling: x fp32 [NB, H, W, C] -> y bf16 [NB, Ho, Wo, C], Ho in {2H - 1, 2H}, Wo in {2W - 1, 2W}
 int launch_upsample2x(const float* x, bf16* y, int NB, int H, int W, int C, int Ho, int Wo, cudaStream_t stream);
-// channel concat (fp32): out[M, Ca + Cb] = [a | b]
-int launch_concat(const float* a, const float* b, float* out, int M, int Ca, int Cb, cudaStream_t stream);
-// fp32 -> bf16 cast
-int launch_cast_bf16(const float* x, bf16* y, size_t n, cudaStream_t stream);
 // UNet conv_in operand: [rgb(4) | target(Ct) | zeros] bf16 NHWC-64 from the fp32 NHWC latents (Ct = 4, or 4 n for IID)
 int launch_pack_latents(const float* rgb, const float* tgt, bf16* out, int M, int Ct, cudaStream_t stream);
 // NCHW fp32 <-> NHWC fp32 (small tensors at the ABI)

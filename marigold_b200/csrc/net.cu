@@ -52,7 +52,7 @@ struct Epi {
   float* aux_out = nullptr;
 };
 
-// Debug only (tools/marginal_cost.py): MGB_SKIP=gn,ln,attn,xattn,concat,gemm drops a kernel family from the graph so
+// Debug only (tools/marginal_cost.py): MGB_SKIP=gn,ln,attn,xattn,gemm drops a kernel family from the graph so
 // that its marginal in-graph cost can be read from the step time. Results are garbage when set.
 static bool skip_family(const char* name) {
   static const char* env = getenv("MGB_SKIP");
@@ -107,13 +107,12 @@ static int matmul_nt(Ctx& c, const bf16* a, const bf16* b, int M, int N, int K, 
 static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const ConvW& W, int kind, const Epi& e,
                    int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr) {
   int tw, th;
-  conv_tile_shape(Hout, Wout, &tw, &th, kind);
+  conv_tile_shape(Hout, Wout, &tw, &th);
   const int m_tiles = NB * ((Wout + tw - 1) / tw) * ((Hout + th - 1) / th);
   int bn, sp, st;
   const bool special = (e.flags & (EPI_SCHED | EPI_DEPTH | EPI_NORMALS | EPI_NCHW)) != 0;
   if ((x2 != nullptr) != (W.k_extra > 0)) { set_error("conv3x3: second operand / weight layout mismatch"); return MGB_ERR_STATE; }
-  choose_tile(m_tiles, W.cout, (9 * W.cin_pad + W.k_extra) / 64, false, !special, &bn, &sp, &st,
-              x2 ? 0 : conv_halo_ring_bytes(kind));
+  choose_tile(m_tiles, W.cout, (9 * W.cin_pad + W.k_extra) / 64, false, !special, &bn, &sp, &st);
   if (special) bn = 16;
   const size_t M = size_t(NB) * Hout * Wout;
   if (sp > 1) c.splitk_need = std::max(c.splitk_need, size_t(sp) * M * W.cout * sizeof(float));

@@ -160,7 +160,6 @@ struct mgb_handle {
   } step_graph;
   std::vector<int> timesteps_idx_scratch;  // [0, 1, 2, ...]: host source for arming the device step counter
   cudaStream_t capture_stream = nullptr;
-  bool use_graph = true;
   unsigned* sync_slab = nullptr;   // GroupNorm grid-barrier counters of one forward
   size_t sync_slab_count = 0;
   // ensemble scratch

@@ -15,7 +15,6 @@
 // Semantics: torch.nn.GroupNorm (biased variance) as used by diffusers ResnetBlock2D / Transformer2DModel / VAE
 // blocks; SURVEY.md App. A.1-A.2. Reached from reference marigold_depth_pipeline.py:461-463,491-492,512-513.
 #include <algorithm>
-#include <cstdlib>
 #include "common.cuh"
 #include "kernels.h"
 #include "launch.h"
@@ -528,6 +527,10 @@ __global__ void __launch_bounds__(256, QL <= 3 ? 4 : QL <= 5 ? 3 : 1)
 // sums and the per-head partial dot products meet in shared memory behind a 128-thread named barrier per token group.
 // (One warp per token leaves 576 tokens x a 20-head serial chain on few warps per SM.)
 constexpr int kXwMaxH = 32;
+// Token count up to which the wide kernel is used. Four warps per token pay while the launch is latency-bound (few
+// tokens: one member's 24^2 / 12^2 levels); with many tokens (batched members) one warp per token has the higher
+// throughput.
+constexpr int kXwMaxTokens = 1024;
 __device__ __forceinline__ void xw_barrier(int g) {
   if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
   else asm volatile("bar.sync 2, 128;" ::: "memory");
@@ -689,11 +692,7 @@ int launch_xattn2_fused(const float* x, bf16* y, bf16* a_out, const float* g2, c
   if (C % 4 != 0 || C / 4 > 32 * kLnMaxQ || H < 1) { set_error("xattn2: unsupported C=%d H=%d", C, H); return MGB_ERR_INVALID; }
   const size_t smem = size_t(2) * H * C * 2 + size_t(5) * C * 4;
   if (smem > 200 * 1024) { set_error("xattn2: C=%d H=%d needs %zu B of shared memory", C, H, smem); return MGB_ERR_INVALID; }
-  // Four warps per token pay while the launch is latency-bound (few tokens: one member's 24^2 / 12^2 levels); with many
-  // tokens (batched members) one warp per token has the higher throughput.
-  // MGB_XATTN_WIDE_MAXM overrides the token count up to which the wide kernel is used.
-  static const int wide_max_m = getenv("MGB_XATTN_WIDE_MAXM") ? atoi(getenv("MGB_XATTN_WIDE_MAXM")) : 1024;
-  if (C % 16 == 0 && C / 16 > 40 && C / 16 <= 96 && H <= kXwMaxH && M <= wide_max_m) {
+  if (C % 16 == 0 && C / 16 > 40 && C / 16 <= 96 && H <= kXwMaxH && M <= kXwMaxTokens) {
     // wide rows: four warps per token (C = 1280: 80 quads per warp quarter)
     static bool wide_attr = false;
     if (!wide_attr) {

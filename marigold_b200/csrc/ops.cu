@@ -2,7 +2,6 @@
 // geometry, tap tables) and pick tile shapes. Used by the network composition (net.cu) and by the
 // operator-level C ABI (api.cu).
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 
 #include "kernels.h"
@@ -14,40 +13,7 @@ static std::atomic<long long> g_launches{0};
 void count_launch(int n) { g_launches += n; }
 long long launch_count() { return g_launches.load(); }
 
-int conv_halo_variant() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MGB_CONV_HALO");
-    v = e ? atoi(e) : 0;   // off by default: an experiment switch
-    if (v == 2) v = 1;     // (variant 2, descriptor base offset set, is numerically WRONG: the swizzle is address based)
-    if (v < 0 || v > 3) v = 0;
-  }
-  return v;
-}
-
-constexpr int kHaloTileW = 8, kHaloTileH = 16;
-static int halo_slots() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("MGB_HALO_SLOTS"); v = e ? atoi(e) : 2; if (v < 2 || v > 4) v = 2; }
-  return v;
-}
-#define kHaloSlots halo_slots()
-static int halo_copy_bytes(int variant) {
-  const int w = variant == 3 ? kHaloTileW : kHaloTileW + 2;
-  return ((w * (kHaloTileH + 2) * 128 + 1023) / 1024) * 1024;
-}
-static int halo_slot_bytes(int variant) { return halo_copy_bytes(variant) * (variant == 3 ? 3 : 1); }
-int conv_halo_ring_bytes(int kind) {
-  const int v = conv_halo_variant();
-  return (kind == 0 && v > 0) ? kHaloSlots * halo_slot_bytes(v) : 0;
-}
-
-void conv_tile_shape(int Hout, int Wout, int* tile_w, int* tile_h, int kind) {
-  if (kind == 0 && conv_halo_variant() > 0) {
-    *tile_w = kHaloTileW;
-    *tile_h = kHaloTileH;
-    return;
-  }
+void conv_tile_shape(int Hout, int Wout, int* tile_w, int* tile_h) {
   int best_w = 16, best_tiles = 1 << 30;
   const int cands[5] = {128, 64, 32, 16, 8};
   for (int tw : cands) {
@@ -104,7 +70,7 @@ int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Ho
   p->M = NB * Hout * Wout;
   p->N = Cout;
   p->H = Hout; p->W = Wout;
-  conv_tile_shape(Hout, Wout, &p->tile_w, &p->tile_h, kind);
+  conv_tile_shape(Hout, Wout, &p->tile_w, &p->tile_h);
   p->tile_w_shift = 0;
   while ((1 << p->tile_w_shift) < p->tile_w) ++p->tile_w_shift;
   p->tiles_x = (Wout + p->tile_w - 1) / p->tile_w;
@@ -150,27 +116,11 @@ int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Ho
   splits = std::min(splits, p->num_kb);
   p->kb_per_split = (p->num_kb + splits - 1) / splits;
   p->stages = stages;
-  const int hv = (kind == 0 && !x2) ? conv_halo_variant() : 0;
-  uint32_t box_w = uint32_t(p->tile_w), box_h = uint32_t(p->tile_h);
-  if (hv > 0) {
-    // operand-reuse path: K order (channel block, tap), splits in whole channel blocks
-    p->mode = 2;
-    splits = std::min(splits, p->cblocks);
-    p->kb_per_split = 9 * ((p->cblocks + splits - 1) / splits);
-    p->halo_copies = hv == 3 ? 3 : 1;
-    p->halo_w = hv == 3 ? p->tile_w : p->tile_w + 2;
-    p->halo_copy_bytes = halo_copy_bytes(hv);
-    p->halo_slot_bytes = halo_slot_bytes(hv);
-    p->halo_slots = kHaloSlots;
-    p->halo_base_off = hv == 2;
-    box_w = uint32_t(p->halo_w);
-    box_h = uint32_t(p->tile_h + 2);
-  }
 
   const uint64_t C2 = uint64_t(Cin) * 2;
   const uint64_t dims[5] = {uint64_t(Cin), uint64_t(Wsrc), uint64_t(Hsrc), uint64_t(planes), uint64_t(NB)};
   const uint64_t strides[4] = {C2, C2 * Wsrc, C2 * Wsrc * Hsrc, C2 * Wsrc * Hsrc * planes};
-  const uint32_t box[5] = {64, box_w, box_h, 1, 1};
+  const uint32_t box[5] = {64, uint32_t(p->tile_w), uint32_t(p->tile_h), 1, 1};
   int rc = make_tmap_5d(&p->tmap_a, x, dims, strides, box);
   if (rc) return rc;
   if (x2) {
@@ -197,14 +147,13 @@ int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) 
   // Multi-wave grids run two CTAs per SM (gemm_tc.cu, MINB = 2): shallow operand rings of <= 113 KB, the epilogue of
   // one tile under the K loop of its neighbour. Single-wave grids, and tiles whose accumulators do not fit half the
   // register file (block_n > 128), keep one CTA per SM with a deep ring.
-  static const int two_cta_env = getenv("MGB_GEMM_2CTA") ? atoi(getenv("MGB_GEMM_2CTA")) : 1;
   // the drained operand ring doubles as the epilogue's staging scratch: it must hold gemm_epi_scratch_bytes()
   const int need = block_n > 16 ? int(gemm_epi_scratch_bytes(block_n)) : 0;
   int ctas_per_sm = 1;
   {
     const long long m_tiles = p.mode == 0 ? (p.M + 127) / 128 : (long long)(p.M / (p.H * p.W)) * p.tiles_x * p.tiles_y;
     const long long ctas = m_tiles * ((p.N + block_n - 1) / block_n) * splits;
-    if (two_cta_env && block_n >= 64 && block_n <= 128 && p.mode != 2 && ctas > kNumSMs) {
+    if (block_n >= 64 && block_n <= 128 && ctas > kNumSMs) {
       const int stage_bytes = 16384 + block_n * 128;
       const int max_st = (113 * 1024 - 1280) / stage_bytes;
       const int st = std::min(max_st, std::max(p.stages, (need + stage_bytes - 1) / stage_bytes));
@@ -215,13 +164,12 @@ int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) 
   if (block_n > 16 && ctas_per_sm == 1) {
     // deepen the pipeline until the ring holds the epilogue scratch
     for (;;) {
-      const int ring = (p.mode == 2 ? p.halo_slots * p.halo_slot_bytes : p.stages * 16384) + p.stages * block_n * 128;
+      const int ring = p.stages * (16384 + block_n * 128);
       if (ring >= need || p.stages >= 16) break;
       ++p.stages;
     }
   }
-  if (p.stages < 2 || p.stages > 8 ||
-      gemm_smem_bytes(block_n, p.stages, p.mode == 2 ? p.halo_slots * p.halo_slot_bytes : -1) > 227 * 1024) {
+  if (p.stages < 2 || p.stages > 8 || gemm_smem_bytes(block_n, p.stages) > 227 * 1024) {
     set_error("gemm: stages=%d does not fit shared memory for block_n=%d", p.stages, block_n);
     return MGB_ERR_INVALID;
   }
@@ -255,17 +203,15 @@ int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) 
   return MGB_OK;
 }
 
-static int tile_model() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("MGB_TILE_MODEL"); v = e ? atoi(e) : 1; }
-  return v;
-}
-
 // Tile-shape heuristic. Cost model (SM cycles): per CTA  num_kb * K-block time + epilogue + prologue; CTAs run in waves
 // of kNumSMs (1 CTA/SM). The H100's dense bf16 rate is 2048 MAC per cycle and SM, so a 128 x BN x 64 K block cannot take
 // less than 4*BN cycles (the tensor-core floor).
+// Measured on an H100 SXM (400 W) with the clock stamps of tools/gemm_phases.py, K = 2880, one CTA per SM:
+// K block 1030 cycles at BN = 256 (floor 1024), 814 at BN = 160 (floor 640), i.e. max(4*BN + 40, ~800);
+// epilogue 6.1 k cycles at BN = 128 / 160 and 9.8 k at BN = 256, ~2.5 k per 64 columns; prologue + first
+// operand ~3.6 k. The split-K reduce launch (~9000 cycles + its traffic) is an estimate, not measured.
 void choose_tile(int m_tiles, int N, int num_kb, bool geglu, bool allow_split, int* block_n, int* splits,
-                 int* stages, int a_ring_bytes) {
+                 int* stages) {
   const int cands[6] = {256, 160, 128, 64, 32, 16};
   double best = 1e30;
   int bbn = 128, bsp = 1;
@@ -274,45 +220,27 @@ void choose_tile(int m_tiles, int N, int num_kb, bool geglu, bool allow_split, i
     if (bn > 64 && N < bn / 2 + 1) continue;  // mostly padding
     if (bn < 64 && N >= 64) continue;         // 16 / 32 wide tiles are for the tiny heads only (N <= 32)
     const int n_tiles = (N + bn - 1) / bn;
-    const double waste = double(n_tiles) * bn / N;  // MMA work on padded columns is still paid
-    (void)waste;
     for (int sp = 1; sp <= (allow_split ? 16 : 1); ++sp) {
       if (sp > 1 && num_kb / sp < 4) break;
-      if (a_ring_bytes > 0 && sp > num_kb / 9) break;
       const long long ctas = (long long)m_tiles * n_tiles * sp;
       const long long waves = (ctas + kNumSMs - 1) / kNumSMs;
-      const int kb = a_ring_bytes > 0 ? 9 * ((num_kb / 9 + sp - 1) / sp) : (num_kb + sp - 1) / sp;
-      double t;
-      if (tile_model() == 0) {
-        // alternative model (MGB_TILE_MODEL=0); its epilogue / fixed / reduce constants are estimates, not measurements
-        double cta_cycles = double(kb) * 4.0 * bn + 6.0 * bn + 3000.0;
-        // small tiles are smem-bandwidth bound: A (16 KB) + B per k-block, B read by both warpgroups, at 128 B/cycle
-        const double smem_cycles = double(kb) * ((a_ring_bytes > 0 ? 2560.0 : 16384.0) + 2.0 * bn * 128.0) / 128.0 + 6.0 * bn + 3000.0;
-        cta_cycles = std::max(cta_cycles, smem_cycles);
-        t = waves * cta_cycles;
-        if (sp > 1) t += 4000.0 + double(m_tiles) * 128.0 * N * sp * 4.0 / (double(kNumSMs) * 64.0);  // reduce pass
-      } else {
-        // Measured on an H100 SXM (400 W) with the clock stamps of tools/gemm_phases.py, K = 2880, one CTA per SM:
-        // K block 1030 cycles at BN = 256 (floor 1024), 814 at BN = 160 (floor 640), i.e. max(4*BN + 40, ~800);
-        // epilogue 6.1 k cycles at BN = 128 / 160 and 9.8 k at BN = 256, ~2.5 k per 64 columns; prologue + first
-        // operand ~3.6 k. The split-K reduce launch (~9000 cycles + its traffic) is an estimate, not measured.
-        const double per_kb = std::max(4.0 * bn + 40.0, 800.0);
-        const double cta_cycles = double(kb) * per_kb + double((bn + 63) / 64) * 2500.0 + 3600.0;
-        t = waves * cta_cycles;
-        if (sp > 1) t += 9000.0 + double(m_tiles) * 128.0 * N * sp * 4.0 / (double(kNumSMs) * 64.0);
-      }
+      const int kb = (num_kb + sp - 1) / sp;
+      const double per_kb = std::max(4.0 * bn + 40.0, 800.0);
+      const double cta_cycles = double(kb) * per_kb + double((bn + 63) / 64) * 2500.0 + 3600.0;
+      double t = waves * cta_cycles;
+      if (sp > 1) t += 9000.0 + double(m_tiles) * 128.0 * N * sp * 4.0 / (double(kNumSMs) * 64.0);
       if (t < best) { best = t; bbn = bn; bsp = sp; }
     }
   }
   *block_n = bbn;
   *splits = bsp;
-  const int stage_bytes = (a_ring_bytes > 0 ? 0 : 16384) + bbn * 128;
+  const int stage_bytes = 16384 + bbn * 128;
   const int kb = (num_kb + bsp - 1) / bsp;
   // Deep pipelines (the whole 200 KB) only pay off for long K loops. Short-K GEMMs are dominated by
   // prologue / first-load / epilogue latency: cap them near 110 KB so that the NEXT kernel's CTA (launched
   // early through PDL) can become resident on the same SM and overlap its prologue and first operand loads
   // with this kernel's epilogue.
-  const int budget = (kb <= 12 ? 110 * 1024 : 200 * 1024) - a_ring_bytes;
+  const int budget = kb <= 12 ? 110 * 1024 : 200 * 1024;
   int st = int((budget - 2048) / stage_bytes);
   st = std::max(2, std::min(st, 8));
   st = std::min(st, std::max(2, kb));

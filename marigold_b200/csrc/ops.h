@@ -9,11 +9,8 @@ namespace mgb {
 void count_launch(int n);
 long long launch_count();
 
-// Halo variant used for 3x3 stride-1 convolutions (kind 0): 0 = off (mode 1, default), 1 = one (tile_h+2) x (tile_w+2)
-// box, 3 = three dx-shifted (tile_h+2) x tile_w boxes. Env MGB_CONV_HALO. Both are bit-compatible with mode 1.
-int conv_halo_variant();
-int conv_halo_ring_bytes(int kind);   // A ring bytes of the halo path (0 when the conv kind does not use it)
-void conv_tile_shape(int Hout, int Wout, int* tile_w, int* tile_h, int kind = -1);
+// Pixel rectangle of one conv output tile: tile_w x tile_h == 128, tile_w a power of two, fewest tiles over the image.
+void conv_tile_shape(int Hout, int Wout, int* tile_w, int* tile_h);
 
 // A [M, K] bf16 row-major, W [N, K] bf16 row-major.
 int fill_linear_params(GemmParams* p, const bf16* a, const bf16* w, int M, int N, int K, int block_n, int splits,
@@ -26,8 +23,8 @@ int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Ho
 int effective_splits(const GemmParams& p);
 // Launch (plus the deferred epilogue when split-K is active). p.epi must be filled by the caller.
 int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream);
-// a_ring_bytes > 0: halo conv (fixed A ring, B-only pipeline stages, split-K in units of 9 K blocks)
+// Tile width, split-K factor and pipeline depth of a GEMM with m_tiles 128-row tiles, N columns and num_kb K blocks of 64.
 void choose_tile(int m_tiles, int N, int num_kb, bool geglu, bool allow_split, int* block_n, int* splits,
-                 int* stages, int a_ring_bytes = 0);
+                 int* stages);
 
 }  // namespace mgb

@@ -206,7 +206,7 @@ def test_bfgs_driver_follows_scipy_default_finite_differences():
 
 
 def test_gelu_exponent_polynomial_matches_erf():
-    """The GEGLU epilogue's erf (csrc/common.cuh gelu_erf_f2: erfc(|x|/sqrt 2) = 2^-Q(|x|), degree-8 Q evaluated in
+    """The GEGLU epilogue's erf (csrc/common.cuh gelu_erf: erfc(|x|/sqrt 2) = 2^-Q(|x|), degree-8 Q evaluated in
     n = -|x|/2) restated in fp32 numpy with the constants read from the source: |gelu error| <= 5e-7 against the exact
     erf form diffusers' GEGLU uses (F.gelu, approximate="none"), over [-12, 12] and at the extremes."""
     import math

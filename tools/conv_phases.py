@@ -1,7 +1,6 @@
-"""Phase breakdown (clock64 stamps) + event timing of the dominant 3x3 conv (96x96, 320->320) under the current
-MGB_CONV_HALO / MGB_HALO_SLOTS environment. Usage: python tools/conv_phases.py [stages ...]"""
+"""Phase breakdown (clock64 stamps) + event timing of the dominant 3x3 conv (96x96, 320->320).
+Usage: python tools/conv_phases.py [stages ...]"""
 import ctypes as C
-import os
 import sys
 from pathlib import Path
 
@@ -41,8 +40,7 @@ def run(H, W, Cin, Cout, bn, stages, reps=20, flags=0):
           "epilogue": d[:, 4] - d[:, 3], "total": d[:, 5] - d[:, 0]}
     s = " ".join(f"{k}={v.median().item():.0f}/{v.max().item():.0f}" for k, v in ph.items())
     fl = 2.0 * H * W * Cout * Cin * 9
-    print(f"halo={os.environ.get('MGB_CONV_HALO', 'default')} slots={os.environ.get('MGB_HALO_SLOTS', '2')} "
-          f"{H}x{W} {Cin}->{Cout} bn{bn} st{stages} flags={flags:#x}: {us:.1f} us ({fl / us * 1e-6:.0f} TF/s) ctas={len(d)} cycles(med/max): {s}",
+    print(f"{H}x{W} {Cin}->{Cout} bn{bn} st{stages} flags={flags:#x}: {us:.1f} us ({fl / us * 1e-6:.0f} TF/s) ctas={len(d)} cycles(med/max): {s}",
           flush=True)
 
 

@@ -7,7 +7,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
 res = {}
-for fam in ["", "gn", "ln", "attn", "xattn", "concat", "gemm", "gn,ln,attn,xattn,concat", "gn,ln,attn,xattn,concat,gemm"]:
+for fam in ["", "gn", "ln", "attn", "xattn", "gemm", "gn,ln,attn,xattn", "gn,ln,attn,xattn,gemm"]:
     env = dict(os.environ)
     if fam:
         env["MGB_SKIP"] = fam
