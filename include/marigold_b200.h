@@ -172,6 +172,23 @@ int mgb_colorize(const float* depth_dev, int64_t HW, float dmin, float dmax, con
 size_t mgb_eval_ws_bytes(void);
 int mgb_eval_depth(const float* pred_dev, const float* gt_dev, const uint8_t* mask_dev, int64_t HW, int32_t least_squares,
                    float dmin, float dmax, float* aligned_out_dev, void* ws_dev, double* out_host, void* stream);
+/* mgb_eval_depth with every alignment of script/depth/eval.py:171-207 (same workspace, same out_host[13]). alignment: 0 none,
+ * 1 least_square, 2 least_square_disparity (:179-199: fit pred to 1 / gt over valid & gt > 0 & pred > 0, clip the aligned
+ * disparity to >= 1e-3 and take its reciprocal before the dataset clip). The metrics always use mask_dev. fit_rows_dev /
+ * fit_cols_dev: int32 [fit_h] / [fit_w] source row / column of each pixel of the downsampled maps the fit uses
+ * (align_depth_least_square's max_resolution, src/util/alignment.py:48-59), or both NULL to fit at full resolution. */
+int mgb_eval_depth_ex(const float* pred_dev, const float* gt_dev, const uint8_t* mask_dev, int32_t H, int32_t W,
+                      int32_t alignment, const int32_t* fit_rows_dev, const int32_t* fit_cols_dev, int32_t fit_h, int32_t fit_w,
+                      float dmin, float dmax, float* aligned_out_dev, void* ws_dev, double* out_host, void* stream);
+/* Surface-normals evaluation of one sample (script/normals/eval.py:145-157): the angular error of compute_cosine_error(
+ * masked=True) (src/util/metric.py:194-219) and the metrics of metric.py:222-257, in four launches and ONE synchronisation.
+ * pred_dev, gt_dev fp32 [3,H,W]; a pixel is valid where ||gt|| > 0 and mask_dev (uint8 [H,W], or NULL) is non-zero.
+ * error_out_dev: fp32 [H,W] angular error in degrees, NaN where not valid, or NULL. ws_dev: mgb_eval_normals_ws_bytes(H*W).
+ * out_host[9] = {n_valid, mean, median (np.median of the errors, exact), rmse, sub5, sub7.5, sub11.25, sub22.5, sub30}
+ * (percentages, unrounded); NaN metrics when n_valid == 0. Deterministic: equal inputs give equal bits. */
+size_t mgb_eval_normals_ws_bytes(int64_t HW);
+int mgb_eval_normals(const float* pred_dev, const float* gt_dev, const uint8_t* mask_dev, int32_t H, int32_t W,
+                     float* error_out_dev, void* ws_dev, double* out_host, void* stream);
 
 /* ---- capacity ------------------------------------------------------------------------------- */
 /* Bytes of the activation arena the handle holds for images of H x W with B members per batch. */

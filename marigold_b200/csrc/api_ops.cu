@@ -147,17 +147,52 @@ int mgb_colorize(const float* depth, int64_t HW, float dmin, float dmax, const u
 
 size_t mgb_eval_ws_bytes(void) { return eval_ws_bytes() + 16 * sizeof(double); }
 
-int mgb_eval_depth(const float* pred, const float* gt, const uint8_t* mask, int64_t HW, int32_t least_squares, float dmin,
-                   float dmax, float* aligned_out, void* ws, double* out_host, void* stream) {
-  if (!pred || !gt || !ws || !out_host || HW <= 0) { set_error("mgb_eval_depth: bad argument"); return MGB_ERR_INVALID; }
+static int eval_depth_run(const char* what, const float* pred, const float* gt, const uint8_t* mask, int64_t H, int64_t W,
+                          int32_t alignment, const int32_t* rows, const int32_t* cols, int32_t fit_h, int32_t fit_w, float dmin,
+                          float dmax, float* aligned_out, void* ws, double* out_host, void* stream) {
   double* out_dev = reinterpret_cast<double*>(static_cast<char*>(ws) + eval_ws_bytes());
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  int rc = launch_eval_depth(pred, gt, mask, HW, least_squares, dmin, dmax, aligned_out, ws, out_dev, s);
+  int rc = launch_eval_depth(pred, gt, mask, H, W, alignment, rows, cols, fit_h, fit_w, dmin, dmax, aligned_out, ws, out_dev, s);
   if (rc) return rc;
   count_launch(4);
   cudaError_t e = cudaMemcpyAsync(out_host, out_dev, 13 * sizeof(double), cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e != cudaSuccess) { set_error("mgb_eval_depth: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+  if (e != cudaSuccess) { set_error("%s: %s", what, cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+  return MGB_OK;
+}
+
+int mgb_eval_depth(const float* pred, const float* gt, const uint8_t* mask, int64_t HW, int32_t least_squares, float dmin,
+                   float dmax, float* aligned_out, void* ws, double* out_host, void* stream) {
+  if (!pred || !gt || !ws || !out_host || HW <= 0) { set_error("mgb_eval_depth: bad argument"); return MGB_ERR_INVALID; }
+  return eval_depth_run("mgb_eval_depth", pred, gt, mask, 1, HW, least_squares ? 1 : 0, nullptr, nullptr, 0, 0, dmin, dmax,
+                        aligned_out, ws, out_host, stream);
+}
+
+int mgb_eval_depth_ex(const float* pred, const float* gt, const uint8_t* mask, int32_t H, int32_t W, int32_t alignment,
+                      const int32_t* fit_rows, const int32_t* fit_cols, int32_t fit_h, int32_t fit_w, float dmin, float dmax,
+                      float* aligned_out, void* ws, double* out_host, void* stream) {
+  const bool tables = fit_rows || fit_cols;
+  if (!pred || !gt || !ws || !out_host || H <= 0 || W <= 0 || alignment < 0 || alignment > 2 ||
+      (tables && (!fit_rows || !fit_cols || fit_h <= 0 || fit_w <= 0))) {
+    set_error("mgb_eval_depth_ex: bad argument");
+    return MGB_ERR_INVALID;
+  }
+  return eval_depth_run("mgb_eval_depth_ex", pred, gt, mask, H, W, alignment, fit_rows, fit_cols, fit_h, fit_w, dmin, dmax,
+                        aligned_out, ws, out_host, stream);
+}
+
+size_t mgb_eval_normals_ws_bytes(int64_t HW) { return eval_normals_ws_bytes(HW); }
+
+int mgb_eval_normals(const float* pred, const float* gt, const uint8_t* mask, int32_t H, int32_t W, float* error_out, void* ws,
+                     double* out_host, void* stream) {
+  if (!pred || !gt || !ws || !out_host || H <= 0 || W <= 0) { set_error("mgb_eval_normals: bad argument"); return MGB_ERR_INVALID; }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  int rc = launch_eval_normals(pred, gt, mask, int64_t(H) * W, error_out, ws, s);
+  if (rc) return rc;
+  count_launch(4);
+  cudaError_t e = cudaMemcpyAsync(out_host, eval_normals_out(ws), 9 * sizeof(double), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) { set_error("mgb_eval_normals: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   return MGB_OK;
 }
 

@@ -2,10 +2,14 @@
 // scale / shift alignment of a prediction to the ground truth over the valid pixels (reference
 // src/util/alignment.py:35-82) and the masked depth metrics (src/util/metric.py:64-191) in two streaming passes and ONE
 // host synchronisation per sample (the reference does a numpy lstsq on the host and one `.item()` per metric).
-//   pass 1  sums n, sum p, sum p^2, sum g, sum p g over the mask (double) -> scale, shift from the 2 x 2 normal equations
-//   pass 2  aligned = clip(clip(p * scale + shift, dmin, dmax), 1e-6) (script/depth/eval.py:201-207) and the sums of every
-//           metric; a last block turns them into the metric values.
+//   pass 1  sums n, sum p, sum p^2, sum g, sum p g over the fit's pixels (double) -> scale, shift from the 2 x 2 normal
+//           equations. The fit is against gt, or against 1 / gt for least_square_disparity, over all pixels or over the
+//           nearest-downsampled map of max_resolution (index tables)
+//   pass 2  aligned = p * scale + shift; for disparity 1 / max(aligned, 1e-3); then clip(clip(., dmin, dmax), 1e-6)
+//           (script/depth/eval.py:196-207) and the sums of every metric over the full-resolution mask; a last block turns
+//           them into the metric values.
 // HBM-bound: 9 bytes / pixel / pass (pred f32, gt f32, mask u8).
+// The surface-normals evaluation (below) computes the angular error and the normals metrics with an exact median.
 #include <cfloat>
 
 #include "common.cuh"
@@ -34,13 +38,20 @@ __device__ __forceinline__ void block_reduce_store(double (&v)[kEvSums], int n, 
   }
 }
 
+// The fit's pixels: the full map (rows == nullptr), or the nearest-downsampled map of fit_h x fit_w pixels whose source row
+// and column are rows[i], cols[j] (align_depth_least_square's max_resolution, alignment.py:48-59). disparity: fit against
+// 1 / gt over valid & gt > 0 & pred > 0 (script/depth/eval.py:180-195; depth2disparity is fp32, alignment.py:85-94).
 __global__ void __launch_bounds__(kEvThreads)
     eval_align_sums_kernel(const float* __restrict__ pred, const float* __restrict__ gt, const uint8_t* __restrict__ mask,
-                           long long HW, double* __restrict__ part) {
+                           long long n_fit, long long W, const int* __restrict__ rows, const int* __restrict__ cols, int fit_w,
+                           int disparity, double* __restrict__ part) {
   double v[kEvSums] = {0};
-  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += (long long)gridDim.x * blockDim.x) {
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n_fit; q += (long long)gridDim.x * blockDim.x) {
+    const long long p = rows ? (long long)rows[q / fit_w] * W + cols[q % fit_w] : q;
     if (mask && !mask[p]) continue;
-    const double a = pred[p], g = gt[p];
+    const float pf = pred[p], gf = gt[p];
+    if (disparity && !(gf > 0.f && pf > 0.f)) continue;
+    const double a = pf, g = disparity ? __fdiv_rn(1.0f, gf) : gf;
     v[0] += 1.0; v[1] += a; v[2] += a * a; v[3] += g; v[4] += a * g;
   }
   block_reduce_store(v, 5, part);
@@ -79,14 +90,15 @@ __global__ void eval_align_solve_kernel(const double* __restrict__ part, int nbl
 
 __global__ void __launch_bounds__(kEvThreads)
     eval_metric_sums_kernel(const float* __restrict__ pred, const float* __restrict__ gt, const uint8_t* __restrict__ mask,
-                            long long HW, const double* __restrict__ st, float dmin, float dmax, float* __restrict__ aligned_out,
-                            double* __restrict__ part) {
+                            long long HW, const double* __restrict__ st, int disparity, float dmin, float dmax,
+                            float* __restrict__ aligned_out, double* __restrict__ part) {
   // numpy: float32 pred * float64 scale + float64 shift is float64, and torch promotes the float64 prediction against the
   // float32 ground truth (script/depth/eval.py:177-213), so the reference's metric arithmetic is double: so is this
   const double scale = st[0], shift = st[1];
   double v[kEvSums] = {0};
   for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += (long long)gridDim.x * blockDim.x) {
     double a = double(pred[p]) * scale + shift;
+    if (disparity) a = 1.0 / fmax(a, 1e-3);              // clip the disparity to >= 1e-3, back to depth (eval.py:196-200)
     a = fmin(fmax(a, double(dmin)), double(dmax));
     a = fmax(a, 1e-6);
     if (aligned_out) aligned_out[p] = float(a);
@@ -132,17 +144,244 @@ __global__ void eval_metric_final_kernel(const double* __restrict__ part, int nb
 size_t eval_ws_bytes() { return size_t(kEvBlocks) * kEvSums * sizeof(double) + 16 * sizeof(double) + 64; }
 
 // out_dev: 13 doubles {scale, shift, n_valid, abs_rel, sq_rel, rmse, rmse_log, log10, delta1, delta2, delta3, i_rmse, silog}
-int launch_eval_depth(const float* pred, const float* gt, const uint8_t* mask, long long HW, int do_align, float dmin, float dmax,
-                      float* aligned_out, void* ws, double* out_dev, cudaStream_t stream) {
+// align: 0 none, 1 least squares on depth, 2 least squares on disparity. rows / cols: the fit's index tables (fit_h x fit_w
+// pixels) or nullptr for a fit over all H x W pixels.
+int launch_eval_depth(const float* pred, const float* gt, const uint8_t* mask, long long H, long long W, int align,
+                      const int* rows, const int* cols, int fit_h, int fit_w, float dmin, float dmax, float* aligned_out,
+                      void* ws, double* out_dev, cudaStream_t stream) {
   double* part = static_cast<double*>(ws);
   double* st = part + size_t(kEvBlocks) * kEvSums;
+  const long long HW = H * W, n_fit = rows ? (long long)fit_h * fit_w : HW;
   const int blocks = int(std::min<long long>((HW + kEvThreads - 1) / kEvThreads, kEvBlocks));
-  eval_align_sums_kernel<<<blocks, kEvThreads, 0, stream>>>(pred, gt, mask, HW, part);
-  eval_align_solve_kernel<<<1, 32, 0, stream>>>(part, blocks, do_align, st);
-  eval_metric_sums_kernel<<<blocks, kEvThreads, 0, stream>>>(pred, gt, mask, HW, st, dmin, dmax, aligned_out, part);
+  const int fit_blocks = int(std::min<long long>((n_fit + kEvThreads - 1) / kEvThreads, kEvBlocks));
+  eval_align_sums_kernel<<<fit_blocks, kEvThreads, 0, stream>>>(pred, gt, mask, n_fit, W, rows, cols, fit_w, align == 2, part);
+  eval_align_solve_kernel<<<1, 32, 0, stream>>>(part, fit_blocks, align != 0, st);
+  eval_metric_sums_kernel<<<blocks, kEvThreads, 0, stream>>>(pred, gt, mask, HW, st, align == 2, dmin, dmax, aligned_out, part);
   eval_metric_final_kernel<<<1, 32, 0, stream>>>(part, blocks, st, out_dev);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_error("eval_depth launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+  return MGB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Surface-normals evaluation (script/normals/eval.py:145-157): compute_cosine_error(masked=True) (src/util/metric.py:
+// 194-219) and the metrics of metric.py:222-257 in four launches and ONE synchronisation.
+//   error    per-pixel angular error, written to the workspace (and error_out); fixed-order double sums of n, e, e^2 and
+//            the five threshold counts; a histogram of the high 16 bits of the errors (shared memory, then global)
+//   locate   one block: the high-16 bins holding the order statistics (n-1)/2 and n/2 and their ranks inside the bins
+//   refine   histograms of the low 16 bits of the errors that fall in those two bins
+//   final    one block: the two order statistics exactly, np.median's mean of them, the other metrics
+// The errors are >= 0, so the unsigned order of their bit patterns is their numeric order, and integer counts do not
+// depend on the order the atomics land in: the median is exact and every output is deterministic.
+constexpr int kNrHiBins = 0x4335 + 1;       // high halves of [0, 180.00002]; the last bin takes anything above (NaN)
+constexpr int kNrLoBins = 1 << 16;
+constexpr int kNrSelThreads = 1024;
+constexpr unsigned kNrInvalid = 0xFFFFFFFFu;  // workspace bits of a pixel that is not valid
+constexpr float kInvPi = 1.0f / 3.14159265358979323846f;
+
+struct NrSel {
+  unsigned n;
+  unsigned bin[2];    // high-16 bin of order statistics (n-1)/2 and n/2 (kNrInvalid when n == 0)
+  unsigned rank[2];   // rank inside that bin
+};
+
+__device__ __forceinline__ unsigned nr_bin(unsigned bits) { return min(bits >> 16, unsigned(kNrHiBins - 1)); }
+
+// torch.cosine_similarity(pred, gt, dim=0) (each vector over max(norm, 1e-8), then the products summed over the channels
+// in order), clamp(-1, 1), acos, * 180.0, / pi. torch's CUDA division by a scalar multiplies by its fp32 reciprocal,
+// which is what the reference's evaluation on the GPU computes. No contraction, in the reference's order.
+__device__ __forceinline__ float angular_error(float x0, float x1, float x2, float y0, float y1, float y2, float ny) {
+  const float nx = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x0, x0), __fmul_rn(x1, x1)), __fmul_rn(x2, x2)));
+  const float dx = fmaxf(nx, 1e-8f), dy = fmaxf(ny, 1e-8f);
+  float c = __fadd_rn(__fadd_rn(__fmul_rn(__fdiv_rn(x0, dx), __fdiv_rn(y0, dy)), __fmul_rn(__fdiv_rn(x1, dx), __fdiv_rn(y1, dy))),
+                      __fmul_rn(__fdiv_rn(x2, dx), __fdiv_rn(y2, dy)));
+  c = fminf(fmaxf(c, -1.0f), 1.0f);
+  return __fmul_rn(__fmul_rn(acosf(c), 180.0f), kInvPi);
+}
+
+// The loops below step over whole warps (base is warp-uniform), so the warp-aggregated atomics can use the full mask:
+// lanes with equal keys add once (heavy ties, e.g. pred == gt, would otherwise serialise on one counter).
+__device__ __forceinline__ void warp_agg_add(unsigned* __restrict__ hist, unsigned key, bool take) {
+  const unsigned k = take ? key : kNrInvalid;
+  const unsigned peers = __match_any_sync(0xffffffffu, k);
+  if (take && (threadIdx.x & 31) == unsigned(__ffs(peers) - 1)) atomicAdd(hist + key, unsigned(__popc(peers)));
+}
+
+__global__ void __launch_bounds__(kEvThreads)
+    eval_normals_error_kernel(const float* __restrict__ pred, const float* __restrict__ gt, const uint8_t* __restrict__ mask,
+                              long long HW, unsigned* __restrict__ err_bits, float* __restrict__ err_out,
+                              unsigned* __restrict__ hist_hi, double* __restrict__ part) {
+  extern __shared__ unsigned sh_hist[];
+  for (int i = threadIdx.x; i < kNrHiBins; i += blockDim.x) sh_hist[i] = 0;
+  __syncthreads();
+  double v[kEvSums] = {0};
+  for (long long base = (long long)blockIdx.x * blockDim.x; base < HW; base += (long long)gridDim.x * blockDim.x) {
+    const long long p = base + threadIdx.x;
+    bool valid = false;
+    unsigned bits = kNrInvalid;
+    if (p < HW) {
+      const float y0 = gt[p], y1 = gt[p + HW], y2 = gt[p + 2 * HW];
+      // torch.norm(gt, dim=0) > 0 (metric.py:205-211), ANDed with the caller's mask
+      const float ny = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(y0, y0), __fmul_rn(y1, y1)), __fmul_rn(y2, y2)));
+      valid = ny > 0.f && (!mask || mask[p]);
+      float e = __int_as_float(0x7fffffff);
+      if (valid) {
+        e = angular_error(pred[p], pred[p + HW], pred[p + 2 * HW], y0, y1, y2, ny);
+        bits = e == e ? __float_as_uint(e) : 0x7fffffffu;
+        const double d = e;
+        v[0] += 1.0; v[1] += d; v[2] += d * d;
+        v[3] += e < 5.0f ? 1.0 : 0.0;
+        v[4] += e < 7.5f ? 1.0 : 0.0;
+        v[5] += e < 11.25f ? 1.0 : 0.0;
+        v[6] += e < 22.5f ? 1.0 : 0.0;
+        v[7] += e < 30.0f ? 1.0 : 0.0;
+      }
+      err_bits[p] = bits;
+      if (err_out) err_out[p] = e;
+    }
+    warp_agg_add(sh_hist, nr_bin(bits), valid);
+  }
+  block_reduce_store(v, 8, part);
+  __syncthreads();
+  for (int i = threadIdx.x; i < kNrHiBins; i += blockDim.x)
+    if (sh_hist[i]) atomicAdd(hist_hi + i, sh_hist[i]);
+}
+
+// Exclusive prefix sum over a block of kNrSelThreads threads; *total = the sum of all.
+__device__ __forceinline__ unsigned block_exclusive_scan(unsigned x, unsigned* total) {
+  __shared__ unsigned sh[kNrSelThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned inc = x;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  __syncthreads();                     // sh may still be read by a previous call
+  if (lane == 31) sh[warp] = inc;
+  __syncthreads();
+  unsigned before = 0, all = 0;
+  for (int w = 0; w < kNrSelThreads / 32; ++w) {
+    if (w < warp) before += sh[w];
+    all += sh[w];
+  }
+  *total = all;
+  return before + inc - x;
+}
+
+// Thread t owns bins [t * per, (t + 1) * per): finds the bin holding rank k and the rank inside it.
+__device__ __forceinline__ void find_rank(const unsigned* __restrict__ hist, int nbins, unsigned k, unsigned* bin_out,
+                                          unsigned* rank_out) {
+  const int per = (nbins + kNrSelThreads - 1) / kNrSelThreads;
+  const int b0 = threadIdx.x * per, b1 = min(b0 + per, nbins);
+  unsigned local = 0;
+  for (int b = b0; b < b1; ++b) local += hist[b];
+  unsigned total;
+  unsigned c = block_exclusive_scan(local, &total);
+  if (k < c || k >= c + local) return;
+  for (int b = b0; b < b1; ++b) {
+    if (k < c + hist[b]) { *bin_out = b; *rank_out = k - c; return; }
+    c += hist[b];
+  }
+}
+
+__global__ void __launch_bounds__(kNrSelThreads) eval_normals_locate_kernel(const unsigned* __restrict__ hist_hi, NrSel* sel) {
+  unsigned local = 0;
+  const int per = (kNrHiBins + kNrSelThreads - 1) / kNrSelThreads;
+  for (int b = threadIdx.x * per; b < min((int(threadIdx.x) + 1) * per, kNrHiBins); ++b) local += hist_hi[b];
+  unsigned n;
+  block_exclusive_scan(local, &n);
+  if (threadIdx.x == 0) {
+    sel->n = n;
+    sel->bin[0] = sel->bin[1] = kNrInvalid;
+  }
+  __syncthreads();
+  if (n == 0) return;
+  find_rank(hist_hi, kNrHiBins, (n - 1) / 2, &sel->bin[0], &sel->rank[0]);
+  find_rank(hist_hi, kNrHiBins, n / 2, &sel->bin[1], &sel->rank[1]);
+}
+
+__global__ void __launch_bounds__(kEvThreads)
+    eval_normals_refine_kernel(const unsigned* __restrict__ err_bits, long long HW, const NrSel* __restrict__ sel,
+                               unsigned* __restrict__ hist_lo) {
+  const unsigned b0 = sel->bin[0], b1 = sel->bin[1];
+  for (long long base = (long long)blockIdx.x * blockDim.x; base < HW; base += (long long)gridDim.x * blockDim.x) {
+    const long long p = base + threadIdx.x;
+    const unsigned bits = p < HW ? err_bits[p] : kNrInvalid;
+    const unsigned bin = bits == kNrInvalid ? kNrInvalid : nr_bin(bits);
+    const unsigned which = bin == b0 ? 0u : 1u;     // both ranks in one bin: one histogram serves both
+    warp_agg_add(hist_lo, which * kNrLoBins + (bits & 0xFFFFu), bin == b0 || bin == b1);
+  }
+}
+
+// out: {n_valid, mean, median, rmse, sub5, sub7.5, sub11.25, sub22.5, sub30}
+__global__ void __launch_bounds__(kNrSelThreads)
+    eval_normals_final_kernel(const double* __restrict__ part, int nblocks, NrSel* sel, const unsigned* __restrict__ hist_lo,
+                              double* __restrict__ out) {
+  __shared__ unsigned lo[2], rank_unused;
+  const unsigned n = sel->n;
+  if (n > 0) {
+    find_rank(hist_lo, kNrLoBins, sel->rank[0], &lo[0], &rank_unused);
+    find_rank(hist_lo + (sel->bin[1] == sel->bin[0] ? 0 : kNrLoBins), kNrLoBins, sel->rank[1], &lo[1], &rank_unused);
+  }
+  __shared__ double s[8];
+  if (threadIdx.x < 32)
+    for (int k = 0; k < 8; ++k) {
+      const double t = warp_sum_partials(part, nblocks, k);
+      if (threadIdx.x == 0) s[k] = t;
+    }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  out[0] = s[0];
+  if (n == 0) {                        // numpy's statistics of an empty array
+#pragma unroll
+    for (int k = 1; k < 9; ++k) out[k] = __longlong_as_double(0x7ff8000000000000ll);
+    return;
+  }
+  const unsigned nan_bits = 0x7fffffffu, top = kNrHiBins - 1;
+  const float v0 = __uint_as_float(sel->bin[0] == top ? nan_bits : (sel->bin[0] << 16) | lo[0]);
+  const float v1 = __uint_as_float(sel->bin[1] == top ? nan_bits : (sel->bin[1] << 16) | lo[1]);
+  out[1] = s[1] / s[0];
+  out[2] = __fdiv_rn(__fadd_rn(v0, v1), 2.0f);       // np.median: float32 mean of the two middle values
+  out[3] = sqrt(s[2] / s[0]);
+#pragma unroll
+  for (int k = 0; k < 5; ++k) out[4 + k] = 100.0 * (s[3 + k] / s[0]);
+}
+
+// Workspace: partials | 16 doubles of results | NrSel | high and low histograms | the error map (4 B per pixel).
+constexpr size_t kNrOutOff = size_t(kEvBlocks) * kEvSums * sizeof(double);
+constexpr size_t kNrSelOff = kNrOutOff + 16 * sizeof(double);
+constexpr size_t kNrHistOff = kNrSelOff + 64;
+constexpr size_t kNrHistBytes = (size_t(kNrHiBins + 3) / 4 * 4 + 2 * kNrLoBins) * sizeof(unsigned);
+constexpr size_t kNrErrOff = kNrHistOff + kNrHistBytes;
+
+size_t eval_normals_ws_bytes(long long HW) { return kNrErrOff + size_t(HW) * sizeof(unsigned); }
+double* eval_normals_out(void* ws) { return reinterpret_cast<double*>(static_cast<char*>(ws) + kNrOutOff); }
+
+int launch_eval_normals(const float* pred, const float* gt, const uint8_t* mask, long long HW, float* err_out, void* ws,
+                        cudaStream_t stream) {
+  char* w = static_cast<char*>(ws);
+  double* part = reinterpret_cast<double*>(w);
+  NrSel* sel = reinterpret_cast<NrSel*>(w + kNrSelOff);
+  unsigned* hist_hi = reinterpret_cast<unsigned*>(w + kNrHistOff);
+  unsigned* hist_lo = hist_hi + (kNrHiBins + 3) / 4 * 4;
+  unsigned* err_bits = reinterpret_cast<unsigned*>(w + kNrErrOff);
+  constexpr size_t smem = kNrHiBins * sizeof(unsigned);
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(eval_normals_error_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) { set_error("eval_normals: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+    attr_set = true;
+  }
+  const int blocks = int(std::min<long long>((HW + kEvThreads - 1) / kEvThreads, kEvBlocks));
+  cudaError_t e = cudaMemsetAsync(hist_hi, 0, kNrHistBytes, stream);
+  if (e != cudaSuccess) { set_error("eval_normals memset: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+  eval_normals_error_kernel<<<blocks, kEvThreads, smem, stream>>>(pred, gt, mask, HW, err_bits, err_out, hist_hi, part);
+  eval_normals_locate_kernel<<<1, kNrSelThreads, 0, stream>>>(hist_hi, sel);
+  eval_normals_refine_kernel<<<blocks, kEvThreads, 0, stream>>>(err_bits, HW, sel, hist_lo);
+  eval_normals_final_kernel<<<1, kNrSelThreads, 0, stream>>>(part, blocks, sel, hist_lo, eval_normals_out(ws));
+  e = cudaGetLastError();
+  if (e != cudaSuccess) { set_error("eval_normals launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   return MGB_OK;
 }
 

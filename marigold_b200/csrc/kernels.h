@@ -170,8 +170,16 @@ int launch_resize(const void* src, int src_is_u8, int NC, int H, int W, float* d
 int launch_colorize(const float* depth, long long HW, float dmin, float dmax, const uint8_t* lut, uint8_t* out,
                     cudaStream_t stream);
 size_t eval_ws_bytes();
-int launch_eval_depth(const float* pred, const float* gt, const uint8_t* mask, long long HW, int do_align, float dmin, float dmax,
-                      float* aligned_out, void* ws, double* out_dev, cudaStream_t stream);
+// align 0 none, 1 least squares on depth, 2 least squares on disparity; rows / cols: int32 [fit_h] / [fit_w] source indices
+// of a nearest-downsampled fit, or nullptr to fit over all H x W pixels. out_dev: 13 doubles (mgb_eval_depth's order).
+int launch_eval_depth(const float* pred, const float* gt, const uint8_t* mask, long long H, long long W, int align,
+                      const int* rows, const int* cols, int fit_h, int fit_w, float dmin, float dmax, float* aligned_out,
+                      void* ws, double* out_dev, cudaStream_t stream);
+// pred, gt fp32 [3, HW]; mask u8 [HW] or nullptr; err_out fp32 [HW] or nullptr. Results: 9 doubles at eval_normals_out(ws).
+size_t eval_normals_ws_bytes(long long HW);
+double* eval_normals_out(void* ws);
+int launch_eval_normals(const float* pred, const float* gt, const uint8_t* mask, long long HW, float* err_out, void* ws,
+                        cudaStream_t stream);
 
 // ---------------------------------------------------------------------------------------------
 // Ensemble kernels (ensemble.cu)

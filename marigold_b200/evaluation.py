@@ -1,6 +1,10 @@
-"""Device-side evaluation step that follows the hot path in dataset evaluation (csrc/eval.cu): least-squares scale / shift
-alignment (reference src/util/alignment.py:35-82), the clips of script/depth/eval.py:201-207 and the masked depth metrics
-of src/util/metric.py:64-191 — two streaming passes and one host synchronisation per sample."""
+"""Device-side evaluation step that follows the hot path in dataset evaluation (csrc/eval.cu).
+
+Depth: least-squares scale / shift alignment in depth or disparity space (reference src/util/alignment.py:35-82,
+script/depth/eval.py:171-207), the dataset clips and the masked depth metrics of src/util/metric.py:64-191 — two
+streaming passes and one host synchronisation per sample.
+Surface normals: the angular error of compute_cosine_error(masked=True) and the metrics of src/util/metric.py:194-257,
+including the exact median — four launches and one host synchronisation per sample."""
 from __future__ import annotations
 
 import ctypes as C
@@ -14,30 +18,79 @@ from ._lib import check, ptr, stream_ptr
 
 METRIC_NAMES = ("abs_relative_difference", "squared_relative_difference", "rmse_linear", "rmse_log", "log10", "delta1_acc",
                 "delta2_acc", "delta3_acc", "i_rmse", "silog_rmse")
+NORMALS_METRIC_NAMES = ("mean_angular_error", "median_angular_error", "rmse_angular_error", "sub5_error", "sub7_5_error",
+                        "sub11_25_error", "sub22_5_error", "sub30_error")
+ALIGNMENTS = (None, "least_square", "least_square_disparity")
 _ws = {}
+_normals_ws = {}
 
 
-def _run(pred, gt, mask, least_squares: bool, dmin: float, dmax: float, want_aligned: bool):
+def _inputs(pred, gt, mask):
     if not (pred.is_cuda and gt.is_cuda):
         raise _lib.MgbError("marigold_b200.evaluation needs CUDA tensors (no CPU fallback)")
-    lib = _lib.load()
     p = pred.to(torch.float32).contiguous().reshape(-1)
     g = gt.to(torch.float32).contiguous().reshape(-1)
     assert p.numel() == g.numel(), f"{tuple(pred.shape)} vs {tuple(gt.shape)}"
     m = None
     if mask is not None:
         m = mask.to(device=p.device).to(torch.uint8).contiguous().reshape(-1)
-        assert m.numel() == p.numel()
+    return p, g, m
+
+
+def _depth_ws(lib, device):
+    ws = _ws.get(device)
+    if ws is None:
+        ws = torch.empty(int(lib.mgb_eval_ws_bytes()), dtype=torch.uint8, device=device)
+        _ws[device] = ws
+    return ws
+
+
+def _run(pred, gt, mask, least_squares: bool, dmin: float, dmax: float, want_aligned: bool):
+    p, g, m = _inputs(pred, gt, mask)
+    assert m is None or m.numel() == p.numel()
+    lib = _lib.load()
     with torch.cuda.device(p.device):
-        ws = _ws.get(p.device)
-        if ws is None:
-            ws = torch.empty(int(lib.mgb_eval_ws_bytes()), dtype=torch.uint8, device=p.device)
-            _ws[p.device] = ws
+        ws = _depth_ws(lib, p.device)
         aligned = torch.empty_like(p) if want_aligned else None
         out = np.zeros(13, dtype=np.float64)
         check(lib.mgb_eval_depth(ptr(p), ptr(g), ptr(m), p.numel(), int(least_squares), float(dmin), float(dmax), ptr(aligned),
                                  ptr(ws), out.ctypes.data_as(C.c_void_p), stream_ptr()), "mgb_eval_depth")
     return out, (aligned.reshape(pred.shape) if aligned is not None else None)
+
+
+def fit_index_tables(H: int, W: int, max_resolution: Optional[int]):
+    """Source rows and columns of the maps align_depth_least_square fits when given max_resolution (alignment.py:48-59),
+    or None when the fit uses the full maps. The reference hands torch.nn.Upsample a [1, H, W] tensor (the squeezed map
+    with one leading dimension), which Upsample reads as a batch of H one-dimensional signals of length W: only the width
+    is downsampled. The tables are that same Upsample applied to the indices themselves, so its rounding is torch's."""
+    if max_resolution is None:
+        return None
+    sf = np.min(max_resolution / np.array((H, W)))
+    if not sf < 1:
+        return None
+    down = torch.nn.Upsample(scale_factor=sf, mode="nearest")
+    cols = down(torch.arange(W, dtype=torch.float64).reshape(1, 1, W)).reshape(-1)
+    rows = torch.arange(H, dtype=torch.float64)
+    return rows.to(torch.int32), cols.to(torch.int32)
+
+
+def _run_ex(pred, gt, mask, mode: int, max_resolution, dmin: float, dmax: float):
+    H, W = pred.shape[-2:]
+    p, g, m = _inputs(pred, gt, mask)
+    lib = _lib.load()
+    assert p.numel() == H * W and (m is None or m.numel() == p.numel()), "depth maps must be [H, W] (or squeeze to it)"
+    tables = fit_index_tables(H, W, max_resolution) if mode else None
+    with torch.cuda.device(p.device):
+        ws = _depth_ws(lib, p.device)
+        rows = cols = None
+        if tables is not None:
+            rows, cols = (t.to(p.device) for t in tables)
+        out = np.zeros(13, dtype=np.float64)
+        check(lib.mgb_eval_depth_ex(ptr(p), ptr(g), ptr(m), H, W, mode, ptr(rows), ptr(cols),
+                                    0 if rows is None else rows.numel(), 0 if cols is None else cols.numel(), float(dmin),
+                                    float(dmax), None, ptr(ws), out.ctypes.data_as(C.c_void_p), stream_ptr()),
+              "mgb_eval_depth_ex")
+    return out
 
 
 def align_depth_least_square(gt: torch.Tensor, pred: torch.Tensor, valid_mask: Optional[torch.Tensor],
@@ -59,12 +112,56 @@ def align_depth_least_square(gt: torch.Tensor, pred: torch.Tensor, valid_mask: O
 
 
 def evaluate_depth(pred: torch.Tensor, gt: torch.Tensor, valid_mask: Optional[torch.Tensor] = None,
-                   alignment: Optional[str] = "least_square", min_depth: float = 1e-6, max_depth: float = 3.0e38
-                   ) -> Tuple[Dict[str, float], Dict[str, float]]:
+                   alignment: Optional[str] = "least_square", min_depth: float = 1e-6, max_depth: float = 3.0e38,
+                   alignment_max_res: Optional[int] = None) -> Tuple[Dict[str, float], Dict[str, float]]:
     """One sample of script/depth/eval.py:171-217: align (or not), clip to the dataset range and to d > 1e-6, all metrics.
+
+    alignment: None, "least_square" (fit pred to gt) or "least_square_disparity" (fit pred to 1 / gt over the valid
+    pixels where gt > 0 and pred > 0, clip the aligned disparity to >= 1e-3 and take its reciprocal). The metrics always
+    use `valid_mask`. alignment_max_res: fit on the maps downsampled as align_depth_least_square(max_resolution=...)
+    downsamples them (see fit_index_tables); the metrics use the full-resolution maps.
     Returns (metrics by the reference's function names, {"scale", "shift", "n_valid"})."""
-    if alignment not in (None, "least_square"):
-        raise ValueError(f"unsupported alignment {alignment!r} (least_square_disparity is not implemented on the device)")
-    out, _ = _run(pred, gt, valid_mask, alignment == "least_square", min_depth, max_depth, False)
+    if alignment not in ALIGNMENTS:
+        raise ValueError(f"unsupported alignment {alignment!r}; expected one of {ALIGNMENTS}")
+    if alignment in (None, "least_square") and alignment_max_res is None:
+        out, _ = _run(pred, gt, valid_mask, alignment == "least_square", min_depth, max_depth, False)
+    else:
+        out = _run_ex(pred, gt, valid_mask, ALIGNMENTS.index(alignment), alignment_max_res, min_depth, max_depth)
     metrics = dict(zip(METRIC_NAMES, (float(v) for v in out[3:13])))
     return metrics, {"scale": float(out[0]), "shift": float(out[1]), "n_valid": int(out[2])}
+
+
+def evaluate_normals(pred: torch.Tensor, gt: torch.Tensor, valid_mask: Optional[torch.Tensor] = None,
+                     return_error_map: bool = False) -> Tuple[Dict[str, float], Dict[str, object]]:
+    """One sample of script/normals/eval.py:145-157: the angular error in degrees of compute_cosine_error(pred, gt,
+    masked=True) (src/util/metric.py:194-219) and the metrics of metric.py:222-257 over it.
+
+    pred, gt: [3, H, W] or [1, 3, H, W] CUDA tensors, channel first. A pixel counts where ||gt|| > 0, as in the
+    reference, and, when `valid_mask` ([H, W]) is given, where it is also true. The median is np.median's exactly: the
+    middle error for odd n, the float32 mean of the two middle errors for even n. The values are NOT rounded; the
+    reference rounds each to 4 decimals (round(x, 4)). With no valid pixel every metric is NaN, as numpy gives for an
+    empty array. Returns (metrics by the reference's function names, {"n_valid"[, "error_map"]}), where "error_map" is
+    the [H, W] float32 error, NaN where the pixel does not count."""
+    if pred.dim() == 4:
+        pred = pred.squeeze(0)
+    if gt.dim() == 4:
+        gt = gt.squeeze(0)
+    assert pred.shape[0] == 3 and gt.shape == pred.shape, f"expected [3, H, W], got {tuple(pred.shape)} and {tuple(gt.shape)}"
+    H, W = pred.shape[-2:]
+    p, g, m = _inputs(pred, gt, valid_mask)
+    assert m is None or m.numel() == H * W
+    lib = _lib.load()
+    with torch.cuda.device(p.device):
+        need = int(lib.mgb_eval_normals_ws_bytes(H * W))
+        ws = _normals_ws.get(p.device)
+        if ws is None or ws.numel() < need:
+            ws = torch.empty(need, dtype=torch.uint8, device=p.device)
+            _normals_ws[p.device] = ws
+        err = torch.empty(H, W, dtype=torch.float32, device=p.device) if return_error_map else None
+        out = np.zeros(9, dtype=np.float64)
+        check(lib.mgb_eval_normals(ptr(p), ptr(g), ptr(m), H, W, ptr(err), ptr(ws), out.ctypes.data_as(C.c_void_p),
+                                   stream_ptr()), "mgb_eval_normals")
+    info = {"n_valid": int(out[0])}
+    if err is not None:
+        info["error_map"] = err
+    return dict(zip(NORMALS_METRIC_NAMES, (float(v) for v in out[1:]))), info
