@@ -115,22 +115,17 @@ int mgb_decode(mgb_handle* h, const float* latent_dev, int32_t B, int32_t lh, in
                float* out_dev, void* stream);
 
 /* ---- ensembling (marigold/util/ensemble.py) ------------------------------------------------- */
-/* cost_fn of ensemble_depth (ensemble.py:138-152) in ONE pass and ONE host sync:
+/* cost_fn of ensemble_depth (ensemble.py:138-152) at one point, in ONE host sync:
  * depth_dev [E,HW] fp32; param_host = [s_0..s_{E-1}, t_0..t_{E-1}] (or only s when !shift);
  * returns sum_{i<j} RMSE(a_i - a_j) + reg * (|min(med)| + |1 - max(med)|). Synchronises. */
 int mgb_ens_depth_cost(mgb_handle* h, const float* depth_dev, const double* param_host, int32_t E, int64_t HW,
                        int32_t scale_invariant, int32_t shift_invariant, int32_t reduction_median,
                        double regularizer, double* cost_out, void* stream);
-/* The same objective for P parameter vectors (params_host [P][2E], or [P][E] when !shift) in ONE launch and ONE
- * synchronisation: the 2E forward-difference points of one scipy BFGS gradient (ensemble.py:165-171; scipy's
- * approx_derivative) are one call. costs_out_host [P]. cost(x) is bit-identical to mgb_ens_depth_cost(x). */
-int mgb_ens_depth_cost_batch(mgb_handle* h, const float* depth_dev, const double* params_host, int32_t P, int32_t E,
-                             int64_t HW, int32_t scale_invariant, int32_t shift_invariant, int32_t reduction_median,
-                             double regularizer, double* costs_out_host, void* stream);
-/* One forward-difference gradient of that objective in a single pass (scipy approx_derivative as BFGS calls it,
- * ensemble.py:165-171): base_host [n] is the current point, pert_host [n] the same vector with EVERY coordinate moved to
- * its perturbed value x_i + h_i; costs_out_host [1 + n]: [0] = cost(base), [1 + i] = cost(base with coordinate i
- * perturbed), each bit-identical to mgb_ens_depth_cost of that vector. n = 2E (or E when !shift); E <= 16. */
+/* That objective and the points of one forward-difference gradient in ONE host sync (scipy approx_derivative as BFGS
+ * calls it, ensemble.py:165-171): base_host [n] is the current point, pert_host [n] the same vector with EVERY
+ * coordinate moved to its perturbed value x_i + h_i; costs_out_host [1 + n]: [0] = cost(base), [1 + i] = cost(base with
+ * coordinate i perturbed), each bit-identical to mgb_ens_depth_cost of that vector. n = 2E (or E when !shift); any E up
+ * to mgb_ens_max_members(). */
 int mgb_ens_depth_cost_fd(mgb_handle* h, const float* depth_dev, const double* base_host, const double* pert_host,
                           int32_t E, int64_t HW, int32_t scale_invariant, int32_t shift_invariant,
                           int32_t reduction_median, double regularizer, double* costs_out_host, void* stream);

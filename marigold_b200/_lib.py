@@ -54,7 +54,6 @@ SIGNATURES = {
     "mgb_denoise_range": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "mgb_decode": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     "mgb_ens_depth_cost": (_i32, [_vp, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _f64, C.POINTER(_f64), _vp]),
-    "mgb_ens_depth_cost_batch": (_i32, [_vp, _vp, _vp, _i32, _i32, _i64, _i32, _i32, _i32, _f64, _vp, _vp]),
     "mgb_ens_depth_cost_fd": (_i32, [_vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _f64, _vp, _vp]),
     "mgb_ens_max_members": (_i32, []),
     "mgb_ens_minmax": (_i32, [_vp, _vp, _i32, _i64, _vp, _vp, _vp]),

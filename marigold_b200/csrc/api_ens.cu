@@ -46,68 +46,51 @@ static int make_st(const double* param, int E, int scale_inv, int shift_inv, flo
   return MGB_OK;
 }
 
-extern "C" {
-
-int mgb_ens_depth_cost_batch(mgb_handle* h, const float* depth, const double* params, int32_t P, int32_t E, int64_t HW,
-                             int32_t scale_inv, int32_t shift_inv, int32_t median, double reg, double* costs_out,
-                             void* stream) {
+// The objective at base and, when pert is given, at the n points that each move one coordinate of base to its value
+// in pert: costs_out [1 + n].
+static int ens_depth_cost(mgb_handle* h, const float* depth, const double* base, const double* pert, int32_t E, int64_t HW,
+                          int32_t scale_inv, int32_t shift_inv, int32_t median, double reg, double* costs_out,
+                          void* stream) {
   int rc = ens_prepare(h);
   if (rc) return rc;
-  if (!depth || !params || !costs_out || HW <= 0 || P < 1) { set_error("ens_depth_cost: bad argument"); return MGB_ERR_INVALID; }
+  if (!depth || !base || !costs_out || HW <= 0) { set_error("ens_depth_cost: bad argument"); return MGB_ERR_INVALID; }
   if (E < 2 || E > ens_max_members()) { set_error("ensemble size %d outside [2,%d]", E, ens_max_members()); return MGB_ERR_UNSUPPORTED; }
-  const int n_param = shift_inv ? 2 * E : E;
+  const int n = pert ? (shift_inv ? 2 * E : E) : 0;
   // the staging area is reused by every call: wait for earlier users of this stream (each cost call ends with a
   // synchronisation, so this is only ever non-trivial after an asynchronous reduce)
   CUDA_TRY(cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(stream)));
-  for (int p0 = 0; p0 < P; p0 += ens_max_batch()) {
-    const int pn = std::min<int>(ens_max_batch(), P - p0);
-    float* st = pinned_st(h);
-    for (int i = 0; i < pn; ++i) {
-      rc = make_st(params + size_t(p0 + i) * n_param, E, scale_inv, shift_inv, st + size_t(i) * 2 * E);
-      if (rc) return rc;
-    }
-    int launches = 0;
-    rc = launch_ens_depth_cost(depth, st, pn, E, HW, shift_inv, median, reg, h->ens_ws, h->ens_pinned, &launches,
-                               reinterpret_cast<cudaStream_t>(stream));
-    if (rc) return rc;
-    count_launch(launches);
-    for (int i = 0; i < pn; ++i) costs_out[p0 + i] = h->ens_pinned[3 * i];
-  }
-  return MGB_OK;
-}
-
-int mgb_ens_depth_cost_fd(mgb_handle* h, const float* depth, const double* base, const double* pert, int32_t E, int64_t HW,
-                          int32_t scale_inv, int32_t shift_inv, int32_t median, double reg, double* costs_out, void* stream) {
-  int rc = ens_prepare(h);
-  if (rc) return rc;
-  if (!depth || !base || !pert || !costs_out || HW <= 0) { set_error("ens_depth_cost_fd: bad argument"); return MGB_ERR_INVALID; }
-  if (E < 2 || E > 16) { set_error("ens_depth_cost_fd: ensemble size %d outside [2,16] (use mgb_ens_depth_cost_batch)", E); return MGB_ERR_UNSUPPORTED; }
-  CUDA_TRY(cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(stream)));   // previous user of the staging area
   float* st = pinned_st(h);
   rc = make_st(base, E, scale_inv, shift_inv, st);
+  if (!rc && pert) rc = make_st(pert, E, scale_inv, shift_inv, st + 2 * E);
   if (rc) return rc;
-  rc = make_st(pert, E, scale_inv, shift_inv, st + 2 * E);
-  if (rc) return rc;
-  if (size_t(HW) * 3 * sizeof(float) > h->ens_v3_bytes) {     // per-pixel order statistics of the base point
+  // per-pixel order statistics of the base point for the register-resident perturbation pass
+  if (pert && E <= kEnsMaxE && size_t(HW) * 3 * sizeof(float) > h->ens_v3_bytes) {
     if (h->ens_v3) CUDA_TRY(cudaFree(h->ens_v3));
     h->ens_v3 = nullptr; h->ens_v3_bytes = 0;
     CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&h->ens_v3), size_t(HW) * 3 * sizeof(float)));
     h->ens_v3_bytes = size_t(HW) * 3 * sizeof(float);
   }
   int launches = 0;
-  rc = launch_ens_depth_cost_fd(depth, st, E, HW, shift_inv, median, reg, h->ens_ws, h->ens_v3, h->ens_pinned, &launches,
-                                reinterpret_cast<cudaStream_t>(stream));
+  rc = launch_ens_depth_cost(depth, st, n, E, HW, shift_inv, median, reg, h->ens_ws, h->ens_v3, h->ens_pinned, &launches,
+                             reinterpret_cast<cudaStream_t>(stream));
   if (rc) return rc;
   count_launch(launches);
-  const int n = shift_inv ? 2 * E : E;
   for (int i = 0; i <= n; ++i) costs_out[i] = h->ens_pinned[3 * i];
   return MGB_OK;
+}
+
+extern "C" {
+
+int mgb_ens_depth_cost_fd(mgb_handle* h, const float* depth, const double* base, const double* pert, int32_t E, int64_t HW,
+                          int32_t scale_inv, int32_t shift_inv, int32_t median, double reg, double* costs_out, void* stream) {
+  if (!pert) { set_error("ens_depth_cost_fd: bad argument"); return MGB_ERR_INVALID; }
+  return ens_depth_cost(h, depth, base, pert, E, HW, scale_inv, shift_inv, median, reg, costs_out, stream);
 }
 
 int mgb_ens_depth_cost(mgb_handle* h, const float* depth, const double* param, int32_t E, int64_t HW,
                        int32_t scale_inv, int32_t shift_inv, int32_t median, double reg, double* cost_out,
                        void* stream) {
-  return mgb_ens_depth_cost_batch(h, depth, param, 1, E, HW, scale_inv, shift_inv, median, reg, cost_out, stream);
+  return ens_depth_cost(h, depth, param, nullptr, E, HW, scale_inv, shift_inv, median, reg, cost_out, stream);
 }
 
 int mgb_ens_max_members(void) { return ens_max_members(); }

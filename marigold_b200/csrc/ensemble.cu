@@ -1,11 +1,11 @@
 // Test-time ensembling on the device (reference marigold/util/ensemble.py).
 //
-//  * ens_depth_cost   : the BFGS objective of ensemble_depth (ensemble.py:138-152) for P parameter vectors in ONE
-//                       launch (grid.y = parameter set) and ONE host synchronisation: the 2E forward-difference
-//                       points of one scipy gradient are one call (the reference does C(E,2)+2 `.item()` syncs
-//                       per point). The E maps are L2-resident (E x 2.4 MB at 768 px), so re-reading them per
-//                       parameter set costs L2 bandwidth only. Every parameter set runs the same code with the same
-//                       grid.x, so cost(x) is bit-identical whether evaluated alone or inside a batch.
+//  * ens_depth_cost   : the BFGS objective of ensemble_depth (ensemble.py:138-152) at a base point and, optionally,
+//                       the 2E forward-difference points of one scipy gradient, in ONE host synchronisation (the
+//                       reference does C(E,2)+2 `.item()` syncs per point). E <= 16: a base pass and a pass that
+//                       only updates what one perturbed coordinate changes; E > 16: one generic pass per point
+//                       (grid.y). The E maps are L2-resident (E x 2.4 MB at 768 px), so re-reading them per point
+//                       costs L2 bandwidth only. Every value is bit-identical to the point evaluated alone.
 //  * ens_depth_reduce : align (ensemble.py:107-118) + median/mean (+MAD/std) (:120-136) + min-max
 //                       renormalisation (:184-194), plus the index of the member the lower median picks.
 //  * ens_normals      : ensemble_normals (:199-249): mean -> normalise -> cosine -> clamp -> argmax -> gather.
@@ -13,7 +13,9 @@
 // These are HBM-bound streaming kernels: each reads the E maps exactly once (E*4 bytes / pixel).
 // Arithmetic that decides an index (median / argmax) uses explicitly un-fused fp32 ops
 // (__fmul_rn/__fadd_rn) in the reference's operation order so that ties break identically.
+#include <algorithm>
 #include <cfloat>
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -22,10 +24,9 @@ namespace mgb {
 
 constexpr int kEnsThreads = 256;
 constexpr int kEnsMaxBlocks = kNumSMs * 4;    // reduce / normals kernels
-constexpr int kEnsCostBlocks = kNumSMs * 2;   // cost kernels: blocks per parameter set
-constexpr int kEnsMaxE = 16;               // register-resident (templated) kernels; larger ensembles take the *_dyn path
+constexpr int kEnsCostBlocks = kNumSMs * 2;   // register-resident cost kernels: blocks per pass
 constexpr int kEnsDynMaxE = 64;
-constexpr int kEnsMaxP = 2 * kEnsDynMaxE + 1;   // parameter sets per batch call (one forward-difference gradient)
+constexpr int kEnsMaxP = 2 * kEnsDynMaxE + 1;   // points per cost call: a base point and its forward-difference points
 constexpr int kDynPairs = 32;              // pairs per blockIdx.z chunk of the generic cost kernel
 constexpr int kDynBlocks = 48;
 constexpr size_t kDynPartialBytes = size_t(16) << 20;
@@ -143,44 +144,38 @@ __device__ __forceinline__ void cost_block(const float* __restrict__ depth, cons
   if (threadIdx.x == 0) { out->pmin = pmin; out->pmax = pmax; }
 }
 
-template <int E>
-__global__ void __launch_bounds__(kEnsThreads)
-    ens_cost_kernel(const float* __restrict__ depth, const float* __restrict__ st_all, long long HW, int shift, int median,
-                    CostPartial* __restrict__ partials_all) {
-  cost_block<E>(depth, st_all + size_t(blockIdx.y) * 2 * E, HW, shift, median,
-                partials_all + size_t(blockIdx.y) * gridDim.x + blockIdx.x);
-}
-
-// ---- one forward-difference gradient in ONE round trip: the base point plus the n = 2E (or E) single-coordinate
-// perturbations scipy's approx_derivative evaluates. Perturbing member m only changes the E - 1 pairs (m, j) and moves
-// one element of the per-pixel order statistics, so after the base pass (which also stores three order statistics per
-// pixel) block row m of the second kernel recomputes just those, without sorting: ~5x less arithmetic than 2E + 1
-// independent evaluations. Every sum is formed exactly as cost_block forms it (same pixel-to-thread map, same
-// reduction order), and the final kernel assembles each perturbed objective from base + perturbed pair sums in pair
-// order, so the values equal ens_cost_kernel's bit for bit (tests/test_ensemble_gpu.py).
-struct FdPartial {
+// ---- E <= 16: the objective and one forward-difference gradient in ONE round trip: the base point plus the n = 2E (or
+// E) single-coordinate perturbations scipy's approx_derivative evaluates. Perturbing member m only changes the E - 1
+// pairs (m, j) and moves one element of the per-pixel order statistics, so after the base pass (which also stores three
+// order statistics per pixel) block row m of the perturbation pass recomputes just those, without sorting: ~5x less
+// arithmetic than 2E + 1 independent evaluations. Every sum is formed exactly as cost_block forms it (same
+// pixel-to-thread map, same reduction order), and the final kernel assembles each perturbed objective from base +
+// perturbed pair sums in pair order, so each value equals the base pass run at that point, bit for bit
+// (tests/test_ensemble_gpu.py).
+struct PertPartial {
   double pair_sum[2][kEnsMaxE];   // [s' | t'][other member j]
   float pmin[2], pmax[2];
 };
 
+// v3 (median only; null for a point without perturbations): the order statistics the perturbation pass reads
 template <int E>
 __global__ void __launch_bounds__(kEnsThreads)
-    ens_cost_fd_base_kernel(const float* __restrict__ depth, const float* __restrict__ st, long long HW, int shift, int median,
-                            CostPartial* __restrict__ base_part, float* __restrict__ v3) {
+    ens_cost_base_kernel(const float* __restrict__ depth, const float* __restrict__ st, long long HW, int shift, int median,
+                         CostPartial* __restrict__ base_part, float* __restrict__ v3) {
   cost_block<E>(depth, st, HW, shift, median, base_part + blockIdx.x, median ? v3 : nullptr);
 }
 
 // block row m: member m perturbed (s_m -> s', and t_m -> t' when shift): the E - 1 pair sums with the other members, and
-// min / max of the re-ensembled map. No sort here: with v = the sorted base values (from ens_cost_fd_base_kernel) and w = v
+// min / max of the re-ensembled map. No sort here: with v = the sorted base values (from ens_cost_base_kernel) and w = v
 // without one instance of a_m, the perturbed lower median is clamp(x', w[R-1], w[R]), where
 //   a_m <= v[R-1]          : w[R-1] = v[R],   w[R] = v[R+1]
 //   v[R-1] < a_m <= v[R]   : w[R-1] = v[R-1], w[R] = v[R+1]      (a_m is v[R])
 //   a_m > v[R]             : w[R-1] = v[R-1], w[R] = v[R]
 template <int E>
 __global__ void __launch_bounds__(kEnsThreads)
-    ens_cost_fd_pert_kernel(const float* __restrict__ depth, const float* __restrict__ st /* [2E] base */,
-                            const float* __restrict__ pert /* [2E]: s'_0..s'_{E-1} | t'_0..t'_{E-1} */, long long HW, int shift,
-                            int median, const float* __restrict__ v3, FdPartial* __restrict__ fd_part) {
+    ens_cost_pert_kernel(const float* __restrict__ depth, const float* __restrict__ st /* [2E] base */,
+                         const float* __restrict__ pert /* [2E]: s'_0..s'_{E-1} | t'_0..t'_{E-1} */, long long HW, int shift,
+                         int median, const float* __restrict__ v3, PertPartial* __restrict__ pert_part) {
   const int m = blockIdx.y;
   const int nk = shift ? 2 : 1;
   float s[E], t[E];
@@ -227,7 +222,7 @@ __global__ void __launch_bounds__(kEnsThreads)
   }
   __shared__ double sh[kEnsThreads / 32];
   __shared__ float shf[2][kEnsThreads / 32];
-  FdPartial* out = fd_part + size_t(m) * gridDim.x + blockIdx.x;
+  PertPartial* out = pert_part + size_t(m) * gridDim.x + blockIdx.x;
 #pragma unroll
   for (int j = 0; j < E; ++j) {
     const double t0 = block_sum_double(acc0[j], sh);
@@ -239,8 +234,8 @@ __global__ void __launch_bounds__(kEnsThreads)
   if (threadIdx.x == 0) { out->pmin[0] = mn0; out->pmax[0] = mx0; out->pmin[1] = mn1; out->pmax[1] = mx1; }
 }
 
-// Sum over the blocks' partials of one pair, one warp per call: lane l takes blocks l, l + 32, ...; xor tree. Both final
-// kernels use it, so a pair total has ONE value no matter which kernel produced the partials.
+// Sum over the blocks' partials of one pair, one warp per call: lane l takes blocks l, l + 32, ...; xor tree. Base and
+// perturbed pair sums are combined the same way, so a pair total has ONE value no matter which pass produced it.
 template <typename F>
 __device__ __forceinline__ double warp_total(int nblocks, F&& get) {
   double tot = 0.0;
@@ -250,46 +245,22 @@ __device__ __forceinline__ double warp_total(int nblocks, F&& get) {
   return tot;
 }
 
-__global__ void __launch_bounds__(256) ens_cost_final_kernel(const CostPartial* __restrict__ partials_all, int nblocks, int E,
-                                                             long long HW, double reg, double* __restrict__ out_all) {
-  // one block per parameter set; one warp per pair (warps stride over the pairs)
-  const CostPartial* partials = partials_all + size_t(blockIdx.x) * nblocks;
-  double* out = out_all + 3 * blockIdx.x;
-  const int NP = E * (E - 1) / 2;
-  __shared__ double c[kEnsMaxE * (kEnsMaxE - 1) / 2];
-  for (int k = threadIdx.x >> 5; k < NP; k += blockDim.x >> 5) {
-    const double tot = warp_total(nblocks, [&](int b) { return partials[b].pair_sum[k]; });
-    // reference: (diff**2).mean().sqrt() evaluated in fp32
-    if ((threadIdx.x & 31) == 0) c[k] = double(sqrtf(float(tot / double(HW))));
-  }
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float pmin = FLT_MAX, pmax = -FLT_MAX;
-    for (int b = threadIdx.x; b < nblocks; b += 32) { pmin = fminf(pmin, partials[b].pmin); pmax = fmaxf(pmax, partials[b].pmax); }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      pmin = fminf(pmin, __shfl_xor_sync(0xffffffffu, pmin, o));
-      pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, o));
-    }
-    if (threadIdx.x == 0) {
-      double cost = 0.0;
-      for (int k = 0; k < NP; ++k) cost += c[k];          // pair order, like the reference's Python loop
-      if (reg > 0.0) cost += (double(fabsf(0.0f - pmin)) + double(fabsf(1.0f - pmax))) * reg;
-      out[0] = cost;
-      out[1] = double(pmin);
-      out[2] = double(pmax);
-    }
-  }
+// {cost, min, max} of one point from its summed pair RMSEs and the range of its ensembled map (ensemble.py:147-152)
+__device__ __forceinline__ void store_cost(double cost, float pmin, float pmax, double reg, double* out) {
+  if (reg > 0.0) cost += (double(fabsf(0.0f - pmin)) + double(fabsf(1.0f - pmax))) * reg;
+  out[0] = cost;
+  out[1] = double(pmin);
+  out[2] = double(pmax);
 }
 
-// set q: 0 = the base point; q >= 1: coordinate i = q - 1 perturbed (i < E: s_i, else t_{i-E})
-__global__ void __launch_bounds__(256) ens_cost_fd_final_kernel(const CostPartial* __restrict__ base_part,
-                                                                const FdPartial* __restrict__ fd_part, int nblocks, int E,
-                                                                long long HW, double reg, double* __restrict__ out_all) {
+// one block per point q: 0 = the base point; q >= 1: coordinate i = q - 1 perturbed (i < E: s_i, else t_{i-E});
+// one warp per pair (warps stride over the pairs)
+__global__ void __launch_bounds__(256) ens_cost_final_kernel(const CostPartial* __restrict__ base_part,
+                                                             const PertPartial* __restrict__ pert_part, int nblocks, int E,
+                                                             long long HW, double reg, double* __restrict__ out_all) {
   const int q = blockIdx.x;
   const int m = q == 0 ? -1 : (q - 1) % E, kk = q == 0 ? 0 : (q - 1) / E;
-  const FdPartial* fp = q == 0 ? nullptr : fd_part + size_t(m) * nblocks;
-  double* out = out_all + 3 * q;
+  const PertPartial* fp = q == 0 ? nullptr : pert_part + size_t(m) * nblocks;
   const int NP = E * (E - 1) / 2;
   __shared__ double c[kEnsMaxE * (kEnsMaxE - 1) / 2];
   for (int k = threadIdx.x >> 5; k < NP; k += blockDim.x >> 5) {
@@ -300,6 +271,7 @@ __global__ void __launch_bounds__(256) ens_cost_fd_final_kernel(const CostPartia
     if (i == m) tot = warp_total(nblocks, [&](int b) { return fp[b].pair_sum[kk][j]; });
     else if (j == m) tot = warp_total(nblocks, [&](int b) { return fp[b].pair_sum[kk][i]; });
     else tot = warp_total(nblocks, [&](int b) { return base_part[b].pair_sum[k]; });
+    // reference: (diff**2).mean().sqrt() evaluated in fp32
     if ((threadIdx.x & 31) == 0) c[k] = double(sqrtf(float(tot / double(HW))));
   }
   __syncthreads();
@@ -316,19 +288,10 @@ __global__ void __launch_bounds__(256) ens_cost_fd_final_kernel(const CostPartia
     }
     if (threadIdx.x == 0) {
       double cost = 0.0;
-      for (int k = 0; k < NP; ++k) cost += c[k];
-      if (reg > 0.0) cost += (double(fabsf(0.0f - pmin)) + double(fabsf(1.0f - pmax))) * reg;
-      out[0] = cost;
-      out[1] = double(pmin);
-      out[2] = double(pmax);
+      for (int k = 0; k < NP; ++k) cost += c[k];          // pair order, like the reference's Python loop
+      store_cost(cost, pmin, pmax, reg, out_all + 3 * q);
     }
   }
-}
-
-template <int E>
-static void launch_cost_t(const float* depth, const float* st, long long HW, int shift, int median,
-                          CostPartial* partials, int blocks, int P, cudaStream_t stream) {
-  ens_cost_kernel<E><<<dim3(blocks, P), kEnsThreads, 0, stream>>>(depth, st, HW, shift, median, partials);
 }
 
 // ---- generic ensemble size (E > 16): values in local memory, pairs in chunks of 32 over blockIdx.z ------------------
@@ -392,32 +355,15 @@ __global__ void __launch_bounds__(kEnsThreads)
       pmax = fmaxf(pmax, pred);
     }
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
   for (int k = 0; k < kDynPairs; ++k) {
     if (k >= nk) break;
-    double v = double(acc[k]);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) sh[warp] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double tot = 0.0;
-      for (int w = 0; w < kEnsThreads / 32; ++w) tot += sh[w];
-      pair_part[(size_t(ps) * NP + k0 + k) * gridDim.x + blockIdx.x] = tot;
-    }
-    __syncthreads();
+    const double tot = block_sum_double(acc[k], sh);
+    if (threadIdx.x == 0) pair_part[(size_t(ps) * NP + k0 + k) * gridDim.x + blockIdx.x] = tot;
   }
   if (blockIdx.z == 0) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      pmin = fminf(pmin, __shfl_xor_sync(0xffffffffu, pmin, o));
-      pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, o));
-    }
-    if (lane == 0) { shf[0][warp] = pmin; shf[1][warp] = pmax; }
-    __syncthreads();
+    block_minmax(pmin, pmax, shf);
     if (threadIdx.x == 0) {
-      for (int w = 1; w < kEnsThreads / 32; ++w) { pmin = fminf(pmin, shf[0][w]); pmax = fmaxf(pmax, shf[1][w]); }
       mm_part[(size_t(ps) * gridDim.x + blockIdx.x) * 2] = pmin;
       mm_part[(size_t(ps) * gridDim.x + blockIdx.x) * 2 + 1] = pmax;
     }
@@ -444,19 +390,16 @@ __global__ void ens_cost_dyn_final_kernel(const double* __restrict__ pair_part, 
       pmin = fminf(pmin, mm_part[(size_t(ps) * nblocks + b) * 2]);
       pmax = fmaxf(pmax, mm_part[(size_t(ps) * nblocks + b) * 2 + 1]);
     }
-    if (reg > 0.0) cost += (double(fabsf(0.0f - pmin)) + double(fabsf(1.0f - pmax))) * reg;
-    double* out = out_all + 3 * ps;
-    out[0] = cost; out[1] = double(pmin); out[2] = double(pmax);
+    store_cost(cost, pmin, pmax, reg, out_all + 3 * ps);
   }
 }
 
-// ws layout: [partials: max(CostPartial x kEnsCostBlocks x (2 kEnsMaxE + 1), kDynPartialBytes + min/max)]
+// ws layout: [partials: max(register-resident: base + E perturbation rows per block, generic: kDynPartialBytes + min/max)]
 //            [st: kEnsMaxP x 2 kEnsDynMaxE floats][out: kEnsMaxP x 3 doubles]
 static size_t ens_partial_bytes() {
-  const size_t t = std::max(sizeof(CostPartial) * kEnsCostBlocks * (2 * kEnsMaxE + 1),
-                            sizeof(CostPartial) * kEnsCostBlocks + sizeof(FdPartial) * kEnsCostBlocks * kEnsMaxE);
+  const size_t t = (sizeof(CostPartial) + sizeof(PertPartial) * kEnsMaxE) * kEnsCostBlocks;
   const size_t d = kDynPartialBytes + size_t(kEnsMaxP) * kDynBlocks * 2 * sizeof(float);
-  return ((t > d ? t : d) + 255) & ~size_t(255);
+  return (std::max(t, d) + 255) & ~size_t(255);
 }
 size_t ens_ws_bytes() {
   return ens_partial_bytes() + size_t(kEnsMaxP) * 2 * kEnsDynMaxE * sizeof(float) + size_t(kEnsMaxP) * 3 * sizeof(double) + 256;
@@ -466,77 +409,73 @@ static double* ens_ws_out(void* ws) { return reinterpret_cast<double*>(ens_ws_st
 int ens_max_batch() { return kEnsMaxP; }
 int ens_max_members() { return kEnsDynMaxE; }
 
-// st_host: float [P][2E] = {s_0..s_{E-1}, t_0..t_{E-1}} per parameter set (pinned); out_host_pinned: double [P][3] =
-// {cost, min(pred), max(pred)}. One synchronisation for the whole batch.
-int launch_ens_depth_cost(const float* depth, const float* st_host, int P, int E, long long HW, int shift, int median,
-                          double reg, void* ws, double* out_host_pinned, int* launches, cudaStream_t stream) {
-  if (E < 2 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [2, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
-  if (P < 1 || P > kEnsMaxP) { set_error("ens cost: %d parameter sets outside [1, %d]", P, kEnsMaxP); return MGB_ERR_INVALID; }
-  float* st = ens_ws_st(ws);
-  double* out = ens_ws_out(ws);
-  cudaError_t e = cudaMemcpyAsync(st, st_host, sizeof(float) * 2 * E * P, cudaMemcpyHostToDevice, stream);
-  if (e != cudaSuccess) { set_error("ens cost H2D: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  *launches = 0;
-  if (E <= kEnsMaxE) {
-    CostPartial* partials = reinterpret_cast<CostPartial*>(ws);
-    const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kEnsCostBlocks));
-    switch (E) {
-#define CASE(n) case n: launch_cost_t<n>(depth, st, HW, shift, median, partials, blocks, P, stream); break;
-      CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7) CASE(8) CASE(9) CASE(10) CASE(11) CASE(12) CASE(13) CASE(14)
-      CASE(15) CASE(16)
-#undef CASE
-    }
-    ens_cost_final_kernel<<<P, 256, 0, stream>>>(partials, blocks, E, HW, reg, out);
-    *launches = 2;
-  } else {
-    const int NP = E * (E - 1) / 2, chunks = (NP + kDynPairs - 1) / kDynPairs;
-    const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kDynBlocks));
-    double* pair_part = reinterpret_cast<double*>(ws);
-    float* mm_part = reinterpret_cast<float*>(static_cast<char*>(ws) + kDynPartialBytes);
-    const int p_max = std::max<int>(1, int(kDynPartialBytes / (size_t(NP) * blocks * sizeof(double))));
-    for (int p0 = 0; p0 < P; p0 += p_max) {
-      const int pn = std::min(p_max, P - p0);
-      ens_cost_dyn_kernel<<<dim3(blocks, pn, chunks), kEnsThreads, 0, stream>>>(depth, st + size_t(p0) * 2 * E, E, HW, shift,
-                                                                               median, pair_part, mm_part);
-      ens_cost_dyn_final_kernel<<<pn, 128, 0, stream>>>(pair_part, mm_part, blocks, E, HW, reg, out + 3 * p0);
-      *launches += 2;
-    }
-  }
-  e = cudaMemcpyAsync(out_host_pinned, out, size_t(P) * 3 * sizeof(double), cudaMemcpyDeviceToHost, stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("ens cost: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
-}
-
-// st_host (pinned): float [4E] = base {s | t} then perturbed {s' | t'}; out_host_pinned: double [1 + n][3] with n = 2E
-// (shift) or E: set 0 = base, set 1 + i = coordinate i perturbed. One launch pair, one synchronisation.
-int launch_ens_depth_cost_fd(const float* depth, const float* st_host, int E, long long HW, int shift, int median,
-                             double reg, void* ws, float* v3 /* 3 HW floats of scratch */, double* out_host_pinned,
-                             int* launches, cudaStream_t stream) {
-  if (E < 2 || E > kEnsMaxE) { set_error("ens cost fd: ensemble size %d outside [2, %d]", E, kEnsMaxE); return MGB_ERR_UNSUPPORTED; }
-  float* st = ens_ws_st(ws);
-  double* out = ens_ws_out(ws);
-  cudaError_t e = cudaMemcpyAsync(st, st_host, sizeof(float) * 4 * E, cudaMemcpyHostToDevice, stream);
-  if (e != cudaSuccess) { set_error("ens cost fd H2D: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  CostPartial* base_part = reinterpret_cast<CostPartial*>(ws);
-  FdPartial* fd_part = reinterpret_cast<FdPartial*>(base_part + kEnsCostBlocks);
-  const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kEnsCostBlocks));
-  const int n = shift ? 2 * E : E;
+// f(std::integral_constant<int, E>()) for the register-resident sizes E <= kEnsMaxE, f(std::integral_constant<int, 0>())
+// for the larger ones
+template <typename F>
+static void dispatch_members(int E, F&& f) {
   switch (E) {
-#define CASE(k) case k: \
-      ens_cost_fd_base_kernel<k><<<blocks, kEnsThreads, 0, stream>>>(depth, st, HW, shift, median, base_part, v3); \
-      ens_cost_fd_pert_kernel<k><<<dim3(blocks, E), kEnsThreads, 0, stream>>>(depth, st, st + 2 * E, HW, shift, median, v3, fd_part); break;
+#define CASE(n) case n: f(std::integral_constant<int, n>()); return;
     CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7) CASE(8) CASE(9) CASE(10) CASE(11) CASE(12) CASE(13) CASE(14)
     CASE(15) CASE(16)
 #undef CASE
   }
-  ens_cost_fd_final_kernel<<<1 + n, 256, 0, stream>>>(base_part, fd_part, blocks, E, HW, reg, out);
-  *launches = 3;
-  e = cudaMemcpyAsync(out_host_pinned, out, size_t(1 + n) * 3 * sizeof(double), cudaMemcpyDeviceToHost, stream);
+  f(std::integral_constant<int, 0>());
+}
+
+int launch_ens_depth_cost(const float* depth, float* st_host, int n, int E, long long HW, int shift, int median,
+                          double reg, void* ws, float* v3, double* out_host_pinned, int* launches, cudaStream_t stream) {
+  if (E < 2 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [2, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
+  const int P = 1 + n;
+  int rows = n > 0 ? 2 : 1;
+  if (E > kEnsMaxE && n > 0) {
+    // the generic kernels evaluate whole points: row 1 + i = the base with coordinate i moved (each coordinate was
+    // converted to float on its own, so these are the rows of the moved double vectors)
+    float moved[2 * kEnsDynMaxE];
+    std::copy(st_host + 2 * E, st_host + 4 * E, moved);
+    for (int i = 0; i < n; ++i) {
+      float* row = st_host + size_t(1 + i) * 2 * E;
+      std::copy(st_host, st_host + 2 * E, row);
+      row[i] = moved[i];
+    }
+    rows = P;
+  }
+  float* st = ens_ws_st(ws);
+  double* out = ens_ws_out(ws);
+  cudaError_t e = cudaMemcpyAsync(st, st_host, sizeof(float) * 2 * E * rows, cudaMemcpyHostToDevice, stream);
+  if (e != cudaSuccess) { set_error("ens cost H2D: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+  *launches = 0;
+  dispatch_members(E, [&](auto members) {
+    constexpr int kE = decltype(members)::value;
+    if constexpr (kE > 0) {
+      CostPartial* base_part = reinterpret_cast<CostPartial*>(ws);
+      PertPartial* pert_part = reinterpret_cast<PertPartial*>(base_part + kEnsCostBlocks);
+      const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kEnsCostBlocks));
+      ens_cost_base_kernel<kE><<<blocks, kEnsThreads, 0, stream>>>(depth, st, HW, shift, median, base_part,
+                                                                   n > 0 ? v3 : nullptr);
+      if (n > 0)
+        ens_cost_pert_kernel<kE><<<dim3(blocks, E), kEnsThreads, 0, stream>>>(depth, st, st + 2 * E, HW, shift, median, v3,
+                                                                              pert_part);
+      ens_cost_final_kernel<<<P, 256, 0, stream>>>(base_part, pert_part, blocks, E, HW, reg, out);
+      *launches = n > 0 ? 3 : 2;
+    } else {
+      const int NP = E * (E - 1) / 2, chunks = (NP + kDynPairs - 1) / kDynPairs;
+      const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kDynBlocks));
+      double* pair_part = reinterpret_cast<double*>(ws);
+      float* mm_part = reinterpret_cast<float*>(static_cast<char*>(ws) + kDynPartialBytes);
+      const int p_max = std::max<int>(1, int(kDynPartialBytes / (size_t(NP) * blocks * sizeof(double))));
+      for (int p0 = 0; p0 < P; p0 += p_max) {
+        const int pn = std::min(p_max, P - p0);
+        ens_cost_dyn_kernel<<<dim3(blocks, pn, chunks), kEnsThreads, 0, stream>>>(depth, st + size_t(p0) * 2 * E, E, HW,
+                                                                                 shift, median, pair_part, mm_part);
+        ens_cost_dyn_final_kernel<<<pn, 128, 0, stream>>>(pair_part, mm_part, blocks, E, HW, reg, out + 3 * p0);
+        *launches += 2;
+      }
+    }
+  });
+  e = cudaMemcpyAsync(out_host_pinned, out, size_t(P) * 3 * sizeof(double), cudaMemcpyDeviceToHost, stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
   if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("ens cost fd: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+  if (e != cudaSuccess) { set_error("ens cost: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   return MGB_OK;
 }
 
@@ -550,15 +489,8 @@ __global__ void __launch_bounds__(kEnsThreads) ens_minmax_kernel(const float* __
     mn = fminf(mn, v); mx = fmaxf(mx, v);
   }
   __shared__ float sh[2][kEnsThreads / 32];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  }
-  if ((threadIdx.x & 31) == 0) { sh[0][threadIdx.x >> 5] = mn; sh[1][threadIdx.x >> 5] = mx; }
-  __syncthreads();
+  block_minmax(mn, mx, sh);
   if (threadIdx.x == 0) {
-    for (int w = 1; w < kEnsThreads / 32; ++w) { mn = fminf(mn, sh[0][w]); mx = fmaxf(mx, sh[1][w]); }
     out[((long long)e * gridDim.x + blockIdx.x) * 2 + 0] = mn;
     out[((long long)e * gridDim.x + blockIdx.x) * 2 + 1] = mx;
   }
@@ -578,34 +510,47 @@ int launch_ens_minmax(const float* depth, int E, long long HW, float* ws, float*
 }
 
 // ---- reduce: align + (median | mean) (+ uncertainty) ; then global min-max renormalisation ------
-template <int E>
-__global__ void __launch_bounds__(kEnsThreads)
-    ens_reduce_kernel(const float* __restrict__ depth, const float* __restrict__ st, long long HW, int shift,
-                      int median, float* __restrict__ pred_out, float* __restrict__ unc_out,
-                      int* __restrict__ idx_out, float* __restrict__ block_minmax) {
-  float s[E], t[E];
+// lower median with torch's stable tie order: its value, and in *pick (when given) the member it comes from. kE > 0:
+// sorting network over kE register values; kE = 0: rank counting over E values (the same value and member).
+template <int kE, int N>
+__device__ __forceinline__ float lower_median(const float (&a)[N], int E, int* pick) {
+  if constexpr (kE > 0) {
+    float v[kE]; int idx[kE];
 #pragma unroll
-  for (int e = 0; e < E; ++e) { s[e] = st[e]; t[e] = st[E + e]; }
+    for (int e = 0; e < kE; ++e) { v[e] = a[e]; idx[e] = e; }
+    sort_small<kE>(v, idx);
+    if (pick) *pick = idx[(kE - 1) / 2];
+    return v[(kE - 1) / 2];
+  } else {
+    return select_lower_median(a, E, pick);
+  }
+}
+
+// kE > 0: exactly kE members, values in registers; kE = 0: any E <= kEnsDynMaxE members, values in local memory
+template <int kE>
+__global__ void __launch_bounds__(kEnsThreads)
+    ens_reduce_kernel(const float* __restrict__ depth, const float* __restrict__ st, int n_members, long long HW, int shift,
+                      int median, float* __restrict__ pred_out, float* __restrict__ unc_out,
+                      int* __restrict__ idx_out, float* __restrict__ bmm) {
+  constexpr int N = kE > 0 ? kE : kEnsDynMaxE;
+  const int E = kE > 0 ? kE : n_members;
+  __shared__ float s_s[N], s_t[N];
+  if (threadIdx.x < E) { s_s[threadIdx.x] = st[threadIdx.x]; s_t[threadIdx.x] = st[E + threadIdx.x]; }
+  __syncthreads();
   float pmin = FLT_MAX, pmax = -FLT_MAX;
   for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += (long long)gridDim.x * blockDim.x) {
-    float a[E];
+    float a[N];
 #pragma unroll
-    for (int e = 0; e < E; ++e) a[e] = align1(__ldg(depth + (long long)e * HW + p), s[e], t[e], shift);
+    for (int e = 0; e < E; ++e) a[e] = align1(__ldg(depth + (long long)e * HW + p), s_s[e], s_t[e], shift);
     float pred, unc = 0.f;
-    int pick = 0;
+    int pick = -1;
     if (median) {
-      float v[E]; int idx[E];
-#pragma unroll
-      for (int e = 0; e < E; ++e) { v[e] = a[e]; idx[e] = e; }
-      sort_small<E>(v, idx);
-      pred = v[(E - 1) / 2];            // torch.median: LOWER median for even E
-      pick = idx[(E - 1) / 2];
+      pred = lower_median<kE>(a, E, &pick);        // torch.median: LOWER median for even E
       if (unc_out) {
-        float dv[E]; int di[E];
+        float dv[N];
 #pragma unroll
-        for (int e = 0; e < E; ++e) { dv[e] = fabsf(a[e] - pred); di[e] = e; }
-        sort_small<E>(dv, di);
-        unc = dv[(E - 1) / 2];          // MAD
+        for (int e = 0; e < E; ++e) dv[e] = fabsf(a[e] - pred);
+        unc = lower_median<kE>(dv, E, nullptr);    // MAD
       }
     } else {
       float sm = 0.f;
@@ -618,25 +563,15 @@ __global__ void __launch_bounds__(kEnsThreads)
         for (int e = 0; e < E; ++e) { const float d = a[e] - pred; q += d * d; }
         unc = sqrtf(q / float(E - 1));
       }
-      pick = -1;
     }
     pred_out[p] = pred;
     if (unc_out) unc_out[p] = unc;
     if (idx_out) idx_out[p] = pick;
     pmin = fminf(pmin, pred); pmax = fmaxf(pmax, pred);
   }
-  __shared__ float sh[2][kEnsThreads / 32];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    pmin = fminf(pmin, __shfl_xor_sync(0xffffffffu, pmin, o));
-    pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, o));
-  }
-  if ((threadIdx.x & 31) == 0) { sh[0][threadIdx.x >> 5] = pmin; sh[1][threadIdx.x >> 5] = pmax; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < kEnsThreads / 32; ++w) { pmin = fminf(pmin, sh[0][w]); pmax = fmaxf(pmax, sh[1][w]); }
-    block_minmax[2 * blockIdx.x] = pmin; block_minmax[2 * blockIdx.x + 1] = pmax;
-  }
+  __shared__ float shf[2][kEnsThreads / 32];
+  block_minmax(pmin, pmax, shf);
+  if (threadIdx.x == 0) { bmm[2 * blockIdx.x] = pmin; bmm[2 * blockIdx.x + 1] = pmax; }
 }
 
 __global__ void __launch_bounds__(kEnsThreads)
@@ -662,55 +597,6 @@ __global__ void __launch_bounds__(kEnsThreads)
   }
 }
 
-// generic ensemble size: values in local memory, order statistics by rank counting (same tie order as the sort)
-__global__ void __launch_bounds__(kEnsThreads)
-    ens_reduce_dyn_kernel(const float* __restrict__ depth, const float* __restrict__ st, int E, long long HW, int shift,
-                          int median, float* __restrict__ pred_out, float* __restrict__ unc_out,
-                          int* __restrict__ idx_out, float* __restrict__ block_minmax) {
-  __shared__ float s_s[kEnsDynMaxE], s_t[kEnsDynMaxE];
-  if (threadIdx.x < E) { s_s[threadIdx.x] = st[threadIdx.x]; s_t[threadIdx.x] = st[E + threadIdx.x]; }
-  __syncthreads();
-  float pmin = FLT_MAX, pmax = -FLT_MAX;
-  float a[kEnsDynMaxE], dv[kEnsDynMaxE];
-  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += (long long)gridDim.x * blockDim.x) {
-    for (int e = 0; e < E; ++e) a[e] = align1(__ldg(depth + (long long)e * HW + p), s_s[e], s_t[e], shift);
-    float pred, unc = 0.f;
-    int pick = -1;
-    if (median) {
-      pred = select_lower_median(a, E, &pick);
-      if (unc_out) {
-        for (int e = 0; e < E; ++e) dv[e] = fabsf(a[e] - pred);
-        unc = select_lower_median(dv, E, nullptr);
-      }
-    } else {
-      float sm = 0.f;
-      for (int e = 0; e < E; ++e) sm += a[e];
-      pred = sm / float(E);
-      if (unc_out) {
-        float q = 0.f;
-        for (int e = 0; e < E; ++e) { const float d = a[e] - pred; q += d * d; }
-        unc = sqrtf(q / float(E - 1));
-      }
-    }
-    pred_out[p] = pred;
-    if (unc_out) unc_out[p] = unc;
-    if (idx_out) idx_out[p] = pick;
-    pmin = fminf(pmin, pred); pmax = fmaxf(pmax, pred);
-  }
-  __shared__ float sh[2][kEnsThreads / 32];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    pmin = fminf(pmin, __shfl_xor_sync(0xffffffffu, pmin, o));
-    pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, o));
-  }
-  if ((threadIdx.x & 31) == 0) { sh[0][threadIdx.x >> 5] = pmin; sh[1][threadIdx.x >> 5] = pmax; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < kEnsThreads / 32; ++w) { pmin = fminf(pmin, sh[0][w]); pmax = fmaxf(pmax, sh[1][w]); }
-    block_minmax[2 * blockIdx.x] = pmin; block_minmax[2 * blockIdx.x + 1] = pmax;
-  }
-}
-
 int launch_ens_depth_reduce(const float* depth, const float* st_host, int E, long long HW, int shift, int median,
                             int use_min, float* pred, float* unc, int* idx, void* ws, cudaStream_t stream) {
   if (E < 2 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [2, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
@@ -719,14 +605,10 @@ int launch_ens_depth_reduce(const float* depth, const float* st_host, int E, lon
   cudaError_t e = cudaMemcpyAsync(st, st_host, sizeof(float) * 2 * E, cudaMemcpyHostToDevice, stream);
   if (e != cudaSuccess) { set_error("ens reduce H2D: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kEnsMaxBlocks));
-  switch (E) {
-#define CASE(n) case n: ens_reduce_kernel<n><<<blocks, kEnsThreads, 0, stream>>>(depth, st, HW, shift, median, pred, unc, idx, bmm); break;
-    CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7) CASE(8) CASE(9) CASE(10) CASE(11) CASE(12) CASE(13) CASE(14)
-    CASE(15) CASE(16)
-#undef CASE
-    default:
-      ens_reduce_dyn_kernel<<<blocks, kEnsThreads, 0, stream>>>(depth, st, E, HW, shift, median, pred, unc, idx, bmm);
-  }
+  dispatch_members(E, [&](auto members) {
+    ens_reduce_kernel<decltype(members)::value><<<blocks, kEnsThreads, 0, stream>>>(depth, st, E, HW, shift, median, pred,
+                                                                                    unc, idx, bmm);
+  });
   ens_renorm_kernel<<<blocks, kEnsThreads, 0, stream>>>(pred, unc, HW, bmm, blocks, use_min);
   e = cudaGetLastError();
   if (e != cudaSuccess) { set_error("ens reduce: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }

@@ -184,16 +184,17 @@ int launch_eval_normals(const float* pred, const float* gt, const uint8_t* mask,
 // ---------------------------------------------------------------------------------------------
 // Ensemble kernels (ensemble.cu)
 // ---------------------------------------------------------------------------------------------
+constexpr int kEnsMaxE = 16;   // largest ensemble the register-resident (templated) kernels take; larger: generic kernels
 size_t ens_ws_bytes();
-int ens_max_batch();     // parameter sets per launch_ens_depth_cost call
+int ens_max_batch();     // points per launch_ens_depth_cost call (1 + 2 ens_max_members())
 int ens_max_members();   // largest supported ensemble size
-// st_host (pinned): float [P][2E] = {s_0..s_{E-1}, t_0..t_{E-1}} per parameter set; out_host_pinned: double [P][3] =
-// {cost, min(pred), max(pred)}; one synchronisation per call. *launches = kernels launched.
-int launch_ens_depth_cost(const float* depth, const float* st_host, int P, int E, long long HW, int shift, int median,
-                          double reg, void* ws, double* out_host_pinned, int* launches, cudaStream_t stream);
-// One forward-difference gradient: st_host (pinned) float [4E] = base {s | t}, perturbed {s' | t'}; out double [1 + n][3]
-int launch_ens_depth_cost_fd(const float* depth, const float* st_host, int E, long long HW, int shift, int median,
-                             double reg, void* ws, float* v3, double* out_host_pinned, int* launches, cudaStream_t stream);
+// The objective at a base point and at the n points that each move one of its coordinates (n = 0, or 2E / E without
+// shift; coordinate i < E is s_i, else t_{i-E}). st_host (pinned, room for ens_max_batch() rows of 2E floats): the base
+// {s_0..s_{E-1}, t_0..t_{E-1}}, then when n > 0 the moved value of every coordinate in the same layout.
+// out_host_pinned: double [1 + n][3] = {cost, min(pred), max(pred)}, row 0 the base point, row 1 + i coordinate i moved.
+// v3: 3 HW floats of scratch when n > 0 and E <= kEnsMaxE. One synchronisation per call; *launches = kernels launched.
+int launch_ens_depth_cost(const float* depth, float* st_host, int n, int E, long long HW, int shift, int median,
+                          double reg, void* ws, float* v3, double* out_host_pinned, int* launches, cudaStream_t stream);
 int launch_ens_minmax(const float* depth, int E, long long HW, float* ws, float* host_pinned, int* blocks_out,
                       cudaStream_t stream);
 int launch_ens_depth_reduce(const float* depth, const float* st_host, int E, long long HW, int shift, int median,

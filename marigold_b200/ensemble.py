@@ -2,11 +2,10 @@
 252-270) backed by the CUDA kernels in csrc/ensemble.cu.
 
 Same signatures, defaults, error behaviour and return shapes as the reference. The scipy BFGS driver
-stays on the host exactly as in the reference (ensemble.py:165-171); what changes is the objective:
-one fused pass + one host sync per evaluation instead of C(E,2)+2 `.item()` syncs, and the 2E
-forward-difference points of one gradient are ONE launch + ONE sync (`mgb_ens_depth_cost_batch`): scipy's
-own `approx_derivative` still forms the differences (its `workers=` map hook receives the perturbed
-vectors), so the trajectory semantics are the reference's.
+stays on the host as in the reference (ensemble.py:165-171); what changes is the objective: f(x) and
+the 2E forward-difference points of its gradient are ONE device round trip (`mgb_ens_depth_cost_fd`)
+instead of C(E,2)+2 `.item()` syncs per point. The gradient is formed from those points with scipy's
+own step and arithmetic, so the trajectory is the one scipy's default (jac=None) takes.
 """
 from __future__ import annotations
 
@@ -60,15 +59,16 @@ def _fd_grad(x: np.ndarray, f0: float, costs: np.ndarray, pert: np.ndarray) -> n
     return (np.asarray(costs, dtype=np.float64) - f0) / (pert - x)
 
 
-def _bfgs(cost_fn, grad_fn, param0, tol, max_iter):
+def _bfgs(fun, param0, tol, max_iter):
     """scipy.optimize.minimize(..., method="BFGS", tol=tol, options={"maxiter": max_iter}) as the reference calls it
-    (ensemble.py:165-171). The reference leaves jac=None, i.e. scipy's forward differences; `grad_fn` restates exactly
-    those (`_scipy_fd_points`, `_fd_grad`: same points, same arithmetic, hence the same trajectory bit for bit) from
-    one batched device pass, and handing it over as `jac` keeps approx_derivative's per-call Python overhead
-    (~2x the device time of a cost pass) out of the loop."""
+    (ensemble.py:165-171). The reference leaves jac=None, i.e. scipy's forward differences; `fun(x) -> (f, grad)`
+    restates exactly those (`_scipy_fd_points`, `_fd_grad`: same points, same arithmetic, hence the same trajectory bit
+    for bit) from one device pass, and jac=True keeps approx_derivative's per-call Python overhead (~2x the device time
+    of a cost pass) out of the loop. scipy keeps the gradient of the last point it evaluated, so every new point is one
+    call of `fun`."""
     import scipy.optimize
 
-    res = scipy.optimize.minimize(cost_fn, param0, jac=grad_fn, method="BFGS", tol=tol,
+    res = scipy.optimize.minimize(fun, param0, jac=True, method="BFGS", tol=tol,
                                   options={"maxiter": max_iter, "disp": False})
     return res.x, res.nit
 
@@ -86,7 +86,6 @@ def ensemble_depth(
     engine=None,
     return_aux: bool = False,
     param: Optional[np.ndarray] = None,
-    speculate: bool = True,
 ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     if depth.dim() != 4 or depth.shape[1] != 1:
         raise ValueError(f"Expecting 4D tensor of shape [B,1,H,W]; got {depth.shape}.")
@@ -125,80 +124,43 @@ def ensemble_depth(
             param0 = (np.float32(1.0) / np.maximum(mx, np.float32(1e-6))).astype(np.float64)
 
         n_eval = [0, 0]   # objective evaluations, device round trips
-
-        def cost_batch(params) -> np.ndarray:
-            """cost_fn (ensemble.py:138-152) for a stack of parameter vectors: one launch, one sync."""
-            P = np.ascontiguousarray(np.atleast_2d(np.asarray(params, dtype=np.float64)))
-            out = np.empty(P.shape[0], dtype=np.float64)
-            check(lib.mgb_ens_depth_cost_batch(h, ptr(d_align), P.ctypes.data_as(C.c_void_p), P.shape[0], E, hw_a, sc,
-                                               sh, median, float(regularizer_strength),
-                                               out.ctypes.data_as(C.c_void_p), stream_ptr()),
-                  "mgb_ens_depth_cost_batch")
-            n_eval[0] += P.shape[0]
-            n_eval[1] += 1
-            return out
-
-        memo = {"x": None, "f": None, "pert": None, "costs": None}   # the last point evaluated
-
-        def _fd_call(base: np.ndarray, pert: np.ndarray) -> np.ndarray:
-            out = np.empty(base.size + 1, dtype=np.float64)
-            check(lib.mgb_ens_depth_cost_fd(h, ptr(d_align), base.ctypes.data_as(C.c_void_p),
-                                            pert.ctypes.data_as(C.c_void_p), E, hw_a, sc, sh, median,
-                                            float(regularizer_strength), out.ctypes.data_as(C.c_void_p), stream_ptr()),
-                  "mgb_ens_depth_cost_fd")
-            n_eval[0] += base.size + 1
-            n_eval[1] += 1
-            return out
-
-        def _fd_rows(x: np.ndarray, pert: np.ndarray) -> np.ndarray:
-            xs = np.repeat(x[None], x.size, 0)
-            xs[np.arange(x.size), np.arange(x.size)] = pert
-            return xs
+        n_param = 2 * E if shift_invariant else E
+        reg = float(regularizer_strength)
 
         def cost_fn(param: np.ndarray) -> float:
-            """The objective at `param`. BFGS asks for the gradient at (almost) every point it evaluates, so the
-            forward-difference points of that gradient (x + h e_i, scipy's default absolute step) ride along in the
-            same pass and the same synchronisation; `grad_fn` is then served from here."""
+            """cost_fn (ensemble.py:138-152) at one point (`mgb_ens_depth_cost`)."""
             x = np.ascontiguousarray(param, dtype=np.float64)
-            if not speculate:
-                f = float(cost_batch(x)[0])
-                memo.update(x=x.copy(), f=f, pert=None, costs=None)
-                return f
+            out = C.c_double()
+            check(lib.mgb_ens_depth_cost(h, ptr(d_align), x.ctypes.data_as(C.c_void_p), E, hw_a, sc, sh, median, reg,
+                                         C.byref(out), stream_ptr()), "mgb_ens_depth_cost")
+            return out.value
+
+        def cost_fd(base: np.ndarray, pert: np.ndarray) -> np.ndarray:
+            """[1 + n]: the objective at `base`, then at `base` with coordinate i moved to pert[i], for each i. One
+            device round trip (`mgb_ens_depth_cost_fd`)."""
+            base = np.ascontiguousarray(base, dtype=np.float64)
+            pert = np.ascontiguousarray(pert, dtype=np.float64)
+            if base.shape != (n_param,) or pert.shape != (n_param,):
+                raise ValueError(f"cost_fd expects two vectors of {n_param} parameters; got {base.shape}, {pert.shape}")
+            out = np.empty(1 + n_param, dtype=np.float64)
+            # plain integer addresses: this runs once per BFGS evaluation, and each data_as() costs ~2 us of host time
+            check(lib.mgb_ens_depth_cost_fd(h, ptr(d_align), base.ctypes.data, pert.ctypes.data, E, hw_a, sc, sh,
+                                            median, reg, out.ctypes.data, stream_ptr()), "mgb_ens_depth_cost_fd")
+            n_eval[0] += out.size
+            n_eval[1] += 1
+            return out
+
+        def fun(param: np.ndarray) -> Tuple[float, np.ndarray]:
+            """f(param) and scipy's forward-difference gradient of it, from one `cost_fd` round trip."""
+            x = np.ascontiguousarray(param, dtype=np.float64)
             pert = _scipy_fd_points(x)
-            if E <= 16 and x.size >= 2:
-                out = _fd_call(x, pert)                         # structured pass: base + one perturbed coordinate per row
-            else:
-                out = cost_batch(np.concatenate([x[None], _fd_rows(x, pert)]))
-            memo.update(x=x.copy(), f=float(out[0]), pert=pert, costs=out[1:])
-            return memo["f"]
-
-        def cost_fd(xs: np.ndarray) -> Optional[np.ndarray]:
-            """xs [n, n]: row i = a common base point with coordinate i perturbed (what a 2-point scheme evaluates).
-            One structured pass on the device (`mgb_ens_depth_cost_fd`); None if xs is not of that form."""
-            n = xs.shape[1]
-            if E > 16 or xs.shape[0] != n or n < 2:
-                return None
-            base = xs[1].copy()
-            base[1] = xs[0][1]                                  # row 0 is unperturbed at coordinate 1
-            pert = np.ascontiguousarray(np.diagonal(xs))
-            if not np.array_equal(_fd_rows(base, pert), xs):
-                return None
-            return _fd_call(base, pert)[1:]
-
-        def grad_fn(param: np.ndarray) -> np.ndarray:
-            x = np.ascontiguousarray(param, dtype=np.float64)
-            if memo["x"] is None or not np.array_equal(memo["x"], x):
-                cost_fn(x)
-            if memo["costs"] is None:                           # speculate=False: the gradient points are a second pass
-                pert = _scipy_fd_points(x)
-                xs = _fd_rows(x, pert)
-                costs = cost_fd(xs)
-                memo.update(pert=pert, costs=costs if costs is not None else cost_batch(xs))
-            return _fd_grad(x, memo["f"], memo["costs"], memo["pert"])
+            out = cost_fd(x, pert)
+            f = float(out[0])
+            return f, _fd_grad(x, f, out[1:], pert)
 
         nit = 0
         if param is None:
-            param, nit = _bfgs(cost_fn, grad_fn, param0, tol, max_iter)
+            param, nit = _bfgs(fun, param0, tol, max_iter)
         param = np.ascontiguousarray(param, dtype=np.float64)   # (tests may inject the alignment)
 
         pred = torch.empty(1, 1, H, W, dtype=torch.float32, device=depth.device)
@@ -211,7 +173,7 @@ def ensemble_depth(
         unc = unc.to(depth.dtype)
     if return_aux:
         return pred, unc, {"param": param, "param0": param0, "member_idx": idx, "nit": nit, "nfev": n_eval[0],
-                            "round_trips": n_eval[1], "cost_fn": cost_fn, "cost_batch": cost_batch, "cost_fd": cost_fd}
+                            "round_trips": n_eval[1], "cost_fn": cost_fn, "cost_fd": cost_fd}
     return pred, unc
 
 

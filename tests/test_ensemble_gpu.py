@@ -144,42 +144,43 @@ def test_median_and_argmax_index_properties_full_size(E):
     assert torch.equal(out.cpu(), torch.gather(n, 0, idx.repeat(1, 3, 1, 1)))
 
 
-def test_cost_batch_is_one_round_trip_and_bit_identical():
-    """One forward-difference gradient (2E points) = ONE device round trip, and cost(x) evaluated inside a batch
-    equals cost(x) evaluated alone bit for bit (otherwise scipy's f(x+h) - f(x) would pick up summation noise)."""
+def test_cost_fd_is_one_round_trip_and_bit_identical():
+    """f(x) and the forward-difference points of its gradient are ONE device round trip, and each of those values equals
+    the objective evaluated alone at that point bit for bit (otherwise scipy's f(x+h) - f(x) would pick up summation
+    noise), for the register-resident (E <= 16) and the generic kernels. The BFGS run built on it follows scipy's own
+    default (jac=None, the reference's call) step for step."""
+    import scipy.optimize
+
     from marigold_b200.ensemble import ensemble_depth
 
-    E = 10
-    g = torch.Generator().manual_seed(3)
-    d = torch.rand(E, 1, 96, 128, generator=g).cuda()
-    p0 = np.concatenate([np.ones(E), np.zeros(E)])
-    _, _, aux = ensemble_depth(d, return_aux=True, param=p0)
     rng = np.random.default_rng(0)
-    P = p0[None] + rng.normal(0, 1e-2, (2 * E + 1, 2 * E))
-    batch = aux["cost_batch"](P)
-    single = np.array([aux["cost_fn"](p) for p in P])
-    np.testing.assert_array_equal(batch, single)
-    # the structured forward-difference pass (base + one perturbed coordinate per row) gives the same bits again
-    for red, shift in (("median", True), ("mean", True), ("median", False)):
-        kw = dict(reduction=red, shift_invariant=shift)
-        n = 2 * E if shift else E
-        b = p0[:n] + rng.normal(0, 1e-2, n)
-        _, _, ax = ensemble_depth(d, return_aux=True, param=b, **kw)
-        X = np.repeat(b[None], n, 0)
-        X[np.arange(n), np.arange(n)] += rng.choice([1.5e-8, 1e-3], n)
-        fd = ax["cost_fd"](X)
-        assert fd is not None
-        np.testing.assert_array_equal(fd, np.array([ax["cost_fn"](x) for x in X]))
-        assert ax["cost_fd"](X[::-1].copy()) is None               # not of the single-coordinate form: generic batch
-    # end to end: round trips = objective calls + gradient calls, far fewer than evaluated points
-    _, _, aux2 = ensemble_depth(d, return_aux=True)
-    assert aux2["nfev"] >= aux2["round_trips"]
-    if aux2["nit"] > 0:   # f(x) and the 2E forward-difference points of its gradient share one round trip
-        assert aux2["round_trips"] * 2 * E <= aux2["nfev"]
-    # the speculation is invisible to scipy: same trajectory with and without it
-    _, _, aux3 = ensemble_depth(d, return_aux=True, speculate=False)
-    np.testing.assert_array_equal(aux2["param"], aux3["param"])
-    assert aux3["round_trips"] > aux2["round_trips"]
+    for E in (10, 17, 33):
+        g = torch.Generator().manual_seed(3)
+        d = torch.rand(E, 1, 96, 128, generator=g).cuda()
+        p0 = np.concatenate([np.ones(E), np.zeros(E)])
+        for red, shift in (("median", True), ("mean", True), ("median", False)):
+            kw = dict(reduction=red, shift_invariant=shift)
+            n = 2 * E if shift else E
+            b = p0[:n] + rng.normal(0, 1e-2, n)
+            _, _, ax = ensemble_depth(d, return_aux=True, param=b, **kw)
+            pert = b + rng.choice([1.5e-8, 1e-3], n)
+            X = np.repeat(b[None], n, 0)
+            X[np.arange(n), np.arange(n)] = pert
+            fd = ax["cost_fd"](b, pert)
+            assert fd.shape == (1 + n,)
+            assert fd[0] == ax["cost_fn"](b)
+            np.testing.assert_array_equal(fd[1:], np.array([ax["cost_fn"](x) for x in X]))
+    # end to end: f(x) and the 2E points of its gradient share one round trip, and the trajectory is scipy's default one
+    for E, max_iter in ((10, 50), (17, 8)):
+        g = torch.Generator().manual_seed(3)
+        d = torch.rand(E, 1, 96, 128, generator=g).cuda()
+        _, _, aux = ensemble_depth(d, return_aux=True, max_iter=max_iter)
+        assert aux["nit"] > 0
+        assert aux["round_trips"] * 2 * E <= aux["nfev"]
+        ref = scipy.optimize.minimize(aux["cost_fn"], aux["param0"], method="BFGS", tol=1e-6,
+                                      options={"maxiter": max_iter, "disp": False})
+        np.testing.assert_array_equal(aux["param"], ref.x)
+        assert aux["nit"] == ref.nit
 
 
 @pytest.mark.parametrize("E,reduction", [(20, "median"), (17, "mean"), (33, "median")])

@@ -171,10 +171,10 @@ def test_iid_output_container_follows_the_reference():
         out.fill_entry("normals", pred[:, :3], None, props)
 
 
-def test_bfgs_driver_follows_scipy_default_finite_differences():
-    """marigold_b200.ensemble._bfgs hands scipy a gradient built from one batch of forward-difference points; the
-    trajectory must be the one scipy's own default (jac=None, as the reference calls it: marigold/util/ensemble.py:
-    165-171) produces, bit for bit."""
+def test_bfgs_driver_one_callback_follows_scipy_default_finite_differences():
+    """marigold_b200.ensemble._bfgs hands scipy one callback that returns f and a gradient built from one batch of
+    forward-difference points (jac=True); the trajectory must be the one scipy's own default (jac=None, as the
+    reference calls it: marigold/util/ensemble.py:165-171) produces, bit for bit."""
     import scipy.optimize
 
     from marigold_b200.ensemble import _bfgs, _fd_grad, _scipy_fd_points
@@ -190,17 +190,18 @@ def test_bfgs_driver_follows_scipy_default_finite_differences():
 
     batches = []
 
-    def grad(x):
+    def fun(x):
         x = np.asarray(x, dtype=np.float64)
         pert = _scipy_fd_points(x)
         xs = np.repeat(x[None], x.size, 0)
         xs[np.arange(x.size), np.arange(x.size)] = pert
         batches.append(len(xs))
-        return _fd_grad(x, f(x), np.array([f(r) for r in xs]), pert)
+        f0 = f(x)
+        return f0, _fd_grad(x, f0, np.array([f(r) for r in xs]), pert)
 
     for x0 in (rng.standard_normal(6), np.array([0.0, 1e9, -1e9, 1.0, -1.0, 3e17])):   # incl. x + eps == x coordinates
         ref = scipy.optimize.minimize(f, x0, method="BFGS", tol=1e-6, options={"maxiter": 50, "disp": False})
-        x1, nit1 = _bfgs(f, grad, x0, 1e-6, 50)
+        x1, nit1 = _bfgs(fun, x0, 1e-6, 50)
         np.testing.assert_array_equal(x1, ref.x)
         assert nit1 == ref.nit and batches and all(c == 6 for c in batches)
 

@@ -1,4 +1,5 @@
-"""Time ensemble_depth (host BFGS + device cost kernels) at the quoted size, and the FD cost call alone.
+"""Time ensemble_depth (host BFGS + device cost kernels) at the quoted size, and its per-iteration call alone: f and
+the forward-difference points of its gradient (`cost_fd`).
 
     python tools/ens_time.py [--res 768] [--members 4 8 10]
 """
@@ -10,7 +11,7 @@ from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import torch  # noqa: E402
 
-from marigold_b200.ensemble import ensemble_depth  # noqa: E402
+from marigold_b200.ensemble import _scipy_fd_points, ensemble_depth  # noqa: E402
 
 
 def main():
@@ -34,9 +35,10 @@ def main():
         ms = (time.perf_counter() - t0) / n * 1e3
         _, _, aux = ensemble_depth(d, scale_invariant=True, shift_invariant=True, output_uncertainty=False, return_aux=True)
         x = aux["param"]
+        pert = _scipy_fd_points(x)
         t0 = time.perf_counter()
         for _ in range(50):
-            aux["cost_fn"](x)
+            aux["cost_fd"](x, pert)
         torch.cuda.synchronize()
         trip = (time.perf_counter() - t0) / 50 * 1e6
         print(f"E={E} res={a.res}: {ms:.2f} ms per ensemble_depth, {aux['round_trips']} round trips, nit {aux['nit']}, "

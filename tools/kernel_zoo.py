@@ -73,10 +73,7 @@ ops.groupnorm(rn(1, 768 * 768, 128), rn(128), rn(128), 1, 768 * 768, 128, 32, 1e
 d = torch.rand(10, 1, 768, 768, device="cuda", generator=g)
 p0 = np.concatenate([np.ones(10), np.zeros(10)])
 _, _, aux = ensemble_depth(d, return_aux=True, param=p0, output_uncertainty=True)     # minmax + reduce + renorm
-aux["cost_batch"](np.repeat(p0[None], 21, 0))            # generic batch: 21 parameter sets, one launch
-X = np.repeat(p0[None], 20, 0)
-X[np.arange(20), np.arange(20)] += 1.5e-8
-aux["cost_fd"](X)                                        # one BFGS gradient, structured: base pass + perturbation rows
+aux["cost_fd"](p0, p0 + 1.5e-8)                          # f and one BFGS gradient: base pass + perturbation rows
 n = torch.nn.functional.normalize(rn(10, 3, 768, 768), dim=1)
 ensemble_normals(n, output_uncertainty=True)
 # ---- bookends and evaluation ----
