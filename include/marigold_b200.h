@@ -203,6 +203,28 @@ int mgb_op_conv2d(const void* x_bf16_dev, const void* w_bf16_dev, const float* b
                   float* out_f32_dev, void* out_bf16_dev, int32_t NB, int32_t Hout, int32_t Wout, int32_t Cin,
                   int32_t Cout, int32_t kind, int32_t flags, int32_t block_n, int32_t splits, int32_t stages,
                   float* splitk_ws_dev, void* stream);
+/* The same two operators with every input the network's GEMMs use (test entry points: each reaches a path of the
+ * network that the plain calls above cannot):
+ *   a2_bf16_dev [M, K2] (or NULL): K concatenation A = [a | a2], w [N, K + K2]  (ff.net.2 + proj_out as one GEMM)
+ *   x2_bf16_dev NHWC [NB, Hout, Wout, Cin2] (or NULL, kinds 0 / 1): a 1x1 convolution appended along K, w
+ *     [Cout, taps*Cin + Cin2]                                                    (ResnetBlock conv2 + 1x1 shortcut)
+ *   ldo: row stride of residual / outputs (0: N, or N / 2 with GEGLU); the conv always uses Cout
+ *   Hsrc, Wsrc: extent of the tensor the taps address (one parity plane for kinds 2 / 3: ceil(Hin / 2) x ceil(Win / 2));
+ *     0 = the output size
+ *   scale (EPI_SCALE), sched_x / sched_z / sched_k_dev {kx, kv, kz} / aux_out (EPI_SCHED): see the epilogue flags.
+ * block_n <= 0 picks the tile; a special epilogue (EPI_SCHED / DEPTH / NORMALS / NCHW) always takes block_n 16, and
+ * an explicit block_n != 16 or N > 16 with one of them returns MGB_ERR_INVALID before anything is launched. */
+int mgb_op_linear_ex(const void* a_bf16_dev, const void* a2_bf16_dev, const void* w_bf16_dev, const float* bias_dev,
+                     const float* residual_dev, float* out_f32_dev, void* out_bf16_dev, int32_t M, int32_t N, int32_t K,
+                     int32_t K2, int32_t ldo, int32_t flags, float scale, const float* sched_x_dev,
+                     const float* sched_z_dev, const float* sched_k_dev, float* aux_out_dev, int32_t block_n,
+                     int32_t splits, int32_t stages, float* splitk_ws_dev, void* stream);
+int mgb_op_conv2d_ex(const void* x_bf16_dev, const void* x2_bf16_dev, const void* w_bf16_dev, const float* bias_dev,
+                     const float* residual_dev, float* out_f32_dev, void* out_bf16_dev, int32_t NB, int32_t Hout,
+                     int32_t Wout, int32_t Cin, int32_t Cin2, int32_t Cout, int32_t kind, int32_t Hsrc, int32_t Wsrc,
+                     int32_t flags, float scale, const float* sched_x_dev, const float* sched_z_dev,
+                     const float* sched_k_dev, float* aux_out_dev, int32_t block_n, int32_t splits, int32_t stages,
+                     float* splitk_ws_dev, void* stream);
 /* Flash self-attention, head size 64 (replaces F.scaled_dot_product_attention under diffusers' Attention, reached
  * from marigold_depth_pipeline.py:461-463). qkv: [NB*T, 3C] (Q | K | V column blocks), out: [NB*T, C]. Long
  * sequences are split over KV ranges and merged by a second kernel; the operator-level entry point keeps the
@@ -217,6 +239,11 @@ size_t mgb_op_groupnorm_ws_bytes(int32_t NB, int32_t HW, int32_t C, int32_t G);
 int mgb_op_groupnorm(const float* x_dev, void* y_bf16_dev, const float* gamma_dev, const float* beta_dev,
                      float* ws_dev, int32_t NB, int32_t HW, int32_t C, int32_t G, float eps, int32_t silu,
                      void* stream);
+/* GroupNorm over the channel concat [xa | xb] (xb NULL with Cb = 0: one source), groups may straddle the boundary;
+ * raw_copy_bf16_dev (or NULL): bf16 copy of the un-normalised concat. ws_dev: mgb_op_groupnorm_ws_bytes(NB, HW, Ca + Cb, G). */
+int mgb_op_groupnorm_ex(const float* xa_dev, int32_t Ca, const float* xb_dev, int32_t Cb, void* y_bf16_dev,
+                        void* raw_copy_bf16_dev, const float* gamma_dev, const float* beta_dev, float* ws_dev, int32_t NB,
+                        int32_t HW, int32_t G, float eps, int32_t silu, void* stream);
 int mgb_op_layernorm(const float* x_dev, void* y_bf16_dev, const float* gamma_dev, const float* beta_dev, int32_t M,
                      int32_t C, float eps, void* stream);
 /* attn2 of diffusers' BasicTransformerBlock against the FIXED two-token context CLIP(""), collapsed (marigold_depth_pipeline.py
@@ -231,6 +258,13 @@ int mgb_op_space_to_depth(const float* x_dev, void* y_bf16_dev, int32_t NB, int3
                           void* stream);
 int mgb_op_upsample2x(const float* x_dev, void* y_bf16_dev, int32_t NB, int32_t H, int32_t W, int32_t C,
                       void* stream);
+/* nearest upsampling to Ho x Wo, Ho in {2H - 1, 2H}, Wo in {2W - 1, 2W} (the UNet's crop to an odd skip size) */
+int mgb_op_upsample2x_ex(const float* x_dev, void* y_bf16_dev, int32_t NB, int32_t H, int32_t W, int32_t C, int32_t Ho,
+                         int32_t Wo, void* stream);
+/* VAE attention helpers. Row softmax: fp32 s[M, ld] (first n columns valid) -> bf16 p[M, ld], columns [n, ld) zero.
+ * Transpose: bf16 x[M, N] -> bf16 y[N, ld], columns [M, ld) zero. */
+int mgb_op_softmax_rows(const float* s_dev, void* p_bf16_dev, int32_t M, int32_t n, int32_t ld, void* stream);
+int mgb_op_transpose_bf16(const void* x_bf16_dev, void* y_bf16_dev, int32_t M, int32_t N, int32_t ld, void* stream);
 
 #ifdef __cplusplus
 }

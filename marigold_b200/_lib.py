@@ -72,13 +72,21 @@ SIGNATURES = {
     "mgb_op_linear": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "mgb_op_conv2d": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32,
                               _i32, _vp, _vp]),
+    "mgb_op_linear_ex": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp,
+                                 _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "mgb_op_conv2d_ex": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32,
+                                 _i32, _f32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "mgb_op_flash_attn64": (_i32, [_vp, _vp, _i32, _i32, _i32, _f32, _vp]),
     "mgb_op_groupnorm_ws_bytes": (C.c_size_t, [_i32, _i32, _i32, _i32]),
     "mgb_op_xattn2": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32, _vp]),
     "mgb_op_groupnorm": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _i32, _vp]),
+    "mgb_op_groupnorm_ex": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _i32, _vp]),
     "mgb_op_layernorm": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp]),
     "mgb_op_space_to_depth": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "mgb_op_upsample2x": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "mgb_op_upsample2x_ex": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mgb_op_softmax_rows": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp]),
+    "mgb_op_transpose_bf16": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp]),
 }
 
 

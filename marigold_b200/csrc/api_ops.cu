@@ -31,55 +31,78 @@ int64_t mgb_launch_count(void) { return launch_count(); }
 void mgb_debug_gemm_timing(void* dev_buffer) { set_gemm_debug_buffer(reinterpret_cast<long long*>(dev_buffer)); }
 
 static void fill_epi(GemmEpilogue* e, const float* bias, const float* residual, float* out_f32, void* out_bf16,
-                     int ldo, int flags) {
+                     int ldo, int flags, float scale, const float* sched_x, const float* sched_z, const float* sched_k,
+                     float* aux_out) {
   memset(e, 0, sizeof(*e));
   e->bias = bias; e->residual = residual; e->out_f32 = out_f32;
   e->out_bf16 = reinterpret_cast<bf16*>(out_bf16);
-  e->ldo = ldo; e->flags = flags; e->scale = 1.0f;
+  e->ldo = ldo; e->flags = flags; e->scale = scale;
+  e->sched_x = sched_x; e->sched_z = sched_z; e->sched_k = sched_k; e->aux_out = aux_out;
 }
 
-int mgb_op_linear(const void* a, const void* w, const float* bias, const float* residual, float* out_f32,
-                  void* out_bf16, int32_t M, int32_t N, int32_t K, int32_t flags, int32_t block_n, int32_t splits,
-                  int32_t stages, float* splitk_ws, void* stream) {
-  if (!a || !w || (!out_f32 && !out_bf16)) { set_error("op_linear: null pointer"); return MGB_ERR_INVALID; }
+int mgb_op_linear_ex(const void* a, const void* a2, const void* w, const float* bias, const float* residual,
+                     float* out_f32, void* out_bf16, int32_t M, int32_t N, int32_t K, int32_t K2, int32_t ldo,
+                     int32_t flags, float scale, const float* sched_x, const float* sched_z, const float* sched_k,
+                     float* aux_out, int32_t block_n, int32_t splits, int32_t stages, float* splitk_ws, void* stream) {
+  if (!a || !w || (!out_f32 && !out_bf16) || (a2 && K2 <= 0)) { set_error("op_linear: null pointer or K2"); return MGB_ERR_INVALID; }
+  if (!a2) K2 = 0;
+  const int n_out = (flags & EPI_GEGLU) ? N / 2 : N;
+  if (ldo <= 0) ldo = n_out;
+  if (ldo < n_out) { set_error("op_linear: ldo %d < %d output columns", ldo, n_out); return MGB_ERR_INVALID; }
   if (block_n <= 0) {
     int bn, sp, st;
-    choose_tile((M + 127) / 128, N, K / 64, (flags & EPI_GEGLU) != 0, splitk_ws != nullptr && !(flags & EPI_GEGLU), &bn, &sp,
-                &st);
+    choose_tile((M + 127) / 128, N, (K + K2) / 64, flags, splitk_ws != nullptr && !(flags & EPI_GEGLU), &bn, &sp, &st);
     block_n = bn; if (splits <= 0) splits = sp; if (stages <= 0) stages = st;
   }
   if (splits <= 0) splits = 1;
   if (stages <= 0) stages = 4;
   GemmParams p;
   int rc = fill_linear_params(&p, reinterpret_cast<const bf16*>(a), reinterpret_cast<const bf16*>(w), M, N, K, block_n,
-                              splits, stages);
+                              splits, stages, reinterpret_cast<const bf16*>(a2), K2);
   if (rc) return rc;
-  fill_epi(&p.epi, bias, residual, out_f32, out_bf16, (flags & EPI_GEGLU) ? N / 2 : N, flags);
+  fill_epi(&p.epi, bias, residual, out_f32, out_bf16, ldo, flags, scale, sched_x, sched_z, sched_k, aux_out);
   return run_gemm(p, block_n, splitk_ws, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int mgb_op_conv2d(const void* x, const void* w, const float* bias, const float* residual, float* out_f32,
-                  void* out_bf16, int32_t NB, int32_t Hout, int32_t Wout, int32_t Cin, int32_t Cout, int32_t kind,
-                  int32_t flags, int32_t block_n, int32_t splits, int32_t stages, float* splitk_ws, void* stream) {
-  if (!x || !w || (!out_f32 && !out_bf16)) { set_error("op_conv2d: null pointer"); return MGB_ERR_INVALID; }
+int mgb_op_linear(const void* a, const void* w, const float* bias, const float* residual, float* out_f32,
+                  void* out_bf16, int32_t M, int32_t N, int32_t K, int32_t flags, int32_t block_n, int32_t splits,
+                  int32_t stages, float* splitk_ws, void* stream) {
+  return mgb_op_linear_ex(a, nullptr, w, bias, residual, out_f32, out_bf16, M, N, K, 0, 0, flags, 1.0f, nullptr, nullptr,
+                          nullptr, nullptr, block_n, splits, stages, splitk_ws, stream);
+}
+
+int mgb_op_conv2d_ex(const void* x, const void* x2, const void* w, const float* bias, const float* residual,
+                     float* out_f32, void* out_bf16, int32_t NB, int32_t Hout, int32_t Wout, int32_t Cin, int32_t Cin2,
+                     int32_t Cout, int32_t kind, int32_t Hsrc, int32_t Wsrc, int32_t flags, float scale,
+                     const float* sched_x, const float* sched_z, const float* sched_k, float* aux_out, int32_t block_n,
+                     int32_t splits, int32_t stages, float* splitk_ws, void* stream) {
+  if (!x || !w || (!out_f32 && !out_bf16) || (x2 && Cin2 <= 0)) { set_error("op_conv2d: null pointer or Cin2"); return MGB_ERR_INVALID; }
+  if (!x2) Cin2 = 0;
   const int taps = kind == 1 ? 1 : 9;
   if (block_n <= 0) {
     int tw, th;
     conv_tile_shape(Hout, Wout, &tw, &th);
     const int m_tiles = NB * ((Wout + tw - 1) / tw) * ((Hout + th - 1) / th);
     int bn, sp, st;
-    choose_tile(m_tiles, Cout, taps * Cin / 64, false, splitk_ws != nullptr, &bn, &sp, &st);
+    choose_tile(m_tiles, Cout, (taps * Cin + Cin2) / 64, flags, splitk_ws != nullptr, &bn, &sp, &st);
     block_n = bn; if (splits <= 0) splits = sp; if (stages <= 0) stages = st;
   }
   if (splits <= 0) splits = 1;
   if (stages <= 0) stages = 4;
   GemmParams p;
   int rc = fill_conv_params(&p, reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(w), NB, Hout, Wout,
-                            Cin, Cout, kind, block_n, splits, stages);
+                            Cin, Cout, kind, block_n, splits, stages, Hsrc, Wsrc, reinterpret_cast<const bf16*>(x2), Cin2);
   if (rc) return rc;
-  fill_epi(&p.epi, bias, residual, out_f32, out_bf16, Cout, flags);
+  fill_epi(&p.epi, bias, residual, out_f32, out_bf16, Cout, flags, scale, sched_x, sched_z, sched_k, aux_out);
   p.epi.hw = Hout * Wout;
   return run_gemm(p, block_n, splitk_ws, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int mgb_op_conv2d(const void* x, const void* w, const float* bias, const float* residual, float* out_f32,
+                  void* out_bf16, int32_t NB, int32_t Hout, int32_t Wout, int32_t Cin, int32_t Cout, int32_t kind,
+                  int32_t flags, int32_t block_n, int32_t splits, int32_t stages, float* splitk_ws, void* stream) {
+  return mgb_op_conv2d_ex(x, nullptr, w, bias, residual, out_f32, out_bf16, NB, Hout, Wout, Cin, 0, Cout, kind, 0, 0, flags,
+                          1.0f, nullptr, nullptr, nullptr, nullptr, block_n, splits, stages, splitk_ws, stream);
 }
 
 int mgb_op_flash_attn64(const void* qkv, void* out, int32_t NB, int32_t T, int32_t C, float scale, void* stream) {
@@ -107,6 +130,23 @@ int mgb_op_groupnorm(const float* x, void* y, const float* gamma, const float* b
                      int32_t C, int32_t G, float eps, int32_t silu, void* stream) {
   int rc = launch_groupnorm(x, reinterpret_cast<bf16*>(y), nullptr, gamma, beta, ws, NB, HW, C, G, eps, silu,
                             reinterpret_cast<cudaStream_t>(stream));
+  if (!rc) count_launch(2);
+  return rc;
+}
+
+int mgb_op_groupnorm_ex(const float* xa, int32_t Ca, const float* xb, int32_t Cb, void* y, void* raw_copy,
+                        const float* gamma, const float* beta, float* ws, int32_t NB, int32_t HW, int32_t G, float eps,
+                        int32_t silu, void* stream) {
+  if (!xa || !y || !ws || (xb == nullptr) != (Cb == 0)) { set_error("op_groupnorm_ex: null pointer or Cb"); return MGB_ERR_INVALID; }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const size_t pb = (groupnorm_part_bytes(NB, HW, Ca + Cb, G) + 255) & ~size_t(255);
+  unsigned* counters = reinterpret_cast<unsigned*>(reinterpret_cast<char*>(ws) + pb);
+  if (cudaMemsetAsync(counters, 0, size_t(NB) * sizeof(unsigned), s) != cudaSuccess) {
+    set_error("op_groupnorm_ex: counter memset failed");
+    return MGB_ERR_CUDA;
+  }
+  int rc = launch_gn_fused(xa, Ca, xb, Cb, reinterpret_cast<bf16*>(y), reinterpret_cast<bf16*>(raw_copy), gamma, beta, NB,
+                           HW, G, eps, silu, ws, counters, s);
   if (!rc) count_launch(2);
   return rc;
 }
@@ -202,8 +242,28 @@ int mgb_op_space_to_depth(const float* x, void* y, int32_t NB, int32_t H, int32_
   return rc;
 }
 
+int mgb_op_upsample2x_ex(const float* x, void* y, int32_t NB, int32_t H, int32_t W, int32_t C, int32_t Ho, int32_t Wo,
+                         void* stream) {
+  int rc = launch_upsample2x(x, reinterpret_cast<bf16*>(y), NB, H, W, C, Ho, Wo, reinterpret_cast<cudaStream_t>(stream));
+  if (!rc) count_launch(1);
+  return rc;
+}
+
 int mgb_op_upsample2x(const float* x, void* y, int32_t NB, int32_t H, int32_t W, int32_t C, void* stream) {
-  int rc = launch_upsample2x(x, reinterpret_cast<bf16*>(y), NB, H, W, C, 2 * H, 2 * W, reinterpret_cast<cudaStream_t>(stream));
+  return mgb_op_upsample2x_ex(x, y, NB, H, W, C, 2 * H, 2 * W, stream);
+}
+
+int mgb_op_softmax_rows(const float* s, void* p, int32_t M, int32_t n, int32_t ld, void* stream) {
+  if (!s || !p || M <= 0 || n <= 0 || ld < n) { set_error("op_softmax_rows: bad argument (M=%d n=%d ld=%d)", M, n, ld); return MGB_ERR_INVALID; }
+  int rc = launch_softmax_rows(s, reinterpret_cast<bf16*>(p), M, n, ld, reinterpret_cast<cudaStream_t>(stream));
+  if (!rc) count_launch(1);
+  return rc;
+}
+
+int mgb_op_transpose_bf16(const void* x, void* y, int32_t M, int32_t N, int32_t ld, void* stream) {
+  if (!x || !y || M <= 0 || N <= 0 || ld < M) { set_error("op_transpose_bf16: bad argument (M=%d N=%d ld=%d)", M, N, ld); return MGB_ERR_INVALID; }
+  int rc = launch_transpose_bf16(reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(y), M, N, ld,
+                                 reinterpret_cast<cudaStream_t>(stream));
   if (!rc) count_launch(1);
   return rc;
 }

@@ -370,6 +370,7 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
           v[i] = src[i];
           if (e.flags & EPI_SCALE) v[i] *= e.scale;
           if (e.bias && (n0 + i) < p.N) v[i] += __ldg(e.bias + n0 + i);
+          if (e.flags & EPI_SILU) v[i] = silu_f(v[i]);
         }
         if (e.flags & (EPI_SCHED | EPI_DEPTH | EPI_NORMALS | EPI_NCHW)) {
           epilogue_special(e, rc, v, p.N);

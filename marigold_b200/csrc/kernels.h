@@ -34,6 +34,8 @@ enum : int {
   EPI_SCALE = 64,       // acc *= scale before bias (used for attention-score GEMMs)
   EPI_UNIT = 128,       // with EPI_NCHW: out = (clip(v, -1, 1) + 1) / 2                     (IID decode head)
 };
+// Epilogues that only the 16-wide GEMM instantiation implements (a whole output row per lane, N <= 16)
+constexpr int kSpecialEpilogues = EPI_SCHED | EPI_DEPTH | EPI_NORMALS | EPI_NCHW;
 
 struct GemmEpilogue {
   const float* bias;      // [N] in accumulator-column order, or nullptr

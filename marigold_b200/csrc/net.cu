@@ -84,7 +84,7 @@ static int linear(Ctx& c, const bf16* a, int M, const LinW& W, const Epi& e, int
   // a2 != nullptr: K concatenation, A = [a (K1 columns) | a2 (W.k - K1 columns)]
   int bn, sp, st;
   const bool geglu = (e.flags & EPI_GEGLU) != 0;
-  choose_tile((M + 127) / 128, W.n, W.k / 64, geglu, true, &bn, &sp, &st);
+  choose_tile((M + 127) / 128, W.n, W.k / 64, e.flags, true, &bn, &sp, &st);
   if (geglu) { bn = 256; sp = 1; st = (W.k / 64 <= 12) ? 2 : 4; }
   if (sp > 1) c.splitk_need = std::max(c.splitk_need, size_t(sp) * M * W.n * sizeof(float));
   if (c.dry) return MGB_OK;
@@ -110,10 +110,8 @@ static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const Conv
   conv_tile_shape(Hout, Wout, &tw, &th);
   const int m_tiles = NB * ((Wout + tw - 1) / tw) * ((Hout + th - 1) / th);
   int bn, sp, st;
-  const bool special = (e.flags & (EPI_SCHED | EPI_DEPTH | EPI_NORMALS | EPI_NCHW)) != 0;
   if ((x2 != nullptr) != (W.k_extra > 0)) { set_error("conv3x3: second operand / weight layout mismatch"); return MGB_ERR_STATE; }
-  choose_tile(m_tiles, W.cout, (9 * W.cin_pad + W.k_extra) / 64, false, !special, &bn, &sp, &st);
-  if (special) bn = 16;
+  choose_tile(m_tiles, W.cout, (9 * W.cin_pad + W.k_extra) / 64, e.flags, true, &bn, &sp, &st);
   const size_t M = size_t(NB) * Hout * Wout;
   if (sp > 1) c.splitk_need = std::max(c.splitk_need, size_t(sp) * M * W.cout * sizeof(float));
   if (c.dry) return MGB_OK;

@@ -140,6 +140,18 @@ int effective_splits(const GemmParams& p) { return (p.num_kb + p.kb_per_split - 
 
 int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) {
   const int splits = effective_splits(p);
+  // The special epilogues exist only in the 16-wide instantiation, where one lane holds a whole output row: any other
+  // width would silently take the plain NHWC epilogue, and N > 16 would index past that row.
+  const int special = p.epi.flags & kSpecialEpilogues;
+  if (special) {
+    const bool three = (special & (EPI_DEPTH | EPI_NORMALS)) != 0;
+    if (block_n != 16 || p.N > 16 || (three && p.N != 3) || !p.epi.out_f32 ||
+        ((special & EPI_SCHED) ? (!p.epi.sched_x || !p.epi.sched_k) : p.epi.hw <= 0)) {
+      set_error("special epilogue (flags %d) needs block_n 16 (got %d), N <= 16 (N == 3 for depth / normals; got %d), "
+                "out_f32, and sched_x + sched_k or hw", p.epi.flags, block_n, p.N);
+      return MGB_ERR_INVALID;
+    }
+  }
   if ((p.epi.flags & EPI_GEGLU) && (block_n % 64 != 0)) {
     set_error("GEGLU epilogue needs block_n %% 64 == 0 (got %d)", block_n);
     return MGB_ERR_INVALID;
@@ -210,12 +222,16 @@ int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) 
 // K block 1030 cycles at BN = 256 (floor 1024), 814 at BN = 160 (floor 640), i.e. max(4*BN + 40, ~800);
 // epilogue 6.1 k cycles at BN = 128 / 160 and 9.8 k at BN = 256, ~2.5 k per 64 columns; prologue + first
 // operand ~3.6 k. The split-K reduce launch (~9000 cycles + its traffic) is an estimate, not measured.
-void choose_tile(int m_tiles, int N, int num_kb, bool geglu, bool allow_split, int* block_n, int* splits,
+void choose_tile(int m_tiles, int N, int num_kb, int flags, bool allow_split, int* block_n, int* splits,
                  int* stages) {
   const int cands[6] = {256, 160, 128, 64, 32, 16};
+  const bool geglu = (flags & EPI_GEGLU) != 0;
+  // the special epilogues run only in the 16-wide instantiation and never under split-K (run_gemm enforces both)
+  const bool special = (flags & kSpecialEpilogues) != 0;
   double best = 1e30;
-  int bbn = 128, bsp = 1;
+  int bbn = special ? 16 : 128, bsp = 1;
   for (int bn : cands) {
+    if (special) break;
     if (geglu && (bn % 64 != 0)) continue;
     if (bn > 64 && N < bn / 2 + 1) continue;  // mostly padding
     if (bn < 64 && N >= 64) continue;         // 16 / 32 wide tiles are for the tiny heads only (N <= 32)

@@ -21,10 +21,12 @@ int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Ho
                      int kind, int block_n, int splits, int stages, int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr,
                      int Cin2 = 0);
 int effective_splits(const GemmParams& p);
-// Launch (plus the deferred epilogue when split-K is active). p.epi must be filled by the caller.
+// Launch (plus the deferred epilogue when split-K is active). p.epi must be filled by the caller. Rejects, before any
+// launch, a special epilogue with block_n != 16, N > 16 (N != 3 for depth / normals) or missing epilogue inputs.
 int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream);
-// Tile width, split-K factor and pipeline depth of a GEMM with m_tiles 128-row tiles, N columns and num_kb K blocks of 64.
-void choose_tile(int m_tiles, int N, int num_kb, bool geglu, bool allow_split, int* block_n, int* splits,
+// Tile width, split-K factor and pipeline depth of a GEMM with m_tiles 128-row tiles, N columns and num_kb K blocks of 64,
+// for epilogue flags `flags` (EPI_GEGLU: widths that are multiples of 64; a special epilogue: width 16, no split-K).
+void choose_tile(int m_tiles, int N, int num_kb, int flags, bool allow_split, int* block_n, int* splits,
                  int* stages);
 
 }  // namespace mgb

@@ -41,6 +41,31 @@ def conv2d(x, w_packed, bias, NB, Hout, Wout, Cin, Cout, kind=0, residual=None, 
     return of, ob
 
 
+def linear_ex(a, w, bias=None, residual=None, a2=None, out=None, out_bf16=None, ldo=0, flags=0, scale=1.0,
+              sched_x=None, sched_z=None, sched_k=None, aux_out=None, block_n=0, splits=0, stages=0, ws=None):
+    """mgb_op_linear_ex: every input the network's GEMMs use; outputs are caller-allocated ([M, ldo] rows)."""
+    lib = _lib.load()
+    M, K = a.shape
+    N = w.shape[0]
+    K2 = a2.shape[1] if a2 is not None else 0
+    check(lib.mgb_op_linear_ex(ptr(a), ptr(a2), ptr(w), ptr(bias), ptr(residual), ptr(out), ptr(out_bf16), M, N, K, K2,
+                               ldo, flags, float(scale), ptr(sched_x), ptr(sched_z), ptr(sched_k), ptr(aux_out), block_n,
+                               splits, stages, ptr(ws), stream_ptr()), "mgb_op_linear_ex")
+    return out, out_bf16
+
+
+def conv2d_ex(x, w_packed, bias, NB, Hout, Wout, Cin, Cout, kind=0, x2=None, Cin2=0, Hsrc=0, Wsrc=0, residual=None,
+              out=None, out_bf16=None, flags=0, scale=1.0, sched_x=None, sched_z=None, sched_k=None, aux_out=None,
+              block_n=0, splits=0, stages=0, ws=None):
+    """mgb_op_conv2d_ex: second (1x1) operand, source extent, scale and scheduler inputs; outputs caller-allocated."""
+    lib = _lib.load()
+    check(lib.mgb_op_conv2d_ex(ptr(x), ptr(x2), ptr(w_packed), ptr(bias), ptr(residual), ptr(out), ptr(out_bf16), NB, Hout,
+                               Wout, Cin, Cin2, Cout, kind, Hsrc, Wsrc, flags, float(scale), ptr(sched_x), ptr(sched_z),
+                               ptr(sched_k), ptr(aux_out), block_n, splits, stages, ptr(ws), stream_ptr()),
+          "mgb_op_conv2d_ex")
+    return out, out_bf16
+
+
 def flash_attn64(qkv, NB, T, C, scale):
     lib = _lib.load()
     out = torch.empty(NB * T, C, dtype=torch.bfloat16, device=qkv.device)
@@ -58,6 +83,22 @@ def groupnorm(x, gamma, beta, NB, HW, C, G, eps, silu):
     check(lib.mgb_op_groupnorm(ptr(x), ptr(y), ptr(gamma), ptr(beta), ptr(ws), NB, HW, C, G, float(eps), int(silu),
                                stream_ptr()), "mgb_op_groupnorm")
     return y
+
+
+def groupnorm_ex(xa, xb, gamma, beta, NB, HW, G, eps, silu, raw_copy=False):
+    """GroupNorm over the channel concat [xa | xb] (xb may be None); returns (y, raw bf16 copy of the concat or None)."""
+    lib = _lib.load()
+    Ca = xa.shape[-1]
+    Cb = xb.shape[-1] if xb is not None else 0
+    y = torch.empty(NB, HW, Ca + Cb, dtype=torch.bfloat16, device=xa.device)
+    raw = torch.empty_like(y) if raw_copy else None
+    nbytes = int(lib.mgb_op_groupnorm_ws_bytes(NB, HW, Ca + Cb, G))
+    if nbytes == 0:
+        raise _lib.MgbError(f"groupnorm: unsupported shape NB={NB} HW={HW} C={Ca}+{Cb} G={G}")
+    ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=xa.device)
+    check(lib.mgb_op_groupnorm_ex(ptr(xa), Ca, ptr(xb), Cb, ptr(y), ptr(raw), ptr(gamma), ptr(beta), ptr(ws), NB, HW, G,
+                                  float(eps), int(silu), stream_ptr()), "mgb_op_groupnorm_ex")
+    return y, raw
 
 
 def xattn2(x, ln2_g, ln2_b, ln3_g, ln3_b, GU, c1, H, scale, eps=1e-5):
@@ -88,9 +129,29 @@ def space_to_depth(x):
     return y
 
 
-def upsample2x(x):
+def upsample2x(x, Ho=None, Wo=None):
+    """Nearest x2 upsampling, optionally cropped to Ho = 2H - 1 / Wo = 2W - 1."""
     lib = _lib.load()
     NB, H, W, Cc = x.shape
-    y = torch.empty(NB, 2 * H, 2 * W, Cc, dtype=torch.bfloat16, device=x.device)
-    check(lib.mgb_op_upsample2x(ptr(x), ptr(y), NB, H, W, Cc, stream_ptr()), "mgb_op_upsample2x")
+    Ho, Wo = Ho or 2 * H, Wo or 2 * W
+    y = torch.empty(NB, Ho, Wo, Cc, dtype=torch.bfloat16, device=x.device)
+    check(lib.mgb_op_upsample2x_ex(ptr(x), ptr(y), NB, H, W, Cc, Ho, Wo, stream_ptr()), "mgb_op_upsample2x_ex")
+    return y
+
+
+def softmax_rows(s, n):
+    """fp32 scores [M, ld] (first n columns valid) -> bf16 probabilities [M, ld], pad columns zero."""
+    lib = _lib.load()
+    M, ld = s.shape
+    p = torch.empty(M, ld, dtype=torch.bfloat16, device=s.device)
+    check(lib.mgb_op_softmax_rows(ptr(s), ptr(p), M, n, ld, stream_ptr()), "mgb_op_softmax_rows")
+    return p
+
+
+def transpose_bf16(x, ld):
+    """bf16 [M, N] -> bf16 [N, ld], columns [M, ld) zero."""
+    lib = _lib.load()
+    M, N = x.shape
+    y = torch.empty(N, ld, dtype=torch.bfloat16, device=x.device)
+    check(lib.mgb_op_transpose_bf16(ptr(x), ptr(y), M, N, ld, stream_ptr()), "mgb_op_transpose_bf16")
     return y
