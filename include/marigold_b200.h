@@ -77,13 +77,16 @@ int mgb_finalize_weights(mgb_handle* h);
 
 /* ---- conditioning --------------------------------------------------------------------------- */
 /* Empty-prompt embedding [n_tokens, cross_dim] fp32 HOST (marigold_depth_pipeline.py:381-394,
- * 438-442; n_tokens == 2). Cross-attention K/V of every block are folded here, once. */
+ * 438-442; n_tokens == 2). Cross-attention K/V of every block are folded here, once.
+ * A call rejected for its arguments changes nothing; a call that fails after that leaves no embedding set, so
+ * denoising returns MGB_ERR_STATE until a later call succeeds. */
 int mgb_set_text_embedding(mgb_handle* h, const float* embed_host, int32_t n_tokens);
 
 /* scheduler.set_timesteps + the per-step coefficients of scheduler.step, computed by the host in
  * float64 (marigold_b200/schedulers.py) so scheduler-config handling stays in Python:
  *     x_prev = kx[i] * x + kv[i] * model_output + kz[i] * noise_i
- * (DDIM eta=0: kz = 0; LCM: kz != 0 on every step but the last). All arrays have n entries. */
+ * (DDIM eta=0: kz = 0; LCM: kz != 0 on every step but the last). All arrays have n entries.
+ * A call that fails for any reason leaves the previous schedule in place and usable. */
 int mgb_set_schedule(mgb_handle* h, int32_t n, const int32_t* timesteps, const float* kx, const float* kv,
                      const float* kz);
 

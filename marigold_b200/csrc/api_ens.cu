@@ -7,30 +7,21 @@
 
 using namespace mgb;
 
-#define CUDA_TRY(expr)                                                                   \
-  do {                                                                                   \
-    cudaError_t _e = (expr);                                                             \
-    if (_e != cudaSuccess) {                                                             \
-      set_error("%s:%d %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e));    \
-      return MGB_ERR_CUDA;                                                               \
-    }                                                                                    \
-  } while (0)
-
 // pinned staging: [out: kMaxP x 3 doubles][st: kMaxP x 2 x maxE floats][min/max: maxE x 64 x 2 floats]
 static size_t pinned_out_doubles() { return size_t(ens_max_batch()) * 3; }
 static size_t pinned_bytes() {
   return pinned_out_doubles() * sizeof(double) + size_t(ens_max_batch()) * 2 * ens_max_members() * sizeof(float) +
          size_t(ens_max_members()) * 64 * 2 * sizeof(float);
 }
-static float* pinned_st(mgb_handle* h) { return reinterpret_cast<float*>(h->ens_pinned + pinned_out_doubles()); }
+static float* pinned_st(mgb_handle* h) { return reinterpret_cast<float*>(h->ens_pinned.get() + pinned_out_doubles()); }
 
+// The device workspace and the pinned staging, allocated by the first call: the handle holds both or neither.
 static int ens_prepare(mgb_handle* h) {
   if (!h) { set_error("null handle"); return MGB_ERR_INVALID; }
-  if (!h->ens_ws) {
-    CUDA_TRY(cudaMalloc(&h->ens_ws, std::max(ens_ws_bytes(), size_t(ens_max_members()) * 64 * 2 * 4)));
-    CUDA_TRY(cudaMallocHost(reinterpret_cast<void**>(&h->ens_pinned), pinned_bytes()));
-  }
-  return MGB_OK;
+  int rc = h->ens_ws.grow(std::max(ens_ws_bytes(), size_t(ens_max_members()) * 64 * 2 * 4));
+  if (!rc) rc = h->ens_pinned.grow(pinned_bytes());
+  if (rc) h->ens_ws.reset();
+  return rc;
 }
 
 static int make_st(const double* param, int E, int scale_inv, int shift_inv, float* st) {
@@ -64,11 +55,9 @@ static int ens_depth_cost(mgb_handle* h, const float* depth, const double* base,
   if (!rc && pert) rc = make_st(pert, E, scale_inv, shift_inv, st + 2 * E);
   if (rc) return rc;
   // per-pixel order statistics of the base point for the register-resident perturbation pass
-  if (pert && E <= kEnsMaxE && size_t(HW) * 3 * sizeof(float) > h->ens_v3_bytes) {
-    if (h->ens_v3) CUDA_TRY(cudaFree(h->ens_v3));
-    h->ens_v3 = nullptr; h->ens_v3_bytes = 0;
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&h->ens_v3), size_t(HW) * 3 * sizeof(float)));
-    h->ens_v3_bytes = size_t(HW) * 3 * sizeof(float);
+  if (pert && E <= kEnsMaxE) {
+    rc = h->ens_v3.grow(size_t(HW) * 3 * sizeof(float));
+    if (rc) return rc;
   }
   int launches = 0;
   rc = launch_ens_depth_cost(depth, st, n, E, HW, shift_inv, median, reg, h->ens_ws, h->ens_v3, h->ens_pinned, &launches,
@@ -103,7 +92,7 @@ int mgb_ens_minmax(mgb_handle* h, const float* depth, int32_t E, int64_t HW, flo
   int blocks = 0;
   CUDA_TRY(cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(stream)));
   float* hp = pinned_st(h) + size_t(ens_max_batch()) * 2 * ens_max_members();
-  rc = launch_ens_minmax(depth, E, HW, reinterpret_cast<float*>(h->ens_ws), hp, &blocks,
+  rc = launch_ens_minmax(depth, E, HW, h->ens_ws, hp, &blocks,
                          reinterpret_cast<cudaStream_t>(stream));
   if (rc) return rc;
   count_launch(1);

@@ -20,18 +20,21 @@ using namespace mgb;
     int _rc = (expr);              \
     if (_rc != MGB_OK) return _rc; \
   } while (0)
-#define CUDA_TRY(expr)                                                                   \
-  do {                                                                                   \
-    cudaError_t _e = (expr);                                                             \
-    if (_e != cudaSuccess) {                                                             \
-      set_error("%s:%d %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e));    \
-      return MGB_ERR_CUDA;                                                               \
-    }                                                                                    \
-  } while (0)
 
 // -------------------------------------------------------------------------------------------------
 // host helpers
 // -------------------------------------------------------------------------------------------------
+static void invalidate_step_graph(mgb_handle* h) { h->step_graph.exec.reset(); }
+
+// Grows a buffer the step graph may have captured: waits for the device and drops the graph before freeing it.
+template <class T>
+static int grow_captured(mgb_handle* h, DevBuf<T>& buf, size_t need) {
+  if (need <= buf.bytes()) return MGB_OK;
+  CUDA_TRY(cudaDeviceSynchronize());
+  invalidate_step_graph(h);
+  return buf.grow(need);
+}
+
 static inline uint16_t f2bf(float f) {  // round-to-nearest-even, NaN preserved
   uint32_t u;
   memcpy(&u, &f, 4);
@@ -55,40 +58,33 @@ static inline float half2f(uint16_t h) {
 }
 
 struct Loader {
-  mgb_handle* h;
+  const std::map<std::string, HostTensor>& host;
+  std::vector<DevBuf<void>> weights;   // handed to the handle only if every upload succeeds
   int rc = MGB_OK;
   const HostTensor* get(const std::string& key) {
-    auto it = h->host.find(key);
-    if (it == h->host.end()) {
+    auto it = host.find(key);
+    if (it == host.end()) {
       if (rc == MGB_OK) { set_error("finalize_weights: tensor '%s' was not loaded", key.c_str()); rc = MGB_ERR_STATE; }
       return nullptr;
     }
     return &it->second;
   }
-  void* dev_alloc(size_t bytes) {
-    void* p = nullptr;
-    if (cudaMalloc(&p, bytes) != cudaSuccess) {
-      if (rc == MGB_OK) { set_error("cudaMalloc(%zu) failed", bytes); rc = MGB_ERR_NOMEM; }
+  // A new device array, filled from src unless null. Nothing more is allocated after a failure: it keeps its text.
+  void* upload(const void* src, size_t bytes) {
+    DevBuf<void> b;
+    if (rc != MGB_OK || (rc = b.grow(bytes)) != MGB_OK) return nullptr;
+    if (src && cudaMemcpy(b, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
+      set_error("cudaMemcpy H2D failed"); rc = MGB_ERR_CUDA;
       return nullptr;
     }
-    h->dev_allocs.push_back(p);
-    return p;
+    weights.push_back(std::move(b));
+    return weights.back();
   }
-  float* up_f32(const std::vector<float>& v) {
-    float* d = static_cast<float*>(dev_alloc(v.size() * 4));
-    if (d && cudaMemcpy(d, v.data(), v.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess && rc == MGB_OK) {
-      set_error("cudaMemcpy H2D failed"); rc = MGB_ERR_CUDA;
-    }
-    return d;
-  }
+  float* up_f32(const std::vector<float>& v) { return static_cast<float*>(upload(v.data(), v.size() * 4)); }
   bf16* up_bf16(const std::vector<float>& v) {
     std::vector<uint16_t> b(v.size());
     for (size_t i = 0; i < v.size(); ++i) b[i] = f2bf(v[i]);
-    bf16* d = static_cast<bf16*>(dev_alloc(b.size() * 2));
-    if (d && cudaMemcpy(d, b.data(), b.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess && rc == MGB_OK) {
-      set_error("cudaMemcpy H2D failed"); rc = MGB_ERR_CUDA;
-    }
-    return d;
+    return static_cast<bf16*>(upload(b.data(), b.size() * 2));
   }
   bool shape_is(const HostTensor* t, std::initializer_list<int64_t> s, const std::string& key) {
     if (!t) return false;
@@ -217,6 +213,10 @@ struct Loader {
     if (shape_is(k2, {C, ctx}, t + ".attn2.to_k.weight") && shape_is(v2, {C, ctx}, t + ".attn2.to_v.weight")) {
       x.k2w = up_f32(k2->data); x.v2w = up_f32(v2->data);
     }
+    // folded against the empty prompt's two tokens by set_text_embedding, in place
+    x.kv = static_cast<float*>(upload(nullptr, size_t(2) * 2 * C * 4));
+    x.xGU = static_cast<bf16*>(upload(nullptr, size_t(2) * (C / 64) * C * 2));
+    x.xc1 = static_cast<float*>(upload(nullptr, size_t(C) * 4));
     // GEGLU: interleave [value | gate] per 256-column accumulator tile
     const HostTensor *fw = get(t + ".ff.net.0.proj.weight"), *fb = get(t + ".ff.net.0.proj.bias");
     if (shape_is(fw, {8 * C, C}, t + ".ff.net.0.proj.weight") && shape_is(fb, {8 * C}, t + ".ff.net.0.proj.bias")) {
@@ -249,15 +249,13 @@ struct Loader {
         x.ffpo.n = C; x.ffpo.k = K;
         x.ffpo.w = up_bf16(wl);
         x.ffpo.b = up_f32(b);
-        float *dA = nullptr, *dB = nullptr;
-        if (x.ffpo.w && cudaMalloc(&dA, size_t(C) * C * 4) == cudaSuccess && cudaMalloc(&dB, size_t(C) * 4 * C * 4) == cudaSuccess &&
+        DevBuf<float> dA, dB;
+        if (x.ffpo.w && dA.grow(size_t(C) * C * 4) == MGB_OK && dB.grow(size_t(C) * 4 * C * 4) == MGB_OK &&
             cudaMemcpy(dA, wpo->data.data(), size_t(C) * C * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
             cudaMemcpy(dB, w2->data.data(), size_t(C) * 4 * C * 4, cudaMemcpyHostToDevice) == cudaSuccess &&
             launch_fold_matmul(dA, dB, x.ffpo.w, C, 4 * C, C, K, C, nullptr) == MGB_OK &&
             cudaDeviceSynchronize() == cudaSuccess) {
         } else if (rc == MGB_OK) { set_error("folding proj_out . ff.net.2 failed for %s", p.c_str()); rc = MGB_ERR_CUDA; }
-        if (dA) cudaFree(dA);
-        if (dB) cudaFree(dB);
       }
     }
     return x;
@@ -308,24 +306,7 @@ int mgb_create(const mgb_config* cfg, mgb_handle** out) {
   return MGB_OK;
 }
 
-void mgb_destroy(mgb_handle* h) {
-  if (!h) return;
-  for (void* p : h->dev_allocs) cudaFree(p);
-  if (h->arena.base) cudaFree(h->arena.base);
-  if (h->splitk_ws) cudaFree(h->splitk_ws);
-  if (h->sched_k) cudaFree(h->sched_k);
-  if (h->sync_slab) cudaFree(h->sync_slab);
-  if (h->bias_table) cudaFree(h->bias_table);
-  if (h->cur_bias) cudaFree(h->cur_bias);
-  if (h->cur_sched_k) cudaFree(h->cur_sched_k);
-  if (h->step_counter) cudaFree(h->step_counter);
-  if (h->step_graph.exec) cudaGraphExecDestroy(h->step_graph.exec);
-  if (h->capture_stream) cudaStreamDestroy(h->capture_stream);
-  if (h->ens_ws) cudaFree(h->ens_ws);
-  if (h->ens_pinned) cudaFreeHost(h->ens_pinned);
-  if (h->ens_v3) cudaFree(h->ens_v3);
-  delete h;
-}
+void mgb_destroy(mgb_handle* h) { delete h; }
 
 int mgb_load_tensor(mgb_handle* h, const char* key, const void* data, const int64_t* shape, int32_t ndim,
                     int32_t dtype) {
@@ -347,15 +328,16 @@ int mgb_load_tensor(mgb_handle* h, const char* key, const void* data, const int6
   return MGB_OK;
 }
 
+// All or nothing: a failed call leaves the handle unfinalized and holding none of its uploads, so it can be retried.
 int mgb_finalize_weights(mgb_handle* h) {
   if (!h) { set_error("null handle"); return MGB_ERR_INVALID; }
   if (h->finalized) { set_error("finalize_weights called twice"); return MGB_ERR_STATE; }
-  Loader L{h};
+  Loader L{h->host, {}};
   const mgb_config& cfg = h->cfg;
   const int* ch = cfg.unet_block_channels;
   const int nl = cfg.unet_layers_per_block;
   const int temb = ch[0] * 4, ctx = cfg.unet_cross_dim;
-  UNetW& U = h->unet;
+  UNetW U;
   U.temb_dim = temb;
   U.conv_in = L.conv("unet.conv_in", cfg.unet_in_channels, ch[0]);
   {
@@ -399,7 +381,7 @@ int mgb_finalize_weights(mgb_handle* h) {
   U.conv_out = L.conv("unet.conv_out", ch[0], cfg.unet_out_channels);
 
   // ---- VAE ----
-  VaeW& V = h->vae;
+  VaeW V;
   const int* vc = cfg.vae_block_channels;
   const int vl = cfg.vae_layers_per_block;
   V.enc_in = L.conv("vae.encoder.conv_in", 3, vc[0]);
@@ -462,13 +444,25 @@ int mgb_finalize_weights(mgb_handle* h) {
   V.dec_out = L.conv("vae.decoder.conv_out", vc[0], 3);
 
   if (L.rc != MGB_OK) return L.rc;
-  // per-transformer folded K/V buffers (filled by set_text_embedding) -- allocated lazily there
+  // what the step graph selects each step into: a row of every resnet's (conv1.bias + time_emb_proj(silu(temb))),
+  // {kx, kv, kz}, and the step counter. Their sizes are fixed by the network, so a retried call reuses them.
+  int total = 0;
+  for (ResnetW& r : U.resnets) { r.bias_off = total; total += r.cout; }
+  TRY(h->cur_bias.grow(size_t(total) * 4));
+  TRY(h->cur_sched_k.grow(3 * 4));
+  TRY(h->step_counter.grow(4));
+  CUDA_TRY(cudaMemset(h->step_counter, 0, 4));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->weights = std::move(L.weights);
+  h->unet = std::move(U);
+  h->vae = std::move(V);
+  h->bias_total = total;
   h->host.clear();
   h->finalized = true;
-  CUDA_TRY(cudaDeviceSynchronize());
   return MGB_OK;
 }
 
+// The folded kv / xGU / xc1 are rewritten in place: a captured step graph reads them.
 int mgb_set_text_embedding(mgb_handle* h, const float* embed_host, int32_t n_tokens) {
   if (!h || !embed_host) { set_error("set_text_embedding: null argument"); return MGB_ERR_INVALID; }
   if (!h->finalized) { set_error("set_text_embedding before finalize_weights"); return MGB_ERR_STATE; }
@@ -477,34 +471,18 @@ int mgb_set_text_embedding(mgb_handle* h, const float* embed_host, int32_t n_tok
               n_tokens);
     return MGB_ERR_UNSUPPORTED;
   }
+  h->text_set = false;
   const int ctx = h->cfg.unet_cross_dim;
-  float* d_ctx = nullptr;
-  CUDA_TRY(cudaMalloc(&d_ctx, size_t(n_tokens) * ctx * 4));
+  DevBuf<float> d_ctx;
+  TRY(d_ctx.grow(size_t(n_tokens) * ctx * 4));
   CUDA_TRY(cudaMemcpy(d_ctx, embed_host, size_t(n_tokens) * ctx * 4, cudaMemcpyHostToDevice));
   for (XfmrW& x : h->unet.xfmrs) {
-    if (!x.kv) {
-      void* p = nullptr;
-      CUDA_TRY(cudaMalloc(&p, size_t(2) * n_tokens * x.C * 4));
-      h->dev_allocs.push_back(p);
-      x.kv = static_cast<float*>(p);
-    }
     TRY(launch_linear_small(d_ctx, x.k2w, nullptr, x.kv, n_tokens, x.C, ctx, 0, 0, nullptr));
     TRY(launch_linear_small(d_ctx, x.v2w, nullptr, x.kv + size_t(n_tokens) * x.C, n_tokens, x.C, ctx, 0, 0, nullptr));
-    if (!x.xGU) {
-      const int H = x.C / 64;
-      void *g = nullptr, *c1 = nullptr;
-      CUDA_TRY(cudaMalloc(&g, size_t(2) * H * x.C * 2));
-      h->dev_allocs.push_back(g);
-      CUDA_TRY(cudaMalloc(&c1, size_t(x.C) * 4));
-      h->dev_allocs.push_back(c1);
-      x.xGU = static_cast<bf16*>(g); x.xc1 = static_cast<float*>(c1);
-    }
     TRY(launch_xattn2_fold(x.q2w, x.o2w, x.o2b, x.kv, x.xGU, x.xc1, x.C, nullptr));
     count_launch(3);
   }
   CUDA_TRY(cudaDeviceSynchronize());
-  CUDA_TRY(cudaFree(d_ctx));
-  h->n_ctx = n_tokens;
   h->text_set = true;
   return MGB_OK;
 }
@@ -514,56 +492,38 @@ int mgb_set_schedule(mgb_handle* h, int32_t n, const int32_t* timesteps, const f
   if (!h || n <= 0 || !timesteps || !kx || !kv || !kz) { set_error("set_schedule: bad argument"); return MGB_ERR_INVALID; }
   if (!h->finalized) { set_error("set_schedule before finalize_weights"); return MGB_ERR_STATE; }
   const UNetW& U = h->unet;
-  const int c0 = h->cfg.unet_block_channels[0], temb = U.temb_dim;
+  const int c0 = h->cfg.unet_block_channels[0], temb = U.temb_dim, total = h->bias_total;
   std::vector<float> t(n), k(size_t(n) * 3);
-  h->timesteps.assign(timesteps, timesteps + n);
-  h->timesteps_idx_scratch.resize(n);
-  for (int i = 0; i < n; ++i) h->timesteps_idx_scratch[i] = i;
-  h->kz_host.assign(kz, kz + n);
   for (int i = 0; i < n; ++i) { t[i] = float(timesteps[i]); k[3 * i] = kx[i]; k[3 * i + 1] = kv[i]; k[3 * i + 2] = kz[i]; }
-  if (h->sched_k) { CUDA_TRY(cudaFree(h->sched_k)); h->sched_k = nullptr; }
-  CUDA_TRY(cudaMalloc(&h->sched_k, k.size() * 4));
-  CUDA_TRY(cudaMemcpy(h->sched_k, k.data(), k.size() * 4, cudaMemcpyHostToDevice));
-  float *d_t = nullptr, *d_emb = nullptr, *d_h1 = nullptr, *d_temb = nullptr;
-  CUDA_TRY(cudaMalloc(&d_t, n * 4));
-  CUDA_TRY(cudaMalloc(&d_emb, size_t(n) * c0 * 4));
-  CUDA_TRY(cudaMalloc(&d_h1, size_t(n) * temb * 4));
-  CUDA_TRY(cudaMalloc(&d_temb, size_t(n) * temb * 4));
+  int max_c = 0;
+  for (const ResnetW& r : U.resnets) max_c = std::max(max_c, r.cout);
+  DevBuf<float> sched_k, d_t, d_emb, d_h1, d_temb, bias_table, tmp;
+  TRY(sched_k.grow(k.size() * 4));
+  CUDA_TRY(cudaMemcpy(sched_k, k.data(), k.size() * 4, cudaMemcpyHostToDevice));
+  TRY(d_t.grow(size_t(n) * 4));
+  TRY(d_emb.grow(size_t(n) * c0 * 4));
+  TRY(d_h1.grow(size_t(n) * temb * 4));
+  TRY(d_temb.grow(size_t(n) * temb * 4));
   CUDA_TRY(cudaMemcpy(d_t, t.data(), n * 4, cudaMemcpyHostToDevice));
   TRY(launch_timestep_embedding(d_t, d_emb, n, c0, nullptr));
   TRY(launch_linear_small(d_emb, U.te_w1, U.te_b1, d_h1, n, temb, c0, 0, 1, nullptr));
   TRY(launch_linear_small(d_h1, U.te_w2, U.te_b2, d_temb, n, temb, temb, 0, 0, nullptr));
   count_launch(3);
   // one contiguous table [n, bias_total]: row i = every resnet's (conv1.bias + time_emb_proj(silu(temb_i)))
-  int total = 0;
-  for (ResnetW& r : h->unet.resnets) { r.bias_off = total; total += r.cout; }
-  h->bias_total = total;
-  if (h->bias_table) { CUDA_TRY(cudaFree(h->bias_table)); h->bias_table = nullptr; }
-  CUDA_TRY(cudaMalloc(&h->bias_table, size_t(n) * total * 4));
-  if (!h->cur_bias) {
-    CUDA_TRY(cudaMalloc(&h->cur_bias, size_t(total) * 4));
-    CUDA_TRY(cudaMalloc(&h->cur_sched_k, 3 * 4));
-    CUDA_TRY(cudaMalloc(&h->step_counter, 4));
-    CUDA_TRY(cudaMemset(h->step_counter, 0, 4));
-  }
-  {
-    float* tmp = nullptr;
-    int max_c = 0;
-    for (ResnetW& r : h->unet.resnets) max_c = std::max(max_c, r.cout);
-    CUDA_TRY(cudaMalloc(&tmp, size_t(n) * max_c * 4));
-    for (ResnetW& r : h->unet.resnets) {
-      TRY(launch_linear_small(d_temb, r.temb_w, r.temb_b, tmp, n, r.cout, temb, 1, 0, nullptr));
-      CUDA_TRY(cudaMemcpy2DAsync(h->bias_table + r.bias_off, size_t(total) * 4, tmp, size_t(r.cout) * 4,
-                                 size_t(r.cout) * 4, n, cudaMemcpyDeviceToDevice, nullptr));
-      count_launch(1);
-    }
-    CUDA_TRY(cudaDeviceSynchronize());
-    CUDA_TRY(cudaFree(tmp));
+  TRY(bias_table.grow(size_t(n) * total * 4));
+  TRY(tmp.grow(size_t(n) * max_c * 4));
+  for (const ResnetW& r : U.resnets) {
+    TRY(launch_linear_small(d_temb, r.temb_w, r.temb_b, tmp, n, r.cout, temb, 1, 0, nullptr));
+    CUDA_TRY(cudaMemcpy2DAsync(bias_table.get() + r.bias_off, size_t(total) * 4, tmp, size_t(r.cout) * 4,
+                               size_t(r.cout) * 4, n, cudaMemcpyDeviceToDevice, nullptr));
+    count_launch(1);
   }
   CUDA_TRY(cudaDeviceSynchronize());
-  cudaFree(d_t); cudaFree(d_emb); cudaFree(d_h1); cudaFree(d_temb);
+  invalidate_step_graph(h);
+  h->sched_k = std::move(sched_k);
+  h->bias_table = std::move(bias_table);
+  h->kz_host.assign(kz, kz + n);
   h->n_steps = n;
-  if (h->step_graph.exec) { cudaGraphExecDestroy(h->step_graph.exec); h->step_graph.exec = nullptr; }
   return MGB_OK;
 }
 
@@ -572,48 +532,15 @@ int mgb_set_schedule(mgb_handle* h, int32_t n, const int32_t* timesteps, const f
 // -------------------------------------------------------------------------------------------------
 enum { OP_UNET = 0, OP_ENCODE = 1, OP_DECODE = 2 };
 
-static int run_graph(mgb_handle* h, Ctx& c, int op, const float* a0, float* a1, const float* a2, float* a3, int step,
-                     int NB, int d0, int d1, int mode);
-
-static int ensure_workspace(mgb_handle* h, int op, int NB, int d0, int d1) {
-  Arena dry;
-  dry.dry = true;
-  Ctx c;
-  c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups;
-  c.splitk_cap = ~size_t(0);
-  TRY(run_graph(h, c, op, nullptr, nullptr, nullptr, nullptr, 0, NB, d0, d1, 0));
-  const size_t need = dry.peak + (1 << 20);
-  if (need > h->arena.cap) {
-    CUDA_TRY(cudaDeviceSynchronize());
-    if (h->step_graph.exec) { cudaGraphExecDestroy(h->step_graph.exec); h->step_graph.exec = nullptr; }
-    if (h->arena.base) CUDA_TRY(cudaFree(h->arena.base));
-    h->arena.base = nullptr; h->arena.cap = 0;
-    void* p = nullptr;
-    if (cudaMalloc(&p, need) != cudaSuccess) { set_error("workspace cudaMalloc(%zu) failed", need); return MGB_ERR_NOMEM; }
-    h->arena.base = static_cast<char*>(p);
-    h->arena.cap = need;
-  }
-  if (c.splitk_need > h->splitk_cap) {
-    CUDA_TRY(cudaDeviceSynchronize());
-    if (h->step_graph.exec) { cudaGraphExecDestroy(h->step_graph.exec); h->step_graph.exec = nullptr; }
-    if (h->splitk_ws) CUDA_TRY(cudaFree(h->splitk_ws));
-    h->splitk_ws = nullptr; h->splitk_cap = 0;
-    void* p = nullptr;
-    if (cudaMalloc(&p, c.splitk_need) != cudaSuccess) { set_error("split-K cudaMalloc(%zu) failed", c.splitk_need); return MGB_ERR_NOMEM; }
-    h->splitk_ws = static_cast<float*>(p);
-    h->splitk_cap = c.splitk_need;
-  }
-  if (c.sync_need > h->sync_slab_count) {
-    CUDA_TRY(cudaDeviceSynchronize());
-    if (h->step_graph.exec) { cudaGraphExecDestroy(h->step_graph.exec); h->step_graph.exec = nullptr; }
-    if (h->sync_slab) CUDA_TRY(cudaFree(h->sync_slab));
-    h->sync_slab = nullptr; h->sync_slab_count = 0;
-    void* p = nullptr;
-    CUDA_TRY(cudaMalloc(&p, c.sync_need * sizeof(unsigned)));
-    h->sync_slab = static_cast<unsigned*>(p);
-    h->sync_slab_count = c.sync_need;
-  }
-  return MGB_OK;
+// The UNet step's NHWC staging buffers, carved from the start of the arena in this order (a braced list is evaluated
+// left to right). The captured step graph bakes in their addresses, so the single step and the denoising loop must
+// lay them out identically.
+struct UNetStaging { float *rgb, *tgt, *nz, *raw; };
+static UNetStaging stage_unet(mgb_handle* h, Arena& a, int NB, int HW) {
+  const size_t n = size_t(NB) * HW * h->cfg.unet_out_channels * 4;
+  auto f32 = [&a](size_t bytes) { return reinterpret_cast<float*>(a.alloc(bytes)); };
+  a.off = 0;
+  return {f32(size_t(NB) * HW * 4 * 4), f32(n), f32(n), f32(n)};
 }
 
 // a0..a3 meaning per op:
@@ -627,24 +554,39 @@ static int run_graph(mgb_handle* h, Ctx& c, int op, const float* a0, float* a1, 
   if (op == OP_DECODE) return vae_decode_forward(h, c, a0, a1, NB, d0, d1, mode);
   // UNET single step through NCHW <-> NHWC conversions
   const int HW = d0 * d1, Ct = h->cfg.unet_out_channels;
-  const size_t n = size_t(NB) * HW * Ct;
-  float* rgb = reinterpret_cast<float*>(c.arena->alloc(size_t(NB) * HW * 4 * 4));
-  float* tgt = reinterpret_cast<float*>(c.arena->alloc(n * 4));
-  float* nz = reinterpret_cast<float*>(c.arena->alloc(n * 4));
-  float* raw = reinterpret_cast<float*>(c.arena->alloc(n * 4));
+  const UNetStaging s = stage_unet(h, *c.arena, NB, HW);
   if (!c.dry) {
-    TRY(launch_nchw_to_nhwc(a0, rgb, NB, 4, HW, 1.f, c.stream));
-    TRY(launch_nchw_to_nhwc(a1, tgt, NB, Ct, HW, 1.f, c.stream));
+    TRY(launch_nchw_to_nhwc(a0, s.rgb, NB, 4, HW, 1.f, c.stream));
+    TRY(launch_nchw_to_nhwc(a1, s.tgt, NB, Ct, HW, 1.f, c.stream));
     count_launch(2);
-    if (a2) { TRY(launch_nchw_to_nhwc(a2, nz, NB, Ct, HW, 1.f, c.stream)); count_launch(1); }
+    if (a2) { TRY(launch_nchw_to_nhwc(a2, s.nz, NB, Ct, HW, 1.f, c.stream)); count_launch(1); }
   }
-  TRY(unet_forward(h, c, rgb, tgt, a2 ? nz : nullptr, a3 ? raw : nullptr, step, NB, d0, d1));
+  TRY(unet_forward(h, c, s.rgb, s.tgt, a2 ? s.nz : nullptr, a3 ? s.raw : nullptr, step, NB, d0, d1));
   if (!c.dry) {
-    TRY(launch_nhwc_to_nchw(tgt, a1, NB, Ct, HW, 1.f, c.stream));
+    TRY(launch_nhwc_to_nchw(s.tgt, a1, NB, Ct, HW, 1.f, c.stream));
     count_launch(1);
-    if (a3) { TRY(launch_nhwc_to_nchw(raw, a3, NB, Ct, HW, 1.f, c.stream)); count_launch(1); }
+    if (a3) { TRY(launch_nhwc_to_nchw(s.raw, a3, NB, Ct, HW, 1.f, c.stream)); count_launch(1); }
   }
   return MGB_OK;
+}
+
+struct WorkspaceNeed { size_t arena = 0, splitk = 0, sync = 0; };   // bytes
+
+// Dry-runs one graph: its arena peak, split-K workspace and GroupNorm barrier counters.
+static int workspace_need(mgb_handle* h, int op, int NB, int d0, int d1, WorkspaceNeed* need) {
+  Arena dry; dry.dry = true;
+  Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
+  TRY(run_graph(h, c, op, nullptr, nullptr, nullptr, nullptr, 0, NB, d0, d1, 0));
+  *need = {dry.peak, c.splitk_need, c.sync_need * sizeof(unsigned)};
+  return MGB_OK;
+}
+
+static int ensure_workspace(mgb_handle* h, int op, int NB, int d0, int d1) {
+  WorkspaceNeed need;
+  TRY(workspace_need(h, op, NB, d0, d1, &need));
+  TRY(grow_captured(h, h->arena_buf, need.arena + (1 << 20)));
+  TRY(grow_captured(h, h->splitk_ws, need.splitk));
+  return grow_captured(h, h->sync_slab, need.sync);
 }
 
 static int check_ready(mgb_handle* h, bool need_sched) {
@@ -661,13 +603,24 @@ static Ctx make_ctx(mgb_handle* h, void* stream) {
   Ctx c;
   c.stream = reinterpret_cast<cudaStream_t>(stream);
   c.arena = &h->arena;
+  c.arena->base = h->arena_buf; c.arena->cap = h->arena_buf.bytes();
   c.arena->dry = false; c.arena->overflow = false;
   c.dry = false;
-  c.splitk_ws = h->splitk_ws; c.splitk_cap = h->splitk_cap;
+  c.splitk_ws = h->splitk_ws; c.splitk_cap = h->splitk_ws.bytes();
   c.groups = h->cfg.norm_groups;
   c.sync_base = h->sync_slab;
-  c.sync_cap = h->sync_slab_count;
+  c.sync_cap = h->sync_slab.bytes() / sizeof(unsigned);
   return c;
+}
+
+// Sizes the workspace for one graph, then runs it once on `stream` (run_graph's arguments).
+static int run_once(mgb_handle* h, void* stream, int op, const float* a0, float* a1, const float* a2, float* a3,
+                    int step, int NB, int d0, int d1, int mode) {
+  TRY(ensure_workspace(h, op, NB, d0, d1));
+  Ctx c = make_ctx(h, stream);
+  TRY(run_graph(h, c, op, a0, a1, a2, a3, step, NB, d0, d1, mode));
+  if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
+  return MGB_OK;
 }
 
 int mgb_encode(mgb_handle* h, const float* rgb, int32_t B, int32_t H, int32_t W, float* latent, void* stream) {
@@ -676,11 +629,7 @@ int mgb_encode(mgb_handle* h, const float* rgb, int32_t B, int32_t H, int32_t W,
     set_error("mgb_encode: need B > 0 and H, W >= 8 (got %d x %d)", H, W);
     return MGB_ERR_INVALID;
   }
-  TRY(ensure_workspace(h, OP_ENCODE, B, H, W));
-  Ctx c = make_ctx(h, stream);
-  TRY(run_graph(h, c, OP_ENCODE, rgb, latent, nullptr, nullptr, 0, B, H, W, 0));
-  if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
-  return MGB_OK;
+  return run_once(h, stream, OP_ENCODE, rgb, latent, nullptr, nullptr, 0, B, H, W, 0);
 }
 
 int mgb_unet_step(mgb_handle* h, const float* rgb_latent, float* target, const float* noise, float* model_out,
@@ -692,11 +641,7 @@ int mgb_unet_step(mgb_handle* h, const float* rgb_latent, float* target, const f
   }
   if (step_index < 0 || step_index >= h->n_steps) { set_error("step_index %d outside schedule of %d", step_index, h->n_steps); return MGB_ERR_INVALID; }
   if (h->kz_host[step_index] != 0.f && !noise) { set_error("step %d needs noise (kz != 0)", step_index); return MGB_ERR_INVALID; }
-  TRY(ensure_workspace(h, OP_UNET, B, lh, lw));
-  Ctx c = make_ctx(h, stream);
-  TRY(run_graph(h, c, OP_UNET, rgb_latent, target, noise, model_out, step_index, B, lh, lw, 0));
-  if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
-  return MGB_OK;
+  return run_once(h, stream, OP_UNET, rgb_latent, target, noise, model_out, step_index, B, lh, lw, 0);
 }
 
 int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, const float* step_noise,
@@ -716,64 +661,62 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
   Ctx c = make_ctx(h, stream);
   const int HW = lh * lw, Ct = h->cfg.unet_out_channels;
   const size_t n = size_t(B) * HW * Ct;
-  c.arena->off = 0;
-  float* rgb = reinterpret_cast<float*>(c.arena->alloc(size_t(B) * HW * 4 * 4));
-  float* tgt = reinterpret_cast<float*>(c.arena->alloc(n * 4));
-  float* nz = reinterpret_cast<float*>(c.arena->alloc(n * 4));
-  (void)c.arena->alloc(n * 4);
+  const UNetStaging s = stage_unet(h, *c.arena, B, HW);
   const size_t base = c.arena->mark();
-  TRY(launch_nchw_to_nhwc(rgb_latent, rgb, B, 4, HW, 1.f, c.stream));
-  TRY(launch_nchw_to_nhwc(target, tgt, B, Ct, HW, 1.f, c.stream));
+  TRY(launch_nchw_to_nhwc(rgb_latent, s.rgb, B, 4, HW, 1.f, c.stream));
+  TRY(launch_nchw_to_nhwc(target, s.tgt, B, Ct, HW, 1.f, c.stream));
   count_launch(2);
   const bool any_noise = step_noise != nullptr;
-  if (!any_noise) CUDA_TRY(cudaMemsetAsync(nz, 0, n * 4, c.stream));   // kz * 0 must stay finite
+  if (!any_noise) CUDA_TRY(cudaMemsetAsync(s.nz, 0, n * 4, c.stream));   // kz * 0 must stay finite
   static const bool graphs = getenv("MGB_NO_GRAPH") == nullptr;
   mgb_handle::StepGraph& G = h->step_graph;
   for (int i = first_step; i < first_step + num_steps; ++i) {
     if (h->kz_host[i] != 0.f) {
-      TRY(launch_nchw_to_nhwc(step_noise + size_t(i) * n, nz, B, Ct, HW, 1.f, c.stream));
+      TRY(launch_nchw_to_nhwc(step_noise + size_t(i) * n, s.nz, B, Ct, HW, 1.f, c.stream));
       count_launch(1);
     }
-    const bool graph_ok = graphs && G.exec && G.NB == B && G.lh == lh && G.lw == lw &&
-                          G.arena_base == h->arena.base && G.splitk == h->splitk_ws;
-    if (graph_ok) {
+    if (graphs && G.exec && G.NB == B && G.lh == lh && G.lw == lw) {
       // arm the device step counter for this replay (pageable 4-byte H2D: staged by the driver, so the
       // source may be reused immediately)
-      CUDA_TRY(cudaMemcpyAsync(h->step_counter, &h->timesteps_idx_scratch[i], 4, cudaMemcpyHostToDevice, c.stream));
-      CUDA_TRY(cudaGraphLaunch(G.exec, c.stream));
+      CUDA_TRY(cudaMemcpyAsync(h->step_counter, &i, 4, cudaMemcpyHostToDevice, c.stream));
+      CUDA_TRY(cudaGraphLaunch(G.exec.get(), c.stream));
       count_launch(int(G.launches));
       continue;
     }
     c.arena->release(base);
-    TRY(unet_forward(h, c, rgb, tgt, nz, nullptr, i, B, lh, lw));      // eager (also warms one-time attributes)
+    TRY(unet_forward(h, c, s.rgb, s.tgt, s.nz, nullptr, i, B, lh, lw));  // eager (also warms one-time attributes)
     if (graphs && !G.exec_failed) {
       // capture one step (reads the step index from the device counter) for all later steps of this shape
-      if (G.exec) { cudaGraphExecDestroy(G.exec); G.exec = nullptr; }
-      if (!h->capture_stream) CUDA_TRY(cudaStreamCreateWithFlags(&h->capture_stream, cudaStreamNonBlocking));
+      invalidate_step_graph(h);
       Ctx cc = c;
-      cc.stream = h->capture_stream;
+      cc.stream = h->capture_stream.get();
+      if (!cc.stream) {
+        CUDA_TRY(cudaStreamCreateWithFlags(&cc.stream, cudaStreamNonBlocking));
+        h->capture_stream.reset(cc.stream);
+      }
       const long long l0 = launch_count();
       cudaGraph_t graph = nullptr;
-      cudaError_t ce = cudaStreamBeginCapture(h->capture_stream, cudaStreamCaptureModeThreadLocal);
+      cudaError_t ce = cudaStreamBeginCapture(cc.stream, cudaStreamCaptureModeThreadLocal);
       int rc = MGB_OK;
       if (ce == cudaSuccess) {
         c.arena->release(base);
-        rc = unet_forward(h, cc, rgb, tgt, nz, nullptr, -1, B, lh, lw);
-        ce = cudaStreamEndCapture(h->capture_stream, &graph);
+        rc = unet_forward(h, cc, s.rgb, s.tgt, s.nz, nullptr, -1, B, lh, lw);
+        ce = cudaStreamEndCapture(cc.stream, &graph);
       }
       const long long nl = launch_count() - l0;
       count_launch(-int(nl));                                            // capture launched nothing
-      if (rc == MGB_OK && ce == cudaSuccess && graph) ce = cudaGraphInstantiate(&G.exec, graph, 0);
+      cudaGraphExec_t exec = nullptr;
+      if (rc == MGB_OK && ce == cudaSuccess && graph) ce = cudaGraphInstantiate(&exec, graph, 0);
       if (graph) cudaGraphDestroy(graph);
-      if (rc != MGB_OK || ce != cudaSuccess || !G.exec) {
-        cudaGetLastError();
-        G.exec = nullptr; G.exec_failed = true;                          // stay on the eager path
+      if (rc == MGB_OK && ce == cudaSuccess && exec) {
+        G.exec.reset(exec); G.NB = B; G.lh = lh; G.lw = lw; G.launches = nl;
       } else {
-        G.NB = B; G.lh = lh; G.lw = lw; G.arena_base = h->arena.base; G.splitk = h->splitk_ws; G.launches = nl;
+        cudaGetLastError();
+        G.exec_failed = true;                                            // stay on the eager path
       }
     }
   }
-  TRY(launch_nhwc_to_nchw(tgt, target, B, Ct, HW, 1.f, c.stream));
+  TRY(launch_nhwc_to_nchw(s.tgt, target, B, Ct, HW, 1.f, c.stream));
   count_launch(1);
   if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
   return MGB_OK;
@@ -792,11 +735,7 @@ int mgb_decode(mgb_handle* h, const float* latent, int32_t B, int32_t lh, int32_
     set_error("mgb_decode: bad argument (latent %d x %d, mode %d)", lh, lw, mode);
     return MGB_ERR_INVALID;
   }
-  TRY(ensure_workspace(h, OP_DECODE, B, lh, lw));
-  Ctx c = make_ctx(h, stream);
-  TRY(run_graph(h, c, OP_DECODE, latent, out, nullptr, nullptr, 0, B, lh, lw, mode));
-  if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
-  return MGB_OK;
+  return run_once(h, stream, OP_DECODE, latent, out, nullptr, nullptr, 0, B, lh, lw, mode);
 }
 
 /* debug hooks (not in the public header) */
@@ -805,11 +744,10 @@ size_t mgb_workspace_bytes(mgb_handle* h, int32_t B, int32_t H, int32_t W) {
   if (!h || !h->finalized || B <= 0 || H < 8 || W < 8) return 0;
   size_t peak = 0;
   for (int op = 0; op < 3; ++op) {
-    Arena dry; dry.dry = true;
-    Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
     const int d0 = op == OP_ENCODE ? H : H / 8, d1 = op == OP_ENCODE ? W : W / 8;
-    if (run_graph(h, c, op, nullptr, nullptr, nullptr, nullptr, 0, B, d0, d1, 0) != MGB_OK) return 0;
-    peak = std::max(peak, dry.peak + c.splitk_need);
+    WorkspaceNeed need;
+    if (workspace_need(h, op, B, d0, d1, &need) != MGB_OK) return 0;
+    peak = std::max(peak, need.arena + need.splitk);
   }
   return peak;
 }

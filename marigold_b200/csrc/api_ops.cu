@@ -3,6 +3,7 @@
 #include <cstdio>
 #include <cstring>
 
+#include "device.h"
 #include "kernels.h"
 #include "ops.h"
 
@@ -29,6 +30,8 @@ const char* mgb_build_info(void) {
 int64_t mgb_launch_count(void) { return launch_count(); }
 /* debug hook (not in the public header): per-CTA clock64 phase stamps of subsequent GEMM launches */
 void mgb_debug_gemm_timing(void* dev_buffer) { set_gemm_debug_buffer(reinterpret_cast<long long*>(dev_buffer)); }
+/* debug hook (not in the public header): bytes of device and pinned host memory the library's buffers hold now */
+int64_t mgb_debug_live_device_bytes(void) { return g_live_bytes.load(); }
 
 static void fill_epi(GemmEpilogue* e, const float* bias, const float* residual, float* out_f32, void* out_bf16,
                      int ldo, int flags, float scale, const float* sched_x, const float* sched_z, const float* sched_k,
@@ -107,19 +110,16 @@ int mgb_op_conv2d(const void* x, const void* w, const float* bias, const float* 
 
 int mgb_op_flash_attn64(const void* qkv, void* out, int32_t NB, int32_t T, int32_t C, float scale, void* stream) {
   // split-KV workspace of the operator-level entry point: a process-wide buffer grown on demand (the network
-  // path carves it out of its arena instead)
-  static float* ws = nullptr;
-  static size_t ws_bytes = 0;
+  // path carves it out of its arena instead). Never destroyed, so it is not freed during static destruction,
+  // after the CUDA runtime may have unloaded.
+  static DevBuf<float>& ws = *new DevBuf<float>();
   const size_t need = flash_attn64_ws_bytes(NB, T, C);
-  if (need > ws_bytes) {
+  if (need > ws.bytes()) {
     cudaDeviceSynchronize();
-    if (ws) cudaFree(ws);
-    ws = nullptr; ws_bytes = 0;
-    if (cudaMalloc(&ws, need) != cudaSuccess) { set_error("op_flash_attn64: workspace cudaMalloc(%zu) failed", need); return MGB_ERR_NOMEM; }
-    ws_bytes = need;
+    if (int rc = ws.grow(need)) return rc;
   }
   int rc = launch_flash_attn64(reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(out), NB, T, C, scale,
-                               need ? ws : nullptr, need ? ws_bytes : 0, reinterpret_cast<cudaStream_t>(stream));
+                               need ? ws.get() : nullptr, need ? ws.bytes() : 0, reinterpret_cast<cudaStream_t>(stream));
   if (!rc) count_launch(need ? 2 : 1);
   return rc;
 }

@@ -7,6 +7,7 @@
 #include <unordered_set>
 #include <vector>
 
+#include "device.h"
 #include "kernels.h"
 #include "ops.h"
 
@@ -130,41 +131,36 @@ struct mgb_handle {
   mgb_config cfg;
   std::map<std::string, mgb::HostTensor> host;  // until finalize
   bool finalized = false;
-  std::vector<void*> dev_allocs;
+  std::vector<mgb::DevBuf<void>> weights;  // every device array the UNetW / VaeW raw pointers point into
   mgb::UNetW unet;
   mgb::VaeW vae;
-  mgb::Arena arena;
-  float* splitk_ws = nullptr;
-  size_t splitk_cap = 0;
+  mgb::DevBuf<char> arena_buf;
+  mgb::Arena arena;                 // view of arena_buf, refreshed by each call that runs a graph
+  mgb::DevBuf<float> splitk_ws;
+  mgb::DevBuf<unsigned> sync_slab;  // GroupNorm grid-barrier counters of one forward
   // conditioning / schedule
-  int n_ctx = 0;
   bool text_set = false;
   int n_steps = 0;
-  std::vector<int> timesteps;
-  float* sched_k = nullptr;   // device [n_steps, 3]
+  mgb::DevBuf<float> sched_k;       // device [n_steps, 3]
   std::vector<float> kz_host;
   // per-step tables selected on the device (so one CUDA graph serves every step)
-  float* bias_table = nullptr;  // device [n_steps, bias_total]
+  mgb::DevBuf<float> bias_table;    // device [n_steps, bias_total]
   int bias_total = 0;
-  float* cur_bias = nullptr;    // device [bias_total]
-  float* cur_sched_k = nullptr; // device [3]
-  int* step_counter = nullptr;  // device
-  // cached CUDA graph of one UNet step
+  mgb::DevBuf<float> cur_bias;      // device [bias_total]
+  mgb::DevBuf<float> cur_sched_k;   // device [3]
+  mgb::DevBuf<int> step_counter;    // device
+  // ensemble scratch
+  mgb::DevBuf<float> ens_ws;
+  mgb::PinnedBuf<double> ens_pinned;  // pinned host staging (api_ens.cu)
+  mgb::DevBuf<float> ens_v3;          // per-pixel order statistics for the forward-difference objective
+  // Cached CUDA graph of one UNet step. It is keyed by (NB, lh, lw) alone: whatever replaces a buffer whose address
+  // the graph captured (arena, split-K workspace, sync slab, sched_k, bias_table) calls invalidate_step_graph first.
+  // Declared after the buffers so that it is destroyed before them.
   struct StepGraph {
-    cudaGraphExec_t exec = nullptr;
+    mgb::GraphExec exec;
     int NB = 0, lh = 0, lw = 0;
-    const char* arena_base = nullptr;
-    const float* splitk = nullptr;
     long long launches = 0;
     bool exec_failed = false;
   } step_graph;
-  std::vector<int> timesteps_idx_scratch;  // [0, 1, 2, ...]: host source for arming the device step counter
-  cudaStream_t capture_stream = nullptr;
-  unsigned* sync_slab = nullptr;   // GroupNorm grid-barrier counters of one forward
-  size_t sync_slab_count = 0;
-  // ensemble scratch
-  void* ens_ws = nullptr;
-  double* ens_pinned = nullptr;  // pinned host staging (api_ens.cu)
-  float* ens_v3 = nullptr;       // per-pixel order statistics for the forward-difference objective
-  size_t ens_v3_bytes = 0;
+  mgb::Stream capture_stream;
 };
