@@ -191,7 +191,8 @@ int mgb_eval_normals(const float* pred_dev, const float* gt_dev, const uint8_t* 
 /* ---- capacity ------------------------------------------------------------------------------- */
 /* Bytes of the activation arena the handle holds for images of H x W with B members per batch. */
 size_t mgb_workspace_bytes(mgb_handle* h, int32_t B, int32_t H, int32_t W);
-/* Number of kernel launches enqueued by this library since creation (for bench.py gpu_launches). */
+/* Number of kernel launches enqueued by this library since creation (for bench.py gpu_launches). Memsets and copies
+   are not counted; a replay of a captured CUDA graph counts the kernels the graph holds. */
 int64_t mgb_launch_count(void);
 
 /* ---- operator-level entry points (layer parity tests; tests/test_ops_gpu.py) ---------------- */

@@ -59,11 +59,9 @@ static int ens_depth_cost(mgb_handle* h, const float* depth, const double* base,
     rc = h->ens_v3.grow(size_t(HW) * 3 * sizeof(float));
     if (rc) return rc;
   }
-  int launches = 0;
-  rc = launch_ens_depth_cost(depth, st, n, E, HW, shift_inv, median, reg, h->ens_ws, h->ens_v3, h->ens_pinned, &launches,
+  rc = launch_ens_depth_cost(depth, st, n, E, HW, shift_inv, median, reg, h->ens_ws, h->ens_v3, h->ens_pinned,
                              reinterpret_cast<cudaStream_t>(stream));
   if (rc) return rc;
-  count_launch(launches);
   for (int i = 0; i <= n; ++i) costs_out[i] = h->ens_pinned[3 * i];
   return MGB_OK;
 }
@@ -95,7 +93,6 @@ int mgb_ens_minmax(mgb_handle* h, const float* depth, int32_t E, int64_t HW, flo
   rc = launch_ens_minmax(depth, E, HW, h->ens_ws, hp, &blocks,
                          reinterpret_cast<cudaStream_t>(stream));
   if (rc) return rc;
-  count_launch(1);
   for (int e = 0; e < E; ++e) {
     float mn = FLT_MAX, mx = -FLT_MAX;
     for (int b = 0; b < blocks; ++b) { mn = std::min(mn, hp[(e * blocks + b) * 2]); mx = std::max(mx, hp[(e * blocks + b) * 2 + 1]); }
@@ -115,26 +112,20 @@ int mgb_ens_depth_reduce(mgb_handle* h, const float* depth, const double* param,
   float* st_pinned = pinned_st(h);
   rc = make_st(param, E, scale_inv, shift_inv, st_pinned);
   if (rc) return rc;
-  rc = launch_ens_depth_reduce(depth, st_pinned, E, HW, shift_inv, median, shift_inv ? 1 : 0, pred, unc, member_idx,
-                               h->ens_ws, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(2);
-  return rc;
+  return launch_ens_depth_reduce(depth, st_pinned, E, HW, shift_inv, median, shift_inv ? 1 : 0, pred, unc, member_idx,
+                                 h->ens_ws, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_ens_iid(mgb_handle* h, const float* targets, int32_t E, int64_t N, int32_t median, float* pred, float* unc,
                 void* stream) {
   if (!h || !targets || !pred || N <= 0) { set_error("ens_iid: bad argument"); return MGB_ERR_INVALID; }
-  int rc = launch_ens_iid(targets, E, N, median, pred, unc, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_ens_iid(targets, E, N, median, pred, unc, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_ens_normals(mgb_handle* h, const float* normals, int32_t E, int64_t HW, int32_t closest, float* out,
                     float* unc, int32_t* member_idx, void* stream) {
   if (!h || !normals || !out || HW <= 0) { set_error("ens_normals: bad argument"); return MGB_ERR_INVALID; }
-  int rc = launch_ens_normals(normals, E, HW, closest, out, unc, member_idx, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_ens_normals(normals, E, HW, closest, out, unc, member_idx, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

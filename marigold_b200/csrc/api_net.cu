@@ -4,6 +4,7 @@
 #include <cstdlib>
 #include <cstring>
 
+#include "launch.h"
 #include "net.h"
 
 namespace mgb {
@@ -14,12 +15,6 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
 }  // namespace mgb
 
 using namespace mgb;
-
-#define TRY(expr)                  \
-  do {                             \
-    int _rc = (expr);              \
-    if (_rc != MGB_OK) return _rc; \
-  } while (0)
 
 // -------------------------------------------------------------------------------------------------
 // host helpers
@@ -480,7 +475,6 @@ int mgb_set_text_embedding(mgb_handle* h, const float* embed_host, int32_t n_tok
     TRY(launch_linear_small(d_ctx, x.k2w, nullptr, x.kv, n_tokens, x.C, ctx, 0, 0, nullptr));
     TRY(launch_linear_small(d_ctx, x.v2w, nullptr, x.kv + size_t(n_tokens) * x.C, n_tokens, x.C, ctx, 0, 0, nullptr));
     TRY(launch_xattn2_fold(x.q2w, x.o2w, x.o2b, x.kv, x.xGU, x.xc1, x.C, nullptr));
-    count_launch(3);
   }
   CUDA_TRY(cudaDeviceSynchronize());
   h->text_set = true;
@@ -508,7 +502,6 @@ int mgb_set_schedule(mgb_handle* h, int32_t n, const int32_t* timesteps, const f
   TRY(launch_timestep_embedding(d_t, d_emb, n, c0, nullptr));
   TRY(launch_linear_small(d_emb, U.te_w1, U.te_b1, d_h1, n, temb, c0, 0, 1, nullptr));
   TRY(launch_linear_small(d_h1, U.te_w2, U.te_b2, d_temb, n, temb, temb, 0, 0, nullptr));
-  count_launch(3);
   // one contiguous table [n, bias_total]: row i = every resnet's (conv1.bias + time_emb_proj(silu(temb_i)))
   TRY(bias_table.grow(size_t(n) * total * 4));
   TRY(tmp.grow(size_t(n) * max_c * 4));
@@ -516,7 +509,6 @@ int mgb_set_schedule(mgb_handle* h, int32_t n, const int32_t* timesteps, const f
     TRY(launch_linear_small(d_temb, r.temb_w, r.temb_b, tmp, n, r.cout, temb, 1, 0, nullptr));
     CUDA_TRY(cudaMemcpy2DAsync(bias_table.get() + r.bias_off, size_t(total) * 4, tmp, size_t(r.cout) * 4,
                                size_t(r.cout) * 4, n, cudaMemcpyDeviceToDevice, nullptr));
-    count_launch(1);
   }
   CUDA_TRY(cudaDeviceSynchronize());
   invalidate_step_graph(h);
@@ -558,14 +550,12 @@ static int run_graph(mgb_handle* h, Ctx& c, int op, const float* a0, float* a1, 
   if (!c.dry) {
     TRY(launch_nchw_to_nhwc(a0, s.rgb, NB, 4, HW, 1.f, c.stream));
     TRY(launch_nchw_to_nhwc(a1, s.tgt, NB, Ct, HW, 1.f, c.stream));
-    count_launch(2);
-    if (a2) { TRY(launch_nchw_to_nhwc(a2, s.nz, NB, Ct, HW, 1.f, c.stream)); count_launch(1); }
+    if (a2) TRY(launch_nchw_to_nhwc(a2, s.nz, NB, Ct, HW, 1.f, c.stream));
   }
   TRY(unet_forward(h, c, s.rgb, s.tgt, a2 ? s.nz : nullptr, a3 ? s.raw : nullptr, step, NB, d0, d1));
   if (!c.dry) {
     TRY(launch_nhwc_to_nchw(s.tgt, a1, NB, Ct, HW, 1.f, c.stream));
-    count_launch(1);
-    if (a3) { TRY(launch_nhwc_to_nchw(s.raw, a3, NB, Ct, HW, 1.f, c.stream)); count_launch(1); }
+    if (a3) TRY(launch_nhwc_to_nchw(s.raw, a3, NB, Ct, HW, 1.f, c.stream));
   }
   return MGB_OK;
 }
@@ -665,22 +655,18 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
   const size_t base = c.arena->mark();
   TRY(launch_nchw_to_nhwc(rgb_latent, s.rgb, B, 4, HW, 1.f, c.stream));
   TRY(launch_nchw_to_nhwc(target, s.tgt, B, Ct, HW, 1.f, c.stream));
-  count_launch(2);
   const bool any_noise = step_noise != nullptr;
   if (!any_noise) CUDA_TRY(cudaMemsetAsync(s.nz, 0, n * 4, c.stream));   // kz * 0 must stay finite
   static const bool graphs = getenv("MGB_NO_GRAPH") == nullptr;
   mgb_handle::StepGraph& G = h->step_graph;
   for (int i = first_step; i < first_step + num_steps; ++i) {
-    if (h->kz_host[i] != 0.f) {
-      TRY(launch_nchw_to_nhwc(step_noise + size_t(i) * n, s.nz, B, Ct, HW, 1.f, c.stream));
-      count_launch(1);
-    }
+    if (h->kz_host[i] != 0.f) TRY(launch_nchw_to_nhwc(step_noise + size_t(i) * n, s.nz, B, Ct, HW, 1.f, c.stream));
     if (graphs && G.exec && G.NB == B && G.lh == lh && G.lw == lw) {
       // arm the device step counter for this replay (pageable 4-byte H2D: staged by the driver, so the
       // source may be reused immediately)
       CUDA_TRY(cudaMemcpyAsync(h->step_counter, &i, 4, cudaMemcpyHostToDevice, c.stream));
       CUDA_TRY(cudaGraphLaunch(G.exec.get(), c.stream));
-      count_launch(int(G.launches));
+      count_launch(G.launches);
       continue;
     }
     c.arena->release(base);
@@ -704,7 +690,7 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
         ce = cudaStreamEndCapture(cc.stream, &graph);
       }
       const long long nl = launch_count() - l0;
-      count_launch(-int(nl));                                            // capture launched nothing
+      count_launch(-nl);                                                 // capture launched nothing
       cudaGraphExec_t exec = nullptr;
       if (rc == MGB_OK && ce == cudaSuccess && graph) ce = cudaGraphInstantiate(&exec, graph, 0);
       if (graph) cudaGraphDestroy(graph);
@@ -717,7 +703,6 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
     }
   }
   TRY(launch_nhwc_to_nchw(s.tgt, target, B, Ct, HW, 1.f, c.stream));
-  count_launch(1);
   if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
   return MGB_OK;
 }

@@ -5,6 +5,7 @@
 
 #include "device.h"
 #include "kernels.h"
+#include "launch.h"
 #include "ops.h"
 
 namespace mgb {
@@ -118,20 +119,16 @@ int mgb_op_flash_attn64(const void* qkv, void* out, int32_t NB, int32_t T, int32
     cudaDeviceSynchronize();
     if (int rc = ws.grow(need)) return rc;
   }
-  int rc = launch_flash_attn64(reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(out), NB, T, C, scale,
-                               need ? ws.get() : nullptr, need ? ws.bytes() : 0, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(need ? 2 : 1);
-  return rc;
+  return launch_flash_attn64(reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(out), NB, T, C, scale,
+                             need ? ws.get() : nullptr, need ? ws.bytes() : 0, reinterpret_cast<cudaStream_t>(stream));
 }
 
 size_t mgb_op_groupnorm_ws_bytes(int32_t NB, int32_t HW, int32_t C, int32_t G) { return groupnorm_ws_bytes(NB, HW, C, G); }
 
 int mgb_op_groupnorm(const float* x, void* y, const float* gamma, const float* beta, float* ws, int32_t NB, int32_t HW,
                      int32_t C, int32_t G, float eps, int32_t silu, void* stream) {
-  int rc = launch_groupnorm(x, reinterpret_cast<bf16*>(y), nullptr, gamma, beta, ws, NB, HW, C, G, eps, silu,
-                            reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(2);
-  return rc;
+  return launch_groupnorm(x, reinterpret_cast<bf16*>(y), nullptr, gamma, beta, ws, NB, HW, C, G, eps, silu,
+                          reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_op_groupnorm_ex(const float* xa, int32_t Ca, const float* xb, int32_t Cb, void* y, void* raw_copy,
@@ -145,44 +142,33 @@ int mgb_op_groupnorm_ex(const float* xa, int32_t Ca, const float* xb, int32_t Cb
     set_error("op_groupnorm_ex: counter memset failed");
     return MGB_ERR_CUDA;
   }
-  int rc = launch_gn_fused(xa, Ca, xb, Cb, reinterpret_cast<bf16*>(y), reinterpret_cast<bf16*>(raw_copy), gamma, beta, NB,
-                           HW, G, eps, silu, ws, counters, s);
-  if (!rc) count_launch(2);
-  return rc;
+  return launch_gn_fused(xa, Ca, xb, Cb, reinterpret_cast<bf16*>(y), reinterpret_cast<bf16*>(raw_copy), gamma, beta, NB, HW,
+                         G, eps, silu, ws, counters, s);
 }
 
 int mgb_op_layernorm(const float* x, void* y, const float* gamma, const float* beta, int32_t M, int32_t C, float eps,
                      void* stream) {
-  int rc = launch_layernorm(x, reinterpret_cast<bf16*>(y), gamma, beta, M, C, eps,
-                            reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_layernorm(x, reinterpret_cast<bf16*>(y), gamma, beta, M, C, eps, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_op_xattn2(const float* x, void* y, void* a_out, const float* ln2_g, const float* ln2_b, const float* ln3_g,
                   const float* ln3_b, const void* GU, const float* c1, int32_t M, int32_t C, int32_t H, float scale, float eps,
                   void* stream) {
   if (!x || !y || !a_out || !GU || !c1) { set_error("op_xattn2: null pointer"); return MGB_ERR_INVALID; }
-  int rc = launch_xattn2_fused(x, reinterpret_cast<bf16*>(y), reinterpret_cast<bf16*>(a_out), ln2_g, ln2_b, ln3_g, ln3_b,
-                               reinterpret_cast<const bf16*>(GU), c1, M, C, H, scale, eps,
-                               reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_xattn2_fused(x, reinterpret_cast<bf16*>(y), reinterpret_cast<bf16*>(a_out), ln2_g, ln2_b, ln3_g, ln3_b,
+                             reinterpret_cast<const bf16*>(GU), c1, M, C, H, scale, eps,
+                             reinterpret_cast<cudaStream_t>(stream));
 }
 
 /* ---- pre / post-processing and evaluation (image.cu, eval.cu) ---- */
 int mgb_resize(const void* src, int32_t src_is_u8, int32_t NC, int32_t H, int32_t W, float* dst, int32_t h, int32_t w,
                int32_t mode, int32_t post, float* tmp, void* stream) {
   if (!src || !dst || !tmp) { set_error("mgb_resize: null pointer"); return MGB_ERR_INVALID; }
-  int rc = launch_resize(src, src_is_u8, NC, H, W, dst, h, w, mode, post, tmp, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(2);
-  return rc;
+  return launch_resize(src, src_is_u8, NC, H, W, dst, h, w, mode, post, tmp, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_colorize(const float* depth, int64_t HW, float dmin, float dmax, const uint8_t* lut, uint8_t* out_hwc, void* stream) {
-  int rc = launch_colorize(depth, HW, dmin, dmax, lut, out_hwc, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_colorize(depth, HW, dmin, dmax, lut, out_hwc, reinterpret_cast<cudaStream_t>(stream));
 }
 
 size_t mgb_eval_ws_bytes(void) { return eval_ws_bytes() + 16 * sizeof(double); }
@@ -192,9 +178,7 @@ static int eval_depth_run(const char* what, const float* pred, const float* gt, 
                           float dmax, float* aligned_out, void* ws, double* out_host, void* stream) {
   double* out_dev = reinterpret_cast<double*>(static_cast<char*>(ws) + eval_ws_bytes());
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  int rc = launch_eval_depth(pred, gt, mask, H, W, alignment, rows, cols, fit_h, fit_w, dmin, dmax, aligned_out, ws, out_dev, s);
-  if (rc) return rc;
-  count_launch(4);
+  TRY(launch_eval_depth(pred, gt, mask, H, W, alignment, rows, cols, fit_h, fit_w, dmin, dmax, aligned_out, ws, out_dev, s));
   cudaError_t e = cudaMemcpyAsync(out_host, out_dev, 13 * sizeof(double), cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) { set_error("%s: %s", what, cudaGetErrorString(e)); return MGB_ERR_CUDA; }
@@ -227,9 +211,7 @@ int mgb_eval_normals(const float* pred, const float* gt, const uint8_t* mask, in
                      double* out_host, void* stream) {
   if (!pred || !gt || !ws || !out_host || H <= 0 || W <= 0) { set_error("mgb_eval_normals: bad argument"); return MGB_ERR_INVALID; }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  int rc = launch_eval_normals(pred, gt, mask, int64_t(H) * W, error_out, ws, s);
-  if (rc) return rc;
-  count_launch(4);
+  TRY(launch_eval_normals(pred, gt, mask, int64_t(H) * W, error_out, ws, s));
   cudaError_t e = cudaMemcpyAsync(out_host, eval_normals_out(ws), 9 * sizeof(double), cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) { set_error("mgb_eval_normals: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
@@ -237,16 +219,12 @@ int mgb_eval_normals(const float* pred, const float* gt, const uint8_t* mask, in
 }
 
 int mgb_op_space_to_depth(const float* x, void* y, int32_t NB, int32_t H, int32_t W, int32_t C, void* stream) {
-  int rc = launch_space_to_depth(x, reinterpret_cast<bf16*>(y), NB, H, W, C, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_space_to_depth(x, reinterpret_cast<bf16*>(y), NB, H, W, C, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_op_upsample2x_ex(const float* x, void* y, int32_t NB, int32_t H, int32_t W, int32_t C, int32_t Ho, int32_t Wo,
                          void* stream) {
-  int rc = launch_upsample2x(x, reinterpret_cast<bf16*>(y), NB, H, W, C, Ho, Wo, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_upsample2x(x, reinterpret_cast<bf16*>(y), NB, H, W, C, Ho, Wo, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_op_upsample2x(const float* x, void* y, int32_t NB, int32_t H, int32_t W, int32_t C, void* stream) {
@@ -255,17 +233,13 @@ int mgb_op_upsample2x(const float* x, void* y, int32_t NB, int32_t H, int32_t W,
 
 int mgb_op_softmax_rows(const float* s, void* p, int32_t M, int32_t n, int32_t ld, void* stream) {
   if (!s || !p || M <= 0 || n <= 0 || ld < n) { set_error("op_softmax_rows: bad argument (M=%d n=%d ld=%d)", M, n, ld); return MGB_ERR_INVALID; }
-  int rc = launch_softmax_rows(s, reinterpret_cast<bf16*>(p), M, n, ld, reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_softmax_rows(s, reinterpret_cast<bf16*>(p), M, n, ld, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_op_transpose_bf16(const void* x, void* y, int32_t M, int32_t N, int32_t ld, void* stream) {
   if (!x || !y || M <= 0 || N <= 0 || ld < M) { set_error("op_transpose_bf16: bad argument (M=%d N=%d ld=%d)", M, N, ld); return MGB_ERR_INVALID; }
-  int rc = launch_transpose_bf16(reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(y), M, N, ld,
-                                 reinterpret_cast<cudaStream_t>(stream));
-  if (!rc) count_launch(1);
-  return rc;
+  return launch_transpose_bf16(reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(y), M, N, ld,
+                               reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -295,25 +295,13 @@ int launch_flash_attn64(const bf16* qkv, bf16* out, int NB, int T, int C, float 
     }
   }
   const size_t smem = 1024 + kQBytes + 2 * kKvStages * kKvBytes + 256;
-  void (*kern)(AttnParams) = flash_attn64_kernel;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) { set_error("flash_attn64 attr: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-    attr_set = true;
-  }
+  TRY(raise_smem_limit_once<flash_attn64_kernel>("flash_attn64", int(smem)));
   dim3 grid((T + 127) / 128, C / 64, NB * p.splits);
-  cudaError_t e = launch_k(kern, grid, kAttnThreads, smem, stream, p);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("flash_attn64 launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  if (p.splits > 1) {
-    const size_t threads = size_t(NB) * (C / 64) * T * 8;
-    e = launch_k(attn_combine_kernel, dim3(unsigned((threads + 255) / 256)), 256, 0, stream, (const float*)p.part_o,
-                 (const float*)p.part_ml, out, p.splits, NB, C / 64, T, C);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("attn_combine launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  }
-  return MGB_OK;
+  TRY(launch_pdl("flash_attn64", flash_attn64_kernel, grid, kAttnThreads, smem, stream, p));
+  if (p.splits == 1) return MGB_OK;
+  const size_t threads = size_t(NB) * (C / 64) * T * 8;
+  return launch_pdl("attn_combine", attn_combine_kernel, dim3(unsigned((threads + 255) / 256)), 256, 0, stream,
+                    (const float*)p.part_o, (const float*)p.part_ml, out, p.splits, NB, C / 64, T, C);
 }
 
 }  // namespace mgb

@@ -17,6 +17,13 @@
     }                                                                                         \
   } while (0)
 
+// Returns the status of `expr` when it is not MGB_OK.
+#define TRY(expr)                  \
+  do {                             \
+    int _rc = (expr);              \
+    if (_rc != MGB_OK) return _rc; \
+  } while (0)
+
 namespace mgb {
 
 // Bytes that every DevBuf and PinnedBuf together hold now (mgb_debug_live_device_bytes).

@@ -7,21 +7,6 @@
 
 namespace mgb {
 
-static inline int grid_for(size_t n, int threads) {
-  size_t b = (n + threads - 1) / threads;
-  const size_t cap = size_t(kNumSMs) * 16;
-  return int(b < cap ? (b ? b : 1) : cap);
-}
-#define MGB_LAUNCH_CHECK(name)                                       \
-  do {                                                               \
-    cudaError_t _e = cudaGetLastError();                             \
-    if (_e != cudaSuccess) {                                         \
-      set_error(name " launch: %s", cudaGetErrorString(_e));         \
-      return MGB_ERR_CUDA;                                           \
-    }                                                                \
-    return MGB_OK;                                                   \
-  } while (0)
-
 // x fp32 [NB, H, W, C] -> y bf16 [NB, 4, ceil(H/2), ceil(W/2), C], plane = (h & 1) * 2 + (w & 1); plane elements whose
 // source pixel lies outside the image (odd H or W) are zero = the convolution's zero padding there.
 __global__ void s2d_kernel(const float4* __restrict__ x, uint2* __restrict__ y, int NB, int H, int W, int Q) {
@@ -45,9 +30,8 @@ __global__ void s2d_kernel(const float4* __restrict__ x, uint2* __restrict__ y, 
 int launch_space_to_depth(const float* x, bf16* y, int NB, int H, int W, int C, cudaStream_t stream) {
   if (C % 4 || H < 1 || W < 1) { set_error("space_to_depth: C %% 4 == 0 required"); return MGB_ERR_INVALID; }
   const size_t n = (size_t)NB * 4 * ((H + 1) / 2) * ((W + 1) / 2) * (C / 4);
-  launch_k(s2d_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const float4*>(x), reinterpret_cast<uint2*>(y),
-           NB, H, W, C / 4);
-  MGB_LAUNCH_CHECK("space_to_depth");
+  return launch_pdl("space_to_depth", s2d_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const float4*>(x),
+                    reinterpret_cast<uint2*>(y), NB, H, W, C / 4);
 }
 
 // nearest upsampling to Ho x Wo with Ho in {2H - 1, 2H} (same for W): x fp32 [NB, H, W, C] -> y bf16 [NB, Ho, Wo, C].
@@ -75,9 +59,8 @@ int launch_upsample2x(const float* x, bf16* y, int NB, int H, int W, int C, int 
     return MGB_ERR_INVALID;
   }
   const size_t n = (size_t)NB * Ho * Wo * (C / 4);
-  launch_k(upsample2x_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const float4*>(x),
-           reinterpret_cast<uint2*>(y), NB, H, W, Ho, Wo, C / 4);
-  MGB_LAUNCH_CHECK("upsample2x");
+  return launch_pdl("upsample2x", upsample2x_kernel, grid_for(n, 256), 256, 0, stream, reinterpret_cast<const float4*>(x),
+                    reinterpret_cast<uint2*>(y), NB, H, W, Ho, Wo, C / 4);
 }
 
 // UNet conv_in operand (reference marigold_depth_pipeline.py:456-458, marigold_iid_pipeline.py:538-540: rgb latent FIRST):
@@ -102,9 +85,9 @@ __global__ void pack_latents_kernel(const float4* __restrict__ rgb, const float4
 }
 int launch_pack_latents(const float* rgb, const float* tgt, bf16* out, int M, int Ct, cudaStream_t stream) {
   if (Ct < 4 || (Ct & 3) || 4 + Ct > 64) { set_error("pack_latents: target channels %d", Ct); return MGB_ERR_INVALID; }
-  launch_k(pack_latents_kernel, grid_for(size_t(M) * 16, 256), 256, 0, stream, reinterpret_cast<const float4*>(rgb),
-           reinterpret_cast<const float4*>(tgt), reinterpret_cast<uint2*>(out), M, Ct / 4);
-  MGB_LAUNCH_CHECK("pack_latents");
+  return launch_pdl("pack_latents", pack_latents_kernel, grid_for(size_t(M) * 16, 256), 256, 0, stream,
+                    reinterpret_cast<const float4*>(rgb), reinterpret_cast<const float4*>(tgt),
+                    reinterpret_cast<uint2*>(out), M, Ct / 4);
 }
 
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, float* __restrict__ y, int NB, int C, int HW,
@@ -118,8 +101,8 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, float* __restri
   }
 }
 int launch_nchw_to_nhwc(const float* x, float* y, int NB, int C, int HW, float scale, cudaStream_t stream) {
-  nchw_to_nhwc_kernel<<<grid_for((size_t)NB * C * HW, 256), 256, 0, stream>>>(x, y, NB, C, HW, scale);
-  MGB_LAUNCH_CHECK("nchw_to_nhwc");
+  return launch_plain("nchw_to_nhwc", nchw_to_nhwc_kernel, grid_for((size_t)NB * C * HW, 256), 256, 0, stream, x, y, NB,
+                      C, HW, scale);
 }
 __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, float* __restrict__ y, int NB, int C, int HW,
                                     float scale) {
@@ -133,8 +116,8 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, float* __restri
   }
 }
 int launch_nhwc_to_nchw(const float* x, float* y, int NB, int C, int HW, float scale, cudaStream_t stream) {
-  nhwc_to_nchw_kernel<<<grid_for((size_t)NB * C * HW, 256), 256, 0, stream>>>(x, y, NB, C, HW, scale);
-  MGB_LAUNCH_CHECK("nhwc_to_nchw");
+  return launch_plain("nhwc_to_nchw", nhwc_to_nchw_kernel, grid_for((size_t)NB * C * HW, 256), 256, 0, stream, x, y, NB,
+                      C, HW, scale);
 }
 
 // rgb fp32 NCHW [NB, 3, HW] -> bf16 NHWC-64 (3 real channels + zeros): the VAE encoder conv_in operand
@@ -155,9 +138,8 @@ __global__ void pack_rgb_kernel(const float* __restrict__ rgb, uint4* __restrict
   }
 }
 int launch_pack_rgb(const float* rgb_nchw, bf16* out, int NB, int HW, cudaStream_t stream) {
-  pack_rgb_kernel<<<grid_for((size_t)NB * HW * 8, 256), 256, 0, stream>>>(rgb_nchw, reinterpret_cast<uint4*>(out), NB,
-                                                                         size_t(HW));
-  MGB_LAUNCH_CHECK("pack_rgb");
+  return launch_plain("pack_rgb", pack_rgb_kernel, grid_for((size_t)NB * HW * 8, 256), 256, 0, stream, rgb_nchw,
+                      reinterpret_cast<uint4*>(out), NB, size_t(HW));
 }
 
 // One-time weight folding: P[M, N] = A[M, K] B[K, N] in fp32 (32 x 32 tiles through shared memory), written as bf16 into
@@ -180,8 +162,7 @@ __global__ void __launch_bounds__(1024) fold_matmul_kernel(const float* __restri
 }
 int launch_fold_matmul(const float* A, const float* B, bf16* out, int M, int N, int K, int ldo, int col0, cudaStream_t stream) {
   dim3 grid((N + 31) / 32, (M + 31) / 32);
-  fold_matmul_kernel<<<grid, 1024, 0, stream>>>(A, B, out, M, N, K, ldo, col0);
-  MGB_LAUNCH_CHECK("fold_matmul");
+  return launch_plain("fold_matmul", fold_matmul_kernel, grid, 1024, 0, stream, A, B, out, M, N, K, ldo, col0);
 }
 
 // y[M, N] = act_out(act_in(x)[M, K] W[N, K]^T + b); fp32 everywhere; one warp per output element.
@@ -209,8 +190,8 @@ __global__ void __launch_bounds__(256) linear_small_kernel(const float* __restri
 int launch_linear_small(const float* x, const float* w, const float* b, float* y, int M, int N, int K, int silu_in,
                         int silu_out, cudaStream_t stream) {
   const long long warps = (long long)M * N;
-  linear_small_kernel<<<int((warps + 7) / 8), 256, 0, stream>>>(x, w, b, y, M, N, K, silu_in, silu_out);
-  MGB_LAUNCH_CHECK("linear_small");
+  return launch_plain("linear_small", linear_small_kernel, int((warps + 7) / 8), 256, 0, stream, x, w, b, y, M, N, K,
+                      silu_in, silu_out);
 }
 
 // diffusers get_timestep_embedding(flip_sin_to_cos=True, downscale_freq_shift=0): emb = [cos(t f) | sin(t f)],
@@ -227,8 +208,8 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, float* __
   }
 }
 int launch_timestep_embedding(const float* t, float* emb, int M, int dim, cudaStream_t stream) {
-  timestep_embedding_kernel<<<grid_for(size_t(M) * dim / 2, 128), 128, 0, stream>>>(t, emb, M, dim);
-  MGB_LAUNCH_CHECK("timestep_embedding");
+  return launch_plain("timestep_embedding", timestep_embedding_kernel, grid_for(size_t(M) * dim / 2, 128), 128, 0, stream,
+                      t, emb, M, dim);
 }
 
 // Row softmax of fp32 scores s[M, ld] (first n columns valid) -> bf16 probabilities p[M, ld], columns [n, ld) zeroed
@@ -260,8 +241,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
     out[i] = i < n ? __float2bfloat16(__expf(row[i] - mx) * inv) : __float2bfloat16(0.f);
 }
 int launch_softmax_rows(const float* s, bf16* p, int M, int n, int ld, cudaStream_t stream) {
-  softmax_rows_kernel<<<M, 256, 0, stream>>>(s, p, n, ld);
-  MGB_LAUNCH_CHECK("softmax_rows");
+  return launch_plain("softmax_rows", softmax_rows_kernel, M, 256, 0, stream, s, p, n, ld);
 }
 
 // x bf16 [M, N] -> y bf16 [N, ld] (ld >= M; columns [M, ld) zeroed) through a padded smem tile
@@ -280,8 +260,7 @@ __global__ void transpose_bf16_kernel(const bf16* __restrict__ x, bf16* __restri
 }
 int launch_transpose_bf16(const bf16* x, bf16* y, int M, int N, int ld, cudaStream_t stream) {
   dim3 grid((N + 31) / 32, (ld + 31) / 32), block(32, 8);
-  transpose_bf16_kernel<<<grid, block, 0, stream>>>(x, y, M, N, ld);
-  MGB_LAUNCH_CHECK("transpose_bf16");
+  return launch_plain("transpose_bf16", transpose_bf16_kernel, grid, block, 0, stream, x, y, M, N, ld);
 }
 
 // Decoder input: z = post_quant_conv(latent / scale) (1x1, 4 -> 4, fp32) packed as bf16 NHWC-64.
@@ -314,9 +293,8 @@ __global__ void pack_decoder_latent_kernel(const float* __restrict__ lat, const 
 }
 int launch_pack_decoder_latent(const float* latent_nchw, const float* w, const float* b, float inv_scale, bf16* out,
                                int NB, int HW, cudaStream_t stream) {
-  pack_decoder_latent_kernel<<<grid_for((size_t)NB * HW * 8, 256), 256, 0, stream>>>(
-      latent_nchw, w, b, inv_scale, reinterpret_cast<uint4*>(out), NB, size_t(HW));
-  MGB_LAUNCH_CHECK("pack_decoder_latent");
+  return launch_plain("pack_decoder_latent", pack_decoder_latent_kernel, grid_for((size_t)NB * HW * 8, 256), 256, 0,
+                      stream, latent_nchw, w, b, inv_scale, reinterpret_cast<uint4*>(out), NB, size_t(HW));
 }
 
 __global__ void select_step_kernel(const float* __restrict__ table, int total, const float* __restrict__ sched_k,
@@ -331,9 +309,8 @@ __global__ void select_step_kernel(const float* __restrict__ table, int total, c
 }
 int launch_select_step(const float* bias_table, int bias_total, const float* sched_k, float* cur_bias, float* cur_k,
                        const int* counter, int step, cudaStream_t stream) {
-  launch_k(select_step_kernel, grid_for(size_t(bias_total), 256), 256, 0, stream, bias_table, bias_total, sched_k,
-           cur_bias, cur_k, counter, step);
-  MGB_LAUNCH_CHECK("select_step");
+  return launch_pdl("select_step", select_step_kernel, grid_for(size_t(bias_total), 256), 256, 0, stream, bias_table,
+                    bias_total, sched_k, cur_bias, cur_k, counter, step);
 }
 __global__ void advance_counter_kernel(int* counter) {
   pdl_launch_dependents();
@@ -341,8 +318,7 @@ __global__ void advance_counter_kernel(int* counter) {
   *counter += 1;
 }
 int launch_advance_counter(int* counter, cudaStream_t stream) {
-  launch_k(advance_counter_kernel, 1, 1, 0, stream, counter);
-  MGB_LAUNCH_CHECK("advance_counter");
+  return launch_pdl("advance_counter", advance_counter_kernel, 1, 1, 0, stream, counter);
 }
 
 }  // namespace mgb

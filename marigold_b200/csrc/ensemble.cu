@@ -19,6 +19,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "launch.h"
 
 namespace mgb {
 
@@ -410,20 +411,20 @@ int ens_max_batch() { return kEnsMaxP; }
 int ens_max_members() { return kEnsDynMaxE; }
 
 // f(std::integral_constant<int, E>()) for the register-resident sizes E <= kEnsMaxE, f(std::integral_constant<int, 0>())
-// for the larger ones
+// for the larger ones; returns what f returns
 template <typename F>
-static void dispatch_members(int E, F&& f) {
+static int dispatch_members(int E, F&& f) {
   switch (E) {
-#define CASE(n) case n: f(std::integral_constant<int, n>()); return;
+#define CASE(n) case n: return f(std::integral_constant<int, n>());
     CASE(2) CASE(3) CASE(4) CASE(5) CASE(6) CASE(7) CASE(8) CASE(9) CASE(10) CASE(11) CASE(12) CASE(13) CASE(14)
     CASE(15) CASE(16)
 #undef CASE
   }
-  f(std::integral_constant<int, 0>());
+  return f(std::integral_constant<int, 0>());
 }
 
 int launch_ens_depth_cost(const float* depth, float* st_host, int n, int E, long long HW, int shift, int median,
-                          double reg, void* ws, float* v3, double* out_host_pinned, int* launches, cudaStream_t stream) {
+                          double reg, void* ws, float* v3, double* out_host_pinned, cudaStream_t stream) {
   if (E < 2 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [2, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
   const int P = 1 + n;
   int rows = n > 0 ? 2 : 1;
@@ -443,20 +444,19 @@ int launch_ens_depth_cost(const float* depth, float* st_host, int n, int E, long
   double* out = ens_ws_out(ws);
   cudaError_t e = cudaMemcpyAsync(st, st_host, sizeof(float) * 2 * E * rows, cudaMemcpyHostToDevice, stream);
   if (e != cudaSuccess) { set_error("ens cost H2D: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  *launches = 0;
-  dispatch_members(E, [&](auto members) {
+  TRY(dispatch_members(E, [&](auto members) -> int {
     constexpr int kE = decltype(members)::value;
     if constexpr (kE > 0) {
       CostPartial* base_part = reinterpret_cast<CostPartial*>(ws);
       PertPartial* pert_part = reinterpret_cast<PertPartial*>(base_part + kEnsCostBlocks);
       const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kEnsCostBlocks));
-      ens_cost_base_kernel<kE><<<blocks, kEnsThreads, 0, stream>>>(depth, st, HW, shift, median, base_part,
-                                                                   n > 0 ? v3 : nullptr);
+      TRY(launch_plain("ens cost", ens_cost_base_kernel<kE>, blocks, kEnsThreads, 0, stream, depth, st, HW, shift, median,
+                       base_part, n > 0 ? v3 : nullptr));
       if (n > 0)
-        ens_cost_pert_kernel<kE><<<dim3(blocks, E), kEnsThreads, 0, stream>>>(depth, st, st + 2 * E, HW, shift, median, v3,
-                                                                              pert_part);
-      ens_cost_final_kernel<<<P, 256, 0, stream>>>(base_part, pert_part, blocks, E, HW, reg, out);
-      *launches = n > 0 ? 3 : 2;
+        TRY(launch_plain("ens cost", ens_cost_pert_kernel<kE>, dim3(blocks, E), kEnsThreads, 0, stream, depth, st,
+                         st + 2 * E, HW, shift, median, v3, pert_part));
+      return launch_plain("ens cost", ens_cost_final_kernel, P, 256, 0, stream, base_part, pert_part, blocks, E, HW, reg,
+                          out);
     } else {
       const int NP = E * (E - 1) / 2, chunks = (NP + kDynPairs - 1) / kDynPairs;
       const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kDynBlocks));
@@ -465,16 +465,16 @@ int launch_ens_depth_cost(const float* depth, float* st_host, int n, int E, long
       const int p_max = std::max<int>(1, int(kDynPartialBytes / (size_t(NP) * blocks * sizeof(double))));
       for (int p0 = 0; p0 < P; p0 += p_max) {
         const int pn = std::min(p_max, P - p0);
-        ens_cost_dyn_kernel<<<dim3(blocks, pn, chunks), kEnsThreads, 0, stream>>>(depth, st + size_t(p0) * 2 * E, E, HW,
-                                                                                 shift, median, pair_part, mm_part);
-        ens_cost_dyn_final_kernel<<<pn, 128, 0, stream>>>(pair_part, mm_part, blocks, E, HW, reg, out + 3 * p0);
-        *launches += 2;
+        TRY(launch_plain("ens cost", ens_cost_dyn_kernel, dim3(blocks, pn, chunks), kEnsThreads, 0, stream, depth,
+                         st + size_t(p0) * 2 * E, E, HW, shift, median, pair_part, mm_part));
+        TRY(launch_plain("ens cost", ens_cost_dyn_final_kernel, pn, 128, 0, stream, pair_part, mm_part, blocks, E, HW, reg,
+                         out + 3 * p0));
       }
+      return MGB_OK;
     }
-  });
+  }));
   e = cudaMemcpyAsync(out_host_pinned, out, size_t(P) * 3 * sizeof(double), cudaMemcpyDeviceToHost, stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-  if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { set_error("ens cost: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   return MGB_OK;
 }
@@ -500,10 +500,9 @@ int launch_ens_minmax(const float* depth, int E, long long HW, float* ws, float*
                       cudaStream_t stream) {
   const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, 64));
   dim3 grid(blocks, E);
-  ens_minmax_kernel<<<grid, kEnsThreads, 0, stream>>>(depth, HW, ws);
+  TRY(launch_plain("ens minmax", ens_minmax_kernel, grid, kEnsThreads, 0, stream, depth, HW, ws));
   cudaError_t e = cudaMemcpyAsync(host_pinned, ws, sizeof(float) * 2 * blocks * E, cudaMemcpyDeviceToHost, stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-  if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { set_error("ens minmax: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   *blocks_out = blocks;
   return MGB_OK;
@@ -605,14 +604,11 @@ int launch_ens_depth_reduce(const float* depth, const float* st_host, int E, lon
   cudaError_t e = cudaMemcpyAsync(st, st_host, sizeof(float) * 2 * E, cudaMemcpyHostToDevice, stream);
   if (e != cudaSuccess) { set_error("ens reduce H2D: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kEnsMaxBlocks));
-  dispatch_members(E, [&](auto members) {
-    ens_reduce_kernel<decltype(members)::value><<<blocks, kEnsThreads, 0, stream>>>(depth, st, E, HW, shift, median, pred,
-                                                                                    unc, idx, bmm);
-  });
-  ens_renorm_kernel<<<blocks, kEnsThreads, 0, stream>>>(pred, unc, HW, bmm, blocks, use_min);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("ens reduce: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  TRY(dispatch_members(E, [&](auto members) -> int {
+    return launch_plain("ens reduce", ens_reduce_kernel<decltype(members)::value>, blocks, kEnsThreads, 0, stream, depth, st,
+                        E, HW, shift, median, pred, unc, idx, bmm);
+  }));
+  return launch_plain("ens renorm", ens_renorm_kernel, blocks, kEnsThreads, 0, stream, pred, unc, HW, bmm, blocks, use_min);
 }
 
 // ---- ensemble_iid (ensemble.py:252-270): per element, plain median (+ MAD) or mean (+ unbiased std) over E ------------
@@ -647,10 +643,7 @@ __global__ void __launch_bounds__(kEnsThreads)
 int launch_ens_iid(const float* x, int E, long long N, int median, float* pred, float* unc, cudaStream_t stream) {
   if (E < 1 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [1, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
   const int blocks = int(std::min<long long>((N + kEnsThreads - 1) / kEnsThreads, kEnsMaxBlocks * 4));
-  ens_iid_kernel<<<blocks, kEnsThreads, 0, stream>>>(x, E, N, median, pred, unc);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("ens iid: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  return launch_plain("ens iid", ens_iid_kernel, blocks, kEnsThreads, 0, stream, x, E, N, median, pred, unc);
 }
 
 // ---- ensemble_normals -------------------------------------------------------------------------------
@@ -693,10 +686,7 @@ int launch_ens_normals(const float* nrm, int E, long long HW, int closest, float
                        cudaStream_t stream) {
   if (E < 1) { set_error("ensemble size %d", E); return MGB_ERR_INVALID; }
   const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kEnsMaxBlocks));
-  ens_normals_kernel<<<blocks, kEnsThreads, 0, stream>>>(nrm, E, HW, closest, out, unc, idx);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("ens normals: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  return launch_plain("ens normals", ens_normals_kernel, blocks, kEnsThreads, 0, stream, nrm, E, HW, closest, out, unc, idx);
 }
 
 }  // namespace mgb

@@ -14,6 +14,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "launch.h"
 
 namespace mgb {
 
@@ -154,13 +155,12 @@ int launch_eval_depth(const float* pred, const float* gt, const uint8_t* mask, l
   const long long HW = H * W, n_fit = rows ? (long long)fit_h * fit_w : HW;
   const int blocks = int(std::min<long long>((HW + kEvThreads - 1) / kEvThreads, kEvBlocks));
   const int fit_blocks = int(std::min<long long>((n_fit + kEvThreads - 1) / kEvThreads, kEvBlocks));
-  eval_align_sums_kernel<<<fit_blocks, kEvThreads, 0, stream>>>(pred, gt, mask, n_fit, W, rows, cols, fit_w, align == 2, part);
-  eval_align_solve_kernel<<<1, 32, 0, stream>>>(part, fit_blocks, align != 0, st);
-  eval_metric_sums_kernel<<<blocks, kEvThreads, 0, stream>>>(pred, gt, mask, HW, st, align == 2, dmin, dmax, aligned_out, part);
-  eval_metric_final_kernel<<<1, 32, 0, stream>>>(part, blocks, st, out_dev);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("eval_depth launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  TRY(launch_plain("eval_align_sums", eval_align_sums_kernel, fit_blocks, kEvThreads, 0, stream, pred, gt, mask, n_fit, W,
+                   rows, cols, fit_w, align == 2, part));
+  TRY(launch_plain("eval_align_solve", eval_align_solve_kernel, 1, 32, 0, stream, part, fit_blocks, align != 0, st));
+  TRY(launch_plain("eval_metric_sums", eval_metric_sums_kernel, blocks, kEvThreads, 0, stream, pred, gt, mask, HW, st,
+                   align == 2, dmin, dmax, aligned_out, part));
+  return launch_plain("eval_metric_final", eval_metric_final_kernel, 1, 32, 0, stream, part, blocks, st, out_dev);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -367,22 +367,17 @@ int launch_eval_normals(const float* pred, const float* gt, const uint8_t* mask,
   unsigned* hist_lo = hist_hi + (kNrHiBins + 3) / 4 * 4;
   unsigned* err_bits = reinterpret_cast<unsigned*>(w + kNrErrOff);
   constexpr size_t smem = kNrHiBins * sizeof(unsigned);
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(eval_normals_error_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) { set_error("eval_normals: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-    attr_set = true;
-  }
+  TRY(raise_smem_limit_once<eval_normals_error_kernel>("eval_normals", int(smem)));
   const int blocks = int(std::min<long long>((HW + kEvThreads - 1) / kEvThreads, kEvBlocks));
   cudaError_t e = cudaMemsetAsync(hist_hi, 0, kNrHistBytes, stream);
   if (e != cudaSuccess) { set_error("eval_normals memset: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  eval_normals_error_kernel<<<blocks, kEvThreads, smem, stream>>>(pred, gt, mask, HW, err_bits, err_out, hist_hi, part);
-  eval_normals_locate_kernel<<<1, kNrSelThreads, 0, stream>>>(hist_hi, sel);
-  eval_normals_refine_kernel<<<blocks, kEvThreads, 0, stream>>>(err_bits, HW, sel, hist_lo);
-  eval_normals_final_kernel<<<1, kNrSelThreads, 0, stream>>>(part, blocks, sel, hist_lo, eval_normals_out(ws));
-  e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("eval_normals launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  TRY(launch_plain("eval_normals_error", eval_normals_error_kernel, blocks, kEvThreads, smem, stream, pred, gt, mask, HW,
+                   err_bits, err_out, hist_hi, part));
+  TRY(launch_plain("eval_normals_locate", eval_normals_locate_kernel, 1, kNrSelThreads, 0, stream, hist_hi, sel));
+  TRY(launch_plain("eval_normals_refine", eval_normals_refine_kernel, blocks, kEvThreads, 0, stream, err_bits, HW, sel,
+                   hist_lo));
+  return launch_plain("eval_normals_final", eval_normals_final_kernel, 1, kNrSelThreads, 0, stream, part, blocks, sel,
+                      hist_lo, eval_normals_out(ws));
 }
 
 }  // namespace mgb

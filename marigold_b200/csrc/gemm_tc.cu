@@ -545,12 +545,8 @@ static int launch_one(const GemmParams& p_in, int splits, cudaStream_t stream) {
   GemmParams p = p_in;
   p.dbg = g_gemm_dbg;
   const size_t smem = gemm_smem_bytes(BN, p.stages);
-  static bool attr_set = false;  // per template instantiation
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return int(e);
-    attr_set = true;
-  }
+  constexpr auto kernel = gemm_tc_kernel<BN, MINB>;
+  TRY(raise_smem_limit_once<kernel>("gemm_tc", 227 * 1024));
   int m_tiles;
   if (p.mode == 0) {
     m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
@@ -558,9 +554,7 @@ static int launch_one(const GemmParams& p_in, int splits, cudaStream_t stream) {
     m_tiles = (p.M / (p.H * p.W)) * p.tiles_x * p.tiles_y;
   }
   dim3 grid(m_tiles, (p.N + BN - 1) / BN, splits);
-  cudaError_t le = launch_k(gemm_tc_kernel<BN, MINB>, grid, kGemmThreads, smem, stream, p);
-  if (le != cudaSuccess) return int(le);
-  return int(cudaGetLastError());
+  return launch_pdl("gemm_tc", kernel, grid, kGemmThreads, smem, stream, p);
 }
 
 int launch_gemm_tc(const GemmParams& p, int block_n, int splits, int ctas_per_sm, cudaStream_t stream) {
@@ -578,7 +572,7 @@ int launch_gemm_tc(const GemmParams& p, int block_n, int splits, int ctas_per_sm
     case 128: return launch_one<128, 1>(p, splits, stream);
     case 160: return launch_one<160, 1>(p, splits, stream);
     case 256: return launch_one<256, 1>(p, splits, stream);
-    default: return int(cudaErrorInvalidValue);
+    default: set_error("gemm_tc: no kernel for block_n %d", block_n); return MGB_ERR_CUDA;
   }
 }
 
@@ -587,7 +581,7 @@ int launch_splitk_epilogue(const GemmParams& p_in, int block_n, int splits, cuda
   GemmParams p = p_in;
   if ((p.epi.flags & EPI_GEGLU) || (p.N & 3) || (p.epi.ldo & 3) || p.N / 4 > kSkThreads * kSkQuads) {
     set_error("split-K epilogue: unsupported shape/flags (N=%d ldo=%d flags=%d)", p.N, p.epi.ldo, p.epi.flags);
-    return int(cudaErrorInvalidValue);
+    return MGB_ERR_CUDA;
   }
   // blocks never straddle images (rows_per_img = hw when known, else the whole M)
   const int rows_per_img = (p.epi.hw > 0 && p.M % p.epi.hw == 0) ? p.epi.hw : p.M;
@@ -595,10 +589,8 @@ int launch_splitk_epilogue(const GemmParams& p_in, int block_n, int splits, cuda
   int blocks_per_img = std::max(1, std::min(rows_per_img, (kNumSMs * 2) / imgs));
   const int rows_per_block = (rows_per_img + blocks_per_img - 1) / blocks_per_img;
   blocks_per_img = (rows_per_img + rows_per_block - 1) / rows_per_block;
-  cudaError_t e = launch_k(splitk_epilogue_kernel, imgs * blocks_per_img, kSkThreads, 0, stream, p, splits,
-                           rows_per_block, blocks_per_img, rows_per_img);
-  if (e != cudaSuccess) return int(e);
-  return int(cudaGetLastError());
+  return launch_pdl("splitk epilogue", splitk_epilogue_kernel, imgs * blocks_per_img, kSkThreads, 0, stream, p, splits,
+                    rows_per_block, blocks_per_img, rows_per_img);
 }
 
 // ---- tensor maps ----

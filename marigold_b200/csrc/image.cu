@@ -68,8 +68,6 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-static inline int grid_of(long long n) { return int(std::min<long long>((n + 255) / 256, kNumSMs * 16)); }
-
 // src [NC, H, W] (u8 or f32) -> dst f32 [NC, h, w]; tmp: NC * H * w floats. mode: 0 bilinear-aa, 1 bicubic-aa, 2 nearest-exact.
 // post: 0 none, 1 round + clamp to [0, 255], 2 round + clamp, then x / 255 * 2 - 1.
 int launch_resize(const void* src, int src_is_u8, int NC, int H, int W, float* dst, int h, int w, int mode, int post, float* tmp,
@@ -81,18 +79,15 @@ int launch_resize(const void* src, int src_is_u8, int NC, int H, int W, float* d
   // horizontal pass (W -> w), intermediate in float like torch's separable implementation (no rounding in between)
   const long long n1 = (long long)NC * H * w;
   if (src_is_u8)
-    launch_k(resize_pass_kernel<uint8_t>, grid_of(n1), 256, 0, stream, static_cast<const uint8_t*>(src), tmp, NC, W, w, H,
-             (long long)H * W, 1LL, (long long)W, 1, mode, 0);
+    TRY(launch_pdl("resize", resize_pass_kernel<uint8_t>, grid_for(n1, 256), 256, 0, stream,
+                   static_cast<const uint8_t*>(src), tmp, NC, W, w, H, (long long)H * W, 1LL, (long long)W, 1, mode, 0));
   else
-    launch_k(resize_pass_kernel<float>, grid_of(n1), 256, 0, stream, static_cast<const float*>(src), tmp, NC, W, w, H,
-             (long long)H * W, 1LL, (long long)W, 1, mode, 0);
+    TRY(launch_pdl("resize", resize_pass_kernel<float>, grid_for(n1, 256), 256, 0, stream, static_cast<const float*>(src),
+                   tmp, NC, W, w, H, (long long)H * W, 1LL, (long long)W, 1, mode, 0));
   // vertical pass (H -> h)
   const long long n2 = (long long)NC * h * w;
-  launch_k(resize_pass_kernel<float>, grid_of(n2), 256, 0, stream, (const float*)tmp, dst, NC, H, h, w, (long long)H * w,
-           (long long)w, 1LL, 0, mode, post);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("resize launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  return launch_pdl("resize", resize_pass_kernel<float>, grid_for(n2, 256), 256, 0, stream, (const float*)tmp, dst, NC, H,
+                    h, w, (long long)H * w, (long long)w, 1LL, 0, mode, post);
 }
 
 // depth f32 [HW] -> uint8 [HW][3] (HWC); lut: uint8 [256][3] = (colormap LUT * 255) truncated, as the reference casts
@@ -115,10 +110,7 @@ __global__ void __launch_bounds__(256)
 int launch_colorize(const float* depth, long long HW, float dmin, float dmax, const uint8_t* lut, uint8_t* out,
                     cudaStream_t stream) {
   if (!depth || !lut || !out || HW < 1 || !(dmax > dmin)) { set_error("colorize: bad argument"); return MGB_ERR_INVALID; }
-  colorize_kernel<<<grid_of(HW), 256, 0, stream>>>(depth, HW, dmin, dmax, lut, out);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("colorize launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  return launch_plain("colorize", colorize_kernel, grid_for(HW, 256), 256, 0, stream, depth, HW, dmin, dmax, lut, out);
 }
 
 }  // namespace mgb

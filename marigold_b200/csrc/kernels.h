@@ -78,7 +78,7 @@ struct GemmParams {
 };
 
 // Launch. block_n in {16, 32, 64, 128, 160, 256}; ctas_per_sm 1 or 2 (2: p.stages must keep gemm_smem_bytes <= 113 KB,
-// block_n 64 or 128). Returns cudaError_t as int.
+// block_n 64 or 128).
 int launch_gemm_tc(const GemmParams& p, int block_n, int splits, int ctas_per_sm, cudaStream_t stream);
 void set_gemm_debug_buffer(long long* dev_ptr);  // debug hook: phase timestamps of subsequent launches
 // Deferred epilogue for split-K: sums `splits` partials and applies p.epi.
@@ -194,9 +194,9 @@ int ens_max_members();   // largest supported ensemble size
 // shift; coordinate i < E is s_i, else t_{i-E}). st_host (pinned, room for ens_max_batch() rows of 2E floats): the base
 // {s_0..s_{E-1}, t_0..t_{E-1}}, then when n > 0 the moved value of every coordinate in the same layout.
 // out_host_pinned: double [1 + n][3] = {cost, min(pred), max(pred)}, row 0 the base point, row 1 + i coordinate i moved.
-// v3: 3 HW floats of scratch when n > 0 and E <= kEnsMaxE. One synchronisation per call; *launches = kernels launched.
+// v3: 3 HW floats of scratch when n > 0 and E <= kEnsMaxE. One synchronisation per call.
 int launch_ens_depth_cost(const float* depth, float* st_host, int n, int E, long long HW, int shift, int median,
-                          double reg, void* ws, float* v3, double* out_host_pinned, int* launches, cudaStream_t stream);
+                          double reg, void* ws, float* v3, double* out_host_pinned, cudaStream_t stream);
 int launch_ens_minmax(const float* depth, int E, long long HW, float* ws, float* host_pinned, int* blocks_out,
                       cudaStream_t stream);
 int launch_ens_depth_reduce(const float* depth, const float* st_host, int E, long long HW, int shift, int median,

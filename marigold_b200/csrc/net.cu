@@ -15,12 +15,6 @@
 
 namespace mgb {
 
-#define TRY(expr)               \
-  do {                          \
-    int _rc = (expr);           \
-    if (_rc != MGB_OK) return _rc; \
-  } while (0)
-
 // ---------------------------------------------------------------------------------------------
 // arena
 // ---------------------------------------------------------------------------------------------
@@ -122,12 +116,9 @@ static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const Conv
   return gemm_common(c, p, bn, effective_splits(p), e2, W.cout);
 }
 
-#define LAUNCH(call, n)            \
+#define LAUNCH(call)               \
   do {                             \
-    if (!c.dry) {                  \
-      TRY(call);                   \
-      count_launch(n);             \
-    }                              \
+    if (!c.dry) TRY(call);         \
   } while (0)
 
 // fp32 trunk tensor [M, C]
@@ -151,10 +142,8 @@ static int groupnorm(Ctx& c, const Act& a, const Act* b, bf16* y, bf16* raw, con
   if (c.sync_off > c.sync_need) c.sync_need = c.sync_off;
   if (c.dry) return MGB_OK;
   if (c.sync_off > c.sync_cap) { set_error("groupnorm: barrier counter slab exhausted"); return MGB_ERR_STATE; }
-  TRY(launch_gn_fused(a.p, a.C, Cb ? b->p : nullptr, Cb, y, raw, n.g, n.b, NB, HW, c.groups, eps, silu, part,
-                      c.sync_base + coff, c.stream));
-  count_launch(1);
-  return MGB_OK;
+  return launch_gn_fused(a.p, a.C, Cb ? b->p : nullptr, Cb, y, raw, n.g, n.b, NB, HW, c.groups, eps, silu, part,
+                         c.sync_base + coff, c.stream);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -208,15 +197,15 @@ static int xfmr_forward(Ctx& c, const XfmrW& X, Act& x, Act& y, int NB, int T) {
   { Epi e; e.bias = X.proj_in.b; e.out_f32 = hs0; TRY(linear(c, a, int(M), X.proj_in, e)); }
   // self attention
   const bool no_ln = skip_family("ln"), no_attn = skip_family("attn"), no_x = skip_family("xattn");
-  if (!no_ln) LAUNCH(launch_layernorm(hs0, a, X.ln1.g, X.ln1.b, int(M), C, 1e-5f, c.stream), 1);
+  if (!no_ln) LAUNCH(launch_layernorm(hs0, a, X.ln1.g, X.ln1.b, int(M), C, 1e-5f, c.stream));
   { Epi e; e.out_bf16 = qkv; TRY(linear(c, a, int(M), X.qkv, e)); }
-  if (!no_attn) LAUNCH(launch_flash_attn64(qkv, o, NB, T, C, 0.125f, attn_ws, attn_ws_bytes, c.stream), attn_ws ? 2 : 1);
+  if (!no_attn) LAUNCH(launch_flash_attn64(qkv, o, NB, T, C, 0.125f, attn_ws, attn_ws_bytes, c.stream));
   { Epi e; e.bias = X.o1.b; e.residual = hs0; e.out_f32 = hs1; TRY(linear(c, o, int(M), X.o1, e)); }
   // cross attention against the empty-prompt context, collapsed (norm.cu: xattn2_fused_kernel): LN2, to_q, the 2-key
   // softmax, to_out + residual and LN3 are one launch; hsb = bf16 trunk after attn2, a = LN3 of it for the feed-forward
   if (!no_x) {
     LAUNCH(launch_xattn2_fused(hs1, hsb, a, X.ln2.g, X.ln2.b, X.ln3.g, X.ln3.b, X.xGU, X.xc1, int(M), C, C / 64, 0.125f,
-                               1e-5f, c.stream), 1);
+                               1e-5f, c.stream));
   }
   // GEGLU feed-forward
   { Epi e; e.bias = X.ff1.b; e.out_bf16 = ffm; e.flags = EPI_GEGLU; TRY(linear(c, a, int(M), X.ff1, e)); }
@@ -255,8 +244,8 @@ static int vae_attn_forward(Ctx& c, const VaeAttnW& A, Act& x, Act& y, int NB, i
   for (int n = 0; n < NB; ++n) {
     const size_t off = size_t(n) * T * C;
     { Epi e; e.out_f32 = s; e.flags = EPI_SCALE; e.scale = scale; TRY(matmul_nt(c, q + off, k + off, T, T, C, e, Tp)); }
-    LAUNCH(launch_softmax_rows(s, pr, T, T, Tp, c.stream), 1);
-    LAUNCH(launch_transpose_bf16(v + off, vt, T, C, Tp, c.stream), 1);
+    LAUNCH(launch_softmax_rows(s, pr, T, T, Tp, c.stream));
+    LAUNCH(launch_transpose_bf16(v + off, vt, T, C, Tp, c.stream));
     { Epi e; e.out_bf16 = o + off; TRY(matmul_nt(c, pr, vt, T, C, Tp, e)); }
   }
   { Epi e; e.bias = A.o.b; e.residual = x.p; e.out_f32 = y.p; TRY(linear(c, o, int(M), A.o, e)); }
@@ -299,10 +288,10 @@ int unet_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* tgt, const flo
 
   // step < 0: the step index is read from the device counter (CUDA-graph replay)
   LAUNCH(launch_select_step(hd->bias_table, hd->bias_total, hd->sched_k, hd->cur_bias, hd->cur_sched_k,
-                            hd->step_counter, step, c.stream), 1);
+                            hd->step_counter, step, c.stream));
   c.cur_bias = hd->cur_bias;
   bf16* x0 = aalloc<bf16>(c, M * 64);
-  LAUNCH(launch_pack_latents(rgb, tgt, x0, int(M), cfg.unet_out_channels, c.stream), 1);
+  LAUNCH(launch_pack_latents(rgb, tgt, x0, int(M), cfg.unet_out_channels, c.stream));
   Act h = act_alloc(c, M, ch[0]);
   {
     Epi e; e.bias = U.conv_in.b; e.out_f32 = h.p;
@@ -327,7 +316,7 @@ int unet_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* tgt, const flo
     if (!last) {
       const int Hn = lvH[i + 1], Wn = lvW[i + 1];
       bf16* planes = aalloc<bf16>(c, size_t(NB) * 4 * Hn * Wn * cur);
-      LAUNCH(launch_space_to_depth(h.p, planes, NB, H, W, cur, c.stream), 1);
+      LAUNCH(launch_space_to_depth(h.p, planes, NB, H, W, cur, c.stream));
       H = Hn; W = Wn; M = size_t(NB) * H * W;
       Act y = act_alloc(c, M, cur);
       {
@@ -366,7 +355,7 @@ int unet_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* tgt, const flo
     if (i < 3) {
       const int Hn = lvH[2 - i], Wn = lvW[2 - i];
       bf16* up = aalloc<bf16>(c, size_t(NB) * Hn * Wn * cur);
-      LAUNCH(launch_upsample2x(h.p, up, NB, H, W, cur, Hn, Wn, c.stream), 1);
+      LAUNCH(launch_upsample2x(h.p, up, NB, H, W, cur, Hn, Wn, c.stream));
       H = Hn; W = Wn; M = size_t(NB) * H * W;
       Act y = act_alloc(c, M, cur);
       {
@@ -387,7 +376,7 @@ int unet_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* tgt, const flo
     e.sched_k = hd->cur_sched_k;
     TRY(conv3x3(c, t, NB, H, W, U.conv_out, 0, e));
   }
-  if (step < 0) LAUNCH(launch_advance_counter(hd->step_counter, c.stream), 1);
+  if (step < 0) LAUNCH(launch_advance_counter(hd->step_counter, c.stream));
   return MGB_OK;
 }
 
@@ -404,7 +393,7 @@ int vae_encode_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* latent_o
   TRY(zero_counters(c));
   const size_t mk0 = c.arena->mark();
   bf16* x0 = aalloc<bf16>(c, M * 64);
-  LAUNCH(launch_pack_rgb(rgb, x0, NB, H * W, c.stream), 1);
+  LAUNCH(launch_pack_rgb(rgb, x0, NB, H * W, c.stream));
   Act h = act_alloc(c, M, ch[0]);
   { Epi e; e.bias = V.enc_in.b; e.out_f32 = h.p; TRY(conv3x3(c, x0, NB, H, W, V.enc_in, 0, e)); }
   int cur = ch[0];
@@ -420,7 +409,7 @@ int vae_encode_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* latent_o
       // F.pad(x, (0,1,0,1)) + 3x3 stride 2 pad 0: floor(s / 2) outputs; the parity planes hold ceil(s / 2) entries
       const int Hp = (H + 1) / 2, Wp = (W + 1) / 2;
       bf16* planes = aalloc<bf16>(c, size_t(NB) * 4 * Hp * Wp * cur);
-      LAUNCH(launch_space_to_depth(h.p, planes, NB, H, W, cur, c.stream), 1);
+      LAUNCH(launch_space_to_depth(h.p, planes, NB, H, W, cur, c.stream));
       H /= 2; W /= 2; M = size_t(NB) * H * W;
       Act y = act_alloc(c, M, cur);
       { Epi e; e.bias = V.enc_down[i].b; e.out_f32 = y.p; TRY(conv3x3(c, planes, NB, H, W, V.enc_down[i], 3, e, Hp, Wp)); }
@@ -461,7 +450,7 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
   TRY(zero_counters(c));
   const size_t mk0 = c.arena->mark();
   bf16* z = aalloc<bf16>(c, M * 64);
-  LAUNCH(launch_pack_decoder_latent(latent, V.pq_w, V.pq_b, 1.0f / cfg.latent_scale, z, NB, H * W, c.stream), 1);
+  LAUNCH(launch_pack_decoder_latent(latent, V.pq_w, V.pq_b, 1.0f / cfg.latent_scale, z, NB, H * W, c.stream));
   int cur = ch[3];
   Act h = act_alloc(c, M, cur);
   { Epi e; e.bias = V.dec_in.b; e.out_f32 = h.p; TRY(conv3x3(c, z, NB, H, W, V.dec_in, 0, e)); }
@@ -484,7 +473,7 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
     }
     if (i < 3) {
       bf16* up = aalloc<bf16>(c, M * 4 * cur);
-      LAUNCH(launch_upsample2x(h.p, up, NB, H, W, cur, 2 * H, 2 * W, c.stream), 1);
+      LAUNCH(launch_upsample2x(h.p, up, NB, H, W, cur, 2 * H, 2 * W, c.stream));
       H *= 2; W *= 2; M = size_t(NB) * H * W;
       Act y = act_alloc(c, M, cur);
       { Epi e; e.bias = V.dec_up[i].b; e.out_f32 = y.p; TRY(conv3x3(c, up, NB, H, W, V.dec_up[i], 0, e)); }

@@ -275,19 +275,9 @@ int launch_gn_fused(const float* xa, int Ca, const float* xb, int Cb, bf16* y, b
   const size_t smem = std::max(size_t(g.Tp) * C * sizeof(float2), size_t(2) * G * sizeof(float));
   if (smem > 40 * 1024) { set_error("groupnorm: C=%d needs %zu B of shared memory", C, smem); return MGB_ERR_INVALID; }
   float2* pp = static_cast<float2*>(part);
-  cudaError_t e;
-  if (g.Kq == 1)
-    e = launch_k(gn_fused_kernel<1>, grid, kGnThreads, smem, stream, xa, Ca, xb, Cb, y, raw_copy, gamma, beta, HW, G, eps,
-                 silu, g, pp, counters);
-  else if (g.Kq == 2)
-    e = launch_k(gn_fused_kernel<2>, grid, kGnThreads, smem, stream, xa, Ca, xb, Cb, y, raw_copy, gamma, beta, HW, G, eps,
-                 silu, g, pp, counters);
-  else
-    e = launch_k(gn_fused_kernel<4>, grid, kGnThreads, smem, stream, xa, Ca, xb, Cb, y, raw_copy, gamma, beta, HW, G, eps,
-                 silu, g, pp, counters);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("groupnorm launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  auto kern = g.Kq == 1 ? gn_fused_kernel<1> : g.Kq == 2 ? gn_fused_kernel<2> : gn_fused_kernel<4>;
+  return launch_pdl("groupnorm", kern, grid, kGnThreads, smem, stream, xa, Ca, xb, Cb, y, raw_copy, gamma, beta, HW, G, eps,
+                    silu, g, pp, counters);
 }
 
 // Stand-alone GroupNorm (operator-level ABI): ws = groupnorm_ws_bytes() of scratch (counters zeroed here).
@@ -694,38 +684,22 @@ int launch_xattn2_fused(const float* x, bf16* y, bf16* a_out, const float* g2, c
   if (smem > 200 * 1024) { set_error("xattn2: C=%d H=%d needs %zu B of shared memory", C, H, smem); return MGB_ERR_INVALID; }
   if (C % 16 == 0 && C / 16 > 40 && C / 16 <= 96 && H <= kXwMaxH && M <= kXwMaxTokens) {
     // wide rows: four warps per token (C = 1280: 80 quads per warp quarter)
-    static bool wide_attr = false;
-    if (!wide_attr) {
-      cudaError_t e = cudaFuncSetAttribute(xattn2_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      if (e != cudaSuccess) { set_error("xattn2 attr: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-      wide_attr = true;
-    }
+    TRY(raise_smem_limit_once<xattn2_wide_kernel>("xattn2", 200 * 1024));
     const int blocks = std::max(1, std::min((M + 1) / 2, kNumSMs));
-    cudaError_t e = launch_k(xattn2_wide_kernel, blocks, 256, smem, stream, x, y, a_out, g2, b2, g3, b3, GU, c1, M, C, H, scale, eps);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("xattn2 launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-    return MGB_OK;
+    return launch_pdl("xattn2", xattn2_wide_kernel, blocks, 256, smem, stream, x, y, a_out, g2, b2, g3, b3, GU, c1, M, C, H,
+                      scale, eps);
   }
   const int ql = (C / 4 + 31) / 32;
-  void (*kern)(const float*, bf16*, bf16*, const float*, const float*, const float*, const float*, const bf16*, const float*,
-               int, int, int, float, float) =
-      ql <= 3 ? xattn2_fused_kernel<3> : ql <= 5 ? xattn2_fused_kernel<5> : xattn2_fused_kernel<10>;
-  static bool attr_set[3] = {false, false, false};
-  const int vi = ql <= 3 ? 0 : ql <= 5 ? 1 : 2;
-  if (!attr_set[vi]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e != cudaSuccess) { set_error("xattn2 attr: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-    attr_set[vi] = true;
-  }
+  auto kern = ql <= 3 ? xattn2_fused_kernel<3> : ql <= 5 ? xattn2_fused_kernel<5> : xattn2_fused_kernel<10>;
+  TRY(ql <= 3   ? raise_smem_limit_once<xattn2_fused_kernel<3>>("xattn2", 200 * 1024)
+      : ql <= 5 ? raise_smem_limit_once<xattn2_fused_kernel<5>>("xattn2", 200 * 1024)
+                : raise_smem_limit_once<xattn2_fused_kernel<10>>("xattn2", 200 * 1024));
   const int warps_per_block = 8;
   // one wave of resident blocks, each loading the tables once
   const int by_regs = ql <= 3 ? 4 : ql <= 5 ? 3 : 1;
   const int per_sm = std::max(1, std::min<int>(by_regs, int((220 * 1024) / (smem + 1024))));
   const int blocks = std::max(1, std::min((M + warps_per_block - 1) / warps_per_block, kNumSMs * per_sm));
-  cudaError_t e = launch_k(kern, blocks, 256, smem, stream, x, y, a_out, g2, b2, g3, b3, GU, c1, M, C, H, scale, eps);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("xattn2 launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  return launch_pdl("xattn2", kern, blocks, 256, smem, stream, x, y, a_out, g2, b2, g3, b3, GU, c1, M, C, H, scale, eps);
 }
 
 // One-time folding of the empty-prompt context into the bf16 tables GU = [G | U] ([2][H][C]) and c1 [C] (see above). wq, wo fp32 [C, C] in the
@@ -755,10 +729,7 @@ __global__ void xattn2_fold_kernel(const float* __restrict__ wq, const float* __
 int launch_xattn2_fold(const float* wq, const float* wo, const float* bo, const float* kv, bf16* GU, float* c1, int C,
                        cudaStream_t stream) {
   const int H = C / 64, n = C * (H + 1);
-  xattn2_fold_kernel<<<(n + 255) / 256, 256, 0, stream>>>(wq, wo, bo, kv, GU, c1, C, H);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("xattn2 fold launch: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
-  return MGB_OK;
+  return launch_plain("xattn2 fold", xattn2_fold_kernel, (n + 255) / 256, 256, 0, stream, wq, wo, bo, kv, GU, c1, C, H);
 }
 
 int launch_layernorm(const float* x, bf16* y, const float* gamma, const float* beta, int M, int C, float eps,
@@ -769,13 +740,7 @@ int launch_layernorm(const float* x, bf16* y, const float* gamma, const float* b
   }
   const int warps_per_block = 8;
   const int blocks = (M + warps_per_block - 1) / warps_per_block;
-  launch_k(layernorm_kernel, blocks, 256, 0, stream, x, y, gamma, beta, M, C, eps);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("layernorm launch: %s", cudaGetErrorString(e));
-    return MGB_ERR_CUDA;
-  }
-  return MGB_OK;
+  return launch_pdl("layernorm", layernorm_kernel, blocks, 256, 0, stream, x, y, gamma, beta, M, C, eps);
 }
 
 }  // namespace mgb

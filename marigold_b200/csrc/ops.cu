@@ -4,14 +4,11 @@
 #include <algorithm>
 #include <cstring>
 
+#include "device.h"
 #include "kernels.h"
 #include "ops.h"
 
 namespace mgb {
-
-static std::atomic<long long> g_launches{0};
-void count_launch(int n) { g_launches += n; }
-long long launch_count() { return g_launches.load(); }
 
 void conv_tile_shape(int Hout, int Wout, int* tile_w, int* tile_h) {
   int best_w = 16, best_tiles = 1 << 30;
@@ -198,21 +195,8 @@ int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) 
   } else {
     p.partial = nullptr;
   }
-  int e = launch_gemm_tc(p, block_n, splits, kernel_minb, stream);
-  if (e) {
-    set_error("gemm_tc launch failed: %s", cudaGetErrorString(cudaError_t(e)));
-    return MGB_ERR_CUDA;
-  }
-  count_launch(1);
-  if (splits > 1) {
-    e = launch_splitk_epilogue(p, block_n, splits, stream);
-    if (e) {
-      set_error("splitk epilogue launch failed: %s", cudaGetErrorString(cudaError_t(e)));
-      return MGB_ERR_CUDA;
-    }
-    count_launch(1);
-  }
-  return MGB_OK;
+  TRY(launch_gemm_tc(p, block_n, splits, kernel_minb, stream));
+  return splits > 1 ? launch_splitk_epilogue(p, block_n, splits, stream) : MGB_OK;
 }
 
 // Tile-shape heuristic. Cost model (SM cycles): per CTA  num_kb * K-block time + epilogue + prologue; CTAs run in waves

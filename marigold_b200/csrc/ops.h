@@ -1,13 +1,8 @@
 // Host-side operator builders (ops.cu).
 #pragma once
-#include <atomic>
-
 #include "kernels.h"
 
 namespace mgb {
-
-void count_launch(int n);
-long long launch_count();
 
 // Pixel rectangle of one conv output tile: tile_w x tile_h == 128, tile_w a power of two, fewest tiles over the image.
 void conv_tile_shape(int Hout, int Wout, int* tile_w, int* tile_h);
