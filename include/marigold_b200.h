@@ -187,6 +187,25 @@ int mgb_eval_depth_ex(const float* pred_dev, const float* gt_dev, const uint8_t*
 size_t mgb_eval_normals_ws_bytes(int64_t HW);
 int mgb_eval_normals(const float* pred_dev, const float* gt_dev, const uint8_t* mask_dev, int32_t H, int32_t W,
                      float* error_out_dev, void* ws_dev, double* out_host, void* stream);
+/* Intrinsic-image evaluation of one (sample, target) pair: compute_iid_metric (src/util/metric.py:263-338) as
+ * script/iid/eval.py:182-213 calls it, for PSNR and SSIM (torchmetrics, data_range 1), in ONE synchronisation (the
+ * reference does a torch.linalg.lstsq, a torch.quantile read back with float(), one .item() per metric and a 121-tap
+ * grouped conv2d over five stacked maps). pred_dev, gt_dev fp32 [3,H,W]; mask_dev uint8 [3,H,W] (per channel) or NULL.
+ *   transform (applied to both maps first): 0 none, 1 x ** 2.2 (srgb2linear), 2 x ** (1/2.2) (linear2srgb)
+ *   up_to_scale (shading, residual; metric.py:266-270): s = lstsq of the masked elements of all three channels
+ *     (sum pg / sum p^2, 0 when sum p^2 == 0), pred = s * pred; q = torch.quantile(brightness, 0.9) of
+ *     0.3 g0 + 0.59 g1 + 0.11 g2 over the pixels valid in mask channel 0 (float32 rank fl(0.9 (n-1)), exact order
+ *     statistics, torch's lerp; NaN if any brightness is NaN); k = 0 if q < 1e-4 else fl(fl(1 / q) * 0.8) (torch's
+ *     0.8 / q); gt = clamp(k gt, 0, 1), pred = clamp(k pred, 0, 1)
+ *   PSNR = 10 log10(1 / (SSE / n)) over the masked elements (all 3HW without a mask); +inf when SSE = 0, NaN when n = 0
+ *   SSIM: invalid elements set to 0, Gaussian sigma 1.5 (11 taps), c1 = 0.01^2, c2 = 0.03^2, variances clamped at 0,
+ *     the mean over the 3 (H-10)(W-10) windows inside the image (torchmetrics pads by reflection and crops 5 per side)
+ * ws_dev: mgb_eval_iid_ws_bytes(H, W). out_host[6] = {n_valid (masked elements), psnr, ssim, s, q, k}; s = k = 1,
+ * q = NaN when !up_to_scale. MGB_ERR_INVALID for H or W < 11, and for up_to_scale with no pixel valid in mask channel 0
+ * (torch.quantile of an empty tensor raises). Deterministic: equal inputs give equal bits. */
+size_t mgb_eval_iid_ws_bytes(int32_t H, int32_t W);
+int mgb_eval_iid(const float* pred_dev, const float* gt_dev, const uint8_t* mask_dev, int32_t H, int32_t W,
+                 int32_t up_to_scale, int32_t transform, void* ws_dev, double* out_host, void* stream);
 
 /* ---- capacity ------------------------------------------------------------------------------- */
 /* Bytes of the activation arena the handle holds for images of H x W with B members per batch. */

@@ -67,6 +67,8 @@ SIGNATURES = {
     "mgb_eval_depth_ex": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _vp]),
     "mgb_eval_normals_ws_bytes": (C.c_size_t, [_i64]),
     "mgb_eval_normals": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "mgb_eval_iid_ws_bytes": (C.c_size_t, [_i32, _i32]),
+    "mgb_eval_iid": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "mgb_workspace_bytes": (C.c_size_t, [_vp, _i32, _i32, _i32]),
     "mgb_launch_count": (_i64, []),
     "mgb_op_linear": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),

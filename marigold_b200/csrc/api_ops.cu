@@ -218,6 +218,28 @@ int mgb_eval_normals(const float* pred, const float* gt, const uint8_t* mask, in
   return MGB_OK;
 }
 
+size_t mgb_eval_iid_ws_bytes(int32_t H, int32_t W) { return H > 0 && W > 0 ? eval_iid_ws_bytes(H, W) : 0; }
+
+int mgb_eval_iid(const float* pred, const float* gt, const uint8_t* mask, int32_t H, int32_t W, int32_t up_to_scale,
+                 int32_t transform, void* ws, double* out_host, void* stream) {
+  if (!pred || !gt || !ws || !out_host || H < 11 || W < 11 || transform < 0 || transform > 2) {
+    set_error("mgb_eval_iid: bad argument (H=%d W=%d transform=%d; H and W must be >= 11)", H, W, transform);
+    return MGB_ERR_INVALID;
+  }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  TRY(launch_eval_iid(pred, gt, mask, H, W, up_to_scale != 0, transform, ws, s));
+  double res[7];
+  cudaError_t e = cudaMemcpyAsync(res, eval_iid_out(ws, H, W), sizeof(res), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) { set_error("mgb_eval_iid: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+  if (up_to_scale && res[6] == 0.0) {
+    set_error("mgb_eval_iid: no pixel is valid in channel 0 of the mask, so the brightness quantile is undefined");
+    return MGB_ERR_INVALID;
+  }
+  for (int i = 0; i < 6; ++i) out_host[i] = res[i];
+  return MGB_OK;
+}
+
 int mgb_op_space_to_depth(const float* x, void* y, int32_t NB, int32_t H, int32_t W, int32_t C, void* stream) {
   return launch_space_to_depth(x, reinterpret_cast<bf16*>(y), NB, H, W, C, reinterpret_cast<cudaStream_t>(stream));
 }

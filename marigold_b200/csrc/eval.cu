@@ -173,6 +173,8 @@ int launch_eval_depth(const float* pred, const float* gt, const uint8_t* mask, l
 //   final    one block: the two order statistics exactly, np.median's mean of them, the other metrics
 // The errors are >= 0, so the unsigned order of their bit patterns is their numeric order, and integer counts do not
 // depend on the order the atomics land in: the median is exact and every output is deterministic.
+// locate / refine and the low-bin lookup of final (sel_*) serve any 32-bit keys whose unsigned order is the values'
+// order: the intrinsic-image evaluation below selects its brightness quantile with them.
 constexpr int kNrHiBins = 0x4335 + 1;       // high halves of [0, 180.00002]; the last bin takes anything above (NaN)
 constexpr int kNrLoBins = 1 << 16;
 constexpr int kNrSelThreads = 1024;
@@ -181,11 +183,14 @@ constexpr float kInvPi = 1.0f / 3.14159265358979323846f;
 
 struct NrSel {
   unsigned n;
-  unsigned bin[2];    // high-16 bin of order statistics (n-1)/2 and n/2 (kNrInvalid when n == 0)
+  unsigned bin[2];    // high-16 bin of the two order statistics (kNrInvalid when n == 0)
   unsigned rank[2];   // rank inside that bin
+  float frac;         // torch.quantile's interpolation weight between them (0 for the median)
 };
 
-__device__ __forceinline__ unsigned nr_bin(unsigned bits) { return min(bits >> 16, unsigned(kNrHiBins - 1)); }
+// High-16 bin of a key; `top` takes every key above it.
+__device__ __forceinline__ unsigned sel_bin(unsigned bits, unsigned top) { return min(bits >> 16, top); }
+__device__ __forceinline__ unsigned nr_bin(unsigned bits) { return sel_bin(bits, unsigned(kNrHiBins - 1)); }
 
 // torch.cosine_similarity(pred, gt, dim=0) (each vector over max(norm, 1e-8), then the products summed over the channels
 // in order), clamp(-1, 1), acos, * 180.0, / pi. torch's CUDA division by a scalar multiplies by its fp32 reciprocal,
@@ -285,45 +290,63 @@ __device__ __forceinline__ void find_rank(const unsigned* __restrict__ hist, int
   }
 }
 
-__global__ void __launch_bounds__(kNrSelThreads) eval_normals_locate_kernel(const unsigned* __restrict__ hist_hi, NrSel* sel) {
+// One block: n = the keys counted in hist_hi, and the bins and in-bin ranks of two order statistics. q < 0: the
+// median's, (n-1)/2 and n/2 (np.median). Otherwise torch.quantile(q)'s, whose rank is float32: r = fl(q * (n-1)),
+// order statistics floor(r) and ceil(r), weight r - floor(r).
+__global__ void __launch_bounds__(kNrSelThreads)
+    sel_locate_kernel(const unsigned* __restrict__ hist_hi, int nbins, float q, NrSel* sel) {
   unsigned local = 0;
-  const int per = (kNrHiBins + kNrSelThreads - 1) / kNrSelThreads;
-  for (int b = threadIdx.x * per; b < min((int(threadIdx.x) + 1) * per, kNrHiBins); ++b) local += hist_hi[b];
+  const int per = (nbins + kNrSelThreads - 1) / kNrSelThreads;
+  for (int b = threadIdx.x * per; b < min((int(threadIdx.x) + 1) * per, nbins); ++b) local += hist_hi[b];
   unsigned n;
   block_exclusive_scan(local, &n);
+  unsigned k0 = (n - 1) / 2, k1 = n / 2;
+  float frac = 0.f;
+  if (q >= 0.f && n > 0) {
+    const float r = __fmul_rn(q, float(n - 1)), f = floorf(r);
+    k0 = unsigned(f);
+    k1 = min(unsigned(ceilf(r)), n - 1);
+    frac = __fsub_rn(r, f);
+  }
   if (threadIdx.x == 0) {
     sel->n = n;
     sel->bin[0] = sel->bin[1] = kNrInvalid;
+    sel->frac = frac;
   }
   __syncthreads();
   if (n == 0) return;
-  find_rank(hist_hi, kNrHiBins, (n - 1) / 2, &sel->bin[0], &sel->rank[0]);
-  find_rank(hist_hi, kNrHiBins, n / 2, &sel->bin[1], &sel->rank[1]);
+  find_rank(hist_hi, nbins, k0, &sel->bin[0], &sel->rank[0]);
+  find_rank(hist_hi, nbins, k1, &sel->bin[1], &sel->rank[1]);
 }
 
+// Histograms of the low 16 bits of the keys in the two located bins (top: the highest bin, as in sel_bin).
 __global__ void __launch_bounds__(kEvThreads)
-    eval_normals_refine_kernel(const unsigned* __restrict__ err_bits, long long HW, const NrSel* __restrict__ sel,
-                               unsigned* __restrict__ hist_lo) {
+    sel_refine_kernel(const unsigned* __restrict__ keys, long long HW, unsigned top, const NrSel* __restrict__ sel,
+                      unsigned* __restrict__ hist_lo) {
   const unsigned b0 = sel->bin[0], b1 = sel->bin[1];
   for (long long base = (long long)blockIdx.x * blockDim.x; base < HW; base += (long long)gridDim.x * blockDim.x) {
     const long long p = base + threadIdx.x;
-    const unsigned bits = p < HW ? err_bits[p] : kNrInvalid;
-    const unsigned bin = bits == kNrInvalid ? kNrInvalid : nr_bin(bits);
+    const unsigned bits = p < HW ? keys[p] : kNrInvalid;
+    const unsigned bin = bits == kNrInvalid ? kNrInvalid : sel_bin(bits, top);
     const unsigned which = bin == b0 ? 0u : 1u;     // both ranks in one bin: one histogram serves both
     warp_agg_add(hist_lo, which * kNrLoBins + (bits & 0xFFFFu), bin == b0 || bin == b1);
   }
+}
+
+// The low 16 bits of both order statistics (block-wide; sel->n > 0).
+__device__ __forceinline__ void sel_find_low(const NrSel* sel, const unsigned* __restrict__ hist_lo, unsigned* lo) {
+  __shared__ unsigned rank_unused;
+  find_rank(hist_lo, kNrLoBins, sel->rank[0], &lo[0], &rank_unused);
+  find_rank(hist_lo + (sel->bin[1] == sel->bin[0] ? 0 : kNrLoBins), kNrLoBins, sel->rank[1], &lo[1], &rank_unused);
 }
 
 // out: {n_valid, mean, median, rmse, sub5, sub7.5, sub11.25, sub22.5, sub30}
 __global__ void __launch_bounds__(kNrSelThreads)
     eval_normals_final_kernel(const double* __restrict__ part, int nblocks, NrSel* sel, const unsigned* __restrict__ hist_lo,
                               double* __restrict__ out) {
-  __shared__ unsigned lo[2], rank_unused;
+  __shared__ unsigned lo[2];
   const unsigned n = sel->n;
-  if (n > 0) {
-    find_rank(hist_lo, kNrLoBins, sel->rank[0], &lo[0], &rank_unused);
-    find_rank(hist_lo + (sel->bin[1] == sel->bin[0] ? 0 : kNrLoBins), kNrLoBins, sel->rank[1], &lo[1], &rank_unused);
-  }
+  if (n > 0) sel_find_low(sel, hist_lo, lo);
   __shared__ double s[8];
   if (threadIdx.x < 32)
     for (int k = 0; k < 8; ++k) {
@@ -373,11 +396,260 @@ int launch_eval_normals(const float* pred, const float* gt, const uint8_t* mask,
   if (e != cudaSuccess) { set_error("eval_normals memset: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
   TRY(launch_plain("eval_normals_error", eval_normals_error_kernel, blocks, kEvThreads, smem, stream, pred, gt, mask, HW,
                    err_bits, err_out, hist_hi, part));
-  TRY(launch_plain("eval_normals_locate", eval_normals_locate_kernel, 1, kNrSelThreads, 0, stream, hist_hi, sel));
-  TRY(launch_plain("eval_normals_refine", eval_normals_refine_kernel, blocks, kEvThreads, 0, stream, err_bits, HW, sel,
-                   hist_lo));
+  TRY(launch_plain("eval_normals_locate", sel_locate_kernel, 1, kNrSelThreads, 0, stream, hist_hi, kNrHiBins, -1.0f, sel));
+  TRY(launch_plain("eval_normals_refine", sel_refine_kernel, blocks, kEvThreads, 0, stream, err_bits, HW,
+                   unsigned(kNrHiBins - 1), sel, hist_lo));
   return launch_plain("eval_normals_final", eval_normals_final_kernel, 1, kNrSelThreads, 0, stream, part, blocks, sel,
                       hist_lo, eval_normals_out(ws));
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Intrinsic-image evaluation of one (sample, target) pair (script/iid/eval.py:182-213 -> compute_iid_metric,
+// src/util/metric.py:263-338): PSNR and SSIM (torchmetrics, data_range 1) of the optionally colour-transformed maps and,
+// for the up-to-scale targets, after the least-squares scale and the quantile map. ONE synchronisation per call.
+//   stats   (up-to-scale) fixed-order double sums of p g and p^2 over the masked elements -> s = sum pg / sum p^2 (the
+//           1 x 1 lstsq); the brightness 0.3 g0 + 0.59 g1 + 0.11 g2 of every pixel valid in mask channel 0 as an
+//           order-preserving key, and a global histogram of the keys' high 16 bits
+//   locate, refine (sel_*), select   the order statistics floor(r), ceil(r) of torch.quantile(0.9) exactly; q, k
+//   ssim    tiles of 32 x 32 outputs per channel: the mapped maps in shared memory with a 5-pixel halo, the separable
+//           11-tap Gaussian over the five moment maps, SSIM of every window that lies inside the image (torchmetrics'
+//           reflect padding touches only the outputs it crops), the squared error of the masked elements the tile owns
+//   final   PSNR = 10 log10(1 / (SSE / n)), SSIM = the mean over the 3 (H-10)(W-10) windows
+// The non-scale targets run ssim and final only. Atomics add integer counts only: equal inputs give equal bits.
+constexpr int kIidHiBins = 1 << 16;              // brightness keys span every float: the whole high half
+constexpr unsigned kIidNanKey = 0xFFFFFFFEu;     // every NaN: above +inf (0xFF800000), alone in the top bin
+constexpr int kSsTile = 32, kSsHalo = 5, kSsIn = kSsTile + 2 * kSsHalo, kSsTaps = 2 * kSsHalo + 1;
+
+// image_util.py:144-149 as torch evaluates x ** 2.2 and x ** (1 / 2.2) on a float32 tensor: powf, float32 exponent
+__device__ __forceinline__ float iid_transform(float x, int t) {
+  return t == 1 ? powf(x, 2.2f) : t == 2 ? powf(x, float(1.0 / 2.2)) : x;
+}
+
+__device__ __forceinline__ unsigned iid_key(float b) {
+  if (b != b) return kIidNanKey;
+  const unsigned u = __float_as_uint(b);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float iid_key_value(unsigned k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+
+// torch.clamp(x, 0, 1): NaN stays NaN
+__device__ __forceinline__ float clamp01(float x) { return x != x ? x : fminf(fmaxf(x, 0.f), 1.f); }
+
+__global__ void __launch_bounds__(kEvThreads)
+    eval_iid_stats_kernel(const float* __restrict__ pred, const float* __restrict__ gt, const uint8_t* __restrict__ mask,
+                          long long HW, int transform, unsigned* __restrict__ keys, unsigned* __restrict__ hist_hi,
+                          double* __restrict__ part) {
+  double v[kEvSums] = {0};
+  for (long long base = (long long)blockIdx.x * blockDim.x; base < HW; base += (long long)gridDim.x * blockDim.x) {
+    const long long p = base + threadIdx.x;
+    bool take = false;
+    unsigned key = kNrInvalid;
+    if (p < HW) {
+      float g[3];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        g[c] = iid_transform(gt[p + c * HW], transform);
+        if (mask && !mask[p + c * HW]) continue;
+        const double a = iid_transform(pred[p + c * HW], transform), b = g[c];
+        v[0] += a * b; v[1] += a * a;                    // exact products of float32 values
+      }
+      take = !mask || mask[p];                           // quantile_map: brightness[valid_mask[0]]
+      if (take) key = iid_key(__fadd_rn(__fadd_rn(__fmul_rn(0.3f, g[0]), __fmul_rn(0.59f, g[1])), __fmul_rn(0.11f, g[2])));
+      keys[p] = key;
+    }
+    warp_agg_add(hist_hi, key >> 16, take);
+  }
+  block_reduce_store(v, 2, part);
+}
+
+// One block. sk = {s, k} for the ssim pass; out[3..6] = {s, q, k, pixels in the quantile}.
+__global__ void __launch_bounds__(kNrSelThreads)
+    eval_iid_select_kernel(const double* __restrict__ part, int nblocks, const NrSel* sel, const unsigned* __restrict__ hist_hi,
+                           const unsigned* __restrict__ hist_lo, float* __restrict__ sk, double* __restrict__ out) {
+  __shared__ unsigned lo[2];
+  __shared__ double sums[2];
+  const unsigned n = sel->n;
+  if (n > 0) sel_find_low(sel, hist_lo, lo);
+  if (threadIdx.x < 32)
+    for (int k = 0; k < 2; ++k) {
+      const double t = warp_sum_partials(part, nblocks, k);
+      if (threadIdx.x == 0) sums[k] = t;
+    }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  // lstsq of the masked elements: sum pg / sum p^2, and 0 (the minimum-norm solution) when every p is 0
+  const float s = sums[1] == 0.0 ? 0.f : float(sums[0] / sums[1]);
+  float q = __int_as_float(0x7fffffff);
+  if (n > 0 && hist_hi[kIidHiBins - 1] == 0) {            // a NaN brightness makes torch.quantile NaN
+    const float v0 = iid_key_value((sel->bin[0] << 16) | lo[0]), v1 = iid_key_value((sel->bin[1] << 16) | lo[1]);
+    const float w = sel->frac, d = __fsub_rn(v1, v0);      // torch's lerp, un-fused
+    q = w < 0.5f ? __fadd_rn(v0, __fmul_rn(w, d)) : __fsub_rn(v1, __fmul_rn(d, __fsub_rn(1.f, w)));
+  }
+  // quantile_map: 0 below 1e-4, else float(0.8 / q), which torch evaluates as q.reciprocal() * 0.8 in float32
+  const float k = q < 1e-4f ? 0.f : __fmul_rn(__frcp_rn(q), 0.8f);
+  sk[0] = s; sk[1] = k;
+  out[3] = s; out[4] = q; out[5] = k; out[6] = n;
+}
+
+// The Gaussian of torchmetrics' SSIM (sigma 1.5, 11 taps): exp(-(d / 1.5)^2 / 2) over d = -5..5, over its float32 sum
+__device__ __forceinline__ void ssim_gauss(float (&w)[kSsTaps]) {
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < kSsTaps; ++i) {
+    const float t = __fdiv_rn(float(i - kSsHalo), 1.5f);
+    w[i] = expf(__fdiv_rn(-__fmul_rn(t, t), 2.f));
+    sum = __fadd_rn(sum, w[i]);
+  }
+#pragma unroll
+  for (int i = 0; i < kSsTaps; ++i) w[i] = __fdiv_rn(w[i], sum);
+}
+
+// One CTA per (channel, 32 x 32 tile). sk: {s, k} of the up-to-scale targets, or nullptr (maps used as they are).
+// Partials: {sum of SSIM over the tile's interior windows, SSE and count of the masked elements the tile owns}.
+__global__ void __launch_bounds__(kEvThreads)
+    eval_iid_ssim_kernel(const float* __restrict__ pred, const float* __restrict__ gt, const uint8_t* __restrict__ mask,
+                         int H, int W, int transform, const float* __restrict__ sk, int tiles_x, int tiles_y,
+                         double* __restrict__ part) {
+  __shared__ float sp[kSsIn][kSsIn + 1], sg[kSsIn][kSsIn + 1];
+  __shared__ float sh[5][kSsIn][kSsTile + 1];                  // the row pass: five moment maps
+  const int c = blockIdx.x / (tiles_x * tiles_y), t = blockIdx.x % (tiles_x * tiles_y);
+  const int y0 = (t / tiles_x) * kSsTile, x0 = (t % tiles_x) * kSsTile;
+  const long long plane = (long long)c * H * W;
+  const float s = sk ? sk[0] : 1.f, k = sk ? sk[1] : 1.f;
+  double v[kEvSums] = {0};
+  for (int i = threadIdx.x; i < kSsIn * kSsIn; i += blockDim.x) {
+    const int r = i / kSsIn, q = i % kSsIn, y = y0 - kSsHalo + r, x = x0 - kSsHalo + q;
+    float pv = 0.f, gv = 0.f;
+    if (y >= 0 && y < H && x >= 0 && x < W) {
+      const long long e = plane + (long long)y * W + x;
+      pv = iid_transform(pred[e], transform);
+      gv = iid_transform(gt[e], transform);
+      if (sk) {                                             // pred = s * pred, then quantile_map's clamp(k * .)
+        pv = clamp01(__fmul_rn(k, __fmul_rn(s, pv)));
+        gv = clamp01(__fmul_rn(k, gv));
+      }
+      const bool valid = !mask || mask[e];
+      const bool own = r >= kSsHalo && r < kSsHalo + kSsTile && q >= kSsHalo && q < kSsHalo + kSsTile;
+      if (valid && own) {                                   // PSNR of pred[mask], gt[mask]
+        const double d = double(pv) - double(gv);
+        v[1] += d * d; v[2] += 1.0;
+      }
+      if (!valid) pv = gv = 0.f;                            // SSIM: pred[~mask] = gt[~mask] = 0
+    }
+    sp[r][q] = pv; sg[r][q] = gv;
+  }
+  __syncthreads();
+  float w[kSsTaps];
+  ssim_gauss(w);
+  for (int i = threadIdx.x; i < kSsIn * kSsTile; i += blockDim.x) {
+    const int r = i / kSsTile, j = i % kSsTile;
+    float m[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int a = 0; a < kSsTaps; ++a) {
+      const float pv = sp[r][j + a], gv = sg[r][j + a];
+      m[0] = fmaf(w[a], pv, m[0]);
+      m[1] = fmaf(w[a], gv, m[1]);
+      m[2] = fmaf(w[a], __fmul_rn(pv, pv), m[2]);
+      m[3] = fmaf(w[a], __fmul_rn(gv, gv), m[3]);
+      m[4] = fmaf(w[a], __fmul_rn(pv, gv), m[4]);
+    }
+#pragma unroll
+    for (int u = 0; u < 5; ++u) sh[u][r][j] = m[u];
+  }
+  __syncthreads();
+  const float c1 = float(0.01 * 0.01), c2 = float(0.03 * 0.03);
+  for (int i = threadIdx.x; i < kSsTile * kSsTile; i += blockDim.x) {
+    const int a0 = i / kSsTile, j = i % kSsTile, y = y0 + a0, x = x0 + j;
+    if (y < kSsHalo || y >= H - kSsHalo || x < kSsHalo || x >= W - kSsHalo) continue;
+    float m[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int a = 0; a < kSsTaps; ++a)
+#pragma unroll
+      for (int u = 0; u < 5; ++u) m[u] = fmaf(w[a], sh[u][a0 + a][j], m[u]);
+    // torchmetrics _ssim_update, in its order
+    const float mu_pp = __fmul_rn(m[0], m[0]), mu_gg = __fmul_rn(m[1], m[1]), mu_pg = __fmul_rn(m[0], m[1]);
+    float s_pp = __fsub_rn(m[2], mu_pp), s_gg = __fsub_rn(m[3], mu_gg);
+    s_pp = s_pp < 0.f ? 0.f : s_pp;                         // clamp(min=0); NaN stays NaN
+    s_gg = s_gg < 0.f ? 0.f : s_gg;
+    const float s_pg = __fsub_rn(m[4], mu_pg);
+    const float upper = __fadd_rn(__fmul_rn(2.f, s_pg), c2), lower = __fadd_rn(__fadd_rn(s_pp, s_gg), c2);
+    const float num = __fmul_rn(__fadd_rn(__fmul_rn(2.f, mu_pg), c1), upper);
+    const float den = __fmul_rn(__fadd_rn(__fadd_rn(mu_pp, mu_gg), c1), lower);
+    v[0] += double(__fdiv_rn(num, den));
+  }
+  block_reduce_store(v, 3, part);
+}
+
+// out[0..2] = {n_valid, psnr, ssim}; without the up-to-scale passes also out[3..6] = {1, NaN, 1, 0}.
+__global__ void eval_iid_final_kernel(const double* __restrict__ part, int nblocks, double windows, int up_to_scale,
+                                      double* __restrict__ out) {
+  double s[3];
+  for (int k = 0; k < 3; ++k) s[k] = warp_sum_partials(part, nblocks, k);
+  if (threadIdx.x != 0) return;
+  out[0] = s[2];
+  out[1] = 10.0 * log10(1.0 / (s[1] / s[2]));              // SSE 0: +inf; no element: NaN
+  out[2] = s[0] / windows;
+  if (!up_to_scale) {
+    out[3] = 1.0; out[4] = __longlong_as_double(0x7ff8000000000000ll); out[5] = 1.0; out[6] = 0.0;
+  }
+}
+
+// Workspace: partials | 16 doubles of results | NrSel | {s, k} | high and low histograms | the keys (4 B per pixel).
+struct IidLayout {
+  size_t out, sel, sk, hist, keys, total;
+  int tiles_x, tiles_y;
+};
+static IidLayout iid_layout(long long H, long long W) {
+  IidLayout l;
+  l.tiles_x = int((W + kSsTile - 1) / kSsTile);
+  l.tiles_y = int((H + kSsTile - 1) / kSsTile);
+  const size_t blocks = std::max<size_t>(kEvBlocks, size_t(3) * l.tiles_x * l.tiles_y);
+  l.out = blocks * kEvSums * sizeof(double);
+  l.sel = l.out + 16 * sizeof(double);
+  l.sk = l.sel + 64;
+  l.hist = l.sk + 64;
+  l.keys = l.hist + size_t(kIidHiBins + 2 * kNrLoBins) * sizeof(unsigned);
+  l.total = l.keys + size_t(H * W) * sizeof(unsigned);
+  return l;
+}
+
+size_t eval_iid_ws_bytes(long long H, long long W) { return iid_layout(H, W).total; }
+double* eval_iid_out(void* ws, long long H, long long W) {
+  return reinterpret_cast<double*>(static_cast<char*>(ws) + iid_layout(H, W).out);
+}
+
+int launch_eval_iid(const float* pred, const float* gt, const uint8_t* mask, long long H, long long W, int up_to_scale,
+                    int transform, void* ws, cudaStream_t stream) {
+  const IidLayout l = iid_layout(H, W);
+  char* w = static_cast<char*>(ws);
+  double* part = reinterpret_cast<double*>(w);
+  double* out = reinterpret_cast<double*>(w + l.out);
+  const long long HW = H * W;
+  float* sk = nullptr;
+  if (up_to_scale) {
+    NrSel* sel = reinterpret_cast<NrSel*>(w + l.sel);
+    sk = reinterpret_cast<float*>(w + l.sk);
+    unsigned* hist_hi = reinterpret_cast<unsigned*>(w + l.hist);
+    unsigned* hist_lo = hist_hi + kIidHiBins;
+    unsigned* keys = reinterpret_cast<unsigned*>(w + l.keys);
+    const int blocks = int(std::min<long long>((HW + kEvThreads - 1) / kEvThreads, kEvBlocks));
+    cudaError_t e = cudaMemsetAsync(hist_hi, 0, size_t(kIidHiBins + 2 * kNrLoBins) * sizeof(unsigned), stream);
+    if (e != cudaSuccess) { set_error("eval_iid memset: %s", cudaGetErrorString(e)); return MGB_ERR_CUDA; }
+    TRY(launch_plain("eval_iid_stats", eval_iid_stats_kernel, blocks, kEvThreads, 0, stream, pred, gt, mask, HW, transform,
+                     keys, hist_hi, part));
+    TRY(launch_plain("eval_iid_locate", sel_locate_kernel, 1, kNrSelThreads, 0, stream, hist_hi, kIidHiBins, 0.9f, sel));
+    TRY(launch_plain("eval_iid_refine", sel_refine_kernel, blocks, kEvThreads, 0, stream, keys, HW,
+                     unsigned(kIidHiBins - 1), sel, hist_lo));
+    TRY(launch_plain("eval_iid_select", eval_iid_select_kernel, 1, kNrSelThreads, 0, stream, part, blocks, sel, hist_hi,
+                     hist_lo, sk, out));
+  }
+  const int tiles = 3 * l.tiles_x * l.tiles_y;
+  TRY(launch_plain("eval_iid_ssim", eval_iid_ssim_kernel, tiles, kEvThreads, 0, stream, pred, gt, mask, int(H), int(W),
+                   transform, sk, l.tiles_x, l.tiles_y, part));
+  return launch_plain("eval_iid_final", eval_iid_final_kernel, 1, 32, 0, stream, part, tiles,
+                      3.0 * double(H - 2 * kSsHalo) * double(W - 2 * kSsHalo), up_to_scale, out);
 }
 
 }  // namespace mgb

@@ -182,6 +182,12 @@ size_t eval_normals_ws_bytes(long long HW);
 double* eval_normals_out(void* ws);
 int launch_eval_normals(const float* pred, const float* gt, const uint8_t* mask, long long HW, float* err_out, void* ws,
                         cudaStream_t stream);
+// pred, gt fp32 [3, H, W]; mask u8 [3, H, W] or nullptr; transform 0 none, 1 x^2.2, 2 x^(1/2.2). Results: 7 doubles at
+// eval_iid_out(ws, H, W): {n_valid, psnr, ssim, s, q, k, pixels in the quantile}.
+size_t eval_iid_ws_bytes(long long H, long long W);
+double* eval_iid_out(void* ws, long long H, long long W);
+int launch_eval_iid(const float* pred, const float* gt, const uint8_t* mask, long long H, long long W, int up_to_scale,
+                    int transform, void* ws, cudaStream_t stream);
 
 // ---------------------------------------------------------------------------------------------
 // Ensemble kernels (ensemble.cu)

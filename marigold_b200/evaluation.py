@@ -4,7 +4,9 @@ Depth: least-squares scale / shift alignment in depth or disparity space (refere
 script/depth/eval.py:171-207), the dataset clips and the masked depth metrics of src/util/metric.py:64-191 — two
 streaming passes and one host synchronisation per sample.
 Surface normals: the angular error of compute_cosine_error(masked=True) and the metrics of src/util/metric.py:194-257,
-including the exact median — four launches and one host synchronisation per sample."""
+including the exact median — four launches and one host synchronisation per sample.
+Intrinsic images: PSNR and SSIM of compute_iid_metric (src/util/metric.py:263-338) with the up-to-scale targets' lstsq
+scale and quantile map — two launches (six for shading and residual) and one host synchronisation per target."""
 from __future__ import annotations
 
 import ctypes as C
@@ -20,9 +22,13 @@ METRIC_NAMES = ("abs_relative_difference", "squared_relative_difference", "rmse_
                 "delta2_acc", "delta3_acc", "i_rmse", "silog_rmse")
 NORMALS_METRIC_NAMES = ("mean_angular_error", "median_angular_error", "rmse_angular_error", "sub5_error", "sub7_5_error",
                         "sub11_25_error", "sub22_5_error", "sub30_error")
+IID_METRIC_NAMES = ("psnr", "ssim")
+IID_TRANSFORMS = (None, "srgb2linear", "linear2srgb")
 ALIGNMENTS = (None, "least_square", "least_square_disparity")
+_ERR_INVALID = -1     # MGB_ERR_INVALID
 _ws = {}
 _normals_ws = {}
+_iid_ws = {}
 
 
 def _inputs(pred, gt, mask):
@@ -165,3 +171,56 @@ def evaluate_normals(pred: torch.Tensor, gt: torch.Tensor, valid_mask: Optional[
     if err is not None:
         info["error_map"] = err
     return dict(zip(NORMALS_METRIC_NAMES, (float(v) for v in out[1:]))), info
+
+
+def _as_chw(t: torch.Tensor, what: str) -> torch.Tensor:
+    if t.dim() == 4 and t.shape[0] == 1:
+        t = t.squeeze(0)
+    if t.dim() != 3 or t.shape[0] != 3:
+        raise ValueError(f"{what} must be [3, H, W] or [1, 3, H, W], got {tuple(t.shape)}")
+    return t
+
+
+def evaluate_iid(pred: torch.Tensor, gt: torch.Tensor, target_name: str, valid_mask: Optional[torch.Tensor] = None,
+                 transform: Optional[str] = None) -> Tuple[Dict[str, float], Dict[str, object]]:
+    """PSNR and SSIM of one intrinsic-image target of one sample: compute_iid_metric (src/util/metric.py:263-338) as
+    script/iid/eval.py:182-213 calls it, with torchmetrics' PeakSignalNoiseRatio and StructuralSimilarityIndexMeasure
+    (data_range=1.0). LPIPS is not computed.
+
+    pred, gt: [3, H, W] or [1, 3, H, W] CUDA tensors, H and W >= 11. valid_mask: bool [3, H, W] (one mask per channel,
+    as the datasets build it) or None. transform: None, "srgb2linear" or "linear2srgb", applied to both maps first (the
+    caller decides it per dataset and target, as eval.py does). "shading" and "residual" are up to scale: the prediction
+    is fitted to gt by least squares and both are mapped to [0, 1] by the brightness quantile of gt.
+    Returns ({"psnr", "ssim"}, {"n_valid", "scale", "quantile", "quantile_scale"}); the last three are None for the
+    other targets. Raises ValueError for malformed input and, for an up-to-scale target, when no pixel is valid in
+    channel 0 of the mask (the reference's torch.quantile of an empty tensor)."""
+    if transform not in IID_TRANSFORMS:
+        raise ValueError(f"unsupported transform {transform!r}; expected one of {IID_TRANSFORMS}")
+    pred, gt = _as_chw(pred, "pred"), _as_chw(gt, "gt")
+    if gt.shape != pred.shape:
+        raise ValueError(f"pred {tuple(pred.shape)} and gt {tuple(gt.shape)} differ")
+    if valid_mask is not None:
+        valid_mask = _as_chw(valid_mask, "valid_mask")
+        if valid_mask.shape != pred.shape:
+            raise ValueError(f"valid_mask {tuple(valid_mask.shape)} does not match {tuple(pred.shape)}")
+    H, W = pred.shape[-2:]
+    if H < 11 or W < 11:
+        raise ValueError(f"SSIM's 11 x 11 window needs H, W >= 11, got {H} x {W}")
+    up_to_scale = target_name in ("shading", "residual")
+    p, g, m = _inputs(pred, gt, valid_mask)
+    lib = _lib.load()
+    with torch.cuda.device(p.device):
+        need = int(lib.mgb_eval_iid_ws_bytes(H, W))
+        ws = _iid_ws.get(p.device)
+        if ws is None or ws.numel() < need:
+            ws = torch.empty(need, dtype=torch.uint8, device=p.device)
+            _iid_ws[p.device] = ws
+        out = np.zeros(6, dtype=np.float64)
+        rc = lib.mgb_eval_iid(ptr(p), ptr(g), ptr(m), H, W, int(up_to_scale), IID_TRANSFORMS.index(transform), ptr(ws),
+                              out.ctypes.data_as(C.c_void_p), stream_ptr())
+    if rc == _ERR_INVALID:
+        raise ValueError(lib.mgb_last_error().decode("utf-8", "replace"))
+    check(rc, "mgb_eval_iid")
+    scaled = (float(out[3]), float(out[4]), float(out[5])) if up_to_scale else (None, None, None)
+    info = {"n_valid": int(out[0]), **dict(zip(("scale", "quantile", "quantile_scale"), scaled))}
+    return dict(zip(IID_METRIC_NAMES, (float(out[1]), float(out[2])))), info

@@ -1,7 +1,9 @@
 """Time one evaluation call per sample (host clock around the synchronising call, after a warm-up) against the
 reference's path restated on the same GPU: normals = torch CUDA error map, .cpu().numpy(), numpy metrics
 (script/normals/eval.py:145-157); depth = numpy lstsq on the host, torch CUDA metrics with one .item() each
-(script/depth/eval.py:171-217). Prints one JSON line with the card's name and power limit.
+(script/depth/eval.py:171-217); IID = the float32 restatement of compute_iid_metric on the GPU (tests/iid_eval_ref.py:
+torch lstsq, torch.quantile read back with float(), one .item() per metric; the reference repeats the fit and the
+quantile for each metric it computes). Prints one JSON line with the card's name and power limit.
 
     python tools/eval_time.py [--reps 20]
 """
@@ -17,8 +19,8 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from bench import gpu_identity  # noqa: E402
-from marigold_b200.evaluation import evaluate_depth, evaluate_normals  # noqa: E402
-from tests import eval_ref  # noqa: E402
+from marigold_b200.evaluation import evaluate_depth, evaluate_iid, evaluate_normals  # noqa: E402
+from tests import eval_ref, iid_eval_ref  # noqa: E402
 
 
 def _time(fn, reps):
@@ -73,6 +75,9 @@ def main():
         dpred = 0.8 / dgt - 0.05 + 0.01 * torch.randn(H, W, device="cuda", generator=g)
         dmask = torch.rand(H, W, device="cuda", generator=g) > 0.2
         gt_np, pred_np, valid_np = dgt.cpu().numpy(), dpred.cpu().numpy(), dmask.cpu().numpy()
+        igt = torch.rand(3, H, W, device="cuda", generator=g)
+        ipred = (0.6 * igt + 0.05 * torch.randn(3, H, W, device="cuda", generator=g)).abs()
+        imask = (torch.rand(H, W, device="cuda", generator=g) > 0.2).expand(3, H, W).contiguous()
         res["cases"][f"{H}x{W}"] = {
             "normals_device": _time(lambda: evaluate_normals(pred, gt), a.reps),
             "normals_reference_path": _time(ref_normals, a.reps),
@@ -80,6 +85,11 @@ def main():
                                                              min_depth=0.5, max_depth=8.0), a.reps),
             "depth_reference_path_lsd": _time(lambda: _ref_depth(pred_np, gt_np, valid_np, dgt, dmask), a.reps),
         }
+        for target in ("albedo", "shading"):
+            res["cases"][f"{H}x{W}"].update({
+                f"iid_{target}_device": _time(lambda: evaluate_iid(ipred, igt, target, imask), a.reps),
+                f"iid_{target}_reference_path": _time(lambda: iid_eval_ref.evaluate(ipred, igt, target, imask), a.reps),
+            })
     print(json.dumps(res))
 
 
