@@ -288,6 +288,10 @@ int mgb_op_upsample2x_ex(const float* x_dev, void* y_bf16_dev, int32_t NB, int32
  * Transpose: bf16 x[M, N] -> bf16 y[N, ld], columns [M, ld) zero. */
 int mgb_op_softmax_rows(const float* s_dev, void* p_bf16_dev, int32_t M, int32_t n, int32_t ld, void* stream);
 int mgb_op_transpose_bf16(const void* x_bf16_dev, void* y_bf16_dev, int32_t M, int32_t N, int32_t ld, void* stream);
+/* The decoder's input: z = post_quant_conv(latent * inv_scale), a 1x1 conv 4 -> 4 in fp32, written as bf16 NHWC with
+ * 64 channels (4..63 zero). latent_dev fp32 NCHW [NB, 4, HW]; w_dev fp32 [4, 4]; b_dev fp32 [4]; out [NB * HW, 64]. */
+int mgb_op_pack_decoder_latent(const float* latent_dev, const float* w_dev, const float* b_dev, float inv_scale,
+                               void* out_bf16_dev, int32_t NB, int32_t HW, void* stream);
 
 #ifdef __cplusplus
 }

@@ -89,6 +89,7 @@ SIGNATURES = {
     "mgb_op_upsample2x_ex": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "mgb_op_softmax_rows": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "mgb_op_transpose_bf16": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp]),
+    "mgb_op_pack_decoder_latent": (_i32, [_vp, _vp, _vp, _f32, _vp, _i32, _i32, _vp]),
 }
 
 

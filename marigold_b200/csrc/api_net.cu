@@ -723,7 +723,174 @@ int mgb_decode(mgb_handle* h, const float* latent, int32_t B, int32_t lh, int32_
   return run_once(h, stream, OP_DECODE, latent, out, nullptr, nullptr, 0, B, lh, lw, mode);
 }
 
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------------
+// read-back of the handle's device tables (mgb_debug_read): field paths name the structs above in execution order
+// -------------------------------------------------------------------------------------------------
+namespace {
+struct FieldRef {
+  const void* p = nullptr;
+  size_t bytes = 0;
+  bool found = false;
+};
+
+// A dotted field path ("unet.resnets.3.c1.w"), matched one part at a time.
+struct FieldPath {
+  std::vector<std::string> parts;
+  size_t pos = 0;
+  explicit FieldPath(const std::string& s) {
+    for (size_t a = 0;;) {
+      const size_t b = s.find('.', a);
+      parts.push_back(s.substr(a, b == std::string::npos ? std::string::npos : b - a));
+      if (b == std::string::npos) break;
+      a = b + 1;
+    }
+  }
+  bool take(const char* name) {
+    if (pos >= parts.size() || parts[pos] != name) return false;
+    ++pos;
+    return true;
+  }
+  // the next part as a decimal index below n
+  bool index(size_t n, size_t* i) {
+    if (pos >= parts.size()) return false;
+    const std::string& s = parts[pos];
+    if (s.empty() || s.size() > 9 || s.find_first_not_of("0123456789") != std::string::npos) return false;
+    *i = std::stoul(s);
+    if (*i >= n) return false;
+    ++pos;
+    return true;
+  }
+  // The last part is `name`. A weight whose pointer is null does not exist (a bias-free GEMM, a VAE resnet's time
+  // projection); handle state always does, and is empty until it is first set.
+  bool leaf(const char* name, const void* p, size_t bytes, FieldRef* r, bool state = false) {
+    if (pos + 1 != parts.size() || parts[pos] != name) return false;
+    if (p || state) *r = {p, p ? bytes : 0, true};
+    return true;
+  }
+};
+
+void read_norm(FieldPath& f, const NormW& n, FieldRef* r) {
+  f.leaf("g", n.g, size_t(n.c) * 4, r) || f.leaf("b", n.b, size_t(n.c) * 4, r);
+}
+void read_conv(FieldPath& f, const ConvW& c, FieldRef* r) {
+  f.leaf("w", c.w, size_t(c.cout) * (9 * c.cin_pad + c.k_extra) * 2, r) || f.leaf("b", c.b, size_t(c.cout) * 4, r);
+}
+void read_lin(FieldPath& f, const LinW& l, FieldRef* r) {
+  f.leaf("w", l.w, size_t(l.n) * l.k * 2, r) || f.leaf("b", l.b, size_t(l.n) * 4, r);
+}
+void read_resnet(FieldPath& f, const ResnetW& x, int temb_dim, FieldRef* r) {
+  if (f.take("n1")) read_norm(f, x.n1, r);
+  else if (f.take("n2")) read_norm(f, x.n2, r);
+  else if (f.take("c1")) read_conv(f, x.c1, r);
+  else if (f.take("c2")) read_conv(f, x.c2, r);
+  else f.leaf("temb_w", x.temb_w, size_t(x.cout) * temb_dim * 4, r) || f.leaf("temb_b", x.temb_b, size_t(x.cout) * 4, r);
+}
+void read_xfmr(FieldPath& f, const XfmrW& x, int ctx, FieldRef* r) {
+  const size_t C = x.C;
+  if (f.take("gn")) read_norm(f, x.gn, r);
+  else if (f.take("ln1")) read_norm(f, x.ln1, r);
+  else if (f.take("ln2")) read_norm(f, x.ln2, r);
+  else if (f.take("ln3")) read_norm(f, x.ln3, r);
+  else if (f.take("proj_in")) read_lin(f, x.proj_in, r);
+  else if (f.take("qkv")) read_lin(f, x.qkv, r);
+  else if (f.take("o1")) read_lin(f, x.o1, r);
+  else if (f.take("ff1")) read_lin(f, x.ff1, r);
+  else if (f.take("ffpo")) read_lin(f, x.ffpo, r);
+  else f.leaf("q2w", x.q2w, C * C * 4, r) || f.leaf("o2w", x.o2w, C * C * 4, r) || f.leaf("o2b", x.o2b, C * 4, r) ||
+       f.leaf("k2w", x.k2w, C * ctx * 4, r) || f.leaf("v2w", x.v2w, C * ctx * 4, r) ||
+       f.leaf("kv", x.kv, 4 * C * 4, r) || f.leaf("xGU", x.xGU, 2 * (C / 64) * C * 2, r) || f.leaf("xc1", x.xc1, C * 4, r);
+}
+void read_vae_attn(FieldPath& f, const VaeAttnW& a, FieldRef* r) {
+  if (f.take("gn")) read_norm(f, a.gn, r);
+  else if (f.take("q")) read_lin(f, a.q, r);
+  else if (f.take("k")) read_lin(f, a.k, r);
+  else if (f.take("v")) read_lin(f, a.v, r);
+  else if (f.take("o")) read_lin(f, a.o, r);
+}
+template <class T, class Read>
+void read_list(FieldPath& f, const std::vector<T>& v, Read read) {
+  size_t i;
+  if (f.index(v.size(), &i)) read(v[i]);
+}
+
+FieldRef find_field(const mgb_handle* h, const std::string& name) {
+  FieldPath f(name);
+  FieldRef r;
+  auto conv = [&](const ConvW& c) { read_conv(f, c, &r); };
+  auto resnet = [&](const ResnetW& x) { read_resnet(f, x, 0, &r); };
+  if (f.take("unet")) {
+    const UNetW& U = h->unet;
+    const size_t T = U.temb_dim, c0 = h->cfg.unet_block_channels[0];
+    if (f.take("conv_in")) conv(U.conv_in);
+    else if (f.take("conv_out")) conv(U.conv_out);
+    else if (f.take("norm_out")) read_norm(f, U.norm_out, &r);
+    else if (f.take("resnets")) read_list(f, U.resnets, [&](const ResnetW& x) { read_resnet(f, x, U.temb_dim, &r); });
+    else if (f.take("xfmrs")) read_list(f, U.xfmrs, [&](const XfmrW& x) { read_xfmr(f, x, h->cfg.unet_cross_dim, &r); });
+    else if (f.take("downs")) read_list(f, U.downs, conv);
+    else if (f.take("ups")) read_list(f, U.ups, conv);
+    else f.leaf("te_w1", U.te_w1, T * c0 * 4, &r) || f.leaf("te_b1", U.te_b1, T * 4, &r) ||
+         f.leaf("te_w2", U.te_w2, T * T * 4, &r) || f.leaf("te_b2", U.te_b2, T * 4, &r);
+  } else if (f.take("vae")) {
+    const VaeW& V = h->vae;
+    if (f.take("enc_in")) conv(V.enc_in);
+    else if (f.take("enc_out")) conv(V.enc_out);
+    else if (f.take("enc_norm_out")) read_norm(f, V.enc_norm_out, &r);
+    else if (f.take("enc_res")) read_list(f, V.enc_res, resnet);
+    else if (f.take("enc_down")) read_list(f, V.enc_down, conv);
+    else if (f.take("enc_attn")) read_vae_attn(f, V.enc_attn, &r);
+    else if (f.take("dec_in")) conv(V.dec_in);
+    else if (f.take("dec_out")) conv(V.dec_out);
+    else if (f.take("dec_norm_out")) read_norm(f, V.dec_norm_out, &r);
+    else if (f.take("dec_res")) read_list(f, V.dec_res, resnet);
+    else if (f.take("dec_up")) read_list(f, V.dec_up, conv);
+    else if (f.take("dec_attn")) read_vae_attn(f, V.dec_attn, &r);
+    else f.leaf("pq_w", V.pq_w, 16 * 4, &r) || f.leaf("pq_b", V.pq_b, 4 * 4, &r);
+  } else {
+    const size_t n = h->n_steps, total = h->bias_total;
+    f.leaf("bias_table", h->bias_table, n * total * 4, &r, true) || f.leaf("sched_k", h->sched_k, n * 3 * 4, &r, true) ||
+        f.leaf("cur_bias", h->cur_bias, total * 4, &r, true) || f.leaf("cur_sched_k", h->cur_sched_k, 3 * 4, &r, true) ||
+        f.leaf("step_counter", h->step_counter, 4, &r, true);
+  }
+  return r;
+}
+}  // namespace
+
+extern "C" {
+
 /* debug hooks (not in the public header) */
+
+// Copies the device array behind one field (find_field's paths) into dst, when dst is not null, and returns its size in
+// bytes; *dev_addr receives its device address. It copies memory only: no kernel runs and no handle state changes.
+int64_t mgb_debug_read(mgb_handle* h, const char* field, void* dst, int64_t cap_bytes, uint64_t* dev_addr) {
+  if (!h || !field) { set_error("debug_read: null argument"); return MGB_ERR_INVALID; }
+  if (!h->finalized) { set_error("debug_read('%s') before finalize_weights", field); return MGB_ERR_STATE; }
+  const FieldRef r = find_field(h, field);
+  if (!r.found) { set_error("debug_read: unknown field '%s'", field); return MGB_ERR_INVALID; }
+  if (dev_addr) *dev_addr = uint64_t(reinterpret_cast<uintptr_t>(r.p));
+  if (dst && r.bytes) {
+    if (cap_bytes < int64_t(r.bytes)) {
+      set_error("debug_read: field '%s' has %zu bytes, the destination %lld", field, r.bytes, (long long)cap_bytes);
+      return MGB_ERR_INVALID;
+    }
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpy(dst, r.p, r.bytes, cudaMemcpyDeviceToHost));
+  }
+  return int64_t(r.bytes);
+}
+
+// Every device array the weights own (h->weights): addresses and sizes of the first `cap`; returns how many there are.
+int32_t mgb_debug_weight_buffers(mgb_handle* h, uint64_t* addr, int64_t* bytes, int32_t cap) {
+  if (!h) { set_error("debug_weight_buffers: null handle"); return MGB_ERR_INVALID; }
+  if (!h->finalized) { set_error("debug_weight_buffers before finalize_weights"); return MGB_ERR_STATE; }
+  const int32_t n = int32_t(h->weights.size());
+  for (int32_t i = 0; i < n && i < cap; ++i) {
+    if (addr) addr[i] = uint64_t(reinterpret_cast<uintptr_t>(h->weights[i].get()));
+    if (bytes) bytes[i] = int64_t(h->weights[i].bytes());
+  }
+  return n;
+}
 
 size_t mgb_workspace_bytes(mgb_handle* h, int32_t B, int32_t H, int32_t W) {
   if (!h || !h->finalized || B <= 0 || H < 8 || W < 8) return 0;

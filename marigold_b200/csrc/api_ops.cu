@@ -160,6 +160,16 @@ int mgb_op_xattn2(const float* x, void* y, void* a_out, const float* ln2_g, cons
                              reinterpret_cast<cudaStream_t>(stream));
 }
 
+int mgb_op_pack_decoder_latent(const float* latent_dev, const float* w_dev, const float* b_dev, float inv_scale,
+                               void* out_bf16_dev, int32_t NB, int32_t HW, void* stream) {
+  if (!latent_dev || !w_dev || !b_dev || !out_bf16_dev || NB <= 0 || HW <= 0) {
+    set_error("op_pack_decoder_latent: bad argument (NB=%d HW=%d)", NB, HW);
+    return MGB_ERR_INVALID;
+  }
+  return launch_pack_decoder_latent(latent_dev, w_dev, b_dev, inv_scale, reinterpret_cast<bf16*>(out_bf16_dev), NB, HW,
+                                    reinterpret_cast<cudaStream_t>(stream));
+}
+
 /* ---- pre / post-processing and evaluation (image.cu, eval.cu) ---- */
 int mgb_resize(const void* src, int32_t src_is_u8, int32_t NC, int32_t H, int32_t W, float* dst, int32_t h, int32_t w,
                int32_t mode, int32_t post, float* tmp, void* stream) {

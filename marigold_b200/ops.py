@@ -148,6 +148,17 @@ def softmax_rows(s, n):
     return p
 
 
+def pack_decoder_latent(latent, w, b, inv_scale):
+    """fp32 latent NCHW [NB, 4, h, w] -> bf16 [NB * h * w, 64]: post_quant_conv(latent * inv_scale) (w fp32 [4, 4],
+    b fp32 [4]) in channels 0..3, zeros in 4..63."""
+    lib = _lib.load()
+    NB, _, h, w_ = latent.shape
+    z = torch.empty(NB * h * w_, 64, dtype=torch.bfloat16, device=latent.device)
+    check(lib.mgb_op_pack_decoder_latent(ptr(latent), ptr(w), ptr(b), float(inv_scale), ptr(z), NB, h * w_, stream_ptr()),
+          "mgb_op_pack_decoder_latent")
+    return z
+
+
 def transpose_bf16(x, ld):
     """bf16 [M, N] -> bf16 [N, ld], columns [M, ld) zero."""
     lib = _lib.load()

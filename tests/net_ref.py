@@ -22,6 +22,9 @@ state dicts, apply the folds the library applies when it loads them, and round t
             o = bf16(P v); the decoder input is bf16(post_quant_conv(latent * fp32(1 / scale)));
             decode heads: depth (channel mean, clip, (d + 1) / 2), normals (clip, unit length), unit ((clip + 1) / 2), raw.
 
+The folds themselves (ffpo, G / U / c1, the time MLP and the per-step bias, the encoder fold) are the functions of
+tests/weights_ref.py, which holds the device's own tables to them.
+
 Everything else is float64. With `bf16=False` no value is rounded and the folds are exact, so the result is the
 diffusers graph algebra (tests/test_net_ref.py checks it against the fp32 oracle).
 
@@ -39,6 +42,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from tests import weights_ref as WR
 
 LATENT_SCALE = float(np.float32(0.18215))           # mgb_config.latent_scale (fp32)
 INV_LATENT_SCALE = float(np.float32(1.0) / np.float32(0.18215))
@@ -183,12 +188,10 @@ def _xfmr(c, p, x, ctx):
     hs1 = _lin(c, o, t + ".attn1.to_out.0") + hs0
     # cross attention against the two-token context, collapsed: G_h = Wq[h]^T (k0 - k1)_h, U_h = Wo[:, h] (v0 - v1)_h,
     # c1 = Wo v1 + bo
-    nh = C // 64
     kk, vv = ctx @ c.p(t + ".attn2.to_k.weight").t(), ctx @ c.p(t + ".attn2.to_v.weight").t()
-    wq, wo = c.p(t + ".attn2.to_q.weight"), c.p(t + ".attn2.to_out.0.weight")
-    G = c.r(torch.einsum("hdc,hd->hc", wq.reshape(nh, 64, C), (kk[0] - kk[1]).reshape(nh, 64)))
-    U = c.r(torch.einsum("chd,hd->hc", wo.reshape(C, nh, 64), (vv[0] - vv[1]).reshape(nh, 64)))
-    c1 = wo @ vv[1] + c.p(t + ".attn2.to_out.0.bias")
+    G, U, c1 = WR.xattn2_fold(c.p(t + ".attn2.to_q.weight"), c.p(t + ".attn2.to_out.0.weight"),
+                             c.p(t + ".attn2.to_out.0.bias"), kk, vv)
+    G, U = c.r(G), c.r(U)
     z = _ln(c, hs1, t + ".norm2")
     acc = hs1 + c1 + torch.sigmoid(0.125 * (z @ G.t())) @ U
     hsb = c.r(acc)
@@ -197,8 +200,8 @@ def _xfmr(c, p, x, ctx):
     ffm = c.r(pr[..., :4 * C] * _gelu(pr[..., 4 * C:]))
     # ff.net.2 folded into proj_out
     wpo = c.p(p + ".proj_out.weight")
-    fold = c.r((wpo @ c.p(t + ".ff.net.2.weight")).float())
-    bias = c.p(p + ".proj_out.bias") + wpo @ c.p(t + ".ff.net.2.bias")
+    fold = c.r(WR.ffpo_fold(wpo, c.p(t + ".ff.net.2.weight")).float())
+    bias = WR.ffpo_bias(c.p(p + ".proj_out.bias"), wpo, c.p(t + ".ff.net.2.bias"))
     y = hsb @ c.w(p + ".proj_out.weight").t() + ffm @ fold.t() + bias + _tokens(x)
     return _image(y, H, W)
 
@@ -212,14 +215,6 @@ def _vae_attn(c, p, x):
     return x + _image(_lin(c, o, p + ".to_out.0"), H, W)
 
 
-def _timestep_embedding(t, dim):
-    """[cos | sin](t f) with the angle formed in fp32, as the oracle and the device kernel form it."""
-    half = dim // 2
-    f = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=torch.float32) / half)
-    ang = (torch.tensor([float(t)], dtype=torch.float32)[:, None] * f[None, :]).to(torch.float64)
-    return torch.cat([torch.cos(ang), torch.sin(ang)], -1)
-
-
 # ---- graphs -----------------------------------------------------------------------------------------------------------
 @torch.no_grad()
 def unet_step(unet, text, rgb, x, t, kx=1.0, kv=0.0, kz=0.0, noise=None, bf16=True, sd=None):
@@ -231,13 +226,11 @@ def unet_step(unet, text, rgb, x, t, kx=1.0, kv=0.0, kz=0.0, noise=None, bf16=Tr
     ch, L, eps = cfg.block_out_channels, cfg.layers_per_block, cfg.norm_eps
     ctx = text.reshape(-1, text.shape[-1]).to(torch.float64)
     rgb, x = rgb.to(torch.float64), x.to(torch.float64)
-    exact = _Ctx(c.sd, False)                      # the time MLP runs on fp32 weights
-    temb = _timestep_embedding(t, ch[0])
-    temb = _lin(exact, F.silu(_lin(exact, temb, "time_embedding.linear_1")), "time_embedding.linear_2")
-    ste = F.silu(temb)[0]
+    # the time MLP and the per-step bias table run on fp32 weights
+    ste = F.silu(WR.time_mlp(c.p, WR.timestep_embedding([t], ch[0])))[0]
 
     def bias1(p):
-        return c.p(p + ".conv1.bias") + c.p(p + ".time_emb_proj.weight") @ ste + c.p(p + ".time_emb_proj.bias")
+        return WR.step_bias(c.p, p, ste)
 
     h = _conv(c, c.r(torch.cat([rgb, x], 1)), "conv_in")
     skips = [h]
@@ -293,18 +286,10 @@ def encode(vae, rgb, bf16=True, sd=None):
     t_ = c.r(F.silu(_gn(c, h, "encoder.conv_norm_out", 1e-6)))
     # conv_out (C -> 8) then quant_conv (1x1, 8 -> 8), mean half, folded
     sd = c.sd
-    cw, cb = sd["encoder.conv_out.weight"].float(), sd["encoder.conv_out.bias"].to(torch.float64)
-    qw, qb = sd["quant_conv.weight"].float()[:4, :, 0, 0], sd["quant_conv.bias"].to(torch.float64)[:4]
+    w, bias = WR.enc_out_fold(sd["encoder.conv_out.weight"], sd["encoder.conv_out.bias"], sd["quant_conv.weight"],
+                             sd["quant_conv.bias"], LATENT_SCALE, host_fp32=bf16)
     if bf16:
-        w = torch.zeros_like(cw[:4])
-        for j in range(8):
-            w = w + qw[:, j, None, None, None] * cw[j][None]        # fp32, in the host loop's order
-        w = c.r(w)
-    else:
-        w = torch.einsum("oj,jchw->ochw", qw.double(), cw.double())
-    bias = (qb + qw.double() @ cb) * LATENT_SCALE
-    if bf16:
-        bias = bias.float().double()
+        w, bias = c.r(w), bias.float().double()
     return F.conv2d(t_, w, padding=1) * LATENT_SCALE + bias[None, :, None, None]
 
 
