@@ -127,8 +127,8 @@ int mgb_ens_depth_cost(mgb_handle* h, const float* depth_dev, const double* para
 /* That objective and the points of one forward-difference gradient in ONE host sync (scipy approx_derivative as BFGS
  * calls it, ensemble.py:165-171): base_host [n] is the current point, pert_host [n] the same vector with EVERY
  * coordinate moved to its perturbed value x_i + h_i; costs_out_host [1 + n]: [0] = cost(base), [1 + i] = cost(base with
- * coordinate i perturbed), each bit-identical to mgb_ens_depth_cost of that vector. n = 2E (or E when !shift); any E up
- * to mgb_ens_max_members(). */
+ * coordinate i perturbed), each bit-identical to mgb_ens_depth_cost of that vector. n = 2E (or E when !shift); any E
+ * from 1 (no pairs: the regulariser alone) to mgb_ens_max_members(). */
 int mgb_ens_depth_cost_fd(mgb_handle* h, const float* depth_dev, const double* base_host, const double* pert_host,
                           int32_t E, int64_t HW, int32_t scale_invariant, int32_t shift_invariant,
                           int32_t reduction_median, double regularizer, double* costs_out_host, void* stream);

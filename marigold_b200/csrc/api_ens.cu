@@ -45,7 +45,7 @@ static int ens_depth_cost(mgb_handle* h, const float* depth, const double* base,
   int rc = ens_prepare(h);
   if (rc) return rc;
   if (!depth || !base || !costs_out || HW <= 0) { set_error("ens_depth_cost: bad argument"); return MGB_ERR_INVALID; }
-  if (E < 2 || E > ens_max_members()) { set_error("ensemble size %d outside [2,%d]", E, ens_max_members()); return MGB_ERR_UNSUPPORTED; }
+  if (E < 1 || E > ens_max_members()) { set_error("ensemble size %d outside [1,%d]", E, ens_max_members()); return MGB_ERR_UNSUPPORTED; }
   const int n = pert ? (shift_inv ? 2 * E : E) : 0;
   // the staging area is reused by every call: wait for earlier users of this stream (each cost call ends with a
   // synchronisation, so this is only ever non-trivial after an asynchronous reduce)
@@ -55,7 +55,7 @@ static int ens_depth_cost(mgb_handle* h, const float* depth, const double* base,
   if (!rc && pert) rc = make_st(pert, E, scale_inv, shift_inv, st + 2 * E);
   if (rc) return rc;
   // per-pixel order statistics of the base point for the register-resident perturbation pass
-  if (pert && E <= kEnsMaxE) {
+  if (pert && ens_register_resident(E)) {
     rc = h->ens_v3.grow(size_t(HW) * 3 * sizeof(float));
     if (rc) return rc;
   }
@@ -86,7 +86,8 @@ int mgb_ens_minmax(mgb_handle* h, const float* depth, int32_t E, int64_t HW, flo
                    void* stream) {
   int rc = ens_prepare(h);
   if (rc) return rc;
-  if (!depth || !min_host || !max_host || E < 1 || E > ens_max_members() || HW <= 0) { set_error("ens_minmax: bad argument"); return MGB_ERR_INVALID; }
+  if (!depth || !min_host || !max_host || HW <= 0) { set_error("ens_minmax: bad argument"); return MGB_ERR_INVALID; }
+  if (E < 1 || E > ens_max_members()) { set_error("ensemble size %d outside [1,%d]", E, ens_max_members()); return MGB_ERR_UNSUPPORTED; }
   int blocks = 0;
   CUDA_TRY(cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(stream)));
   float* hp = pinned_st(h) + size_t(ens_max_batch()) * 2 * ens_max_members();
@@ -107,7 +108,7 @@ int mgb_ens_depth_reduce(mgb_handle* h, const float* depth, const double* param,
   int rc = ens_prepare(h);
   if (rc) return rc;
   if (!depth || !param || !pred || HW <= 0) { set_error("ens_depth_reduce: bad argument"); return MGB_ERR_INVALID; }
-  if (E < 2 || E > ens_max_members()) { set_error("ensemble size %d outside [2,%d]", E, ens_max_members()); return MGB_ERR_UNSUPPORTED; }
+  if (E < 1 || E > ens_max_members()) { set_error("ensemble size %d outside [1,%d]", E, ens_max_members()); return MGB_ERR_UNSUPPORTED; }
   CUDA_TRY(cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(stream)));  // previous user of the staging area
   float* st_pinned = pinned_st(h);
   rc = make_st(param, E, scale_inv, shift_inv, st_pinned);

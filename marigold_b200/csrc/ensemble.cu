@@ -425,10 +425,10 @@ static int dispatch_members(int E, F&& f) {
 
 int launch_ens_depth_cost(const float* depth, float* st_host, int n, int E, long long HW, int shift, int median,
                           double reg, void* ws, float* v3, double* out_host_pinned, cudaStream_t stream) {
-  if (E < 2 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [2, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
+  if (E < 1 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [1, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
   const int P = 1 + n;
   int rows = n > 0 ? 2 : 1;
-  if (E > kEnsMaxE && n > 0) {
+  if (!ens_register_resident(E) && n > 0) {
     // the generic kernels evaluate whole points: row 1 + i = the base with coordinate i moved (each coordinate was
     // converted to float on its own, so these are the rows of the moved double vectors)
     float moved[2 * kEnsDynMaxE];
@@ -458,11 +458,12 @@ int launch_ens_depth_cost(const float* depth, float* st_host, int n, int E, long
       return launch_plain("ens cost", ens_cost_final_kernel, P, 256, 0, stream, base_part, pert_part, blocks, E, HW, reg,
                           out);
     } else {
-      const int NP = E * (E - 1) / 2, chunks = (NP + kDynPairs - 1) / kDynPairs;
+      // one member (no pairs: the objective is the regulariser alone) still takes one z-slice for the min / max
+      const int NP = E * (E - 1) / 2, chunks = std::max(1, (NP + kDynPairs - 1) / kDynPairs);
       const int blocks = int(std::min<long long>((HW + kEnsThreads - 1) / kEnsThreads, kDynBlocks));
       double* pair_part = reinterpret_cast<double*>(ws);
       float* mm_part = reinterpret_cast<float*>(static_cast<char*>(ws) + kDynPartialBytes);
-      const int p_max = std::max<int>(1, int(kDynPartialBytes / (size_t(NP) * blocks * sizeof(double))));
+      const int p_max = std::max<int>(1, int(kDynPartialBytes / (size_t(std::max(NP, 1)) * blocks * sizeof(double))));
       for (int p0 = 0; p0 < P; p0 += p_max) {
         const int pn = std::min(p_max, P - p0);
         TRY(launch_plain("ens cost", ens_cost_dyn_kernel, dim3(blocks, pn, chunks), kEnsThreads, 0, stream, depth,
@@ -598,7 +599,7 @@ __global__ void __launch_bounds__(kEnsThreads)
 
 int launch_ens_depth_reduce(const float* depth, const float* st_host, int E, long long HW, int shift, int median,
                             int use_min, float* pred, float* unc, int* idx, void* ws, cudaStream_t stream) {
-  if (E < 2 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [2, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
+  if (E < 1 || E > kEnsDynMaxE) { set_error("ensemble size %d outside [1, %d]", E, kEnsDynMaxE); return MGB_ERR_UNSUPPORTED; }
   float* st = ens_ws_st(ws);
   float* bmm = reinterpret_cast<float*>(ws);  // reuse the partial area for block min/max
   cudaError_t e = cudaMemcpyAsync(st, st_host, sizeof(float) * 2 * E, cudaMemcpyHostToDevice, stream);

@@ -223,6 +223,8 @@ const float* lpips_features(const void* ws, int H, int W, int l, int dims[3]);
 // Ensemble kernels (ensemble.cu)
 // ---------------------------------------------------------------------------------------------
 constexpr int kEnsMaxE = 16;   // largest ensemble the register-resident (templated) kernels take; larger: generic kernels
+// sizes 2..kEnsMaxE run the register-resident kernels; one member (no pairs) and E > kEnsMaxE the generic ones
+constexpr bool ens_register_resident(int E) { return E >= 2 && E <= kEnsMaxE; }
 size_t ens_ws_bytes();
 int ens_max_batch();     // points per launch_ens_depth_cost call (1 + 2 ens_max_members())
 int ens_max_members();   // largest supported ensemble size
