@@ -155,10 +155,13 @@ int mgb_ens_iid(mgb_handle* h, const float* targets_dev, int32_t E, int64_t N, i
 /* ---- pre / post-processing bookends and the evaluation step ------------------------------------ */
 /* torchvision resize(antialias=True) as resize_max_res calls it (marigold/util/image_util.py:90-120) and for the final
  * prediction (marigold_depth_pipeline.py:306-312). src_dev [NC,H,W] uint8 (src_is_u8) or fp32 -> dst_dev fp32 [NC,h,w].
- * mode 0 bilinear, 1 bicubic (both antialiased), 2 nearest-exact. post 0: none; 1: round + clamp to [0,255] (a uint8
- * image stays uint8-valued); 2: that, then x / 255 * 2 - 1 (marigold_depth_pipeline.py:252). tmp_dev: NC*H*w floats. */
-int mgb_resize(const void* src_dev, int32_t src_is_u8, int32_t NC, int32_t H, int32_t W, float* dst_dev, int32_t h, int32_t w,
-               int32_t mode, int32_t post, float* tmp_dev, void* stream);
+ * mode 0 bilinear, 1 bicubic (both antialiased), 2 nearest-exact. arith selects whose arithmetic the antialiased modes
+ * reproduce bit for bit (tap windows, weights and accumulation): 0 torch's CPU kernel (the reference resizes the image
+ * on the host), 1 torch's CUDA kernel (the reference resizes the prediction on the device).
+ * post 0: none; 1: clamp to [0,255] and round half to even (a uint8 image stays uint8-valued); 2: that, then x / 255 * 2 - 1 with a true division
+ * (marigold_depth_pipeline.py:252 on the host); 3: x / 255 * 2 - 1 alone (a float image). tmp_dev: NC*H*w floats. */
+int mgb_resize_ex(const void* src_dev, int32_t src_is_u8, int32_t NC, int32_t H, int32_t W, float* dst_dev, int32_t h,
+                  int32_t w, int32_t mode, int32_t arith, int32_t post, float* tmp_dev, void* stream);
 /* colorize_depth_maps + chw2hwc + uint8 (image_util.py:38-76, marigold_depth_pipeline.py:326-331): depth_dev fp32 [HW] ->
  * out_hwc_dev uint8 [HW,3]; lut_dev uint8 [256,3] = the colour map's 256-entry table * 255, truncated. */
 int mgb_colorize(const float* depth_dev, int64_t HW, float dmin, float dmax, const uint8_t* lut_dev, uint8_t* out_hwc_dev,

@@ -61,7 +61,7 @@ SIGNATURES = {
     "mgb_ens_depth_reduce": (_i32, [_vp, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "mgb_ens_iid": (_i32, [_vp, _vp, _i32, _i64, _i32, _vp, _vp, _vp]),
     "mgb_ens_normals": (_i32, [_vp, _vp, _i32, _i64, _i32, _vp, _vp, _vp, _vp]),
-    "mgb_resize": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "mgb_resize_ex": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "mgb_colorize": (_i32, [_vp, _i64, _f32, _f32, _vp, _vp, _vp]),
     "mgb_eval_ws_bytes": (C.c_size_t, []),
     "mgb_eval_depth": (_i32, [_vp, _vp, _vp, _i64, _i32, _f32, _f32, _vp, _vp, _vp, _vp]),

@@ -171,10 +171,10 @@ int mgb_op_pack_decoder_latent(const float* latent_dev, const float* w_dev, cons
 }
 
 /* ---- pre / post-processing and evaluation (image.cu, eval.cu) ---- */
-int mgb_resize(const void* src, int32_t src_is_u8, int32_t NC, int32_t H, int32_t W, float* dst, int32_t h, int32_t w,
-               int32_t mode, int32_t post, float* tmp, void* stream) {
-  if (!src || !dst || !tmp) { set_error("mgb_resize: null pointer"); return MGB_ERR_INVALID; }
-  return launch_resize(src, src_is_u8, NC, H, W, dst, h, w, mode, post, tmp, reinterpret_cast<cudaStream_t>(stream));
+int mgb_resize_ex(const void* src, int32_t src_is_u8, int32_t NC, int32_t H, int32_t W, float* dst, int32_t h, int32_t w,
+                  int32_t mode, int32_t arith, int32_t post, float* tmp, void* stream) {
+  if (!src || !dst || !tmp) { set_error("mgb_resize_ex: null pointer"); return MGB_ERR_INVALID; }
+  return launch_resize(src, src_is_u8, NC, H, W, dst, h, w, mode, arith, post, tmp, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_colorize(const float* depth, int64_t HW, float dmin, float dmax, const uint8_t* lut, uint8_t* out_hwc, void* stream) {

@@ -169,9 +169,9 @@ int launch_transpose_bf16(const bf16* x, bf16* y, int M, int N, int ld, cudaStre
 // Pre / post-processing bookends (image.cu) and the evaluation step (eval.cu)
 // ---------------------------------------------------------------------------------------------
 // src [NC, H, W] (u8 or f32) -> dst f32 [NC, h, w]; tmp: NC * H * w floats. mode 0 bilinear-aa, 1 bicubic-aa, 2 nearest-exact;
-// post 0 none, 1 round + clamp to [0, 255], 2 that and then x / 255 * 2 - 1
-int launch_resize(const void* src, int src_is_u8, int NC, int H, int W, float* dst, int h, int w, int mode, int post, float* tmp,
-                  cudaStream_t stream);
+// arith 0 torch CPU, 1 torch CUDA; post 0 none, 1 clamp to [0, 255] + round, 2 that and then x / 255 * 2 - 1, 3 x / 255 * 2 - 1
+int launch_resize(const void* src, int src_is_u8, int NC, int H, int W, float* dst, int h, int w, int mode, int arith,
+                  int post, float* tmp, cudaStream_t stream);
 int launch_colorize(const float* depth, long long HW, float dmin, float dmax, const uint8_t* lut, uint8_t* out,
                     cudaStream_t stream);
 size_t eval_ws_bytes();

@@ -14,16 +14,21 @@ from . import _lib
 from ._lib import check, ptr, stream_ptr
 
 _MODES = {"bilinear": 0, "bicubic": 1, "nearest-exact": 2}
+_ARITH = {"cpu": 0, "cuda": 1}
 _lut_cache = {}
 
 
-def resize(img: torch.Tensor, size, mode: str, post: int = 0) -> torch.Tensor:
-    """img [N,C,H,W] uint8 or float (CUDA) -> float32 [N,C,h,w]. post: 0 none; 1 round + clamp to [0,255] (what a uint8
-    image becomes); 2 that, then x / 255 * 2 - 1."""
+def resize(img: torch.Tensor, size, mode: str, post: int = 0, arith: str = "cuda") -> torch.Tensor:
+    """img [N,C,H,W] uint8 or float (CUDA) -> float32 [N,C,h,w]. post: 0 none; 1 clamp to [0,255] and round half to even
+    (what a uint8 image becomes); 2 that, then x / 255 * 2 - 1; 3 x / 255 * 2 - 1 alone. arith: whose arithmetic the
+    antialiased modes reproduce bit for bit in their tap windows and weights, torch's "cpu" kernel (an image the
+    reference resizes on the host) or its "cuda" kernel (a prediction the reference resizes on the device)."""
     if not img.is_cuda:
         raise _lib.MgbError("marigold_b200.imageops.resize needs a CUDA tensor (no CPU fallback)")
     if mode not in _MODES:
         raise ValueError(f"Unknown resampling method: {mode}")
+    if arith not in _ARITH:
+        raise ValueError(f"Unknown resize arithmetic: {arith}")
     lib = _lib.load()
     N, Cc, H, W = img.shape
     h, w = int(size[0]), int(size[1])
@@ -32,8 +37,8 @@ def resize(img: torch.Tensor, size, mode: str, post: int = 0) -> torch.Tensor:
     with torch.cuda.device(img.device):
         dst = torch.empty(N, Cc, h, w, dtype=torch.float32, device=img.device)
         tmp = torch.empty(N * Cc * H * w, dtype=torch.float32, device=img.device)
-        check(lib.mgb_resize(ptr(src), int(is_u8), N * Cc, H, W, ptr(dst), h, w, _MODES[mode], int(post), ptr(tmp),
-                             stream_ptr()), "mgb_resize")
+        check(lib.mgb_resize_ex(ptr(src), int(is_u8), N * Cc, H, W, ptr(dst), h, w, _MODES[mode], _ARITH[arith],
+                                int(post), ptr(tmp), stream_ptr()), "mgb_resize_ex")
     return dst
 
 

@@ -56,14 +56,15 @@ def get_tv_resample_method(method_str: str) -> str:
     return m
 
 
-def _resize(img: torch.Tensor, size, mode: str) -> torch.Tensor:
+def _resize(img: torch.Tensor, size, mode: str, arith: str = "cuda") -> torch.Tensor:
     """torchvision.transforms.functional.resize(img, size, interpolation, antialias=True) semantics. CUDA tensors (the
-    pipelines' path) go through the library's own kernels (csrc/image.cu); CPU tensors (host-side helpers in the tests)
-    through torch."""
+    pipelines' path) go through the library's own kernels (csrc/image.cu) in the rounding of torch's `arith` kernel:
+    "cuda" for predictions, which the reference resizes on the device, "cpu" for images, which it resizes on the host.
+    CPU tensors (host-side helpers in the tests) go through torch."""
     if img.is_cuda:
         from . import imageops
 
-        out = imageops.resize(img, size, mode, post=1 if img.dtype == torch.uint8 else 0)
+        out = imageops.resize(img, size, mode, post=1 if img.dtype == torch.uint8 else 0, arith=arith)
         return out.to(img.dtype)
     if mode == "nearest-exact":
         return F.interpolate(img.float(), size=size, mode=mode).to(img.dtype)
@@ -78,7 +79,7 @@ def resize_max_res(img: torch.Tensor, max_edge_resolution: int, resample_method:
     assert 4 == img.dim(), f"Invalid input shape {img.shape}"
     h, w = img.shape[-2:]
     f = min(max_edge_resolution / w, max_edge_resolution / h)
-    return _resize(img, (int(h * f), int(w * f)), resample_method)
+    return _resize(img, (int(h * f), int(w * f)), resample_method, arith="cpu")     # the reference's image is on the host
 
 
 # matplotlib's "Spectral" is the linear interpolation of ColorBrewer's 11-class Spectral palette.
@@ -184,19 +185,31 @@ class _MarigoldBase:
             raise TypeError(f"Unknown input type: {type(input_image) = }")
         input_size = rgb.shape
         assert 4 == rgb.dim() and 3 == input_size[-3], f"Wrong input shape {input_size}, expected [1, rgb, H, W]"
+        # The reference resizes (image_util.py:90-120) and normalises (:252-254) the tensor where it lives: a host image
+        # (PIL, or a CPU tensor) with torch CPU's resize and a true division, a CUDA tensor with torch CUDA's resize and
+        # its division by a scalar, which multiplies by the reciprocal (1 ulp off for 111 of the 256 byte values).
+        on_device = rgb.is_cuda
         rgb = rgb.to(self.device)
-        if processing_res > 0 and rgb.dtype == torch.uint8:
-            # resize_max_res (image_util.py:90-120) with the uint8 rounding and the [-1, 1] normalisation (:252-254) fused
-            # into the second pass of the device resize
-            from . import imageops
+        from . import imageops
 
-            h0, w0 = rgb.shape[-2:]
+        h0, w0 = rgb.shape[-2:]
+        if processing_res > 0:
             f = min(processing_res / w0, processing_res / h0)
-            rgb_norm = imageops.resize(rgb, (int(h0 * f), int(w0 * f)), resample_method, post=2).to(self.dtype)
+            size, mode = (int(h0 * f), int(w0 * f)), resample_method
         else:
+            size, mode = (h0, w0), "nearest-exact"
+        if not on_device and rgb.dtype in (torch.uint8, torch.float32):
+            # both fused into the resize's second pass; at native resolution the resize is the identity (nearest-exact
+            # at the same size copies every value). uint8 is rounded back to uint8 first, float32 is used as it is.
+            post = 2 if rgb.dtype == torch.uint8 else 3
+            rgb_norm = imageops.resize(rgb, size, get_tv_resample_method(mode), post=post, arith="cpu").to(self.dtype)
+        else:
+            # a CUDA tensor, or a float dtype other than float32, which the reference normalises in its own dtype
             if processing_res > 0:
-                rgb = resize_max_res(rgb, max_edge_resolution=processing_res, resample_method=resample_method)
-            rgb_norm = (rgb / 255.0 * 2.0 - 1.0).to(self.dtype)
+                rgb = _resize(rgb, size, get_tv_resample_method(mode), arith="cuda" if on_device else "cpu")
+            if not on_device:
+                rgb = rgb.cpu()
+            rgb_norm = (rgb / 255.0 * 2.0 - 1.0).to(self.device, self.dtype)
         assert rgb_norm.min() >= -1.0 and rgb_norm.max() <= 1.0
         return rgb_norm, input_size
 
