@@ -169,7 +169,8 @@ int mgb_colorize(const float* depth_dev, int64_t HW, float dmin, float dmax, con
 /* Least-squares scale / shift alignment to the ground truth over the valid pixels (src/util/alignment.py:35-82), the
  * clips of script/depth/eval.py:201-207 and the masked depth metrics of src/util/metric.py:64-191 in two passes and ONE
  * synchronisation. mask_dev uint8 [HW] or NULL; aligned_out_dev fp32 [HW] or NULL; ws_dev: mgb_eval_ws_bytes() bytes.
- * out_host[13] = {scale, shift, n_valid, abs_rel, sq_rel, rmse, rmse_log, log10, delta1, delta2, delta3, i_rmse, silog}. */
+ * out_host[13] = {scale, shift, n_valid, abs_rel, sq_rel, rmse, rmse_log, log10, delta1, delta2, delta3, i_rmse, silog}.
+ * NaN metrics when n_valid == 0; scale = shift = 0 when the fit has no pixel (np.linalg.lstsq of no rows). */
 size_t mgb_eval_ws_bytes(void);
 int mgb_eval_depth(const float* pred_dev, const float* gt_dev, const uint8_t* mask_dev, int64_t HW, int32_t least_squares,
                    float dmin, float dmax, float* aligned_out_dev, void* ws_dev, double* out_host, void* stream);

@@ -2,12 +2,13 @@
 // scale / shift alignment of a prediction to the ground truth over the valid pixels (reference
 // src/util/alignment.py:35-82) and the masked depth metrics (src/util/metric.py:64-191) in two streaming passes and ONE
 // host synchronisation per sample (the reference does a numpy lstsq on the host and one `.item()` per metric).
-//   pass 1  sums n, sum p, sum p^2, sum g, sum p g over the fit's pixels (double) -> scale, shift from the 2 x 2 normal
-//           equations. The fit is against gt, or against 1 / gt for least_square_disparity, over all pixels or over the
+//   pass 1  sums n, sum d, sum d^2, sum g, sum d g over the fit's pixels (double, d = p - a pivot) -> scale, shift from the
+//           2 x 2 normal equations, with lstsq's rank rule. The fit is against gt, or against 1 / gt for least_square_disparity, over all pixels or over the
 //           nearest-downsampled map of max_resolution (index tables)
 //   pass 2  aligned = p * scale + shift; for disparity 1 / max(aligned, 1e-3); then clip(clip(., dmin, dmax), 1e-6)
-//           (script/depth/eval.py:196-207) and the sums of every metric over the full-resolution mask; a last block turns
-//           them into the metric values.
+//           (script/depth/eval.py:196-207) and the sums of every metric over the full-resolution mask (double), the delta
+//           counts from the same steps in the reference's float32; a last block turns them into the metric values, NaN
+//           when no pixel is valid.
 // HBM-bound: 9 bytes / pixel / pass (pred f32, gt f32, mask u8).
 // The surface-normals evaluation (below) computes the angular error and the normals metrics with an exact median.
 #include <cfloat>
@@ -40,26 +41,48 @@ __device__ __forceinline__ void block_reduce_store(double (&v)[kEvSums], int n, 
   }
 }
 
+// Moves sums taken about a pivot c to the pivot c - delta (d' = d + delta): v = {n, sum d, sum d^2, sum g, sum d g}.
+__device__ __forceinline__ void repivot(double* v, double delta) {
+  v[2] += 2.0 * delta * v[1] + v[0] * delta * delta;
+  v[1] += v[0] * delta;
+  v[4] += delta * v[3];
+}
+
 // The fit's pixels: the full map (rows == nullptr), or the nearest-downsampled map of fit_h x fit_w pixels whose source row
 // and column are rows[i], cols[j] (align_depth_least_square's max_resolution, alignment.py:48-59). disparity: fit against
 // 1 / gt over valid & gt > 0 & pred > 0 (script/depth/eval.py:180-195; depth2disparity is fp32, alignment.py:85-94).
+// The sums over the prediction are CENTRED: d = p - c about a pivot c that is itself a fit pixel's prediction, so that
+// n sum d^2 - (sum d)^2 loses (mean - c)^2 / var instead of mean^2 / var, and is exactly 0 for a constant prediction.
+// Differences of float32 values are exact in double. Each thread pivots on its first fit pixel, the block on its lowest
+// thread that holds one (part[5]), the solve on the lowest such block: every choice is a function of the input alone.
 __global__ void __launch_bounds__(kEvThreads)
     eval_align_sums_kernel(const float* __restrict__ pred, const float* __restrict__ gt, const uint8_t* __restrict__ mask,
                            long long n_fit, long long W, const int* __restrict__ rows, const int* __restrict__ cols, int fit_w,
                            int disparity, double* __restrict__ part) {
+  __shared__ int sh_first;
+  __shared__ double sh_c;
+  if (threadIdx.x == 0) { sh_first = kEvThreads; sh_c = 0.0; }
   double v[kEvSums] = {0};
+  double c = 0.0;
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n_fit; q += (long long)gridDim.x * blockDim.x) {
     const long long p = rows ? (long long)rows[q / fit_w] * W + cols[q % fit_w] : q;
     if (mask && !mask[p]) continue;
     const float pf = pred[p], gf = gt[p];
     if (disparity && !(gf > 0.f && pf > 0.f)) continue;
-    const double a = pf, g = disparity ? __fdiv_rn(1.0f, gf) : gf;
+    if (v[0] == 0.0) c = pf;
+    const double a = double(pf) - c, g = disparity ? __fdiv_rn(1.0f, gf) : gf;
     v[0] += 1.0; v[1] += a; v[2] += a * a; v[3] += g; v[4] += a * g;
   }
+  __syncthreads();
+  if (v[0] > 0.0) atomicMin(&sh_first, int(threadIdx.x));
+  __syncthreads();
+  if (int(threadIdx.x) == sh_first) sh_c = c;
+  __syncthreads();
+  if (v[0] > 0.0) repivot(v, c - sh_c);
   block_reduce_store(v, 5, part);
+  if (threadIdx.x == 0) part[(size_t)blockIdx.x * kEvSums + 5] = sh_c;
 }
 
-// scale, shift of min || [p 1] [s t]^T - g ||^2 over the valid pixels (np.linalg.lstsq in alignment.py:66-69)
 // Sum of quantity k over the blocks' partials by one warp: lane l takes blocks l, l + 32, ... (independent loads), xor tree.
 // (A single thread would walk blocks x 12 dependent loads.)
 __device__ __forceinline__ double warp_sum_partials(const double* __restrict__ part, int nblocks, int k) {
@@ -70,21 +93,47 @@ __device__ __forceinline__ double warp_sum_partials(const double* __restrict__ p
   return t;
 }
 
+// scale, shift of min || [p 1] [s t]^T - g ||^2 over the fit's pixels (np.linalg.lstsq(rcond=None) in alignment.py:66-69),
+// from the blocks' centred sums moved to one pivot. lstsq drops the singular values of [p 1] at or below
+// eps * max(n, 2) * sigma_max and returns the minimum-norm solution: the same rank rule is applied here to the
+// eigenvalues of the 2 x 2 Gram matrix (sigma^2), whose determinant n sum d^2 - (sum d)^2 does not depend on the pivot.
 __global__ void eval_align_solve_kernel(const double* __restrict__ part, int nblocks, int do_align, double* __restrict__ st) {
-  double s[5];
-  for (int k = 0; k < 5; ++k) s[k] = warp_sum_partials(part, nblocks, k);
+  const int lane = threadIdx.x & 31;
+  int first = nblocks;
+  for (int b = lane; b < nblocks; b += 32)
+    if (part[(size_t)b * kEvSums] > 0.0) { first = b; break; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+  const double c = first < nblocks ? part[(size_t)first * kEvSums + 5] : 0.0;
+  double s[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int b = lane; b < nblocks; b += 32) {
+    double v[5];
+    for (int k = 0; k < 5; ++k) v[k] = part[(size_t)b * kEvSums + k];
+    if (v[0] > 0.0) repivot(v, part[(size_t)b * kEvSums + 5] - c);
+    for (int k = 0; k < 5; ++k) s[k] += v[k];
+  }
+  for (int k = 0; k < 5; ++k)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
   if (threadIdx.x != 0) return;
-  double scale = 1.0, shift = 0.0;
-  if (do_align) {
-    const double n = s[0], sp = s[1], spp = s[2], sg = s[3], spg = s[4];
-    const double det = n * spp - sp * sp;
-    if (n > 0 && fabs(det) > 1e-300) {
-      scale = (n * spg - sp * sg) / det;
-      shift = (spp * sg - sp * spg) / det;
-    } else if (n > 0) {               // constant prediction: lstsq's minimum-norm solution of the rank-1 system
-      const double m = sp / n, gm = sg / n;
-      scale = gm * m / (m * m + 1.0);
-      shift = gm / (m * m + 1.0);
+  double scale = do_align ? 0.0 : 1.0, shift = 0.0;     // a fit over no pixel: lstsq's minimum-norm solution is 0, 0
+  if (do_align && s[0] > 0.0) {
+    const double n = s[0], sd = s[1], sdd = s[2], sg = s[3], sdg = s[4];
+    const double det = n * sdd - sd * sd;
+    const double tr = sdd + 2.0 * c * sd + n * c * c + n;            // sum p^2 + n
+    const double lmax = 0.5 * (tr + sqrt(fmax(tr * tr - 4.0 * det, 0.0)));
+    const double cut = DBL_EPSILON * fmax(n, 2.0) * lmax;            // sigma_min <= rcond sigma_max <=> det <= cut^2
+    if (det > cut * cut) {
+      scale = (n * sdg - sd * sg) / det;
+      shift = (sg - scale * sd) / n - scale * c;
+    } else {     // (nearly) constant prediction: lstsq keeps sigma_max only, x = v (v^T A^T g) / (|v|^2 lambda_max), with
+                 // v the Gram matrix's top eigenvector from whichever of its two rows gives the longer one
+      const double sp = sd + n * c, spp = tr - n, spg = sdg + c * sg;
+      const bool by_first = n >= spp;
+      const double v0 = by_first ? sp : lmax - n, v1 = by_first ? lmax - spp : sp;
+      const double k = (v0 * spg + v1 * sg) / ((v0 * v0 + v1 * v1) * lmax);
+      scale = v0 * k;
+      shift = v1 * k;
     }
   }
   st[0] = scale; st[1] = shift; st[2] = s[0];
@@ -94,21 +143,30 @@ __global__ void __launch_bounds__(kEvThreads)
     eval_metric_sums_kernel(const float* __restrict__ pred, const float* __restrict__ gt, const uint8_t* __restrict__ mask,
                             long long HW, const double* __restrict__ st, int disparity, float dmin, float dmax,
                             float* __restrict__ aligned_out, double* __restrict__ part) {
-  // numpy: float32 pred * float64 scale + float64 shift is float64, and torch promotes the float64 prediction against the
-  // float32 ground truth (script/depth/eval.py:177-213), so the reference's metric arithmetic is double: so is this
+  // The sums are taken in double from the double fit: closer to the exact value than the reference, whose arithmetic is
+  // float32 throughout (np.linalg.lstsq on float32 maps returns a float32 scale and shift, so pred * scale + shift, the
+  // clips, the reciprocal and every torch metric are float32; script/depth/eval.py:177-213). The delta accuracies are
+  // counts decided by a comparison, so they follow the reference's float32 operations one by one, un-fused.
   const double scale = st[0], shift = st[1];
+  const float s32 = float(scale), t32 = float(shift);
   double v[kEvSums] = {0};
+  int d1 = 0, d2 = 0, d3 = 0;
   for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += (long long)gridDim.x * blockDim.x) {
-    double a = double(pred[p]) * scale + shift;
+    const float pf = pred[p];
+    double a = double(pf) * scale + shift;
     if (disparity) a = 1.0 / fmax(a, 1e-3);              // clip the disparity to >= 1e-3, back to depth (eval.py:196-200)
     a = fmin(fmax(a, double(dmin)), double(dmax));
     a = fmax(a, 1e-6);
     if (aligned_out) aligned_out[p] = float(a);
     if (mask && !mask[p]) continue;
-    const double g = double(gt[p]);
+    const float gf = gt[p];
+    float af = __fadd_rn(__fmul_rn(pf, s32), t32);
+    if (disparity) af = __fdiv_rn(1.0f, fmaxf(af, 1e-3f));
+    af = fmaxf(fminf(fmaxf(af, dmin), dmax), 1e-6f);
+    const float r = fmaxf(__fdiv_rn(af, gf), __fdiv_rn(gf, af));     // threshold_percentage, metric.py:131-145
+    const double g = double(gf);
     const double diff = a - g;
     const double dl = log(a) - log(g);
-    const double r = fmax(a / g, g / a);
     const double di = 1.0 / a - 1.0 / g;
     v[0] += 1.0;
     v[1] += fabs(diff) / g;                               // abs_relative_difference
@@ -117,11 +175,10 @@ __global__ void __launch_bounds__(kEvThreads)
     v[4] += dl * dl;                                      // rmse_log / silog first term
     v[5] += dl;                                           // silog second term
     v[6] += fabs(log10(a) - log10(g));                    // log10
-    v[7] += r < 1.25 ? 1.0 : 0.0;                         // delta1
-    v[8] += r < 1.25 * 1.25 ? 1.0 : 0.0;                  // delta2
-    v[9] += r < 1.25 * 1.25 * 1.25 ? 1.0 : 0.0;           // delta3
+    d1 += r < 1.25f; d2 += r < 1.5625f; d3 += r < 1.953125f;   // delta1..3: 1.25^2 and 1.25^3 are exact in float32
     v[10] += di * di;                                     // i_rmse
   }
+  v[7] = d1; v[8] = d2; v[9] = d3;
   block_reduce_store(v, 11, part);
 }
 
@@ -130,7 +187,7 @@ __global__ void eval_metric_final_kernel(const double* __restrict__ part, int nb
   double s[kEvSums] = {0};
   for (int k = 0; k < 11; ++k) s[k] = warp_sum_partials(part, nblocks, k);
   if (threadIdx.x != 0) return;
-  const double n = s[0] > 0 ? s[0] : 1.0;
+  const double n = s[0];                                 // no valid pixel: 0 / 0, NaN, as the reference's torch sums give
   out[0] = st[0]; out[1] = st[1]; out[2] = s[0];
   out[3] = s[1] / n;                                     // abs_relative_difference
   out[4] = s[2] / n;                                     // squared_relative_difference
@@ -140,7 +197,7 @@ __global__ void eval_metric_final_kernel(const double* __restrict__ part, int nb
   out[8] = s[7] / n; out[9] = s[8] / n; out[10] = s[9] / n;   // delta1..3
   out[11] = sqrt(s[10] / n);                             // i_rmse
   const double t = s[4] / n - (s[5] * s[5]) / (n * n);
-  out[12] = sqrt(t > 0 ? t : 0.0) * 100.0;               // silog_rmse
+  out[12] = sqrt(t < 0 ? 0.0 : t) * 100.0;               // silog_rmse (NaN stays NaN)
 }
 
 size_t eval_ws_bytes() { return size_t(kEvBlocks) * kEvSums * sizeof(double) + 16 * sizeof(double) + 64; }

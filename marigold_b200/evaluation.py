@@ -102,17 +102,12 @@ def _run_ex(pred, gt, mask, mode: int, max_resolution, dmin: float, dmax: float)
 
 def align_depth_least_square(gt: torch.Tensor, pred: torch.Tensor, valid_mask: Optional[torch.Tensor],
                              return_scale_shift: bool = True, max_resolution: Optional[int] = None):
-    """src/util/alignment.py:35-82 on the device: (aligned_pred, scale, shift). `max_resolution` downsamples the three
-    maps with the reference's nearest Upsample before the fit; the fitted map is always the full-resolution prediction."""
-    fit_p, fit_g, fit_m = pred, gt, valid_mask
-    if max_resolution is not None:
-        sf = float(np.min(max_resolution / np.array(pred.shape[-2:])))
-        if sf < 1:
-            down = torch.nn.Upsample(scale_factor=sf, mode="nearest")
-            fit_g = down(gt.reshape(1, 1, *gt.shape[-2:]).float())
-            fit_p = down(pred.reshape(1, 1, *pred.shape[-2:]).float())
-            fit_m = down(valid_mask.reshape(1, 1, *valid_mask.shape[-2:]).float()).bool() if valid_mask is not None else None
-    out, _ = _run(fit_p, fit_g, fit_m, True, -3.0e38, 3.0e38, False)      # only the fit is used from this call
+    """src/util/alignment.py:35-82 on the device: (aligned_pred, scale, shift). `max_resolution` fits the pixels the
+    reference's nearest Upsample keeps (fit_index_tables: its [1, H, W] input downsamples the width only), as
+    evaluate_depth(alignment_max_res=...) does; the fitted map is always the full-resolution prediction."""
+    H, W = pred.shape[-2:]
+    out = _run_ex(pred.reshape(H, W), gt.reshape(H, W), None if valid_mask is None else valid_mask.reshape(H, W), 1,
+                  max_resolution, -3.0e38, 3.0e38)                          # only the fit is used from this call
     scale, shift = out[0], out[1]
     aligned = pred.to(torch.float64) * scale + shift
     return (aligned, scale, shift) if return_scale_shift else aligned
@@ -126,7 +121,9 @@ def evaluate_depth(pred: torch.Tensor, gt: torch.Tensor, valid_mask: Optional[to
     alignment: None, "least_square" (fit pred to gt) or "least_square_disparity" (fit pred to 1 / gt over the valid
     pixels where gt > 0 and pred > 0, clip the aligned disparity to >= 1e-3 and take its reciprocal). The metrics always
     use `valid_mask`. alignment_max_res: fit on the maps downsampled as align_depth_least_square(max_resolution=...)
-    downsamples them (see fit_index_tables); the metrics use the full-resolution maps.
+    downsamples them (see fit_index_tables); the metrics use the full-resolution maps. The sums are taken in double;
+    the delta accuracies count the reference's float32 decisions. With no valid pixel every metric is NaN (n_valid 0),
+    as the reference's 0 / 0 gives; a fit over no pixel gives scale 0, shift 0, as np.linalg.lstsq does.
     Returns (metrics by the reference's function names, {"scale", "shift", "n_valid"})."""
     if alignment not in ALIGNMENTS:
         raise ValueError(f"unsupported alignment {alignment!r}; expected one of {ALIGNMENTS}")

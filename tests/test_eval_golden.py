@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from tests import eval_ref
-from tests.golden.eval_cases import DEPTH_EVAL_CASES, DEPTH_EVAL_RANGE, NORMALS_EVAL_CASES, depth_eval_input, normals_eval_input
+from tests.golden.eval_cases import DEPTH_EVAL_RANGE, DEPTH_EVAL_SMOOTH_CASES, NORMALS_EVAL_CASES, depth_eval_input, normals_eval_input
 
 GOLD = np.load(Path(__file__).resolve().parent / "golden" / "eval_golden.npz")
 
@@ -24,9 +24,10 @@ def test_normals_restatement_reproduces_reference(name):
         assert got[k] == float(GOLD[f"normals/{name}/{k}"]), (k, got[k], float(GOLD[f"normals/{name}/{k}"]))
 
 
-@pytest.mark.parametrize("name", list(DEPTH_EVAL_CASES))
+# the other recorded depth cases (dataset ranges, degenerate fits, planted thresholds): tests/test_depth_eval_ref.py
+@pytest.mark.parametrize("name", list(DEPTH_EVAL_SMOOTH_CASES))
 def test_depth_restatement_reproduces_reference(name):
-    cfg = DEPTH_EVAL_CASES[name]
+    cfg = DEPTH_EVAL_SMOOTH_CASES[name]
     pred, gt, valid = depth_eval_input(cfg)
     got, scale, shift = eval_ref.depth_eval(pred, gt, valid, cfg["alignment"], cfg["max_res"], *DEPTH_EVAL_RANGE)
     assert scale == float(GOLD[f"depth/{name}/scale"]) and shift == float(GOLD[f"depth/{name}/shift"])

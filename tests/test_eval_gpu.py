@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from tests import eval_ref
-from tests.golden.eval_cases import DEPTH_EVAL_CASES, DEPTH_EVAL_RANGE, NORMALS_EVAL_CASES, depth_eval_input, normals_eval_input
+from tests.golden.eval_cases import DEPTH_EVAL_CASES, DEPTH_EVAL_RANGE, DEPTH_EVAL_SMOOTH_CASES, NORMALS_EVAL_CASES, depth_eval_input, normals_eval_input
 
 pytestmark = pytest.mark.gpu
 GOLD = np.load(Path(__file__).resolve().parent / "golden" / "eval_golden.npz")
@@ -186,7 +186,8 @@ def _depth_case(cfg):
     return pred, gt, valid, (torch.from_numpy(pred).cuda(), torch.from_numpy(gt).cuda(), torch.from_numpy(valid).cuda())
 
 
-@pytest.mark.parametrize("name", list(DEPTH_EVAL_CASES))
+# the smooth scene at DEPTH_EVAL_RANGE; the dataset-shaped, degenerate and planted cases are test_depth_eval_gpu.py's
+@pytest.mark.parametrize("name", list(DEPTH_EVAL_SMOOTH_CASES))
 def test_depth_alignment_modes_match_reference(name):
     from marigold_b200 import _lib
     from marigold_b200.evaluation import evaluate_depth

@@ -67,7 +67,7 @@ def _ref_eval(pred, gt, mask, dmin, dmax, align):
         A = np.concatenate([p[mask].reshape(-1, 1), np.ones((int(mask.sum()), 1), np.float32)], axis=-1)
         X = np.linalg.lstsq(A, gt[mask].reshape(-1, 1), rcond=None)[0]
         scale, shift = float(X[0, 0]), float(X[1, 0])
-        p = p * X[0] + X[1]                                             # float32 * float64 -> float64, as in the reference
+        p = p * X[0] + X[1]                                             # lstsq returns float32: float32 throughout, as the reference
     p = np.clip(np.clip(p, dmin, dmax), 1e-6, None)
     o, t, m = torch.from_numpy(p), torch.from_numpy(gt), torch.from_numpy(mask)
     n = m.sum()
