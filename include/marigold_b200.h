@@ -93,7 +93,9 @@ int mgb_set_schedule(mgb_handle* h, int32_t n, const int32_t* timesteps, const f
 /* ---- the hot path --------------------------------------------------------------------------- */
 /* encode_rgb: vae.encoder + quant_conv, mean half, * latent_scale  (…pipeline.py:479-496).
  * rgb_dev [B,3,H,W] in [-1,1]; latent_dev [B,4,H/8,W/8] (floor). Any H, W >= 8: like the reference, sizes that are not
- * multiples of 8 lose the remainder rows / columns in the VAE's stride-2 convs. */
+ * multiples of 8 lose the remainder rows / columns in the VAE's stride-2 convs.
+ * Supported maximum (this call and mgb_decode): B * H * W <= 2^26 pixels (one 8192 x 8192 image); larger batches return
+ * MGB_ERR_UNSUPPORTED before anything is allocated or launched. */
 int mgb_encode(mgb_handle* h, const float* rgb_dev, int32_t B, int32_t H, int32_t W, float* latent_dev,
                void* stream);
 /* One denoising iteration i: cat -> unet -> scheduler.step (…pipeline.py:456-468).
@@ -113,7 +115,8 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent_dev, float* target_
 /* decode_depth / decode_normals + the clip / shift / normalise that follow
  * (…depth_pipeline.py:498-516,473-475; …normals_pipeline.py:463-479,438-440).
  * out_dev: DEPTH [B,1,H,W] in [0,1]; NORMALS [B,3,H,W] unit vectors; RAW3 [B,3,H,W]; UNIT3 [B,3,H,W] = (clip(x,-1,1)+1)/2
- * (one IID target, marigold_iid_pipeline.py:562-565,578-585: the caller loops over the targets' 4-channel slices). */
+ * (one IID target, marigold_iid_pipeline.py:562-565,578-585: the caller loops over the targets' 4-channel slices).
+ * B * 8 lh * 8 lw output pixels within the supported maximum of mgb_encode. */
 int mgb_decode(mgb_handle* h, const float* latent_dev, int32_t B, int32_t lh, int32_t lw, int32_t mode,
                float* out_dev, void* stream);
 
@@ -234,8 +237,12 @@ int mgb_eval_iid_lpips(const float* pred_dev, const float* gt_dev, const uint8_t
                        void* stream);
 
 /* ---- capacity ------------------------------------------------------------------------------- */
-/* Bytes of the activation arena the handle holds for images of H x W with B members per batch. */
+/* Bytes of the activation arena the handle holds for images of H x W with B members per batch; 0 beyond the supported
+ * maximum of mgb_encode / mgb_decode. */
 size_t mgb_workspace_bytes(mgb_handle* h, int32_t B, int32_t H, int32_t W);
+/* Bytes of device workspace the handle holds now (activation arena, split-K and barrier scratch); a call that needs more
+ * frees it before allocating the larger size. */
+size_t mgb_workspace_held_bytes(mgb_handle* h);
 /* Number of kernel launches enqueued by this library since creation (for bench.py gpu_launches). Memsets and copies
    are not counted; a replay of a captured CUDA graph counts the kernels the graph holds. */
 int64_t mgb_launch_count(void);

@@ -76,6 +76,7 @@ SIGNATURES = {
     "mgb_lpips_ws_bytes": (C.c_size_t, [_i32, _i32]),
     "mgb_eval_iid_lpips": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "mgb_workspace_bytes": (C.c_size_t, [_vp, _i32, _i32, _i32]),
+    "mgb_workspace_held_bytes": (C.c_size_t, [_vp]),
     "mgb_launch_count": (_i64, []),
     "mgb_op_linear": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "mgb_op_conv2d": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32,

@@ -566,6 +566,7 @@ struct WorkspaceNeed { size_t arena = 0, splitk = 0, sync = 0; };   // bytes
 static int workspace_need(mgb_handle* h, int op, int NB, int d0, int d1, WorkspaceNeed* need) {
   Arena dry; dry.dry = true;
   Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
+  c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
   TRY(run_graph(h, c, op, nullptr, nullptr, nullptr, nullptr, 0, NB, d0, d1, 0));
   *need = {dry.peak, c.splitk_need, c.sync_need * sizeof(unsigned)};
   return MGB_OK;
@@ -589,6 +590,15 @@ static int check_ready(mgb_handle* h, bool need_sched) {
   return MGB_OK;
 }
 
+// B images of H x W pixels (a decode's output size) within kMaxPixels, checked before anything is sized or launched
+static int check_pixels(const char* what, int B, int H, int W) {
+  if (size_t(B) * size_t(H) * size_t(W) > kMaxPixels) {
+    set_error("%s: %d x %d x %d pixels exceed the supported maximum of %zu per call", what, B, H, W, kMaxPixels);
+    return MGB_ERR_UNSUPPORTED;
+  }
+  return MGB_OK;
+}
+
 static Ctx make_ctx(mgb_handle* h, void* stream) {
   Ctx c;
   c.stream = reinterpret_cast<cudaStream_t>(stream);
@@ -598,6 +608,7 @@ static Ctx make_ctx(mgb_handle* h, void* stream) {
   c.dry = false;
   c.splitk_ws = h->splitk_ws; c.splitk_cap = h->splitk_ws.bytes();
   c.groups = h->cfg.norm_groups;
+  c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
   c.sync_base = h->sync_slab;
   c.sync_cap = h->sync_slab.bytes() / sizeof(unsigned);
   return c;
@@ -619,6 +630,7 @@ int mgb_encode(mgb_handle* h, const float* rgb, int32_t B, int32_t H, int32_t W,
     set_error("mgb_encode: need B > 0 and H, W >= 8 (got %d x %d)", H, W);
     return MGB_ERR_INVALID;
   }
+  TRY(check_pixels("mgb_encode", B, H, W));
   return run_once(h, stream, OP_ENCODE, rgb, latent, nullptr, nullptr, 0, B, H, W, 0);
 }
 
@@ -720,6 +732,7 @@ int mgb_decode(mgb_handle* h, const float* latent, int32_t B, int32_t lh, int32_
     set_error("mgb_decode: bad argument (latent %d x %d, mode %d)", lh, lw, mode);
     return MGB_ERR_INVALID;
   }
+  TRY(check_pixels("mgb_decode", B, 8 * lh, 8 * lw));
   return run_once(h, stream, OP_DECODE, latent, out, nullptr, nullptr, 0, B, lh, lw, mode);
 }
 
@@ -892,8 +905,22 @@ int32_t mgb_debug_weight_buffers(mgb_handle* h, uint64_t* addr, int64_t* bytes, 
   return n;
 }
 
+// VAE mid-block attention row blocking of this handle: sets its workspace budget (budget_bytes <= 0: the library's,
+// kVaeAttnBudget) and forced rows per block (force_rows <= 0: none), then reports the rows per block (*rows) and the
+// blocks over all NB images (*blocks) that an (NB, T)-token attention of the VAE's width runs with.
+int mgb_debug_vae_attn_blocks(mgb_handle* h, int64_t budget_bytes, int32_t force_rows, int32_t NB, int32_t T,
+                              int32_t* rows, int32_t* blocks) {
+  if (!h || NB <= 0 || T <= 0) { set_error("debug_vae_attn_blocks: bad argument"); return MGB_ERR_INVALID; }
+  h->vae_attn_budget = budget_bytes > 0 ? size_t(budget_bytes) : kVaeAttnBudget;
+  h->vae_attn_force_rows = force_rows > 0 ? force_rows : 0;
+  const int R = vae_attn_rows(T, h->cfg.vae_block_channels[3], h->vae_attn_budget, h->vae_attn_force_rows);
+  if (rows) *rows = R;
+  if (blocks) *blocks = NB * ((T + R - 1) / R);
+  return MGB_OK;
+}
+
 size_t mgb_workspace_bytes(mgb_handle* h, int32_t B, int32_t H, int32_t W) {
-  if (!h || !h->finalized || B <= 0 || H < 8 || W < 8) return 0;
+  if (!h || !h->finalized || B <= 0 || H < 8 || W < 8 || size_t(B) * size_t(H) * size_t(W) > kMaxPixels) return 0;
   size_t peak = 0;
   for (int op = 0; op < 3; ++op) {
     const int d0 = op == OP_ENCODE ? H : H / 8, d1 = op == OP_ENCODE ? W : W / 8;
@@ -902,6 +929,11 @@ size_t mgb_workspace_bytes(mgb_handle* h, int32_t B, int32_t H, int32_t W) {
     peak = std::max(peak, need.arena + need.splitk);
   }
   return peak;
+}
+
+size_t mgb_workspace_held_bytes(mgb_handle* h) {
+  if (!h) return 0;
+  return h->arena_buf.bytes() + h->splitk_ws.bytes() + h->sync_slab.bytes();
 }
 
 }  // extern "C"

@@ -72,14 +72,25 @@ static int gemm_common(Ctx& c, GemmParams& p, int bn, int splits, const Epi& e, 
   return run_gemm(p, bn, c.splitk_ws, c.stream);
 }
 
+struct Tile { int bn, sp, st; };
+
+// the tile of an M-row linear over W: choose_tile's, or GEGLU's fixed one
+static Tile linear_tile(int M, const LinW& W, int flags) {
+  Tile t;
+  choose_tile((M + 127) / 128, W.n, W.k / 64, flags, true, &t.bn, &t.sp, &t.st);
+  if (flags & EPI_GEGLU) t = {256, 1, (W.k / 64 <= 12) ? 2 : 4};
+  return t;
+}
+
 // y = a[M,K] W^T (+ epilogue); ldo = row stride of the outputs (0: W.n, or W.n / 2 for GEGLU)
+// tile (or null: linear_tile's): a block of rows of a larger problem passes that problem's tile, so that its rows come
+// out bit for bit as they do in the whole (the K split and the epilogue path depend on the tile, never on the row)
 static int linear(Ctx& c, const bf16* a, int M, const LinW& W, const Epi& e, int ldo = 0, const bf16* a2 = nullptr,
-                  int K1 = 0) {
+                  int K1 = 0, const Tile* tile = nullptr) {
   // a2 != nullptr: K concatenation, A = [a (K1 columns) | a2 (W.k - K1 columns)]
-  int bn, sp, st;
   const bool geglu = (e.flags & EPI_GEGLU) != 0;
-  choose_tile((M + 127) / 128, W.n, W.k / 64, e.flags, true, &bn, &sp, &st);
-  if (geglu) { bn = 256; sp = 1; st = (W.k / 64 <= 12) ? 2 : 4; }
+  const Tile t = tile ? *tile : linear_tile(M, W, e.flags);
+  const int bn = t.bn, sp = t.sp, st = t.st;
   if (sp > 1) c.splitk_need = std::max(c.splitk_need, size_t(sp) * M * W.n * sizeof(float));
   if (c.dry) return MGB_OK;
   GemmParams p;
@@ -89,12 +100,17 @@ static int linear(Ctx& c, const bf16* a, int M, const LinW& W, const Epi& e, int
 }
 
 // generic A[M,K] x B[N,K]^T with raw pointers (attention score / PV GEMMs in the VAE)
-static int matmul_nt(Ctx& c, const bf16* a, const bf16* b, int M, int N, int K, const Epi& e, int ldo = 0) {
+static int matmul_nt(Ctx& c, const bf16* a, const bf16* b, int M, int N, int K, const Epi& e, int ldo,
+                     const Tile& tile) {
   LinW W; W.w = const_cast<bf16*>(b); W.n = N; W.k = K;
   // B is an activation written by an earlier kernel of this stream (K, or V^T straight out of the transpose): the
   // GEMM's pre-wait B prefetch must not run ahead of its producer, so no programmatic early launch here.
   PlainLaunchScope no_early_launch;
-  return linear(c, a, M, W, e, ldo);
+  return linear(c, a, M, W, e, ldo, nullptr, 0, &tile);
+}
+static Tile matmul_tile(int M, int N, int K, int flags) {
+  LinW W; W.n = N; W.k = K;
+  return linear_tile(M, W, flags);
 }
 
 // 3x3 conv on NHWC bf16; Hout x Wout output; kind per ops.cu
@@ -222,19 +238,37 @@ static int xfmr_forward(Ctx& c, const XfmrW& X, Act& x, Act& y, int NB, int T) {
 // VAE mid-block attention: single head, dim C (512), over T = h*w tokens. x, y fp32 [NB*T, C].
 // Per image: fp32 scores S = Q K^T / sqrt(C) (T x Tp, Tp = T rounded up to 64), fp32 row softmax -> bf16 P with the
 // pad columns zeroed, O = P V through V^T [C, Tp] (pad zeroed): any T works, and the logits are never rounded to bf16.
+// The queries of an image are taken in blocks of R rows (vae_attn_rows), so S and P take R x Tp, not T x Tp. Both GEMMs
+// run every block with the tile of the whole T-row problem: each row is the same kernel's same arithmetic whatever R
+// is, and the softmax is row-local, so the output is bit-identical to one block. R = T is exactly the unblocked launch
+// sequence.
 // ---------------------------------------------------------------------------------------------
+int vae_attn_rows(int T, int C, size_t budget, int force_rows) {
+  if (force_rows > 0) return std::min(force_rows, T);
+  const int Tp = (T + 63) / 64 * 64;
+  const size_t row_bytes = size_t(Tp) * (sizeof(float) + sizeof(bf16));
+  if (size_t(T) * row_bytes <= budget) return T;
+  const Tile pv = matmul_tile(T, C, Tp, 0);
+  const int ctas_per_128_rows = (C + pv.bn - 1) / pv.bn * pv.sp;
+  const int wave_rows = (kNumSMs + ctas_per_128_rows - 1) / ctas_per_128_rows * 128;
+  const int budget_rows = int(std::min(budget / row_bytes, size_t(T))) / 128 * 128;
+  return std::min(T, std::max(budget_rows, wave_rows));
+}
+
 static int vae_attn_forward(Ctx& c, const VaeAttnW& A, Act& x, Act& y, int NB, int T) {
   const int C = A.C;
   const size_t M = size_t(NB) * T;
   const int Tp = (T + 63) / 64 * 64;
+  const int R = vae_attn_rows(T, C, c.attn_budget, c.attn_rows);
+  const Tile tile_s = matmul_tile(T, T, C, EPI_SCALE), tile_pv = matmul_tile(T, C, Tp, 0);
   const size_t mk = c.arena->mark();
   bf16* a = aalloc<bf16>(c, M * C);
   bf16* q = aalloc<bf16>(c, M * C);
   bf16* k = aalloc<bf16>(c, M * C);
   bf16* v = aalloc<bf16>(c, M * C);
   bf16* vt = aalloc<bf16>(c, size_t(C) * Tp);
-  float* s = aalloc<float>(c, size_t(T) * Tp);
-  bf16* pr = aalloc<bf16>(c, size_t(T) * Tp);
+  float* s = aalloc<float>(c, size_t(R) * Tp);
+  bf16* pr = aalloc<bf16>(c, size_t(R) * Tp);
   bf16* o = aalloc<bf16>(c, M * C);
   TRY(groupnorm(c, x, nullptr, a, nullptr, A.gn, NB, T, 1e-6f, 0));
   { Epi e; e.bias = A.q.b; e.out_bf16 = q; TRY(linear(c, a, int(M), A.q, e)); }
@@ -243,10 +277,14 @@ static int vae_attn_forward(Ctx& c, const VaeAttnW& A, Act& x, Act& y, int NB, i
   const float scale = 1.0f / sqrtf(float(C));
   for (int n = 0; n < NB; ++n) {
     const size_t off = size_t(n) * T * C;
-    { Epi e; e.out_f32 = s; e.flags = EPI_SCALE; e.scale = scale; TRY(matmul_nt(c, q + off, k + off, T, T, C, e, Tp)); }
-    LAUNCH(launch_softmax_rows(s, pr, T, T, Tp, c.stream));
-    LAUNCH(launch_transpose_bf16(v + off, vt, T, C, Tp, c.stream));
-    { Epi e; e.out_bf16 = o + off; TRY(matmul_nt(c, pr, vt, T, C, Tp, e)); }
+    for (int r0 = 0; r0 < T; r0 += R) {
+      const int rows = std::min(R, T - r0);
+      const size_t qo = off + size_t(r0) * C;
+      { Epi e; e.out_f32 = s; e.flags = EPI_SCALE; e.scale = scale; TRY(matmul_nt(c, q + qo, k + off, rows, T, C, e, Tp, tile_s)); }
+      LAUNCH(launch_softmax_rows(s, pr, rows, T, Tp, c.stream));
+      if (r0 == 0) LAUNCH(launch_transpose_bf16(v + off, vt, T, C, Tp, c.stream));
+      { Epi e; e.out_bf16 = o + qo; TRY(matmul_nt(c, pr, vt, rows, C, Tp, e, 0, tile_pv)); }
+    }
   }
   { Epi e; e.bias = A.o.b; e.residual = x.p; e.out_f32 = y.p; TRY(linear(c, o, int(M), A.o, e)); }
   c.arena->release(mk);
@@ -465,6 +503,11 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
   }
   for (int i = 0; i < 4; ++i) {
     const int cout = ch[3 - i];
+    // the next level's input is placed below this level's buffers, which are given back once it is written: at 12 MP
+    // the full-resolution level would otherwise sit on ~15 GB of dead lower-level and upsampling buffers
+    Act next;
+    if (i < 3) next = act_alloc(c, M * 4, cout);
+    const size_t mk = c.arena->mark();
     Act buf[2] = {act_alloc(c, M, cout), act_alloc(c, M, cout)};
     for (int j = 0; j < L + 1; ++j) {
       Act y = buf[j & 1];
@@ -475,9 +518,9 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
       bf16* up = aalloc<bf16>(c, M * 4 * cur);
       LAUNCH(launch_upsample2x(h.p, up, NB, H, W, cur, 2 * H, 2 * W, c.stream));
       H *= 2; W *= 2; M = size_t(NB) * H * W;
-      Act y = act_alloc(c, M, cur);
-      { Epi e; e.bias = V.dec_up[i].b; e.out_f32 = y.p; TRY(conv3x3(c, up, NB, H, W, V.dec_up[i], 0, e)); }
-      h = y;
+      { Epi e; e.bias = V.dec_up[i].b; e.out_f32 = next.p; TRY(conv3x3(c, up, NB, H, W, V.dec_up[i], 0, e)); }
+      h = next;
+      c.arena->release(mk);
     }
   }
   bf16* t = aalloc<bf16>(c, M * cur);

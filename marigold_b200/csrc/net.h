@@ -85,10 +85,27 @@ struct Act {
   int C = 0;
 };
 
+// Largest image batch one encode / decode call accepts: NB * H * W output pixels (e.g. one 8192 x 8192 image, or
+// one 12 MP photo and four more). Below it every 32-bit count of the VAE graph (pixels, GEMM rows, per-row sizes,
+// grid dimensions) stays in range; element counts and offsets are 64-bit.
+constexpr size_t kMaxPixels = size_t(1) << 26;
+
+// Workspace target of the VAE mid-block attention's score rows: fp32 S + bf16 P, 6 bytes per logit. An image whose
+// whole T x Tp score matrix fits runs as one block (every size up to 1024 x 1024 does); above it the query rows are
+// processed in blocks (vae_attn_rows).
+constexpr size_t kVaeAttnBudget = size_t(2) << 30;
+
+// Query rows per block of the VAE mid-block attention over T tokens of width C: T when T * Tp * 6 bytes fit `budget`;
+// else the largest multiple of 128 that fits, raised where needed so that each block's P V GEMM still fills one wave
+// of the SMs. force_rows > 0 overrides the choice (tests).
+int vae_attn_rows(int T, int C, size_t budget, int force_rows);
+
 struct Ctx {
   cudaStream_t stream = nullptr;
   Arena* arena = nullptr;
   bool dry = false;
+  size_t attn_budget = kVaeAttnBudget;  // vae_attn_rows' budget and forced rows (mgb_handle's, see there)
+  int attn_rows = 0;
   float* splitk_ws = nullptr;
   size_t splitk_cap = 0;   // bytes available
   size_t splitk_need = 0;  // bytes needed (dry run)
@@ -138,6 +155,9 @@ struct mgb_handle {
   mgb::Arena arena;                 // view of arena_buf, refreshed by each call that runs a graph
   mgb::DevBuf<float> splitk_ws;
   mgb::DevBuf<unsigned> sync_slab;  // GroupNorm grid-barrier counters of one forward
+  // VAE mid-block attention row blocking: the library's budget unless a test overrides it (mgb_debug_vae_attn_blocks)
+  size_t vae_attn_budget = mgb::kVaeAttnBudget;
+  int vae_attn_force_rows = 0;
   // conditioning / schedule
   bool text_set = false;
   int n_steps = 0;

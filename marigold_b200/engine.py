@@ -164,4 +164,9 @@ class Engine:
         return out
 
     def workspace_bytes(self, B, H, W) -> int:
+        """Device workspace a batch of B members at H x W pixels needs; 0 beyond the supported maximum."""
         return int(self.lib.mgb_workspace_bytes(self._h, B, H, W))
+
+    def held_bytes(self) -> int:
+        """Device workspace the engine holds now (given back before it grows)."""
+        return int(self.lib.mgb_workspace_held_bytes(self._h))

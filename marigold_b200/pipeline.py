@@ -139,6 +139,43 @@ def find_batch_size(ensemble_size: int, input_res: int, dtype: torch.dtype) -> i
     return max(1, min(ensemble_size, 16 if input_res <= 768 else 8))
 
 
+MAX_PIXELS = 1 << 26                 # kMaxPixels (csrc/net.h): members x height x width of one encode / decode call
+
+
+def select_batch_size(engine, n_members: int, h: int, w: int, batch_size: int = 0,
+                      free_bytes: Optional[int] = None) -> int:
+    """Members per batch for n_members at h x w. batch_size > 0 is taken as given; 0 takes find_batch_size's value,
+    lowered to the largest batch whose workspace (engine.workspace_bytes) fits the memory available to the engine: free
+    device memory (`free_bytes`, or the device's) plus the workspace the engine holds, which it gives back before it
+    grows. A batch that cannot fit, explicit or of one member, raises ValueError before any inference work is spent."""
+    if free_bytes is None:
+        free_bytes = torch.cuda.mem_get_info(engine.device)[0]
+    avail = int(free_bytes) + engine.held_bytes()
+    explicit = batch_size > 0
+    bs = min(batch_size, max(n_members, 1)) if explicit else find_batch_size(n_members, max(h, w), torch.float32)
+    while True:
+        need = engine.workspace_bytes(bs, h, w)
+        if 0 < need <= avail:
+            return bs
+        if need == 0 and bs * h * w <= MAX_PIXELS:
+            return bs                    # a shape the engine refuses for another reason, with its own error
+        if explicit or bs == 1:
+            break
+        bs -= 1
+    what = f"a batch of {bs} member{'s' if bs > 1 else ''} at {h} x {w}"
+    if need == 0:
+        raise ValueError(f"{what} exceeds the engine's supported maximum of {MAX_PIXELS} pixels per call")
+    raise ValueError(f"{what} needs {need} bytes of device workspace, but {avail} bytes are available")
+
+
+def _processing_size(h0: int, w0: int, processing_res: int):
+    """(h, w) of the image the pipelines process: resize_max_res's, or the input's own at processing_res = 0."""
+    if processing_res > 0:
+        f = min(processing_res / w0, processing_res / h0)
+        return int(h0 * f), int(w0 * f)
+    return int(h0), int(w0)
+
+
 class _MarigoldBase:
     latent_scale_factor = 0.18215  # depth_pipeline.py:118
 
@@ -192,12 +229,8 @@ class _MarigoldBase:
         rgb = rgb.to(self.device)
         from . import imageops
 
-        h0, w0 = rgb.shape[-2:]
-        if processing_res > 0:
-            f = min(processing_res / w0, processing_res / h0)
-            size, mode = (int(h0 * f), int(w0 * f)), resample_method
-        else:
-            size, mode = (h0, w0), "nearest-exact"
+        size = _processing_size(*rgb.shape[-2:], processing_res)
+        mode = resample_method if processing_res > 0 else "nearest-exact"
         if not on_device and rgb.dtype in (torch.uint8, torch.float32):
             # both fused into the resize's second pass; at native resolution the resize is the identity (nearest-exact
             # at the same size copies every value). uint8 is rounded back to uint8 first, float32 is used as it is.
@@ -212,6 +245,21 @@ class _MarigoldBase:
             rgb_norm = (rgb / 255.0 * 2.0 - 1.0).to(self.device, self.dtype)
         assert rgb_norm.min() >= -1.0 and rgb_norm.max() <= 1.0
         return rgb_norm, input_size
+
+    def _member_batch_size(self, input_image, processing_res, ensemble_size, batch_size):
+        """select_batch_size for this call, from the input's shape alone: an input that cannot run is refused before
+        anything is allocated on the device or launched."""
+        if Image is not None and isinstance(input_image, Image.Image):
+            w0, h0 = input_image.size
+        elif isinstance(input_image, torch.Tensor) and input_image.dim() == 4:
+            h0, w0 = input_image.shape[-2:]
+        else:
+            return batch_size                                # _preprocess rejects it
+        from . import parallel
+
+        rank, G = parallel.world()
+        n = len(parallel.member_indices(ensemble_size, rank, G))
+        return select_batch_size(self.engine, n, *_processing_size(h0, w0, processing_res), batch_size)
 
     def _draw_noise(self, shape, generator, noise):
         if noise is not None:
@@ -233,13 +281,14 @@ class _MarigoldBase:
         one all-gather of the decoded maps (parallel.py); the result is identical on every rank."""
         from . import parallel
 
+        rank, G = parallel.world()
+        mine = parallel.member_indices(ensemble_size, rank, G)
+        _bs = batch_size if batch_size > 0 else select_batch_size(self.engine, len(mine), *rgb_norm.shape[-2:])
         self._set_schedule(denoising_steps)
         rgb_latent1 = self.encode_rgb(rgb_norm)                      # [1,4,h,w]
         lh, lw = rgb_latent1.shape[-2:]
         is_lcm = isinstance(self.scheduler, LCMScheduler)
         need_sn = is_lcm and denoising_steps > 1
-        rank, G = parallel.world()
-        mine = parallel.member_indices(ensemble_size, rank, G)
         ct = self.engine.cfg.unet_out_channels               # 4, or 4 n for an n-target IID model
         if G > 1:
             # every rank draws (or receives) the FULL noise tensors and takes its rows, so member k's noise
@@ -249,7 +298,6 @@ class _MarigoldBase:
                 dev = generator.device if generator is not None else self.device
                 step_noise = torch.randn((denoising_steps - 1, ensemble_size, ct, lh, lw), device=dev, dtype=self.dtype,
                                          generator=generator)
-        _bs = batch_size if batch_size > 0 else find_batch_size(len(mine), max(rgb_norm.shape[1:]), self.dtype)
         preds = []
         for s in range(0, len(mine), _bs):
             ids = mine[s:s + _bs]
@@ -327,6 +375,7 @@ class MarigoldDepthPipeline(_MarigoldBase):
         _check_ensemble_size(self.engine, ensemble_size)          # fail before any inference work is spent
         self._check_inference_step(denoising_steps)
         resample = get_tv_resample_method(resample_method)
+        batch_size = self._member_batch_size(input_image, processing_res, ensemble_size, batch_size)
         rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
 
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
@@ -388,6 +437,7 @@ class MarigoldNormalsPipeline(_MarigoldBase):
         assert ensemble_size >= 1
         self._check_inference_step(denoising_steps)
         resample = get_tv_resample_method(resample_method)
+        batch_size = self._member_batch_size(input_image, processing_res, ensemble_size, batch_size)
         rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
                                            None, _lib_decode_normals)
@@ -457,6 +507,7 @@ class MarigoldIIDPipeline(_MarigoldBase):
         assert ensemble_size >= 1
         self._check_inference_step(denoising_steps)
         resample = get_tv_resample_method(resample_method)
+        batch_size = self._member_batch_size(input_image, processing_res, ensemble_size, batch_size)
         rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
                                            None, _lib_decode_iid)

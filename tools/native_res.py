@@ -1,0 +1,163 @@
+"""Native-resolution inference (processing_res = 0) on synthetic 12-megapixel photos, SD-size random weights: per run the
+stage times from CUDA events (encode, denoise, decode, ensemble: summed over the member batches), mgb_workspace_bytes,
+the member batch select_batch_size chose, and the VAE attention's rows per block and block count; the card's name and
+power limit, read in the same run. Then 24 MP (6048 x 4032): its numbers, or the error with the bytes it needed. Then
+a 1920 x 1080 decode with the VAE attention in one block against its default row blocks, alternated.
+
+    python tools/native_res.py [--out DIR]      (prints one JSON line; with --out also writes DIR/native_res.json)
+"""
+import argparse
+import ctypes as C
+import json
+import sys
+from pathlib import Path
+
+sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
+import torch  # noqa: E402
+
+from bench import gpu_identity  # noqa: E402
+from marigold_b200.ensemble import ensemble_depth, ensemble_iid, ensemble_normals  # noqa: E402
+from marigold_b200.pipeline import select_batch_size  # noqa: E402
+from marigold_b200.schedulers import DDIMScheduler  # noqa: E402
+from tests.helpers import synthetic_image  # noqa: E402
+
+
+def attn_blocks(eng, NB, T, budget=0):
+    f = eng.lib.mgb_debug_vae_attn_blocks        # debug hook outside the public header
+    f.restype = C.c_int32
+    f.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    r, b = C.c_int32(), C.c_int32()
+    assert f(eng._h, budget, 0, NB, T, C.byref(r), C.byref(b)) == 0
+    return r.value, b.value
+
+
+def make_engine(n_targets=1, seed=0):
+    from marigold_b200.engine import Engine, EngineConfig
+    from oracle.unet import UNet2DConditionOracle, UNetConfig
+    from oracle.vae import AutoencoderKLOracle, VAEConfig
+
+    torch.manual_seed(seed)
+    ucfg = UNetConfig()
+    ucfg.in_channels, ucfg.out_channels = 4 * (n_targets + 1), 4 * n_targets
+    unet, vae = UNet2DConditionOracle(ucfg).eval(), AutoencoderKLOracle(VAEConfig()).eval()
+    eng = Engine(EngineConfig(unet_in_channels=ucfg.in_channels, unet_out_channels=ucfg.out_channels))
+    eng.load_state_dict("unet", unet.state_dict())
+    eng.load_state_dict("vae", vae.state_dict())
+    eng.finalize()
+    eng.set_text_embedding(torch.randn(1, 2, ucfg.cross_attention_dim, generator=torch.Generator().manual_seed(7)))
+    return eng
+
+
+class Stages:
+    """Event pairs per stage, summed after one synchronise."""
+
+    def __init__(self):
+        self.pairs = {}
+
+    def time(self, name, fn):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        out = fn()
+        b.record()
+        self.pairs.setdefault(name, []).append((a, b))
+        return out
+
+    def ms(self):
+        torch.cuda.synchronize()
+        return {k: round(sum(a.elapsed_time(b) for a, b in v), 1) for k, v in self.pairs.items()}
+
+
+def run(eng, task, H, W, E, steps):
+    """One prediction of E members at H x W: the pipeline's stages (pipeline.py _infer_members + the ensembling)."""
+    s = DDIMScheduler()
+    s.set_timesteps(steps)
+    eng.set_schedule(s.timesteps, *s.coefficients())
+    rgb = (synthetic_image(max(H, W), seed=3)[..., :H, :W].float() / 255.0 * 2.0 - 1.0).cuda()
+    bs = select_batch_size(eng, E, H, W)
+    ct = eng.cfg.unet_out_channels
+    g = torch.Generator(device="cuda").manual_seed(0)
+    st = Stages()
+    lat = st.time("encode", lambda: eng.encode(rgb))
+    preds = []
+    for s0 in range(0, E, bs):
+        nb = min(bs, E - s0)
+        z = torch.randn(nb, ct, H // 8, W // 8, device="cuda", generator=g)
+        tgt = st.time("denoise", lambda: eng.denoise(lat.expand(nb, -1, -1, -1).contiguous(), z))
+        if task == "iid":
+            preds.append(st.time("decode", lambda: torch.cat([eng.decode(tgt[:, 4 * i:4 * i + 4].contiguous(), 3)
+                                                              for i in range(ct // 4)], 1)))
+        else:
+            preds.append(st.time("decode", lambda: eng.decode(tgt, 0 if task == "depth" else 1)))
+    pred = torch.cat(preds)
+    if E > 1:
+        ens = {"depth": lambda: ensemble_depth(pred, engine=eng, output_uncertainty=True),
+               "normals": lambda: ensemble_normals(pred, engine=eng, output_uncertainty=True),
+               "iid": lambda: ensemble_iid(pred, engine=eng, output_uncertainty=True)}[task]
+        out = st.time("ensemble", ens)[0]
+    else:
+        out = pred
+    ms = st.ms()
+    assert torch.isfinite(out).all()
+    R, blocks = attn_blocks(eng, 1, (H // 8) * (W // 8))
+    return {"task": task, "H": H, "W": W, "E": E, "steps": steps, "stage_ms": ms, "batch_size": bs,
+            "workspace_bytes": eng.workspace_bytes(bs, H, W), "attn_rows": R, "attn_blocks_per_image": blocks,
+            "held_bytes_after": eng.held_bytes()}
+
+
+def attention_ab(eng, reps=5):
+    """Decode of a 1920 x 1080 latent (135 x 240) with the VAE attention in one block and in its default blocks,
+    alternated in this one process; the difference is the attention's."""
+    lat = torch.randn(1, 4, 135, 240, generator=torch.Generator().manual_seed(1)).cuda()
+    T = 135 * 240
+    arms = {"one_block": 8 << 30, "default": 0}
+    ref = {}
+    times = {k: [] for k in arms}
+    for i in range(reps + 1):
+        for name, budget in arms.items():
+            attn_blocks(eng, 1, T, budget)
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            out = eng.decode(lat, 0)
+            b.record()
+            torch.cuda.synchronize()
+            if i:                                            # the first round warms both arms up
+                times[name].append(a.elapsed_time(b))
+            ref.setdefault(name, out)
+    attn_blocks(eng, 1, T)
+    med = {k: round(sorted(v)[len(v) // 2], 2) for k, v in times.items()}
+    return {"decode_ms_median": med, "decode_ms_all": {k: [round(x, 2) for x in v] for k, v in times.items()},
+            "rows": {k: attn_blocks(eng, 1, T, b)[0] for k, b in arms.items()},
+            "bit_equal": bool(torch.equal(ref["one_block"], ref["default"]))}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    res = {"card": gpu_identity(torch.cuda.current_device()), "runs": []}
+    eng = make_engine()
+    for (H, W) in ((3000, 4000), (3024, 4032)):
+        for E in (1, 10):
+            for steps in (1, 4):
+                res["runs"].append(run(eng, "depth", H, W, E, steps))
+                print(json.dumps(res["runs"][-1]), file=sys.stderr, flush=True)
+    res["runs"].append(run(eng, "normals", 3000, 4000, 1, 1))
+    try:
+        res["mp24"] = run(eng, "depth", 4032, 6048, 1, 1)
+    except (ValueError, RuntimeError) as e:           # the batch selection's refusal, or an arena that cannot grow
+        res["mp24"] = {"H": 4032, "W": 6048, "error": str(e)}
+    res["attention_1080p"] = attention_ab(eng)
+    eng.close()
+    torch.cuda.empty_cache()
+    eng = make_engine(n_targets=2)
+    res["runs"].append(run(eng, "iid", 3000, 4000, 1, 1))
+    eng.close()
+    line = json.dumps(res)
+    print(line, flush=True)
+    if a.out:
+        Path(a.out).mkdir(parents=True, exist_ok=True)
+        (Path(a.out) / "native_res.json").write_text(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
