@@ -919,6 +919,28 @@ int mgb_debug_vae_attn_blocks(mgb_handle* h, int64_t budget_bytes, int32_t force
   return MGB_OK;
 }
 
+// The VAE mid-block attention's core (vae_attn_core) alone, as vae_attn_forward runs it: bf16 q, k, v [NB * T, C] ->
+// bf16 o, C = the VAE's mid-block width, in this handle's arena and split-K workspace (grown to a dry pass's need) with
+// the row blocking mgb_debug_vae_attn_blocks set, on the default stream.
+int mgb_debug_vae_attn_core(mgb_handle* h, const void* q, const void* k, const void* v, void* o, int32_t NB,
+                            int32_t T) {
+  TRY(check_ready(h, false));
+  if (!q || !k || !v || !o || NB <= 0 || T <= 0) { set_error("debug_vae_attn_core: bad argument"); return MGB_ERR_INVALID; }
+  const int C = h->cfg.vae_block_channels[3];
+  auto in = [](const void* p) { return reinterpret_cast<const bf16*>(p); };
+  Arena dry; dry.dry = true;
+  Ctx d; d.arena = &dry; d.dry = true; d.splitk_cap = ~size_t(0);
+  d.attn_budget = h->vae_attn_budget; d.attn_rows = h->vae_attn_force_rows;
+  TRY(vae_attn_core(d, in(q), in(k), in(v), reinterpret_cast<bf16*>(o), NB, T, C));
+  TRY(grow_captured(h, h->arena_buf, dry.peak + (1 << 20)));
+  TRY(grow_captured(h, h->splitk_ws, d.splitk_need));
+  Ctx c = make_ctx(h, nullptr);
+  c.arena->off = 0;
+  TRY(vae_attn_core(c, in(q), in(k), in(v), reinterpret_cast<bf16*>(o), NB, T, C));
+  if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
+  return MGB_OK;
+}
+
 size_t mgb_workspace_bytes(mgb_handle* h, int32_t B, int32_t H, int32_t W) {
   if (!h || !h->finalized || B <= 0 || H < 8 || W < 8 || size_t(B) * size_t(H) * size_t(W) > kMaxPixels) return 0;
   size_t peak = 0;

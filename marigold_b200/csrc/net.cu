@@ -255,25 +255,14 @@ int vae_attn_rows(int T, int C, size_t budget, int force_rows) {
   return std::min(T, std::max(budget_rows, wave_rows));
 }
 
-static int vae_attn_forward(Ctx& c, const VaeAttnW& A, Act& x, Act& y, int NB, int T) {
-  const int C = A.C;
-  const size_t M = size_t(NB) * T;
+int vae_attn_core(Ctx& c, const bf16* q, const bf16* k, const bf16* v, bf16* o, int NB, int T, int C) {
   const int Tp = (T + 63) / 64 * 64;
   const int R = vae_attn_rows(T, C, c.attn_budget, c.attn_rows);
   const Tile tile_s = matmul_tile(T, T, C, EPI_SCALE), tile_pv = matmul_tile(T, C, Tp, 0);
   const size_t mk = c.arena->mark();
-  bf16* a = aalloc<bf16>(c, M * C);
-  bf16* q = aalloc<bf16>(c, M * C);
-  bf16* k = aalloc<bf16>(c, M * C);
-  bf16* v = aalloc<bf16>(c, M * C);
   bf16* vt = aalloc<bf16>(c, size_t(C) * Tp);
   float* s = aalloc<float>(c, size_t(R) * Tp);
   bf16* pr = aalloc<bf16>(c, size_t(R) * Tp);
-  bf16* o = aalloc<bf16>(c, M * C);
-  TRY(groupnorm(c, x, nullptr, a, nullptr, A.gn, NB, T, 1e-6f, 0));
-  { Epi e; e.bias = A.q.b; e.out_bf16 = q; TRY(linear(c, a, int(M), A.q, e)); }
-  { Epi e; e.bias = A.k.b; e.out_bf16 = k; TRY(linear(c, a, int(M), A.k, e)); }
-  { Epi e; e.bias = A.v.b; e.out_bf16 = v; TRY(linear(c, a, int(M), A.v, e)); }
   const float scale = 1.0f / sqrtf(float(C));
   for (int n = 0; n < NB; ++n) {
     const size_t off = size_t(n) * T * C;
@@ -286,6 +275,24 @@ static int vae_attn_forward(Ctx& c, const VaeAttnW& A, Act& x, Act& y, int NB, i
       { Epi e; e.out_bf16 = o + qo; TRY(matmul_nt(c, pr, vt, rows, C, Tp, e, 0, tile_pv)); }
     }
   }
+  c.arena->release(mk);
+  return MGB_OK;
+}
+
+static int vae_attn_forward(Ctx& c, const VaeAttnW& A, Act& x, Act& y, int NB, int T) {
+  const int C = A.C;
+  const size_t M = size_t(NB) * T;
+  const size_t mk = c.arena->mark();
+  bf16* a = aalloc<bf16>(c, M * C);
+  bf16* q = aalloc<bf16>(c, M * C);
+  bf16* k = aalloc<bf16>(c, M * C);
+  bf16* v = aalloc<bf16>(c, M * C);
+  bf16* o = aalloc<bf16>(c, M * C);
+  TRY(groupnorm(c, x, nullptr, a, nullptr, A.gn, NB, T, 1e-6f, 0));
+  { Epi e; e.bias = A.q.b; e.out_bf16 = q; TRY(linear(c, a, int(M), A.q, e)); }
+  { Epi e; e.bias = A.k.b; e.out_bf16 = k; TRY(linear(c, a, int(M), A.k, e)); }
+  { Epi e; e.bias = A.v.b; e.out_bf16 = v; TRY(linear(c, a, int(M), A.v, e)); }
+  TRY(vae_attn_core(c, q, k, v, o, NB, T, C));
   { Epi e; e.bias = A.o.b; e.residual = x.p; e.out_f32 = y.p; TRY(linear(c, o, int(M), A.o, e)); }
   c.arena->release(mk);
   return MGB_OK;

@@ -116,6 +116,11 @@ struct Ctx {
   size_t sync_off = 0, sync_cap = 0, sync_need = 0;
 };
 
+// The VAE mid-block attention between its projections: o = softmax(q k^T / sqrt(C)) v per image, on bf16 q, k, v, o
+// [NB * T, C], in blocks of vae_attn_rows(T, C, c.attn_budget, c.attn_rows) query rows. Its scratch (V^T, one block's
+// fp32 scores and bf16 probabilities) comes from the arena and is released on return.
+int vae_attn_core(Ctx& c, const bf16* q, const bf16* k, const bf16* v, bf16* o, int NB, int T, int C);
+
 struct UNetW {
   ConvW conv_in, conv_out;
   NormW norm_out;

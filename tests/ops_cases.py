@@ -6,7 +6,9 @@ Covers the tile shapes the SD-2-size network launches (gemm_tc_kernel<160>/<128>
 split-K + its deferred epilogue, split-KV flash attention + attn_combine, the space-to-depth stride-2 convs, the small-N
 special epilogues) and the paths only the network used to reach: K concatenation in the linear and the conv
 (conv2 + 1x1 shortcut), odd stride-2 inputs, the scheduler epilogue, GroupNorm over a concat with straddling groups and
-its raw copy, the cropped upsample and the VAE attention helpers.
+its raw copy, the cropped upsample and the VAE attention helpers. The attention, softmax, transpose and VAE attention
+GEMM cases also run at the token counts of a 4032 x 3024 photo at native resolution (T = 190 512 at the UNet's level 0
+and in the VAE's mid block); there the attention's float64 reference is held to check_rows' rows only.
 
 Each case returns {"ok": bool, "worst": max |d| / bound, ...}; "rel_to_max" is reported, never asserted."""
 from __future__ import annotations
@@ -49,6 +51,10 @@ def cases():
     add("linear_ldo", case_linear, M=300, N=256, K=256, block_n=128, bias=True, residual=True, bf16out=True, ldo=320)
     # the VAE score GEMM: EPI_SCALE, fp32 out with ldo = T rounded up to 64
     add("linear_vae_score", case_linear, M=84, N=84, K=512, block_n=0, scale=512 ** -0.5, ldo=128)
+    # the VAE attention's GEMMs on a 4032 x 3024 photo (T = 190 512, Tp = 190 528): one block of score rows, and P V
+    # over the whole key range
+    add("linear_vae_score_t190512", case_linear, M=256, N=190512, K=512, block_n=0, scale=512 ** -0.5, ldo=190528)
+    add("linear_vae_pv_k190528", case_linear, M=256, N=512, K=190528, block_n=0, bf16out=True, probs=True)
     # multi-wave grids take the two-CTAs-per-SM instantiation (MINB = 2)
     add("linear_2cta_bn64", case_linear, M=9216, N=256, K=640, block_n=64, bias=True, residual=True)
     add("linear_2cta_bn128", case_linear, M=9216, N=512, K=640, block_n=128, bias=True, bf16out=True)
@@ -115,6 +121,14 @@ def cases():
     add("attn_t324_logits80", case_attn, NB=1, T=324, C=128, qk_std=6.3)
     add("attn_t1500_logits80", case_attn, NB=1, T=1500, C=64, qk_std=6.3)
     add("attn_t129_one_key", case_attn, NB=2, T=129, C=128, dominant=True)
+    # the UNet's levels 0, 1 and 2 on a 4032 x 3024 photo (504 x 378 latents), checked on check_rows' rows; a key that
+    # dominates every query late in the KV loop (past 256 key blocks: the running max grows there) and in the ragged
+    # last key block
+    add("attn_t190512_c320", case_attn, NB=1, T=190512, C=320)
+    add("attn_t47628_c640", case_attn, NB=1, T=47628, C=640)
+    add("attn_t11970_c1280", case_attn, NB=1, T=11970, C=1280)
+    add("attn_t190512_late_key", case_attn, NB=1, T=190512, C=320, dominant_at=120001)
+    add("attn_t190512_last_key", case_attn, NB=1, T=190512, C=320, dominant_at=190511)
     # ---- streaming kernels ------------------------------------------------------------------
     add("groupnorm_320", case_groupnorm, NB=2, HW=2304, C=320, G=32, eps=1e-5, silu=1)
     add("groupnorm_1920", case_groupnorm, NB=1, HW=576, C=1920, G=32, eps=1e-5, silu=1)
@@ -166,8 +180,13 @@ def cases():
     add("softmax_rows_84", case_softmax_rows, M=84, n=84, ld=128)
     add("softmax_rows_324_logits80", case_softmax_rows, M=324, n=324, ld=384, std=40.0)
     add("softmax_rows_4096", case_softmax_rows, M=64, n=4096, ld=4096)
+    # VAE attention score rows at 4032 x 3024 and 4000 x 3000
+    for n, ld in ((190512, 190528), (187500, 187520)):
+        for std in (3.0, 40.0):
+            add(f"softmax_rows_{n}_std{std:g}", case_softmax_rows, M=64, n=n, ld=ld, std=std)
     add("transpose_84x512", case_transpose, M=84, N=512, ld=128)
     add("transpose_4096x512", case_transpose, M=4096, N=512, ld=4096)
+    add("transpose_190512x512", case_transpose, M=190512, N=512, ld=190528)
     return cases
 
 
@@ -226,7 +245,9 @@ def _sched_k(kx, kv, kz):
 
 
 def case_linear(M, N, K, block_n, bias=False, residual=False, bf16out=False, geglu=False, splits=0, stages=0,
-                silu=False, scale=None, ldo=0, K2=0):
+                silu=False, scale=None, ldo=0, K2=0, probs=False):
+    """probs: A holds rows of softmax probabilities (non-negative, summing to 1) and W unit-variance values, as in the
+    VAE attention's P V GEMM."""
     import torch
 
     from marigold_b200 import _lib, ops
@@ -234,9 +255,10 @@ def case_linear(M, N, K, block_n, bias=False, residual=False, bf16out=False, geg
 
     g = torch.Generator(device="cuda").manual_seed(1)
     Kt = K + K2
-    a = (torch.randn(M, K, device="cuda", generator=g)).to(torch.bfloat16)
+    a = torch.randn(M, K, device="cuda", generator=g)
+    a = (torch.softmax(a, dim=1) if probs else a).to(torch.bfloat16)
     a2 = torch.randn(M, K2, device="cuda", generator=g).to(torch.bfloat16) if K2 else None
-    w = (torch.randn(N, Kt, device="cuda", generator=g) / Kt ** 0.5).to(torch.bfloat16)
+    w = (torch.randn(N, Kt, device="cuda", generator=g) / (1.0 if probs else Kt ** 0.5)).to(torch.bfloat16)
     b = torch.randn(N, device="cuda", generator=g) if bias else None
     n_out = N // 2 if geglu else N
     ld = ldo or n_out
@@ -467,7 +489,37 @@ def attn_splits(NB, T, C):
     return best
 
 
-def case_attn(NB, T, C, qk_std=1.0, dominant=False):
+def dominant_key(q, k, at, logit, scale, d, seed):
+    """Make key `at` of every image the dominant one for every query: q gains a shared random +-1 direction u, key
+    `at` becomes logit / (d scale) u, so that each query's logit for it is about `logit` (d: the dot product's length,
+    the head dim) while the others keep their spread. q, k: [NB, T, C], changed in place."""
+    import torch
+
+    g = torch.Generator(device=q.device).manual_seed(seed)
+    u = torch.randint(0, 2, (q.shape[-1],), device=q.device, generator=g).float() * 2 - 1
+    q += u
+    k[:, at] = logit / (d * scale) * u
+
+
+def check_rows(T, block, seed, n_random=2048):
+    """Query rows checked where the float64 reference of every row is out of reach: the first and the last block of
+    `block` rows, the rows either side of every block boundary, the last 64 rows and n_random seeded rows."""
+    import torch
+
+    rows = set(range(min(block, T))) | set(range(max(0, (T - 1) // block * block), T)) | set(range(max(0, T - 64), T))
+    for r0 in range(block, T, block):
+        rows |= {r0 - 1, r0}
+    g = torch.Generator().manual_seed(seed)
+    rows |= set(torch.randint(0, T, (n_random,), generator=g).tolist())
+    return torch.tensor(sorted(rows), dtype=torch.long)
+
+
+# Above this many float64 probabilities (NB heads T^2) case_attn holds its reference to check_rows' rows only
+_ATTN_WHOLE_P = 1 << 30
+
+
+def case_attn(NB, T, C, qk_std=1.0, dominant=False, dominant_at=None):
+    """dominant_at: index of a key made dominant for every query (dominant_key, logit 14)."""
     import torch
 
     from marigold_b200 import _lib, ops
@@ -481,17 +533,38 @@ def case_attn(NB, T, C, qk_std=1.0, dominant=False):
     if dominant and T > 7:
         # key 7 of every image is 6 x query 0: query 0's logit for it exceeds the others by ~48
         k.view(NB, T, C)[:, 7] = 6 * q.view(NB, T, C)[:, 0]
+    if dominant_at is not None:
+        dominant_key(q.view(NB, T, C), k.view(NB, T, C), dominant_at, 14.0, 0.125, 64, seed=T)
     qkv = torch.cat([q, k, v], 1).to(torch.bfloat16).contiguous()
+    del q, k, v
     q64, k64, v64 = [R.f64(t).reshape(NB, T, heads, 64).permute(0, 2, 1, 3) for t in qkv.split(C, dim=1)]
-    p = torch.softmax((q64 @ k64.transpose(-1, -2)) * 0.125, dim=-1)
-    ref = (p @ v64).permute(0, 2, 1, 3).reshape(NB * T, C)
-    pv_abs = (p @ v64.abs()).permute(0, 2, 1, 3).reshape(NB * T, C)
+    # the flash kernel takes queries in tiles of 128 rows
+    rows = check_rows(T, 128, seed=T).cuda() if NB * heads * T * T > _ATTN_WHOLE_P else None
+    if rows is None:
+        p = torch.softmax((q64 @ k64.transpose(-1, -2)) * 0.125, dim=-1)
+        ref = (p @ v64).permute(0, 2, 1, 3).reshape(NB * T, C)
+        pv_abs = (p @ v64.abs()).permute(0, 2, 1, 3).reshape(NB * T, C)
+        del p
+    else:
+        ref = torch.empty(NB, heads, len(rows), 64, dtype=torch.float64, device="cuda")
+        pv_abs = torch.empty_like(ref)
+        step = max(1, (1 << 26) // (NB * heads * T))
+        for i in range(0, len(rows), step):
+            rr = rows[i:i + step]
+            p = torch.softmax((q64[:, :, rr] @ k64.transpose(-1, -2)) * 0.125, dim=-1)
+            ref[:, :, i:i + step], pv_abs[:, :, i:i + step] = p @ v64, p @ v64.abs()
+            del p
+        ref, pv_abs = (t.permute(0, 2, 1, 3).reshape(NB * len(rows), C) for t in (ref, pv_abs))
+    del q64, k64, v64
     lib = _lib.load()
     n0 = lib.mgb_launch_count()
     out = ops.flash_attn64(qkv, NB, T, C, 0.125)
     launches = lib.mgb_launch_count() - n0
     torch.cuda.synchronize()
     res = {"splits": attn_splits(NB, T, C), "launches": launches}
+    if rows is not None:
+        out = out.view(NB, T, C)[:, rows].reshape(NB * len(rows), C)
+        res["rows_checked"] = len(rows)
     _check(res, "bf16", out, ref, R.attn_bound(ref, pv_abs))
     d = (out.double() - ref).abs()
     excess = (d - R.U_BF16 * ref.abs()).clamp(min=0) / (R.U_BF16 * pv_abs + R.TINY)
@@ -668,9 +741,9 @@ def case_softmax_rows(M, n, ld, std=3.0):
     torch.cuda.synchronize()
     s64 = R.f64(s[:, :n])
     ref = torch.softmax(s64, dim=1)
-    # bf16 rounding, plus fp32 exp (argument rounding grows with |s - max|) and the fp32 row sum
+    # bf16 rounding, plus fp32 exp (argument rounding grows with |s - max|) and the fp32 row sum of n terms
     dist = (s64.max(dim=1, keepdim=True).values - s64)
-    bound = ref * (R.U_BF16 + 2.0 ** -18 + 2.0 ** -22 * dist) + R.TINY
+    bound = ref * (R.U_BF16 + R.softmax_rel(n, dist, ref)) + R.TINY
     res = {}
     _check(res, "bf16", p[:, :n], ref, bound)
     _exact(res, "pad_zero", p[:, n:], torch.zeros_like(p[:, n:]))

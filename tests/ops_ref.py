@@ -94,6 +94,19 @@ def attn_bound(ref, pv_abs):
     return U_BF16 * ref.abs() + C_P * U_BF16 * pv_abs + TINY
 
 
+def softmax_rel(n, dist, p):
+    """Relative error of softmax_rows_kernel's fp32 probability p_j = exp(s_j - m) / sum before its bf16 rounding, on
+    rows of n logits; dist = m - s_j >= 0 (float64, [rows, n]), p the float64 softmax.
+      * exp(s_j - m): the fp32 subtraction rounds the argument by 2^-24 dist_j and __expf is within 2 + 1.173 dist_j
+        ulps (CUDA Programming Guide), an ulp being at most 2^-23 relative: 2^-22 (1 + dist_j) together.
+      * the row sum carries its terms' relative errors, at most 2^-22 (1 + sum_j p_j dist_j) weighted by the terms,
+        plus its own fp32 additions: 256 threads each add ceil(n / 256) terms in order, then 5 shuffle levels and 8
+        warp partials: (ceil(n / 256) + 16) 2^-24. At n = 4096 that is 2^-19, at n = 190 512 about 2^-14.4.
+      * 1 / sum and the product: 2^-23."""
+    dbar = (p * dist).sum(dim=-1, keepdim=True)
+    return 2.0 ** -22 * (2 + dist + dbar) + (math.ceil(n / 256) + 16) * U_F32 + 2.0 ** -23
+
+
 # ---- references ---------------------------------------------------------------------------------------------------
 def f64(t):
     return t.detach().to(torch.float64)

@@ -8,15 +8,38 @@
     the torch graphs below, whose libraries keep device memory for the rest of the process;
   * parity at 4000 x 3000: encode, then decode the 500 x 375 latent with the depth, normals and one-IID-target heads,
     against the fp32 oracle run by torch on the GPU with TF32 off, with the bf16 yardstick of test_fullsize_gpu.py. Its
-    mid-block attention is evaluated in row blocks (_blocked_attention): SDPA cannot hold the T x T scores here."""
+    mid-block attention is evaluated in row blocks (_blocked_attention): SDPA cannot hold the T x T scores here;
+  * one UNet + DDIM step at the 504 x 378 and 500 x 375 latents of 4032 x 3024 and 4000 x 3000 photos (T = 190 512 and
+    187 500 tokens at level 0; the 2H - 1 upsample crops fall on different levels), at steps 0 and 5 of 10, against
+    the same fp32 oracle and bf16 yardstick; the fused DDIM update against kx x + kv model_out;
+  * the VAE attention's core (score GEMM, row softmax, V^T, P V GEMM, in row blocks: mgb_debug_vae_attn_core) element
+    by element against float64 at T = 187 500, 190 512, 2 x 32 400 and 10 087, on four kinds of input, and bit for bit
+    across block heights at T = 190 512.
+
+The VAE attention core's bound. The reference is o = softmax(s) v with s = q k^T / sqrt(C) in float64 on the same bf16
+q, k, v; only rows are checked whose float64 probabilities fit (check_rows: both end blocks, both sides of every block
+boundary, the last 64 rows, 2048 seeded rows). Per element of row i, with p the float64 probabilities, Tp the key count
+rounded up to 64 and the constants of tests/ops_ref.py:
+    |o~ - o| <= (2^-8 + 2 R_F32_OUT) |o|                      bf16 output, fp32 epilogue
+              + C_P 2^-8 sum_j p_j |v_j|                      bf16 P
+              + C_ACC Tp 2^-24 sum_j p_j |v_j|                P V fp32 accumulation
+              + sum_j p_j |ds_j| (|v_j| + |o|)                the score error through the softmax (|v_j - o| bounded)
+              + sum_j p_j softmax_rel(T, m - s_j) |v_j|       the softmax's fp32 exp and row sum (ops_ref.softmax_rel)
+    |ds_j| <= C_ACC C 2^-24 |q||k_j| / sqrt(C) + R_F32_OUT |s_j|   the score GEMM's accumulation and epilogue.
+softmax_rel's row-sum term grows with T: (ceil(T / 256) + 16) 2^-24, about 2^-14.4 at T = 190 512."""
 import ctypes as C
+import json
+import os
 import types
+from pathlib import Path
 
 import numpy as np
 import pytest
 import torch
 
-from tests.helpers import engine_from_oracle, oracle_models, rel_err, synthetic_image
+from tests import ops_ref
+from tests.helpers import engine_from_oracle, oracle_models, record, rel_err, synthetic_image
+from tests.ops_cases import check_rows, dominant_key
 
 pytestmark = pytest.mark.gpu
 
@@ -230,3 +253,167 @@ def test_12mp_encode_decode_match_oracle(models):
     e_ours = float((ours["normals"] - r).abs()[strong].max())
     e_yard = float((refs["bf16", "normals"] - r).abs()[strong].max())
     assert e_ours <= e_yard * 1.05 + 1e-3, (e_ours, e_yard)
+
+
+# ---- the UNet step at native resolution --------------------------------------------------------------------------
+PARITY = {}
+
+
+def _record_parity(key, ours, yard):
+    PARITY[key] = {"ours_vs_fp32": ours, "torch_bf16_vs_fp32": yard}
+    if os.environ.get("MGB_PARITY_DIR"):
+        out = Path(os.environ["MGB_PARITY_DIR"])
+        out.mkdir(parents=True, exist_ok=True)
+        (out / "native_res_parity.json").write_text(json.dumps(PARITY, indent=1))
+
+
+def test_unet_step_at_native_resolution_matches_oracle(models):
+    """One UNet + DDIM step at steps 0 and 5 of a 10-step schedule on the latents of 4032 x 3024 and 4000 x 3000
+    photos, within test_fullsize_gpu.py's bf16 yardstick of the fp32 oracle. The engine runs first and is closed before
+    the torch graphs, which keep device memory for the rest of the process."""
+    import copy
+
+    from marigold_b200.schedulers import DDIMScheduler
+
+    unet, vae, text = models
+    s = DDIMScheduler()
+    s.set_timesteps(10)
+    kx, kv, kz = s.coefficients()
+    eng = engine_from_oracle(unet, vae, text)
+    eng.set_schedule(s.timesteps, kx, kv, kz)
+    inputs, ours = {}, {}
+    for lh, lw in ((378, 504), (375, 500)):
+        g = torch.Generator().manual_seed(lh * lw)
+        rgb, x0 = torch.randn(1, 4, lh, lw, generator=g), torch.randn(1, 4, lh, lw, generator=g)
+        inputs[lh, lw] = rgb, x0
+        for step in (0, 5):
+            x = x0.cuda()
+            mo = eng.unet_step(rgb.cuda(), x, step, want_model_out=True)
+            # the fused scheduler epilogue is fp32-exact on the product's own model output
+            assert rel_err(x, float(kx[step]) * x0.cuda() + float(kv[step]) * mo) < 1e-5, (lh, lw, step)
+            assert torch.isfinite(mo).all()
+            ours[lh, lw, step] = mo.cpu()
+            del x, mo
+    eng.close()
+    torch.cuda.empty_cache()
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.backends.cudnn.allow_tf32 = False
+    refs = {}
+    for tag, dt in (("fp32", torch.float32), ("bf16", torch.bfloat16)):
+        u, tx = copy.deepcopy(unet).cuda().to(dt), text.cuda().to(dt)
+        with torch.no_grad():
+            for (lh, lw), (rgb, x0) in inputs.items():
+                for step in (0, 5):
+                    inp = torch.cat([rgb, x0], 1).cuda().to(dt)
+                    refs[tag, lh, lw, step] = u(inp, int(s.timesteps[step]), tx).float().cpu()
+        del u, tx
+        torch.cuda.empty_cache()
+    for (lh, lw, step), mo in ours.items():
+        e_ours, e_yard = rel_err(mo, refs["fp32", lh, lw, step]), rel_err(refs["bf16", lh, lw, step],
+                                                                        refs["fp32", lh, lw, step])
+        _record_parity(f"{lw}x{lh}/unet_step{step}", e_ours, e_yard)
+        assert e_ours <= e_yard * 1.05 + 1e-3, f"{lw}x{lh} step {step}: ours {e_ours:.3e} vs torch-bf16 {e_yard:.3e}"
+
+
+# ---- the VAE attention core at native token counts ---------------------------------------------------------------
+VAE_C = 512
+# 4000 x 3000 (T % 64 = 44), 4032 x 3024 (T % 64 = 48), two 1920 x 1080 images (blocks and per-image offsets) and
+# 77 x 131 latents (one block)
+CORE_SIZES = [(1, 187500), (1, 190512), (2, 32400), (1, 10087)]
+# logits of std 1; of std 40 (up to about +-200); one key dominating every query (logit about 14 against a log-sum of
+# the others of about 13) at T - 1, in the ragged last 64-key tile, and near T / 2
+REGIMES = ("std1", "logits80", "key_last", "key_mid")
+
+
+@pytest.fixture(scope="module")
+def core_engine(models):
+    eng = engine_from_oracle(*models)
+    yield eng
+    eng.close()
+
+
+def attn_core(eng, q, k, v, NB, T):
+    """mgb_debug_vae_attn_core: bf16 q, k, v [NB T, 512] -> bf16 o, with the handle's row blocking."""
+    from marigold_b200._lib import check
+
+    f = _hook("mgb_debug_vae_attn_core", C.c_int32, [C.c_void_p] * 5 + [C.c_int32, C.c_int32])
+    o = torch.empty_like(q)
+    check(f(eng._h, q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), NB, T), "mgb_debug_vae_attn_core")
+    torch.cuda.synchronize()
+    return o
+
+
+def _core_inputs(NB, T, regime):
+    g = torch.Generator(device="cuda").manual_seed(7 * T + NB)
+    std = 6.3 if regime == "logits80" else 1.0
+    q = torch.randn(NB, T, VAE_C, device="cuda", generator=g) * std
+    k = torch.randn(NB, T, VAE_C, device="cuda", generator=g) * std
+    v = torch.randn(NB, T, VAE_C, device="cuda", generator=g)
+    if regime in ("key_last", "key_mid"):
+        dominant_key(q, k, T - 1 if regime == "key_last" else T // 2 + 7, 14.0, VAE_C ** -0.5, VAE_C, seed=T)
+    return [t.reshape(NB * T, VAE_C).to(torch.bfloat16) for t in (q, k, v)]
+
+
+def _core_ref(q, k, v, NB, T, rows):
+    """float64 o, its bound (module docstring) and sum_j p_j |v_j| at `rows` of every image: [NB, len(rows), C]."""
+    R = ops_ref
+    Cc, Tp, scale = VAE_C, (T + 63) // 64 * 64, VAE_C ** -0.5
+    ref = torch.empty(NB, len(rows), Cc, dtype=torch.float64, device="cuda")
+    bound, pv_abs = torch.empty_like(ref), torch.empty_like(ref)
+    step = max(1, (1 << 26) // T)
+    for n in range(NB):
+        k64, v64 = R.f64(k[n * T:(n + 1) * T]), R.f64(v[n * T:(n + 1) * T])
+        ka, va = k64.abs(), v64.abs()
+        for i in range(0, len(rows), step):
+            qr = R.f64(q[n * T + rows[i:i + step]])
+            s = qr @ k64.t() * scale
+            ds = R.C_ACC * Cc * R.U_F32 * scale * (qr.abs() @ ka.t()) + R.R_F32_OUT * s.abs()
+            dist = s.max(dim=1, keepdim=True).values - s
+            del s
+            p = torch.exp(-dist)
+            p /= p.sum(dim=1, keepdim=True)
+            o = p @ v64
+            pds = p * ds
+            del ds
+            w = p * (R.softmax_rel(T, dist, p) + R.C_ACC * Tp * R.U_F32) + pds
+            del dist
+            pa = p @ va
+            sl = slice(i, i + step)
+            ref[n, sl], pv_abs[n, sl] = o, pa
+            bound[n, sl] = ((R.U_BF16 + 2 * R.R_F32_OUT) * o.abs() + R.C_P * R.U_BF16 * pa + w @ va
+                            + o.abs() * pds.sum(dim=1, keepdim=True) + R.TINY)
+            del p, pds, w
+    return ref, bound, pv_abs
+
+
+@pytest.mark.parametrize("regime", REGIMES)
+@pytest.mark.parametrize("NB,T", CORE_SIZES, ids=lambda x: str(x))
+def test_vae_attn_core_within_float64_bound(core_engine, NB, T, regime):
+    R, blocks = attn_blocks(core_engine, NB, T)
+    assert blocks == NB * -(-T // R)
+    q, k, v = _core_inputs(NB, T, regime)
+    o = attn_core(core_engine, q, k, v, NB, T)
+    rows = check_rows(T, R, seed=T).cuda()
+    ref, bound, pv_abs = _core_ref(q, k, v, NB, T, rows)
+    out = o.view(NB, T, VAE_C)[:, rows]
+    r = ops_ref.within(out, ref, bound)
+    record(f"native_res/vae_attn_core/{NB}x{T}/{regime}/worst", r["worst"])
+    # what the rows say about the bf16 P rounding: the error beyond every other term, over 2^-8 sum_j p_j |v_j|
+    other = bound - ops_ref.C_P * ops_ref.U_BF16 * pv_abs
+    c_p = ((out.double() - ref).abs() - other).clamp(min=0) / (ops_ref.U_BF16 * pv_abs + ops_ref.TINY)
+    record(f"native_res/vae_attn_core/{NB}x{T}/{regime}/c_p", float(c_p.max()))
+    assert not r["nan"] and r["worst"] <= 1.0, (R, len(rows), r)
+
+
+def test_vae_attn_core_row_blocks_are_bit_identical_at_12mp(core_engine):
+    """At T = 190 512 one block cannot run (S and P would take 218 GB): the default block height and forced heights
+    of 128 and 1792 rows give the same bits."""
+    T = 190512
+    q, k, v = _core_inputs(1, T, "std1")
+    R0, _ = attn_blocks(core_engine, 1, T)
+    assert R0 not in (128, 1792, T)
+    base = attn_core(core_engine, q, k, v, 1, T)
+    for force in (128, 1792):
+        assert attn_blocks(core_engine, 1, T, force_rows=force) == (force, -(-T // force))
+        assert torch.equal(attn_core(core_engine, q, k, v, 1, T), base), force
+    attn_blocks(core_engine, 1, T)
