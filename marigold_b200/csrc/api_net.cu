@@ -541,7 +541,8 @@ static UNetStaging stage_unet(mgb_handle* h, Arena& a, int NB, int HW) {
 //   DECODE: a0 = latent NCHW, a1 = out NCHW
 static int run_graph(mgb_handle* h, Ctx& c, int op, const float* a0, float* a1, const float* a2, float* a3, int step,
                      int NB, int d0, int d1, int mode) {
-  c.arena->off = 0;
+  c.arena->start();
+  c.planned = op != OP_UNET;
   if (op == OP_ENCODE) return vae_encode_forward(h, c, a0, a1, NB, d0, d1);
   if (op == OP_DECODE) return vae_decode_forward(h, c, a0, a1, NB, d0, d1, mode);
   // UNET single step through NCHW <-> NHWC conversions
@@ -562,19 +563,26 @@ static int run_graph(mgb_handle* h, Ctx& c, int op, const float* a0, float* a1, 
 
 struct WorkspaceNeed { size_t arena = 0, splitk = 0, sync = 0; };   // bytes
 
-// Dry-runs one graph: its arena peak, split-K workspace and GroupNorm barrier counters.
-static int workspace_need(mgb_handle* h, int op, int NB, int d0, int d1, WorkspaceNeed* need) {
+// Dry-runs one graph: its arena peak, split-K workspace and GroupNorm barrier counters. The VAE forwards' arena is
+// planned: their buffers, placed by lifetime (arena_place with the handle's placement), go to *bufs and the arena
+// peak is the plan's. The UNet step keeps the bump allocator's stack layout, which its captured graph holds; *bufs
+// then receives the buffers at their bump offsets.
+static int workspace_need(mgb_handle* h, int op, int NB, int d0, int d1, WorkspaceNeed* need,
+                          std::vector<ArenaBuf>* bufs = nullptr) {
   Arena dry; dry.dry = true;
   Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
   c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
   TRY(run_graph(h, c, op, nullptr, nullptr, nullptr, nullptr, 0, NB, d0, d1, 0));
-  *need = {dry.peak, c.splitk_need, c.sync_need * sizeof(unsigned)};
+  dry.finish();
+  const size_t arena = op == OP_UNET ? dry.peak : arena_place(dry.rec, h->arena_placement);
+  *need = {arena, c.splitk_need, c.sync_need * sizeof(unsigned)};
+  if (bufs) bufs->swap(dry.rec);
   return MGB_OK;
 }
 
 static int ensure_workspace(mgb_handle* h, int op, int NB, int d0, int d1) {
   WorkspaceNeed need;
-  TRY(workspace_need(h, op, NB, d0, d1, &need));
+  TRY(workspace_need(h, op, NB, d0, d1, &need, op == OP_UNET ? nullptr : &h->arena_plan));
   TRY(grow_captured(h, h->arena_buf, need.arena + (1 << 20)));
   TRY(grow_captured(h, h->splitk_ws, need.splitk));
   return grow_captured(h, h->sync_slab, need.sync);
@@ -604,8 +612,9 @@ static Ctx make_ctx(mgb_handle* h, void* stream) {
   c.stream = reinterpret_cast<cudaStream_t>(stream);
   c.arena = &h->arena;
   c.arena->base = h->arena_buf; c.arena->cap = h->arena_buf.bytes();
-  c.arena->dry = false; c.arena->overflow = false;
+  c.arena->dry = false; c.arena->status = MGB_OK; c.arena->plan = nullptr;
   c.dry = false;
+  c.poison = h->arena_poison;
   c.splitk_ws = h->splitk_ws; c.splitk_cap = h->splitk_ws.bytes();
   c.groups = h->cfg.norm_groups;
   c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
@@ -619,8 +628,13 @@ static int run_once(mgb_handle* h, void* stream, int op, const float* a0, float*
                     int step, int NB, int d0, int d1, int mode) {
   TRY(ensure_workspace(h, op, NB, d0, d1));
   Ctx c = make_ctx(h, stream);
+  if (op != OP_UNET) c.arena->plan = &h->arena_plan;
   TRY(run_graph(h, c, op, a0, a1, a2, a3, step, NB, d0, d1, mode));
-  if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
+  TRY(h->arena.status);
+  if (c.arena->plan && c.arena->n != h->arena_plan.size()) {
+    set_error("arena: the forward made %zu allocations, its plan %zu", c.arena->n, h->arena_plan.size());
+    return MGB_ERR_STATE;
+  }
   return MGB_OK;
 }
 
@@ -683,6 +697,7 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
     }
     c.arena->release(base);
     TRY(unet_forward(h, c, s.rgb, s.tgt, s.nz, nullptr, i, B, lh, lw));  // eager (also warms one-time attributes)
+    TRY(h->arena.status);   // a step the arena cut short launched only part of its kernels: never capture it
     if (graphs && !G.exec_failed) {
       // capture one step (reads the step index from the device counter) for all later steps of this shape
       invalidate_step_graph(h);
@@ -706,7 +721,7 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
       cudaGraphExec_t exec = nullptr;
       if (rc == MGB_OK && ce == cudaSuccess && graph) ce = cudaGraphInstantiate(&exec, graph, 0);
       if (graph) cudaGraphDestroy(graph);
-      if (rc == MGB_OK && ce == cudaSuccess && exec) {
+      if (rc == MGB_OK && ce == cudaSuccess && exec && h->arena.status == MGB_OK) {
         G.exec.reset(exec); G.NB = B; G.lh = lh; G.lw = lw; G.launches = nl;
       } else {
         cudaGetLastError();
@@ -715,8 +730,7 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
     }
   }
   TRY(launch_nhwc_to_nchw(s.tgt, target, B, Ct, HW, 1.f, c.stream));
-  if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
-  return MGB_OK;
+  return h->arena.status;
 }
 
 int mgb_denoise(mgb_handle* h, const float* rgb_latent, float* target, const float* step_noise, int32_t B, int32_t lh,
@@ -935,10 +949,64 @@ int mgb_debug_vae_attn_core(mgb_handle* h, const void* q, const void* k, const v
   TRY(grow_captured(h, h->arena_buf, dry.peak + (1 << 20)));
   TRY(grow_captured(h, h->splitk_ws, d.splitk_need));
   Ctx c = make_ctx(h, nullptr);
-  c.arena->off = 0;
+  c.arena->start();
   TRY(vae_attn_core(c, in(q), in(k), in(v), reinterpret_cast<bf16*>(o), NB, T, C));
-  if (h->arena.overflow) { set_error("arena overflow"); return MGB_ERR_NOMEM; }
+  return h->arena.status;
+}
+
+// Debug switches of this handle's arena: poison != 0 fills every buffer a forward's arena hands out with 0xFF bytes
+// (NaN in fp32 and bf16) before the forward uses it; placement is arena_place's placement of the VAE forwards' plans
+// (0: the library's, 1: first fit in reverse allocation order). No result may depend on either.
+int mgb_debug_arena(mgb_handle* h, int32_t poison, int32_t placement) {
+  if (!h || placement < 0 || placement > 1) { set_error("debug_arena: bad argument"); return MGB_ERR_INVALID; }
+  h->arena_poison = poison != 0;
+  h->arena_placement = placement;
   return MGB_OK;
+}
+
+// arena_place on n buffers, a pure host function: sizes and lifetimes [t_alloc, t_free) in, offsets out. Returns the
+// peak, or a negative status.
+int64_t mgb_debug_arena_place(int64_t n, const int64_t* bytes, const int64_t* t_alloc, const int64_t* t_free,
+                              int32_t placement, int64_t* off) {
+  if (n < 0 || (n > 0 && (!bytes || !t_alloc || !t_free || !off)) || placement < 0 || placement > 1) {
+    set_error("debug_arena_place: bad argument");
+    return MGB_ERR_INVALID;
+  }
+  std::vector<ArenaBuf> b(static_cast<size_t>(n));
+  for (int64_t i = 0; i < n; ++i) {
+    if (bytes[i] < 0 || t_free[i] <= t_alloc[i]) {
+      set_error("debug_arena_place: buffer %lld has bytes %lld, lifetime [%lld, %lld)", (long long)i,
+                (long long)bytes[i], (long long)t_alloc[i], (long long)t_free[i]);
+      return MGB_ERR_INVALID;
+    }
+    b[i].bytes = size_t(bytes[i]); b[i].t_alloc = t_alloc[i]; b[i].t_free = t_free[i];
+  }
+  const size_t peak = arena_place(b, placement);
+  for (int64_t i = 0; i < n; ++i) off[i] = int64_t(b[i].off);
+  return int64_t(peak);
+}
+
+// The arena of one forward at this shape (op 0: UNet step on a d0 x d1 latent, 1: encode of d0 x d1 pixels, 2: decode
+// of a d0 x d1 latent), as workspace_need lays it out: per buffer in allocation order its size, lifetime and offset,
+// for the first `cap` buffers. Returns the buffer count, or a negative status.
+int64_t mgb_debug_arena_plan(mgb_handle* h, int32_t op, int32_t B, int32_t d0, int32_t d1, int64_t* bytes,
+                             int64_t* t_alloc, int64_t* t_free, int64_t* off, int64_t cap) {
+  if (!h || op < OP_UNET || op > OP_DECODE || B <= 0 || d0 <= 0 || d1 <= 0) {
+    set_error("debug_arena_plan: bad argument");
+    return MGB_ERR_INVALID;
+  }
+  TRY(check_ready(h, false));
+  TRY(check_pixels("debug_arena_plan", B, op == OP_ENCODE ? d0 : 8 * d0, op == OP_ENCODE ? d1 : 8 * d1));
+  WorkspaceNeed need;
+  std::vector<ArenaBuf> bufs;
+  TRY(workspace_need(h, op, B, d0, d1, &need, &bufs));
+  for (size_t i = 0; i < bufs.size() && int64_t(i) < cap; ++i) {
+    if (bytes) bytes[i] = int64_t(bufs[i].bytes);
+    if (t_alloc) t_alloc[i] = bufs[i].t_alloc;
+    if (t_free) t_free[i] = bufs[i].t_free;
+    if (off) off[i] = int64_t(bufs[i].off);
+  }
+  return int64_t(bufs.size());
 }
 
 size_t mgb_workspace_bytes(mgb_handle* h, int32_t B, int32_t H, int32_t W) {

@@ -6,6 +6,7 @@
 //
 // Numerics: bf16 tensor-core operands, fp32 accumulation, fp32 residual trunk and latent state;
 // GroupNorm/LayerNorm/softmax statistics in fp32.
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -18,16 +19,129 @@ namespace mgb {
 // ---------------------------------------------------------------------------------------------
 // arena
 // ---------------------------------------------------------------------------------------------
+static size_t align1k(size_t x) { return (x + 1023) & ~size_t(1023); }
+static constexpr uintptr_t kDryBase = 0x100000;   // a dry run's addresses: kDryBase + bump offset, never dereferenced
+
+void Arena::start() {
+  off = 0; n = 0; events = 0;
+  rec.clear(); live.clear();
+}
+
 void* Arena::alloc(size_t bytes) {
-  const size_t a = (off + 1023) & ~size_t(1023);
+  const size_t a = align1k(off);
   off = a + bytes;
   if (off > peak) peak = off;
-  if (dry) return reinterpret_cast<void*>(uintptr_t(0x100000) + a);
-  if (off > cap) { overflow = true; return nullptr; }
+  const size_t i = n++;
+  if (dry) {
+    rec.push_back({bytes, a, events++, 0});
+    live.push_back(i);
+    return reinterpret_cast<void*>(kDryBase + a);
+  }
+  if (status != MGB_OK) return nullptr;
+  if (plan) {
+    if (i >= plan->size() || (*plan)[i].bytes != bytes) {
+      set_error("arena: allocation %zu of %zu bytes is not the plan's (%zu buffers)", i, bytes, plan->size());
+      status = MGB_ERR_STATE;
+      return nullptr;
+    }
+    const ArenaBuf& b = (*plan)[i];
+    if (b.off + b.bytes > cap) { set_error("arena overflow"); status = MGB_ERR_NOMEM; return nullptr; }
+    return base + b.off;
+  }
+  if (off > cap) { set_error("arena overflow"); status = MGB_ERR_NOMEM; return nullptr; }
   return base + a;
 }
+
+void Arena::free(const void* p) {
+  if (!dry || !p) return;
+  const size_t a = size_t(reinterpret_cast<uintptr_t>(p) - kDryBase);
+  for (size_t k = live.size(); k-- > 0;) {
+    if (rec[live[k]].off == a) {
+      rec[live[k]].t_free = events++;
+      live.erase(live.begin() + k);
+      return;
+    }
+  }
+}
+
+void Arena::release(size_t m) {
+  off = m;
+  if (!dry) return;
+  // everything allocated since the mark: the live buffers at bump offsets >= m, newest first
+  for (size_t k = live.size(); k-- > 0;) {
+    if (rec[live[k]].off < m) continue;
+    rec[live[k]].t_free = events++;
+    live.erase(live.begin() + k);
+  }
+}
+
+void Arena::finish() {
+  for (size_t i : live) rec[i].t_free = events;
+  live.clear();
+  ++events;
+}
+
+// First fit in the given order: each buffer at the lowest aligned offset clear of every buffer already placed whose
+// lifetime overlaps its own.
+static size_t place_in_order(std::vector<ArenaBuf>& b, const std::vector<size_t>& order) {
+  std::vector<size_t> placed;
+  std::vector<std::pair<size_t, size_t>> busy;
+  placed.reserve(b.size());
+  size_t peak = 0;
+  for (size_t i : order) {
+    busy.clear();
+    for (size_t j : placed)
+      if (b[j].bytes && b[j].t_alloc < b[i].t_free && b[i].t_alloc < b[j].t_free)
+        busy.push_back({b[j].off, b[j].off + b[j].bytes});
+    std::sort(busy.begin(), busy.end());
+    size_t o = 0;
+    for (const auto& r : busy) {
+      if (o + b[i].bytes <= r.first) break;
+      o = std::max(o, align1k(r.second));
+    }
+    b[i].off = o;
+    placed.push_back(i);
+    peak = std::max(peak, o + b[i].bytes);
+  }
+  return peak;
+}
+
+size_t arena_place(std::vector<ArenaBuf>& bufs, int placement) {
+  std::vector<size_t> order(bufs.size());
+  for (size_t i = 0; i < order.size(); ++i) order[i] = i;
+  std::stable_sort(order.begin(), order.end(),
+                   [&](size_t x, size_t y) { return bufs[x].t_alloc < bufs[y].t_alloc; });
+  if (placement == 1) {
+    std::reverse(order.begin(), order.end());
+    return place_in_order(bufs, order);
+  }
+  // In allocation order, every aligned offset below the top of a stack is taken, so a stack-shaped sequence lands
+  // where the bump allocator puts it, whose aligned peak no placement beats. Largest first replaces it only where it
+  // needs strictly less memory (rounded to the alignment).
+  std::vector<ArenaBuf> by_size = bufs;
+  const size_t peak = place_in_order(bufs, order);
+  std::stable_sort(order.begin(), order.end(), [&](size_t x, size_t y) { return bufs[x].bytes > bufs[y].bytes; });
+  const size_t peak2 = place_in_order(by_size, order);
+  if (align1k(peak2) >= align1k(peak)) return peak;
+  bufs.swap(by_size);
+  return peak2;
+}
+
+// Arena memory for n T's. A failed allocation turns the rest of the forward into a dry run: nothing more is launched,
+// and the caller reports the arena's status.
 template <typename T>
-static T* aalloc(Ctx& c, size_t n) { return reinterpret_cast<T*>(c.arena->alloc(n * sizeof(T))); }
+static T* aalloc(Ctx& c, size_t n) {
+  void* p = c.arena->alloc(n * sizeof(T));
+  if (c.dry) return reinterpret_cast<T*>(p);
+  if (!p) {
+    c.dry = true;
+  } else if (c.poison && cudaMemsetAsync(p, 0xFF, n * sizeof(T), c.stream) != cudaSuccess) {
+    set_error("arena poison memset failed");
+    c.arena->status = MGB_ERR_CUDA;
+    c.dry = true;
+  }
+  return reinterpret_cast<T*>(p);
+}
 
 // ---------------------------------------------------------------------------------------------
 // launch wrappers (skipped in dry-run mode, which only measures arena / split-K needs)
@@ -146,41 +260,64 @@ static Act act_alloc(Ctx& c, size_t M, int C) {
 }
 
 // GroupNorm (+SiLU) over [a | b] (b == nullptr: single source) -> bf16 operand; one deterministic launch (norm.cu).
-// Scratch: partials from the arena (released by the caller's mark), one barrier counter per image from the per-forward
+// Scratch: partials from the arena (freed on return in a planned forward, else released by the caller's mark), one
+// barrier counter per image from the per-forward
 // counter slab (zeroed once per forward by zero_counters()).
 static int groupnorm(Ctx& c, const Act& a, const Act* b, bf16* y, bf16* raw, const NormW& n, int NB, int HW, float eps,
                      int silu) {
   if (skip_family("gn")) return MGB_OK;
   const int Cb = (b && b->p) ? b->C : 0;
-  void* part = c.arena->alloc(groupnorm_part_bytes(NB, HW, a.C + Cb, c.groups));
+  void* part = aalloc<char>(c, groupnorm_part_bytes(NB, HW, a.C + Cb, c.groups));
   const size_t coff = c.sync_off;
   c.sync_off += size_t(NB);
   if (c.sync_off > c.sync_need) c.sync_need = c.sync_off;
-  if (c.dry) return MGB_OK;
-  if (c.sync_off > c.sync_cap) { set_error("groupnorm: barrier counter slab exhausted"); return MGB_ERR_STATE; }
-  return launch_gn_fused(a.p, a.C, Cb ? b->p : nullptr, Cb, y, raw, n.g, n.b, NB, HW, c.groups, eps, silu, part,
+  int rc = MGB_OK;
+  if (!c.dry) {
+    if (c.sync_off > c.sync_cap) { set_error("groupnorm: barrier counter slab exhausted"); return MGB_ERR_STATE; }
+    rc = launch_gn_fused(a.p, a.C, Cb ? b->p : nullptr, Cb, y, raw, n.g, n.b, NB, HW, c.groups, eps, silu, part,
                          c.sync_base + coff, c.stream);
+  }
+  if (c.planned) c.arena->free(part);   // read by this launch alone
+  return rc;
 }
 
 // ---------------------------------------------------------------------------------------------
 // ResnetBlock2D: GN -> SiLU -> conv3x3 (+temb) -> GN -> SiLU -> conv3x3 ; + (1x1 shortcut | x)
-//   x fp32 [M, cin] -> y fp32 [M, cout] (y preallocated by the caller)
+//   x fp32 [M, cin] -> y fp32 [M, cout] (y preallocated by the caller, or in a planned forward allocated here if y.p
+//   is null)
+// In a planned forward (c.planned) each buffer is allocated where it is first written and freed after its last read,
+// and with consume_x so is x: after the first GroupNorm where the shortcut reads GroupNorm's raw copy instead, else
+// after conv2. Otherwise (the UNet step) the scratch is allocated at entry, the stack layout its captured graph holds.
 // ---------------------------------------------------------------------------------------------
-static int resnet_forward(Ctx& c, const ResnetW& R, Act& x, Act* skip, Act& y, int NB, int H, int W) {
+static int resnet_forward(Ctx& c, const ResnetW& R, Act& x, Act* skip, Act& y, int NB, int H, int W,
+                          bool consume_x = false) {
+  const bool planned = c.planned;
   // input = x, or the channel concat [x | skip] of an up block (never materialised in fp32: GroupNorm reads both
   // sources, and the 1x1 shortcut reads the bf16 copy GroupNorm emits)
   const size_t M = size_t(NB) * H * W;
   const size_t mk = c.arena->mark();
   bf16* t1 = aalloc<bf16>(c, M * R.cin);
   bf16* raw = R.has_sc ? aalloc<bf16>(c, M * R.cin) : nullptr;
-  Act h = act_alloc(c, M, R.cout);
-  bf16* t2 = aalloc<bf16>(c, M * R.cout);
+  Act h;
+  bf16* t2 = nullptr;
+  if (!planned) {
+    h = act_alloc(c, M, R.cout);
+    t2 = aalloc<bf16>(c, M * R.cout);
+  }
   TRY(groupnorm(c, x, skip, t1, raw, R.n1, NB, H * W, R.eps, 1));
+  if (consume_x && R.has_sc) c.arena->free(x.p);
+  if (planned) h = act_alloc(c, M, R.cout);
   Epi e1;
   e1.bias = (R.bias_off >= 0 && c.cur_bias) ? c.cur_bias + R.bias_off : R.c1.b;
   e1.out_f32 = h.p;
   TRY(conv3x3(c, t1, NB, H, W, R.c1, 0, e1));
+  if (planned) {
+    c.arena->free(t1);
+    t2 = aalloc<bf16>(c, M * R.cout);
+  }
   TRY(groupnorm(c, h, nullptr, t2, nullptr, R.n2, NB, H * W, R.eps, 1));
+  if (planned) c.arena->free(h.p);
+  if (!y.p) y = act_alloc(c, M, R.cout);
   // conv2 (+ residual). Where the block changes the channel count, diffusers adds conv_shortcut(x), a 1x1 convolution:
   // its K blocks are appended to conv2's implicit GEMM (weights [W2 | Wsc], bias b2 + bsc, second A operand = the raw
   // bf16 copy of the block input), which removes a GEMM launch (plus a split-K reduce on the small levels) and the
@@ -188,7 +325,13 @@ static int resnet_forward(Ctx& c, const ResnetW& R, Act& x, Act* skip, Act& y, i
   Epi e2; e2.bias = R.c2.b; e2.out_f32 = y.p;
   if (!R.has_sc) e2.residual = x.p;
   TRY(conv3x3(c, t2, NB, H, W, R.c2, 0, e2, 0, 0, R.has_sc ? raw : nullptr));
-  c.arena->release(mk);
+  if (planned) {
+    c.arena->free(t2);
+    c.arena->free(raw);
+    if (consume_x && !R.has_sc) c.arena->free(x.p);
+  } else {
+    c.arena->release(mk);
+  }
   return MGB_OK;
 }
 
@@ -426,8 +569,25 @@ int unet_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* tgt, const flo
 }
 
 // ---------------------------------------------------------------------------------------------
-// VAE encoder: rgb fp32 NCHW [NB,3,H,W] -> latent fp32 NCHW [NB,4,H/8,W/8] (mean * latent_scale)
+// VAE forwards. Their arena is lifetime-planned (api_net.cu): every buffer is allocated where it is first written and
+// freed after its last read, so the memory live at once stays near the largest working set of one step. At full
+// resolution that is the decoder's first up-level resnet's GroupNorm: its 256-channel fp32 input and the two bf16
+// copies it writes.
 // ---------------------------------------------------------------------------------------------
+// mid block: resnet, attention, resnet; consumes h and leaves the result in it
+static int vae_mid_forward(Ctx& c, const ResnetW& r0, const VaeAttnW& A, const ResnetW& r1, Act& h, int NB, int H,
+                           int W) {
+  Act y1, y3;
+  TRY(resnet_forward(c, r0, h, nullptr, y1, NB, H, W, true));
+  Act y2 = act_alloc(c, size_t(NB) * H * W, y1.C);
+  TRY(vae_attn_forward(c, A, y1, y2, NB, H * W));
+  c.arena->free(y1.p);
+  TRY(resnet_forward(c, r1, y2, nullptr, y3, NB, H, W, true));
+  h = y3;
+  return MGB_OK;
+}
+
+// VAE encoder: rgb fp32 NCHW [NB,3,H,W] -> latent fp32 NCHW [NB,4,H/8,W/8] (mean * latent_scale)
 int vae_encode_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* latent_out, int NB, int H, int W) {
   const VaeW& V = hd->vae;
   const mgb_config& cfg = hd->cfg;
@@ -441,37 +601,35 @@ int vae_encode_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* latent_o
   LAUNCH(launch_pack_rgb(rgb, x0, NB, H * W, c.stream));
   Act h = act_alloc(c, M, ch[0]);
   { Epi e; e.bias = V.enc_in.b; e.out_f32 = h.p; TRY(conv3x3(c, x0, NB, H, W, V.enc_in, 0, e)); }
+  c.arena->free(x0);
   int cur = ch[0];
   for (int i = 0; i < 4; ++i) {
-    // ping-pong trunk buffers for this resolution
-    Act buf[2] = {act_alloc(c, M, ch[i]), act_alloc(c, M, ch[i])};
+    // ping-pong trunk buffers for this resolution, each allocated by the resnet that first writes it
+    Act buf[2];
     for (int j = 0; j < L; ++j) {
-      Act y = buf[j & 1];
-      TRY(resnet_forward(c, V.enc_res[ri++], h, nullptr, y, NB, H, W));
-      h = y; cur = ch[i];
+      TRY(resnet_forward(c, V.enc_res[ri++], h, nullptr, buf[j & 1], NB, H, W, j == 0));
+      h = buf[j & 1]; cur = ch[i];
     }
     if (i < 3) {
       // F.pad(x, (0,1,0,1)) + 3x3 stride 2 pad 0: floor(s / 2) outputs; the parity planes hold ceil(s / 2) entries
       const int Hp = (H + 1) / 2, Wp = (W + 1) / 2;
       bf16* planes = aalloc<bf16>(c, size_t(NB) * 4 * Hp * Wp * cur);
       LAUNCH(launch_space_to_depth(h.p, planes, NB, H, W, cur, c.stream));
+      c.arena->free(buf[0].p);
+      c.arena->free(buf[1].p);
       H /= 2; W /= 2; M = size_t(NB) * H * W;
       Act y = act_alloc(c, M, cur);
       { Epi e; e.bias = V.enc_down[i].b; e.out_f32 = y.p; TRY(conv3x3(c, planes, NB, H, W, V.enc_down[i], 3, e, Hp, Wp)); }
+      c.arena->free(planes);
       h = y;
+    } else {
+      c.arena->free(buf[L & 1].p);   // h's partner; h goes on into the mid block
     }
   }
-  {
-    Act y1 = act_alloc(c, M, cur);
-    TRY(resnet_forward(c, V.enc_res[ri++], h, nullptr, y1, NB, H, W));
-    Act y2 = act_alloc(c, M, cur);
-    TRY(vae_attn_forward(c, V.enc_attn, y1, y2, NB, H * W));
-    Act y3 = act_alloc(c, M, cur);
-    TRY(resnet_forward(c, V.enc_res[ri++], y2, nullptr, y3, NB, H, W));
-    h = y3;
-  }
+  TRY(vae_mid_forward(c, V.enc_res[ri], V.enc_attn, V.enc_res[ri + 1], h, NB, H, W));
   bf16* t = aalloc<bf16>(c, M * cur);
   TRY(groupnorm(c, h, nullptr, t, nullptr, V.enc_norm_out, NB, H * W, 1e-6f, 1));
+  c.arena->free(h.p);
   {
     // conv_out with quant_conv folded in; mean half only; * latent_scale; NCHW output
     Epi e; e.bias = V.enc_out.b; e.out_f32 = latent_out; e.flags = EPI_NCHW | EPI_SCALE; e.scale = cfg.latent_scale;
@@ -481,9 +639,7 @@ int vae_encode_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* latent_o
   return MGB_OK;
 }
 
-// ---------------------------------------------------------------------------------------------
 // VAE decoder: latent fp32 NCHW [NB,4,lh,lw] -> out fp32 NCHW (depth: 1 plane, normals/raw: 3 planes)
-// ---------------------------------------------------------------------------------------------
 int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, int NB, int lh, int lw, int mode) {
   const VaeW& V = hd->vae;
   const mgb_config& cfg = hd->cfg;
@@ -491,7 +647,6 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
   const int L = cfg.vae_layers_per_block;
   int H = lh, W = lw;
   size_t M = size_t(NB) * H * W;
-  size_t ri = 0;
   TRY(zero_counters(c));
   const size_t mk0 = c.arena->mark();
   bf16* z = aalloc<bf16>(c, M * 64);
@@ -499,39 +654,33 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
   int cur = ch[3];
   Act h = act_alloc(c, M, cur);
   { Epi e; e.bias = V.dec_in.b; e.out_f32 = h.p; TRY(conv3x3(c, z, NB, H, W, V.dec_in, 0, e)); }
-  {
-    Act y1 = act_alloc(c, M, cur);
-    TRY(resnet_forward(c, V.dec_res[ri++], h, nullptr, y1, NB, H, W));
-    Act y2 = act_alloc(c, M, cur);
-    TRY(vae_attn_forward(c, V.dec_attn, y1, y2, NB, H * W));
-    Act y3 = act_alloc(c, M, cur);
-    TRY(resnet_forward(c, V.dec_res[ri++], y2, nullptr, y3, NB, H, W));
-    h = y3;
-  }
+  c.arena->free(z);
+  TRY(vae_mid_forward(c, V.dec_res[0], V.dec_attn, V.dec_res[1], h, NB, H, W));
+  size_t ri = 2;
+  Act buf[2];
   for (int i = 0; i < 4; ++i) {
     const int cout = ch[3 - i];
-    // the next level's input is placed below this level's buffers, which are given back once it is written: at 12 MP
-    // the full-resolution level would otherwise sit on ~15 GB of dead lower-level and upsampling buffers
-    Act next;
-    if (i < 3) next = act_alloc(c, M * 4, cout);
-    const size_t mk = c.arena->mark();
-    Act buf[2] = {act_alloc(c, M, cout), act_alloc(c, M, cout)};
+    buf[0] = buf[1] = Act();   // ping-pong trunk buffers, each allocated by the resnet that first writes it
     for (int j = 0; j < L + 1; ++j) {
-      Act y = buf[j & 1];
-      TRY(resnet_forward(c, V.dec_res[ri++], h, nullptr, y, NB, H, W));
-      h = y; cur = cout;
+      TRY(resnet_forward(c, V.dec_res[ri++], h, nullptr, buf[j & 1], NB, H, W, j == 0));
+      h = buf[j & 1]; cur = cout;
     }
     if (i < 3) {
       bf16* up = aalloc<bf16>(c, M * 4 * cur);
       LAUNCH(launch_upsample2x(h.p, up, NB, H, W, cur, 2 * H, 2 * W, c.stream));
+      c.arena->free(buf[0].p);
+      c.arena->free(buf[1].p);
       H *= 2; W *= 2; M = size_t(NB) * H * W;
+      Act next = act_alloc(c, M, cur);
       { Epi e; e.bias = V.dec_up[i].b; e.out_f32 = next.p; TRY(conv3x3(c, up, NB, H, W, V.dec_up[i], 0, e)); }
+      c.arena->free(up);
       h = next;
-      c.arena->release(mk);
     }
   }
   bf16* t = aalloc<bf16>(c, M * cur);
   TRY(groupnorm(c, h, nullptr, t, nullptr, V.dec_norm_out, NB, H * W, 1e-6f, 1));
+  c.arena->free(buf[0].p);
+  c.arena->free(buf[1].p);
   {
     Epi e; e.bias = V.dec_out.b; e.out_f32 = out;
     e.flags = mode == MGB_DECODE_DEPTH ? EPI_DEPTH : mode == MGB_DECODE_NORMALS ? EPI_NORMALS

@@ -69,14 +69,40 @@ struct VaeAttnW {
   LinW q, k, v, o;
 };
 
+// One activation buffer of a forward: its size, its lifetime [t_alloc, t_free) in events (allocations and frees,
+// counted from the forward's start) and its offset in the arena: the bump offset while a dry run records it, the
+// planned one once arena_place has placed it.
+struct ArenaBuf {
+  size_t bytes = 0, off = 0;
+  int64_t t_alloc = 0, t_free = 0;
+};
+
+// Gives each buffer a 1024-aligned offset such that no two buffers whose lifetimes overlap share a byte; returns the
+// peak (the largest off + bytes). Placement 0 places first fit in allocation order, which puts a stack-shaped sequence
+// exactly where the bump allocator does, or first fit largest first where that needs less memory. Placement 1 places
+// first fit in reverse allocation order (tests: results must not depend on where buffers are).
+size_t arena_place(std::vector<ArenaBuf>& bufs, int placement);
+
+// Activation memory of one forward. Without a plan it is a bump allocator: mark / release give back everything
+// allocated since the mark, and free() gives back nothing. A dry run records every allocation's size and lifetime
+// (release() and free() end lifetimes); a real run given that dry run's placed records (`plan`) hands out the planned
+// offsets, so a buffer holds its bytes only from its allocation to its free.
 struct Arena {
   char* base = nullptr;
   size_t cap = 0, off = 0, peak = 0;
   bool dry = false;
-  bool overflow = false;
+  int status = MGB_OK;   // MGB_ERR_NOMEM past cap, MGB_ERR_STATE when a real run leaves its plan
+  std::vector<ArenaBuf> rec;                  // dry run: every allocation so far
+  std::vector<size_t> live;                   // dry run: indices into rec not yet freed
+  int64_t events = 0;
+  const std::vector<ArenaBuf>* plan = nullptr;
+  size_t n = 0;                               // allocations so far
+  void start();                               // begins one forward
   void* alloc(size_t bytes);
+  void free(const void* p);
+  void finish();                              // dry run: ends the lifetimes still open
   size_t mark() const { return off; }
-  void release(size_t m) { off = m; }
+  void release(size_t m);
 };
 
 // A trunk activation: fp32 [M, C]
@@ -106,6 +132,8 @@ struct Ctx {
   bool dry = false;
   size_t attn_budget = kVaeAttnBudget;  // vae_attn_rows' budget and forced rows (mgb_handle's, see there)
   int attn_rows = 0;
+  bool planned = false;    // the arena is lifetime-planned (the VAE forwards): buffers are freed after their last read
+  bool poison = false;     // fill every buffer the arena hands out with 0xFF bytes (NaN in fp32 and bf16) first
   float* splitk_ws = nullptr;
   size_t splitk_cap = 0;   // bytes available
   size_t splitk_need = 0;  // bytes needed (dry run)
@@ -163,6 +191,11 @@ struct mgb_handle {
   // VAE mid-block attention row blocking: the library's budget unless a test overrides it (mgb_debug_vae_attn_blocks)
   size_t vae_attn_budget = mgb::kVaeAttnBudget;
   int vae_attn_force_rows = 0;
+  // The VAE forwards' arena plan: placed by the dry run that sizes each call's workspace, replayed by its real run.
+  // arena_placement and arena_poison are arena_place's placement and Ctx::poison (mgb_debug_arena).
+  std::vector<mgb::ArenaBuf> arena_plan;
+  int arena_placement = 0;
+  bool arena_poison = false;
   // conditioning / schedule
   bool text_set = false;
   int n_steps = 0;

@@ -142,15 +142,23 @@ def find_batch_size(ensemble_size: int, input_res: int, dtype: torch.dtype) -> i
 MAX_PIXELS = 1 << 26                 # kMaxPixels (csrc/net.h): members x height x width of one encode / decode call
 
 
+def call_reserve_bytes(h: int, w: int, ensemble_size: int, channels: int) -> int:
+    """Device memory a pipeline call holds beside the engine's workspace at h x w: the decoded members and their
+    concatenation (ensemble_size fp32 maps of `channels` each), the ensembled prediction and its uncertainty, and the
+    normalised fp32 input. At 24 MP it is 2.4 GB for depth and 6.7 GB for normals with 10 members."""
+    return 4 * h * w * (channels * (2 * ensemble_size + 2) + 3)
+
+
 def select_batch_size(engine, n_members: int, h: int, w: int, batch_size: int = 0,
-                      free_bytes: Optional[int] = None) -> int:
+                      free_bytes: Optional[int] = None, reserve_bytes: int = 0) -> int:
     """Members per batch for n_members at h x w. batch_size > 0 is taken as given; 0 takes find_batch_size's value,
     lowered to the largest batch whose workspace (engine.workspace_bytes) fits the memory available to the engine: free
     device memory (`free_bytes`, or the device's) plus the workspace the engine holds, which it gives back before it
-    grows. A batch that cannot fit, explicit or of one member, raises ValueError before any inference work is spent."""
+    grows, less `reserve_bytes` that the call needs for its own tensors (call_reserve_bytes). A batch that cannot fit,
+    explicit or of one member, raises ValueError before any inference work is spent."""
     if free_bytes is None:
         free_bytes = torch.cuda.mem_get_info(engine.device)[0]
-    avail = int(free_bytes) + engine.held_bytes()
+    avail = int(free_bytes) + engine.held_bytes() - int(reserve_bytes)
     explicit = batch_size > 0
     bs = min(batch_size, max(n_members, 1)) if explicit else find_batch_size(n_members, max(h, w), torch.float32)
     while True:
@@ -165,7 +173,8 @@ def select_batch_size(engine, n_members: int, h: int, w: int, batch_size: int = 
     what = f"a batch of {bs} member{'s' if bs > 1 else ''} at {h} x {w}"
     if need == 0:
         raise ValueError(f"{what} exceeds the engine's supported maximum of {MAX_PIXELS} pixels per call")
-    raise ValueError(f"{what} needs {need} bytes of device workspace, but {avail} bytes are available")
+    left = f" beside the call's own {int(reserve_bytes)}" if reserve_bytes else ""
+    raise ValueError(f"{what} needs {need} bytes of device workspace, but {avail} bytes are available{left}")
 
 
 def _processing_size(h0: int, w0: int, processing_res: int):
@@ -178,6 +187,7 @@ def _processing_size(h0: int, w0: int, processing_res: int):
 
 class _MarigoldBase:
     latent_scale_factor = 0.18215  # depth_pipeline.py:118
+    member_channels = 1            # channels of one decoded member: 1 (depth), 3 (normals), 3 per target (IID)
 
     def __init__(self, engine: Engine, scheduler, empty_text_embed: torch.Tensor,
                  default_denoising_steps: Optional[int] = None, default_processing_resolution: Optional[int] = None):
@@ -259,7 +269,9 @@ class _MarigoldBase:
 
         rank, G = parallel.world()
         n = len(parallel.member_indices(ensemble_size, rank, G))
-        return select_batch_size(self.engine, n, *_processing_size(h0, w0, processing_res), batch_size)
+        h, w = _processing_size(h0, w0, processing_res)
+        return select_batch_size(self.engine, n, h, w, batch_size,
+                                 reserve_bytes=call_reserve_bytes(h, w, ensemble_size, self.member_channels))
 
     def _draw_noise(self, shape, generator, noise):
         if noise is not None:
@@ -407,6 +419,8 @@ class MarigoldDepthPipeline(_MarigoldBase):
 
 
 class MarigoldNormalsPipeline(_MarigoldBase):
+    member_channels = 3
+
     def _check_inference_step(self, n_step: int) -> None:
         """normals_pipeline.py:310-344: LCM is refused."""
         assert n_step >= 1
@@ -468,6 +482,7 @@ class MarigoldIIDPipeline(_MarigoldBase):
         self.target_properties = target_properties
         self.target_names = target_properties["target_names"]          # :228-229 (KeyError / TypeError like the reference)
         self.n_targets = len(self.target_names)
+        self.member_channels = 3 * self.n_targets
         if engine.cfg.unet_out_channels != 4 * self.n_targets:
             raise ValueError(f"the UNet predicts {engine.cfg.unet_out_channels} latent channels, but target_names "
                              f"{self.target_names} needs {4 * self.n_targets}")

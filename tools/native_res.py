@@ -1,8 +1,10 @@
 """Native-resolution inference (processing_res = 0) on synthetic 12-megapixel photos, SD-size random weights: per run the
 stage times from CUDA events (encode, denoise, decode, ensemble: summed over the member batches), mgb_workspace_bytes,
 the member batch select_batch_size chose, and the VAE attention's rows per block and block count; the card's name and
-power limit, read in the same run. Then 24 MP (6048 x 4032): its numbers, or the error with the bytes it needed. Then
-a 1920 x 1080 decode with the VAE attention in one block against its default row blocks, alternated.
+power limit, read in the same run. Then 24 MP (6048 x 4032): depth with E = 1 and 1 step and with E = 10 and 4 steps,
+normals, and a 2-target IID model (each its numbers, or the error with the bytes it needed); the largest 4:3 and 3:2
+photos select_batch_size accepts for one depth member on this card; mgb_workspace_bytes at the batch caps and the
+native sizes. Then a 1920 x 1080 decode with the VAE attention in one block against its default row blocks, alternated.
 
     python tools/native_res.py [--out DIR]      (prints one JSON line; with --out also writes DIR/native_res.json)
 """
@@ -17,7 +19,7 @@ import torch  # noqa: E402
 
 from bench import gpu_identity  # noqa: E402
 from marigold_b200.ensemble import ensemble_depth, ensemble_iid, ensemble_normals  # noqa: E402
-from marigold_b200.pipeline import select_batch_size  # noqa: E402
+from marigold_b200.pipeline import call_reserve_bytes, select_batch_size  # noqa: E402
 from marigold_b200.schedulers import DDIMScheduler  # noqa: E402
 from tests.helpers import synthetic_image  # noqa: E402
 
@@ -73,8 +75,9 @@ def run(eng, task, H, W, E, steps):
     s.set_timesteps(steps)
     eng.set_schedule(s.timesteps, *s.coefficients())
     rgb = (synthetic_image(max(H, W), seed=3)[..., :H, :W].float() / 255.0 * 2.0 - 1.0).cuda()
-    bs = select_batch_size(eng, E, H, W)
     ct = eng.cfg.unet_out_channels
+    ch = {"depth": 1, "normals": 3, "iid": 3 * (ct // 4)}[task]
+    bs = select_batch_size(eng, E, H, W, reserve_bytes=call_reserve_bytes(H, W, E, ch))
     g = torch.Generator(device="cuda").manual_seed(0)
     st = Stages()
     lat = st.time("encode", lambda: eng.encode(rgb))
@@ -102,6 +105,35 @@ def run(eng, task, H, W, E, steps):
     return {"task": task, "H": H, "W": W, "E": E, "steps": steps, "stage_ms": ms, "batch_size": bs,
             "workspace_bytes": eng.workspace_bytes(bs, H, W), "attn_rows": R, "attn_blocks_per_image": blocks,
             "held_bytes_after": eng.held_bytes()}
+
+
+def try_run(eng, task, H, W, E, steps):
+    try:
+        return run(eng, task, H, W, E, steps)
+    except (ValueError, RuntimeError) as e:           # the batch selection's refusal, or an arena that cannot grow
+        return {"task": task, "H": H, "W": W, "E": E, "steps": steps, "error": str(e)}
+
+
+def largest_accepted(eng, aspect):
+    """The largest photo of aspect (w, h) with sides multiples of 8 that select_batch_size accepts for one depth member
+    (E = 1) in the memory free now: its size and workspace."""
+    def fits(k):
+        H, W = 8 * aspect[1] * k, 8 * aspect[0] * k
+        try:
+            select_batch_size(eng, 1, H, W, batch_size=1, reserve_bytes=call_reserve_bytes(H, W, 1, 1))
+            return True
+        except ValueError:
+            return False
+    if not fits(1):
+        return {"error": f"no {aspect[0]}:{aspect[1]} photo fits"}
+    lo, hi = 1, 2
+    while fits(hi):
+        lo, hi = hi, 2 * hi
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        lo, hi = (mid, hi) if fits(mid) else (lo, mid)
+    H, W = 8 * aspect[1] * lo, 8 * aspect[0] * lo
+    return {"H": H, "W": W, "megapixels": round(H * W / 1e6, 1), "workspace_bytes": eng.workspace_bytes(1, H, W)}
 
 
 def attention_ab(eng, reps=5):
@@ -142,15 +174,17 @@ def main():
                 res["runs"].append(run(eng, "depth", H, W, E, steps))
                 print(json.dumps(res["runs"][-1]), file=sys.stderr, flush=True)
     res["runs"].append(run(eng, "normals", 3000, 4000, 1, 1))
-    try:
-        res["mp24"] = run(eng, "depth", 4032, 6048, 1, 1)
-    except (ValueError, RuntimeError) as e:           # the batch selection's refusal, or an arena that cannot grow
-        res["mp24"] = {"H": 4032, "W": 6048, "error": str(e)}
+    res["mp24"] = try_run(eng, "depth", 4032, 6048, 1, 1)
+    res["mp24_runs"] = [try_run(eng, "depth", 4032, 6048, 10, 4), try_run(eng, "normals", 4032, 6048, 1, 1)]
+    res["workspace_bytes"] = {f"{B}x{H}x{W}": eng.workspace_bytes(B, H, W) for B, H, W in
+                              ((16, 768, 768), (8, 1024, 1024), (1, 3024, 4032), (2, 3024, 4032), (1, 4032, 6048))}
+    res["largest_accepted"] = {"4:3": largest_accepted(eng, (4, 3)), "3:2": largest_accepted(eng, (3, 2))}
     res["attention_1080p"] = attention_ab(eng)
     eng.close()
     torch.cuda.empty_cache()
     eng = make_engine(n_targets=2)
     res["runs"].append(run(eng, "iid", 3000, 4000, 1, 1))
+    res["mp24_runs"].append(try_run(eng, "iid", 4032, 6048, 1, 1))
     eng.close()
     line = json.dumps(res)
     print(line, flush=True)
