@@ -53,6 +53,61 @@ def gather_members(local: torch.Tensor, ensemble_size: int, group=None) -> torch
     return torch.stack(members, dim=0)
 
 
+def _collective_device(device: Optional[torch.device]) -> torch.device:
+    """Where a small host value travels for a collective: the caller's device under NCCL, the host under gloo."""
+    if device is not None and dist.get_backend() == "nccl":
+        return torch.device(device)
+    return torch.device("cpu")
+
+
+# ---- lists of images (pipeline.py _infer_list) ----------------------------------------------------------------------
+# A size group's jobs are (image, member) pairs in image-major order; job k belongs to rank k mod G (for a one-image list
+# these are member_indices). In round r every rank runs its r-th batch of at most bs jobs, and one all-gather gives every
+# rank the round's jobs [r G bs, (r + 1) G bs) in job order.
+
+def agree_batch_sizes(sizes: List[int], device: Optional[torch.device] = None) -> List[int]:
+    """The MIN over ranks of each size group's member batch, in one all-reduce: a rank's own choice depends on its free
+    memory, and the rounds' gathers need one slot count on every rank."""
+    rank, G = world()
+    if G == 1 or not sizes:
+        return [int(b) for b in sizes]
+    t = torch.tensor([int(b) for b in sizes], dtype=torch.int64, device=_collective_device(device))
+    dist.all_reduce(t, op=dist.ReduceOp.MIN)
+    return [int(b) for b in t.tolist()]
+
+
+def num_rounds(n_jobs: int, bs: int, world_size: int) -> int:
+    """Rounds of G batches of bs slots that cover n_jobs jobs."""
+    return -(-n_jobs // (world_size * bs))
+
+
+def round_jobs(n_jobs: int, bs: int, rnd: int, rank: int, world_size: int):
+    """(jobs, mine) of round `rnd`: every job index of the round in job order, and this rank's (every G-th from rank)."""
+    jobs = list(range(rnd * world_size * bs, min((rnd + 1) * world_size * bs, n_jobs)))
+    return jobs, jobs[rank::world_size]
+
+
+def open_images(bs: int, ensemble_size: int, world_size: int, n_images: int) -> int:
+    """The most images one round's G bs consecutive jobs can span, E jobs per image: the images a list call holds device
+    tensors for at once."""
+    return min(n_images, -(-(world_size * bs - 1) // ensemble_size) + 1)
+
+
+def gather_round(local: torch.Tensor, bs: int, n_round_jobs: int, group=None) -> torch.Tensor:
+    """local: [n_mine, C, H, W], this rank's jobs of the round in round_jobs order (n_mine <= bs). Returns the round's
+    [n_round_jobs, C, H, W] in job order on every rank: ONE all_gather of bs padded slots per rank. Slot s of rank r holds
+    the round's job s G + r."""
+    rank, G = world()
+    if G == 1:
+        assert local.shape[0] == n_round_jobs
+        return local
+    pad = torch.zeros((bs,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
+    pad[: local.shape[0]] = local
+    out = torch.empty((G * bs,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
+    dist.all_gather_into_tensor(out, pad, group=group)
+    return out.reshape(G, bs, *local.shape[1:]).transpose(0, 1).reshape(G * bs, *local.shape[1:])[:n_round_jobs]
+
+
 def barrier_max_ms(ms: float, device: Optional[torch.device] = None) -> float:
     """Max over ranks of a locally measured duration (multi-GPU numbers are max-over-ranks)."""
     rank, G = world()

@@ -8,6 +8,12 @@ the reference holds as `unet`, `vae`, `scheduler` are replaced by one `Engine` (
 a host-side scheduler mirror. Two keyword-only additions exist because the reference draws noise from
 a generator shared across batches (depth_pipeline.py:430-435), which cannot be reproduced once members
 are sharded across GPUs:  noise=[E,4,h,w]  and  step_noise=[n-1,E,4,h,w] (LCM).
+
+Every pipeline also takes a list (or tuple) of images and returns a list of outputs in input order: the members of
+several images share network batches, and each image is finished (ensembled, resized, copied to the host) by the single
+call's code as soon as its last member is decoded. `generator` is then one generator, drawn from by the images in list
+order, or a list with one generator (or None) per image; `noise` / `step_noise` are lists of per-image tensors (or
+None). Image i's noise is what the single call with its generator draws (_MarigoldBase._infer_list).
 """
 from __future__ import annotations
 
@@ -185,6 +191,61 @@ def _processing_size(h0: int, w0: int, processing_res: int):
     return int(h0), int(w0)
 
 
+def size_groups(sizes):
+    """[(size, [image indices])] in order of first appearance: the images of a list call that may share a batch."""
+    groups = {}
+    for i, s in enumerate(sizes):
+        groups.setdefault(tuple(s), []).append(i)
+    return list(groups.items())
+
+
+def noise_draw_batches(ensemble_size: int, batch_size: int, h: int, w: int, world_size: int = 1):
+    """Member counts of the successive noise draws for one image at h x w: what the single call draws, one batch at a
+    time at world size 1 (batch_size members if given, else find_batch_size's), the whole ensemble under G > 1 ranks. A
+    list call draws each image's noise in these pieces, whatever batches its members are later packed into."""
+    if world_size > 1:
+        return [ensemble_size]
+    b = min(batch_size, ensemble_size) if batch_size > 0 else find_batch_size(ensemble_size, max(h, w), torch.float32)
+    return [b] * (ensemble_size // b) + ([ensemble_size % b] if ensemble_size % b else [])
+
+
+def select_list_batch_size(engine, n_jobs: int, h: int, w: int, ensemble_size: int, channels: int, n_images: int,
+                           world_size: int = 1, batch_size: int = 0, free_bytes: Optional[int] = None) -> int:
+    """Members per batch for a size group of a list call: select_batch_size over the group's n_jobs (image, member) jobs
+    (one rank's share under world_size ranks), beside the call_reserve_bytes of every image one round of batches can
+    hold open (parallel.open_images). The reserve grows with the batch, so the two are lowered together: the result is
+    the largest batch that fits beside its own reserve. Raises ValueError like select_batch_size."""
+    from . import parallel
+
+    if free_bytes is None:
+        free_bytes = torch.cuda.mem_get_info(engine.device)[0]
+    per_image = call_reserve_bytes(h, w, ensemble_size, channels)
+    explicit = batch_size > 0
+    bs = min(batch_size, max(n_jobs, 1)) if explicit else find_batch_size(n_jobs, max(h, w), torch.float32)
+    while True:
+        reserve = parallel.open_images(bs, ensemble_size, world_size, n_images) * per_image
+        if explicit or bs == 1:
+            return select_batch_size(engine, n_jobs, h, w, bs, free_bytes, reserve)
+        try:
+            if select_batch_size(engine, bs, h, w, 0, free_bytes, reserve) == bs:
+                return bs
+        except ValueError:
+            pass                         # not even one member fits beside this batch's reserve; a smaller one reserves less
+        bs -= 1
+
+
+def _image_runs(jobs, idx, ensemble_size):
+    """[(image, [members])] of a job list, one entry per run of consecutive jobs of one image (idx: the group's images)."""
+    runs = []
+    for k in jobs:
+        i, m = idx[k // ensemble_size], k % ensemble_size
+        if runs and runs[-1][0] == i:
+            runs[-1][1].append(m)
+        else:
+            runs.append((i, [m]))
+    return runs
+
+
 class _MarigoldBase:
     latent_scale_factor = 0.18215  # depth_pipeline.py:118
     member_channels = 1            # channels of one decoded member: 1 (depth), 3 (normals), 3 per target (IID)
@@ -329,15 +390,183 @@ class _MarigoldBase:
                     sn = torch.stack([torch.randn((nb, ct, lh, lw), device=dev, dtype=self.dtype, generator=generator)
                                       for _ in range(denoising_steps - 1)]).to(self.device)
             target = self.engine.denoise(rgb_latent1.expand(nb, -1, -1, -1).contiguous(), z0, sn)
-            if decode_mode == _lib_decode_iid:
-                # marigold_iid_pipeline.py:568-585: one VAE decode per 4-channel target slice, concatenated along channels
-                preds.append(torch.cat([self.engine.decode(target[:, 4 * i:4 * i + 4].contiguous(), _lib_decode_iid)
-                                        for i in range(ct // 4)], dim=1))
-            else:
-                preds.append(self.engine.decode(target, decode_mode))
+            preds.append(self._decode(target, decode_mode))
         ch = 1 if decode_mode == 0 else (3 * (ct // 4) if decode_mode == _lib_decode_iid else 3)
         local = torch.concat(preds, dim=0) if preds else torch.empty((0, ch, lh * 8, lw * 8), device=self.device)
         return parallel.gather_members(local, ensemble_size)
+
+    def _decode(self, target, decode_mode):
+        """The decode of one denoised member batch [NB, ct, lh, lw] -> [NB, member_channels, 8 lh, 8 lw]."""
+        if decode_mode == _lib_decode_iid:
+            # marigold_iid_pipeline.py:568-585: one VAE decode per 4-channel target slice, concatenated along channels
+            return torch.cat([self.engine.decode(target[:, 4 * i:4 * i + 4].contiguous(), _lib_decode_iid)
+                              for i in range(target.shape[1] // 4)], dim=1)
+        return self.engine.decode(target, decode_mode)
+
+    # ---- lists of images -------------------------------------------------------------------------------------------
+    def _list_image_hw(self, i, image):
+        """(H, W) of list element i, checked as the single call checks its input, before any work."""
+        if Image is not None and isinstance(image, Image.Image):
+            w0, h0 = image.size
+            return int(h0), int(w0)
+        if not isinstance(image, torch.Tensor):
+            raise TypeError(f"image {i}: Unknown input type: {type(image) = }")
+        assert 4 == image.dim() and 1 == image.shape[0] and 3 == image.shape[1], \
+            f"image {i}: Wrong input shape {tuple(image.shape)}, expected [1, rgb, H, W]"
+        return int(image.shape[-2]), int(image.shape[-1])
+
+    def _call_list(self, images, denoising_steps, ensemble_size, processing_res, match_input_res, resample_method,
+                   batch_size, generator, ensemble_kwargs, noise, step_noise, decode_mode, **finish_kw):
+        """__call__ on a list of images: one output per image, in input order (see _infer_list)."""
+        if denoising_steps is None:
+            denoising_steps = self.default_denoising_steps
+        if processing_res is None:
+            processing_res = self.default_processing_resolution
+        assert processing_res >= 0
+        assert ensemble_size >= 1
+        _check_ensemble_size(self.engine, ensemble_size)
+        self._check_inference_step(denoising_steps)
+        resample = get_tv_resample_method(resample_method)
+        outputs = [None] * len(images)
+
+        def finish(i, member_maps, out_hw):
+            outputs[i] = self._finish(member_maps, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs,
+                                      **finish_kw)
+
+        self._infer_list(images, ensemble_size, denoising_steps, processing_res, resample, batch_size, generator, noise,
+                         step_noise, decode_mode, finish)
+        return outputs
+
+    def _infer_list(self, images, ensemble_size, denoising_steps, processing_res, resample, batch_size, generator,
+                    noise, step_noise, decode_mode, finish):
+        """Every member of every image through shared member batches; finish(i, [E, C, H, W] member maps, (H0, W0)) is
+        called for each image as soon as its last member is decoded, after which the call drops its device tensors.
+
+        Images are grouped by processing size (in order of first appearance); a group's jobs are (image, member) in
+        image-major order, job k on rank k mod G, and each batch takes the next bs of a rank's jobs (select_list_batch_size,
+        agreed by MIN over ranks). An image is preprocessed and encoded alone, as in the single call, when its first
+        member enters a batch. Under G ranks, round r runs every rank's r-th batch and one all-gather joins them.
+
+        Noise: image i draws from generator[i] (a list), or from the one shared generator in list order, exactly what
+        the single call with that generator draws: at world size 1 per noise_draw_batches piece of b members, z0
+        [b, ct, lh, lw] then the n - 1 LCM step-noise draws [b, ct, lh, lw]; under G > 1 z0 [E, ...] then step noise
+        [n - 1, E, ...]. noise[i] / step_noise[i] replace image i's draws. A member's maps depend only on its own inputs
+        and on its batch's size, so a member packed beside other images' members has the single call's bits wherever
+        the single call runs the same batch size (free memory can lower the single call's batch below b)."""
+        from . import parallel
+
+        N = len(images)
+        rank, G = parallel.world()
+        E = ensemble_size
+        ct = self.engine.cfg.unet_out_channels
+        need_sn = isinstance(self.scheduler, LCMScheduler) and denoising_steps > 1
+        # ---- every check before any work
+        hw0 = [self._list_image_hw(i, im) for i, im in enumerate(images)]
+        shared_gen = not isinstance(generator, (list, tuple))
+        for name, per_image in (("generator", None if shared_gen else generator), ("noise", noise),
+                                ("step_noise", step_noise)):
+            if per_image is not None and (not isinstance(per_image, (list, tuple)) or len(per_image) != N):
+                got = f"{len(per_image)} entries" if isinstance(per_image, (list, tuple)) else type(per_image).__name__
+                raise ValueError(f"{name} must be None or a list of one entry per image ({N}); got {got}")
+        groups = size_groups([_processing_size(h0, w0, processing_res) for h0, w0 in hw0])
+        sizes = []
+        for (h, w), idx in groups:
+            n_jobs = len(idx) * E
+            try:
+                sizes.append(select_list_batch_size(self.engine, parallel.slots_per_rank(n_jobs, G), h, w, E,
+                                                    self.member_channels, len(idx), G, batch_size))
+            except ValueError as e:
+                raise ValueError(f"image {idx[0]}: {e}") from None
+            lh, lw = h // 8, w // 8
+            for i in idx:
+                if noise is not None and noise[i] is not None:
+                    assert tuple(noise[i].shape) == (E, ct, lh, lw), \
+                        f"image {i}: noise shape {tuple(noise[i].shape)} != {(E, ct, lh, lw)}"
+                if need_sn and step_noise is not None and step_noise[i] is not None:
+                    assert tuple(step_noise[i].shape) == (denoising_steps - 1, E, ct, lh, lw), \
+                        f"image {i}: step_noise shape {tuple(step_noise[i].shape)} != " \
+                        f"{(denoising_steps - 1, E, ct, lh, lw)}"
+        if N == 0:
+            return
+        sizes = parallel.agree_batch_sizes(sizes, self.device)
+        self._set_schedule(denoising_steps)
+
+        def draw(i):
+            """Image i's z0 [E, ...] and step noise [n - 1, E, ...] (or None), in the single call's draw order."""
+            gen = generator if shared_gen else generator[i]
+            z_i = noise[i] if noise is not None else None
+            s_i = step_noise[i] if (need_sn and step_noise is not None) else None
+            h, w = _processing_size(*hw0[i], processing_res)
+            shape = (ct, h // 8, w // 8)
+            dev = gen.device if gen is not None else self.device
+            if G > 1:
+                z = self._draw_noise((E,) + shape, gen, z_i)
+                if need_sn and s_i is None:
+                    s_i = torch.randn((denoising_steps - 1, E) + shape, device=dev, dtype=self.dtype, generator=gen)
+            else:
+                zs, ss = [], []
+                for b in noise_draw_batches(E, batch_size, h, w):
+                    if z_i is None:
+                        zs.append(self._draw_noise((b,) + shape, gen, None))
+                    if need_sn and s_i is None:
+                        ss.append(torch.stack([torch.randn((b,) + shape, device=dev, dtype=self.dtype, generator=gen)
+                                               for _ in range(denoising_steps - 1)]))
+                z = z_i.to(self.device, torch.float32) if z_i is not None else torch.cat(zs)
+                if ss:
+                    s_i = torch.cat(ss, dim=1)
+            return z, (s_i.to(self.device, torch.float32) if need_sn else None)
+
+        drawn, next_draw = {}, 0
+
+        def noise_of(i):
+            nonlocal next_draw
+            if not shared_gen:
+                return draw(i)
+            while next_draw <= i:                    # one generator: every image draws in list order
+                drawn[next_draw] = draw(next_draw)
+                next_draw += 1
+            return drawn.pop(i)
+
+        for ((h, w), idx), bs in zip(groups, sizes):
+            lh, lw = h // 8, w // 8
+            n_jobs = len(idx) * E
+            lat, z, sn, maps, done = {}, {}, {}, {}, {}
+            for rnd in range(parallel.num_rounds(n_jobs, bs, G)):
+                jobs, mine = parallel.round_jobs(n_jobs, bs, rnd, rank, G)
+                for k in jobs:                       # open the images this round reaches
+                    i = idx[k // E]
+                    if i not in maps:
+                        z[i], sn[i] = noise_of(i)
+                        maps[i] = torch.empty((E, self.member_channels, 8 * lh, 8 * lw), device=self.device)
+                        done[i] = 0
+                if mine:
+                    runs = _image_runs(mine, idx, E)
+                    for i, _ in runs:
+                        if i not in lat:
+                            rgb_norm, _ = self._preprocess(images[i], processing_res, resample)
+                            lat[i] = self.encode_rgb(rgb_norm)
+                            del rgb_norm
+                    rgb_latent = torch.cat([lat[i].expand(len(ms), -1, -1, -1) for i, ms in runs]).contiguous()
+                    z0 = torch.cat([z[i][ms] for i, ms in runs]).contiguous()
+                    s = torch.cat([sn[i][:, ms] for i, ms in runs], dim=1).contiguous() if need_sn else None
+                    local = self._decode(self.engine.denoise(rgb_latent, z0, s), decode_mode)
+                    del rgb_latent, z0, s
+                else:
+                    local = torch.empty((0, self.member_channels, 8 * lh, 8 * lw), device=self.device)
+                pred = parallel.gather_round(local, bs, len(jobs))
+                del local
+                r0 = 0
+                for i, ms in _image_runs(jobs, idx, E):
+                    maps[i][ms[0]:ms[-1] + 1] = pred[r0:r0 + len(ms)]
+                    r0 += len(ms)
+                    done[i] += len(ms)
+                    if done[i] == E:
+                        member_maps = maps.pop(i)
+                        for held in (lat, z, sn, done):
+                            held.pop(i, None)
+                        finish(i, member_maps, hw0[i])
+                        del member_maps
+                del pred
 
 
 class MarigoldDepthPipeline(_MarigoldBase):
@@ -378,6 +607,10 @@ class MarigoldDepthPipeline(_MarigoldBase):
                  show_progress_bar: bool = True, ensemble_kwargs: Dict = None, *,
                  noise: Optional[torch.Tensor] = None, step_noise: Optional[torch.Tensor] = None
                  ) -> MarigoldDepthOutput:
+        if isinstance(input_image, (list, tuple)):
+            return self._call_list(input_image, denoising_steps, ensemble_size, processing_res, match_input_res,
+                                   resample_method, batch_size, generator, ensemble_kwargs, noise, step_noise,
+                                   _lib_decode_depth, color_map=color_map)
         if denoising_steps is None:
             denoising_steps = self.default_denoising_steps
         if processing_res is None:
@@ -392,6 +625,11 @@ class MarigoldDepthPipeline(_MarigoldBase):
 
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
                                            step_noise, _lib_decode_depth)
+        return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
+                            ensemble_kwargs, color_map=color_map)
+
+    def _finish(self, target_preds, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs, color_map):
+        """One image's [E, 1, h, w] member maps -> MarigoldDepthOutput (depth_pipeline.py:292-338)."""
         if ensemble_size > 1:
             final_pred, pred_uncert = ensemble_depth(target_preds, scale_invariant=self.scale_invariant,
                                                      shift_invariant=self.shift_invariant, engine=self.engine,
@@ -399,7 +637,7 @@ class MarigoldDepthPipeline(_MarigoldBase):
         else:
             final_pred, pred_uncert = target_preds, None
         if match_input_res:
-            final_pred = _resize(final_pred, tuple(input_size[-2:]), resample)
+            final_pred = _resize(final_pred, out_hw, resample)
         final_pred = final_pred.squeeze().cpu().numpy()
         if pred_uncert is not None:
             pred_uncert = pred_uncert.squeeze().cpu().numpy()
@@ -443,6 +681,10 @@ class MarigoldNormalsPipeline(_MarigoldBase):
                  resample_method: str = "bilinear", batch_size: int = 0,
                  generator: Union[torch.Generator, None] = None, show_progress_bar: bool = True,
                  ensemble_kwargs: Dict = None, *, noise: Optional[torch.Tensor] = None) -> MarigoldNormalsOutput:
+        if isinstance(input_image, (list, tuple)):
+            return self._call_list(input_image, denoising_steps, ensemble_size, processing_res, match_input_res,
+                                   resample_method, batch_size, generator, ensemble_kwargs, noise, None,
+                                   _lib_decode_normals)
         if denoising_steps is None:
             denoising_steps = self.default_denoising_steps
         if processing_res is None:
@@ -455,12 +697,17 @@ class MarigoldNormalsPipeline(_MarigoldBase):
         rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
                                            None, _lib_decode_normals)
+        return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
+                            ensemble_kwargs)
+
+    def _finish(self, target_preds, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs):
+        """One image's [E, 3, h, w] member maps -> MarigoldNormalsOutput (normals_pipeline.py:278-308)."""
         if ensemble_size > 1:
             final_pred, pred_uncert = ensemble_normals(target_preds, engine=self.engine, **(ensemble_kwargs or {}))
         else:
             final_pred, pred_uncert = target_preds, None
         if match_input_res:
-            final_pred = _resize(final_pred, tuple(input_size[-2:]), resample)
+            final_pred = _resize(final_pred, out_hw, resample)
         final_pred = final_pred.squeeze().cpu().numpy()
         if pred_uncert is not None:
             pred_uncert = pred_uncert.squeeze().cpu().numpy()
@@ -512,8 +759,10 @@ class MarigoldIIDPipeline(_MarigoldBase):
                  resample_method: str = "bilinear", batch_size: int = 0,
                  generator: Union[torch.Generator, None] = None, show_progress_bar: bool = True,
                  ensemble_kwargs: Dict = None, *, noise: Optional[torch.Tensor] = None):
-        from .iid import MarigoldIIDOutput, fill_outputs
-
+        if isinstance(input_image, (list, tuple)):
+            return self._call_list(input_image, denoising_steps, ensemble_size, processing_res, match_input_res,
+                                   resample_method, batch_size, generator, ensemble_kwargs, noise, None,
+                                   _lib_decode_iid)
         if denoising_steps is None:
             denoising_steps = self.default_denoising_steps
         if processing_res is None:
@@ -526,13 +775,20 @@ class MarigoldIIDPipeline(_MarigoldBase):
         rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
                                            None, _lib_decode_iid)
+        return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
+                            ensemble_kwargs)
+
+    def _finish(self, target_preds, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs):
+        """One image's [E, 3 n, h, w] member maps -> MarigoldIIDOutput (marigold_iid_pipeline.py:367-411)."""
+        from .iid import MarigoldIIDOutput, fill_outputs
+
         assert target_preds.dim() == 4 and target_preds.shape[1] == 3 * self.n_targets      # :367-370
         if ensemble_size > 1:
             final_pred, pred_uncert = ensemble_iid(target_preds, engine=self.engine, **(ensemble_kwargs or {}))
         else:
             final_pred, pred_uncert = target_preds, None
         if match_input_res:
-            final_pred = _resize(final_pred, tuple(input_size[-2:]), resample)      # (:386-392; uncertainty is NOT resized)
+            final_pred = _resize(final_pred, out_hw, resample)      # (:386-392; uncertainty is NOT resized)
         output = MarigoldIIDOutput(target_names=self.target_names)
         fill_outputs(output, final_pred, pred_uncert, self.target_names, self.target_properties)
         assert output.is_complete
