@@ -221,17 +221,37 @@ int mgb_eval_iid(const float* pred_dev, const float* gt_dev, const uint8_t* mask
 typedef struct mgb_lpips mgb_lpips;
 int mgb_lpips_create(const float* const conv_w[5], const int32_t conv_w_shape[5][4], const float* const conv_b[5],
                      const float* const lin_w[5], const int32_t lin_channels[5], mgb_lpips** out);
+/* LPIPS weights of any of torchmetrics' three backbones (net_type "alex", "vgg", "squeeze"). conv_w[i], conv_b[i]: host
+ * fp32 weight [Cout, Cin, k, k] and bias [Cout] of the net's i-th convolution in torchvision's order, conv_w_shape[4 i ..
+ * 4 i + 3] that weight's shape; lin_w[l]: host fp32 lin{l}.model.1.weight of lin_channels[l] elements.
+ *   MGB_LPIPS_ALEX     5 convs:  alexnet().features.{0,3,6,8,10}; 5 lin layers of 64, 192, 384, 256, 256 channels
+ *   MGB_LPIPS_VGG      13 convs: vgg16().features.{0,2,5,7,10,12,14,17,19,21,24,26,28}; 5 lin layers of 64, 128, 256, 512,
+ *                      512 channels (relu1_2, relu2_2, relu3_3, relu4_3, relu5_3)
+ *   MGB_LPIPS_SQUEEZE  25 convs: squeezenet1_1().features.0, then features.{3,4,6,7,9,10,11,12}.{squeeze, expand1x1,
+ *                      expand3x3}; 7 lin layers of 64, 128, 256, 384, 384, 512, 512 channels
+ * MGB_ERR_INVALID for an unknown net_type and for any count or shape but the net's. mgb_lpips_create is this call with
+ * MGB_LPIPS_ALEX. */
+typedef enum { MGB_LPIPS_ALEX = 0, MGB_LPIPS_VGG = 1, MGB_LPIPS_SQUEEZE = 2 } mgb_lpips_net_type;
+int mgb_lpips_create_net(int32_t net_type, int32_t n_conv, const float* const* conv_w, const int32_t* conv_w_shape,
+                         const float* const* conv_b, int32_t n_lin, const float* const* lin_w, const int32_t* lin_channels,
+                         mgb_lpips** out);
 void mgb_lpips_destroy(mgb_lpips* h);
-/* Workspace of mgb_eval_iid_lpips (it includes mgb_eval_iid's); 0 when H or W < 31. */
+/* The smallest H (and W) for which every tapped layer of the net is non-empty: 31 (AlexNet), 16 (VGG16), 17 (SqueezeNet
+ * 1.1); 0 for an unknown net_type. */
+int32_t mgb_lpips_min_size(int32_t net_type);
+/* Workspace of mgb_eval_iid_lpips with the AlexNet weights (it includes mgb_eval_iid's); 0 when H or W < 31. */
 size_t mgb_lpips_ws_bytes(int32_t H, int32_t W);
+/* Workspace of mgb_eval_iid_lpips with the weights h; 0 when H or W is below the net's minimum size. */
+size_t mgb_lpips_ws_bytes_h(const mgb_lpips* h, int32_t H, int32_t W);
 /* mgb_eval_iid, then LPIPS of the same maps (compute_iid_metric with "lpips", src/util/metric.py:263-288), in ONE
  * synchronisation. The maps the metric sees are SSIM's (mapped, invalid elements 0); they must lie in [0, 1]
  * (normalize=True), else MGB_ERR_INVALID with torchmetrics' message (a NaN fails). Then 2 x - 1, the scaling layer,
- * AlexNet's five conv + ReLU stages (bf16 operands, fp32 accumulation and features), per layer the unit-normalised
- * (x / sqrt(1e-8 + sum x^2)) squared difference weighted by lin and averaged over the pixels, and the float32 sum of the
- * five means. out_host[7] = mgb_eval_iid's six values, then lpips. H, W >= 31 (AlexNet's second pool needs a 3 x 3
- * input). Deterministic: equal inputs give equal bits; for the targets that are not up to scale, swapping pred and gt
- * gives the same lpips. */
+ * the net's conv + ReLU layers and pools (bf16 operands, fp32 accumulation and features), per tapped layer the
+ * unit-normalised (x / sqrt(1e-8 + sum x^2)) squared difference weighted by lin and averaged over the pixels, and the
+ * float32 sum of the means in layer order. out_host[7] = mgb_eval_iid's six values, then lpips. H, W >= the net's
+ * minimum size (mgb_lpips_min_size; 31 for AlexNet, whose second pool needs a 3 x 3 input). ws_dev:
+ * mgb_lpips_ws_bytes_h. Deterministic: equal inputs give equal bits; for the targets that are not up to scale, swapping
+ * pred and gt gives the same lpips. */
 int mgb_eval_iid_lpips(const float* pred_dev, const float* gt_dev, const uint8_t* mask_dev, int32_t H, int32_t W,
                        int32_t up_to_scale, int32_t transform, const mgb_lpips* lpips, void* ws_dev, double* out_host,
                        void* stream);

@@ -72,8 +72,12 @@ SIGNATURES = {
     "mgb_eval_iid": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "mgb_lpips_create": (_i32, [C.POINTER(_vp), C.POINTER(_i32), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_i32),
                                  C.POINTER(_vp)]),
+    "mgb_lpips_create_net": (_i32, [_i32, _i32, C.POINTER(_vp), C.POINTER(_i32), C.POINTER(_vp), _i32, C.POINTER(_vp),
+                                     C.POINTER(_i32), C.POINTER(_vp)]),
     "mgb_lpips_destroy": (None, [_vp]),
+    "mgb_lpips_min_size": (_i32, [_i32]),
     "mgb_lpips_ws_bytes": (C.c_size_t, [_i32, _i32]),
+    "mgb_lpips_ws_bytes_h": (C.c_size_t, [_vp, _i32, _i32]),
     "mgb_eval_iid_lpips": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "mgb_workspace_bytes": (C.c_size_t, [_vp, _i32, _i32, _i32]),
     "mgb_workspace_held_bytes": (C.c_size_t, [_vp]),

@@ -195,10 +195,42 @@ int launch_eval_iid(const float* pred, const float* gt, const uint8_t* mask, lon
 float* eval_iid_sk(void* ws, long long H, long long W);
 
 // ---------------------------------------------------------------------------------------------
-// LPIPS (AlexNet, lpips.cu) of the maps the IID evaluation scores
+// LPIPS (lpips.cu) of the maps the IID evaluation scores: AlexNet, VGG16 or SqueezeNet 1.1 features
 // ---------------------------------------------------------------------------------------------
-constexpr int kLpipsLayers = 5;
-constexpr int kLpipsMinSize = 31;              // pool2 needs a conv2 output of at least 3 x 3
+constexpr int kLpipsLayers = 5;                // AlexNet's tapped layers
+constexpr int kLpipsMinSize = 31;              // AlexNet: pool2 needs a conv2 output of at least 3 x 3
+constexpr int kLpMaxLayers = 7;                // tapped layers of any net (SqueezeNet)
+constexpr int kLpMaxConvs = 25;                // convolutions of any net (SqueezeNet: conv1 + 8 Fire modules x 3)
+constexpr int kLpMaxSteps = 32;                // convolutions and pools of any net
+
+// One convolution of a backbone as torchvision defines it, and how the GEMM runs it.
+struct LpConv {
+  int cout, cin, k;            // torchvision weight [cout, cin, k, k]
+  int n, cin_pad;              // GEMM columns (cout, or 64 for a Fire squeeze) and operand channels (a multiple of 64)
+};
+// One launch of the backbone. A conv writes bf16 [2, h, w, ldo] (the next step's operand) and, at a tap, fp32 [2, h, w,
+// ldo] at column `col` of the buffer of step `buf` (itself, or the expand1x1 whose output the expand3x3 completes).
+enum : int { LP_CONV = 0, LP_POOL2 = 1, LP_POOL3 = 2, LP_POOL3_CEIL = 3 };
+struct LpStep {
+  int op;
+  int in;                      // step whose output this reads, -1: the prep operand
+  int buf, col, ldo;           // output buffer (a step index), column offset and row pitch in elements
+  int conv, kind;              // LP_CONV: index into LpNet::conv, fill_conv_params kind
+  int tap;                     // head layer of the fp32 output, -1: none
+  bool bf16_out;               // false only for the last tap, which no step reads
+};
+enum : int { LP_PREP_S2D4 = 0, LP_PREP_PLAIN = 1, LP_PREP_PARITY = 2 };
+struct LpNet {
+  const char* name;
+  int prep;                    // LP_PREP_*: the layout of the first conv's operand
+  int nconv, nsteps, L;
+  LpConv conv[kLpMaxConvs];
+  LpStep step[kLpMaxSteps];
+  int C[kLpMaxLayers];         // channels of each tapped layer
+  int min_size;                // the smallest H (and W) for which every tapped layer is non-empty
+};
+// MGB_LPIPS_ALEX / _VGG / _SQUEEZE; nullptr for any other value
+const LpNet* lpips_net(int net);
 // Conv1 (11 x 11, stride 4, pad 2) runs as a 3 x 3 unpadded convolution (kind 4) over 4 x 4 blocks of the padded input:
 // output row o reads padded rows 4 o .. 4 o + 10, i.e. rows r of blocks o + kb with 4 kb + r < 11. A block is 64
 // channels, pixel (rh, rw) of the block and colour c at channel s2d_channel(rh, rw, c), channels 48..63 zero. The input
@@ -206,18 +238,22 @@ constexpr int kLpipsMinSize = 31;              // pool2 needs a conv2 output of 
 __host__ __device__ constexpr int s2d_channel(int rh, int rw, int c) { return (rh * 4 + rw) * 3 + c; }
 constexpr int kLpipsS2dC = 64;
 struct LpipsWeights {
-  const bf16* w[kLpipsLayers];                 // [Cout, taps * Cin] tap-major; conv1 in the factor-4 block layout
-  const float* b[kLpipsLayers];                // [Cout]
-  const float* lin;                            // [64 + 192 + 384 + 256 + 256], layer after layer
+  const bf16* w[kLpMaxConvs];                  // [n, taps * cin_pad] tap-major; AlexNet conv1 in the factor-4 block layout
+  const float* b[kLpMaxConvs];                 // [n]
+  const float* lin;                            // the tapped layers' channels, layer after layer
 };
-size_t lpips_ws_bytes(int H, int W);
-// Forward of both maps after the IID passes that left {s, k} at sk (nullptr: not up to scale). ws: lpips_ws_bytes(H, W).
+// 0 when H or W is below net.min_size
+size_t lpips_ws_bytes(const LpNet& net, int H, int W);
+// Forward of both maps after the IID passes that left {s, k} at sk (nullptr: not up to scale). ws: lpips_ws_bytes.
 // Results: lpips_out(ws): {lpips, elements out of [0, 1], min and max keys of each map (4 doubles)}.
-int launch_lpips(const float* pred, const float* gt, const uint8_t* mask, int H, int W, int transform, const float* sk,
-                 const LpipsWeights& wts, void* ws, cudaStream_t stream);
-const void* lpips_out(const void* ws, int H, int W);
-// The fp32 post-ReLU features of layer l (0..4) in ws: [2, h, w, C]; dims = {h, w, C}
-const float* lpips_features(const void* ws, int H, int W, int l, int dims[3]);
+int launch_lpips(const LpNet& net, const float* pred, const float* gt, const uint8_t* mask, int H, int W, int transform,
+                 const float* sk, const LpipsWeights& wts, void* ws, cudaStream_t stream);
+const void* lpips_out(const LpNet& net, const void* ws, int H, int W);
+// The fp32 post-ReLU features of tapped layer l in ws: [2, h, w, C]; dims = {h, w, C}
+const float* lpips_features(const LpNet& net, const void* ws, int H, int W, int l, int dims[3]);
+// The bf16 output buffer of step s (-1: the prep operand) in ws: [2, h, w, ldo] (the prep operand of a parity layout:
+// [2, 4, h, w, 64]); dims = {h, w, ldo}
+const bf16* lpips_step_output(const LpNet& net, const void* ws, int H, int W, int s, int dims[3]);
 
 // ---------------------------------------------------------------------------------------------
 // Ensemble kernels (ensemble.cu)

@@ -7,7 +7,8 @@ Surface normals: the angular error of compute_cosine_error(masked=True) and the 
 including the exact median — four launches and one host synchronisation per sample.
 Intrinsic images: PSNR and SSIM of compute_iid_metric (src/util/metric.py:263-338) with the up-to-scale targets' lstsq
 scale and quantile map — two launches (six for shading and residual) and one host synchronisation per target — and,
-with LPIPS weights, the AlexNet LPIPS of the same maps in the same synchronisation (csrc/lpips.cu)."""
+with LPIPS weights, the AlexNet, VGG16 or SqueezeNet 1.1 LPIPS of the same maps in the same synchronisation
+(csrc/lpips.cu)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -184,13 +185,57 @@ _ALEX_CONVS = ((0, (64, 3, 11, 11)), (3, (192, 64, 5, 5)), (6, (384, 192, 3, 3))
                (10, (256, 256, 3, 3)))
 
 
-class LPIPS:
-    """The weights of torchmetrics' LearnedPerceptualImagePatchSimilarity(net_type="alex") on the device, for
-    evaluate_iid(..., lpips=...). alexnet_state_dict: torchvision AlexNet keys features.{0,3,6,8,10}.{weight,bias} (other
-    keys are ignored); lin_state_dict: lpips / torchmetrics keys lin{0..4}.model.1.weight ([1, C, 1, 1]). Loading the
-    files is the caller's (torch.load(path, weights_only=True)). The convolutions are held in bf16, lin in fp32."""
+def _vgg16_convs():
+    """vgg16().features: (key prefix, weight shape) of the thirteen 3 x 3 convolutions."""
+    idx = (0, 2, 5, 7, 10, 12, 14, 17, 19, 21, 24, 26, 28)
+    cout = (64, 64, 128, 128, 256, 256, 256, 512, 512, 512, 512, 512, 512)
+    return tuple((f"features.{i}", (co, ci, 3, 3)) for i, co, ci in zip(idx, cout, (3,) + cout[:-1]))
 
-    def __init__(self, alexnet_state_dict, lin_state_dict, device=None):
+
+def _squeezenet1_1_convs():
+    """squeezenet1_1().features: (key prefix, weight shape) of conv1 and each Fire module's squeeze, expand1x1 and
+    expand3x3, in that order."""
+    convs = [("features.0", (64, 3, 3, 3))]
+    fires = ((3, 64, 16, 64), (4, 128, 16, 64), (6, 128, 32, 128), (7, 256, 32, 128), (9, 256, 48, 192),
+             (10, 384, 48, 192), (11, 384, 64, 256), (12, 512, 64, 256))
+    for i, cin, sq, e in fires:
+        convs += [(f"features.{i}.squeeze", (sq, cin, 1, 1)), (f"features.{i}.expand1x1", (e, sq, 1, 1)),
+                  (f"features.{i}.expand3x3", (e, sq, 3, 3))]
+    return tuple(convs)
+
+
+# net_type -> (C ABI net, name, convolutions, channels of each lin layer): torchmetrics' vendored lpips pretrained_networks
+LPIPS_NETS = {
+    "alex": (0, "AlexNet", tuple((f"features.{i}", shape) for i, shape in _ALEX_CONVS), (64, 192, 384, 256, 256)),
+    "vgg": (1, "VGG16", _vgg16_convs(), (64, 128, 256, 512, 512)),
+    "squeeze": (2, "SqueezeNet 1.1", _squeezenet1_1_convs(), (64, 128, 256, 384, 384, 512, 512)),
+}
+
+
+def lpips_min_size(net_type: str = "alex") -> int:
+    """The smallest H (and W) evaluate_iid accepts with LPIPS weights of `net_type`: the smallest for which every tapped
+    layer of the torchvision module is non-empty (31 alex, 16 vgg, 17 squeeze)."""
+    if net_type not in LPIPS_NETS:
+        raise ValueError(f"unsupported net_type {net_type!r}; expected one of {tuple(LPIPS_NETS)}")
+    return int(_lib.load().mgb_lpips_min_size(LPIPS_NETS[net_type][0]))
+
+
+class LPIPS:
+    """The weights of torchmetrics' LearnedPerceptualImagePatchSimilarity(net_type=net_type) on the device, for
+    evaluate_iid(..., lpips=...). net_state_dict: the torchvision state dict of the backbone (other keys are ignored):
+      "alex" (default)  alexnet() keys features.{0,3,6,8,10}.{weight,bias}
+      "vgg"             vgg16() keys features.{0,2,5,7,10,12,14,17,19,21,24,26,28}.{weight,bias}
+      "squeeze"         squeezenet1_1() keys features.0.{weight,bias} and
+                        features.{3,4,6,7,9,10,11,12}.{squeeze,expand1x1,expand3x3}.{weight,bias}
+    lin_state_dict: lpips / torchmetrics keys lin{0..4}.model.1.weight (lin{0..6} for "squeeze"), each [1, C, 1, 1].
+    Loading the files is the caller's (torch.load(path, weights_only=True)). The convolutions are held in bf16, lin in
+    fp32. A missing key, a misshaped tensor or an unknown net_type raises ValueError."""
+
+    def __init__(self, net_state_dict, lin_state_dict, device=None, *, net_type: str = "alex"):
+        if net_type not in LPIPS_NETS:
+            raise ValueError(f"unsupported net_type {net_type!r}; expected one of {tuple(LPIPS_NETS)}")
+        net, self.net_name, convs, chans = LPIPS_NETS[net_type]
+
         def get(sd, key, shape, what):
             if key not in sd:
                 raise ValueError(f"{what} has no {key!r}")
@@ -199,26 +244,27 @@ class LPIPS:
                 raise ValueError(f"{what}[{key!r}] has shape {tuple(t.shape)}, expected {tuple(shape)}")
             return t.to("cpu", torch.float32).contiguous()
 
-        host = []
-        for l, (idx, shape) in enumerate(_ALEX_CONVS):
-            host.append((get(alexnet_state_dict, f"features.{idx}.weight", shape, "alexnet_state_dict"),
-                         get(alexnet_state_dict, f"features.{idx}.bias", shape[:1], "alexnet_state_dict"),
-                         get(lin_state_dict, f"lin{l}.model.1.weight", (1, shape[0], 1, 1), "lin_state_dict")))
+        what = "alexnet_state_dict" if net_type == "alex" else "net_state_dict"
+        ws = [get(net_state_dict, f"{k}.weight", shape, what) for k, shape in convs]
+        bs = [get(net_state_dict, f"{k}.bias", shape[:1], what) for k, shape in convs]
+        lins = [get(lin_state_dict, f"lin{l}.model.1.weight", (1, c, 1, 1), "lin_state_dict") for l, c in enumerate(chans)]
         dev = torch.device("cuda" if device is None else device)
         self.device = dev if dev.index is not None else torch.device("cuda", torch.cuda.current_device())
-        vp5 = C.c_void_p * 5
-        shapes = (C.c_int32 * 20)(*[s for _, shape in _ALEX_CONVS for s in shape])
-        chans = (C.c_int32 * 5)(*[shape[0] for _, shape in _ALEX_CONVS])
+        self.net_type = net_type
+        vp = lambda ts: (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])  # noqa: E731
+        shapes = (C.c_int32 * (4 * len(convs)))(*[s for _, shape in convs for s in shape])
+        lin_c = (C.c_int32 * len(chans))(*chans)
         lib = _lib.load()
         h = C.c_void_p()
         with torch.cuda.device(self.device):
-            check(lib.mgb_lpips_create(vp5(*[w.data_ptr() for w, _, _ in host]), shapes, vp5(*[b.data_ptr() for _, b, _ in host]),
-                                       vp5(*[n.data_ptr() for _, _, n in host]), chans, C.byref(h)), "mgb_lpips_create")
+            check(lib.mgb_lpips_create_net(net, len(convs), vp(ws), shapes, vp(bs), len(chans), vp(lins), lin_c, C.byref(h)),
+                  "mgb_lpips_create_net")
         self._lib, self._h = lib, h
+        self.min_size = int(lib.mgb_lpips_min_size(net))
         self._ws = None
 
     def _workspace(self, H: int, W: int) -> torch.Tensor:
-        need = int(self._lib.mgb_lpips_ws_bytes(H, W))
+        need = int(self._lib.mgb_lpips_ws_bytes_h(self._h, H, W))
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         return self._ws
@@ -241,11 +287,11 @@ def evaluate_iid(pred: torch.Tensor, gt: torch.Tensor, target_name: str, valid_m
                  transform: Optional[str] = None, lpips: Optional[LPIPS] = None) -> Tuple[Dict[str, float], Dict[str, object]]:
     """PSNR, SSIM and, given `lpips`, LPIPS of one intrinsic-image target of one sample: compute_iid_metric
     (src/util/metric.py:263-338) as script/iid/eval.py:182-213 calls it, with torchmetrics' PeakSignalNoiseRatio and
-    StructuralSimilarityIndexMeasure (data_range=1.0) and LearnedPerceptualImagePatchSimilarity(net_type="alex",
+    StructuralSimilarityIndexMeasure (data_range=1.0) and LearnedPerceptualImagePatchSimilarity(net_type=lpips.net_type,
     normalize=True), one host synchronisation per call.
 
-    pred, gt: [3, H, W] or [1, 3, H, W] CUDA tensors, H and W >= 11 (>= 31 with lpips: AlexNet's second pool needs a
-    3 x 3 input). valid_mask: bool [3, H, W] (one mask per channel, as the datasets build it) or None. transform: None,
+    pred, gt: [3, H, W] or [1, 3, H, W] CUDA tensors, H and W >= 11 and, with lpips, >= lpips.min_size (31 alex: its
+    second pool needs a 3 x 3 input; 16 vgg; 17 squeeze). valid_mask: bool [3, H, W] (one mask per channel, as the datasets build it) or None. transform: None,
     "srgb2linear" or "linear2srgb", applied to both maps first (the caller decides it per dataset and target, as eval.py
     does). "shading" and "residual" are up to scale: the prediction is fitted to gt by least squares and both are mapped
     to [0, 1] by the brightness quantile of gt. LPIPS sees the maps SSIM sees (invalid elements 0), which must lie in
@@ -266,8 +312,8 @@ def evaluate_iid(pred: torch.Tensor, gt: torch.Tensor, target_name: str, valid_m
     H, W = pred.shape[-2:]
     if H < 11 or W < 11:
         raise ValueError(f"SSIM's 11 x 11 window needs H, W >= 11, got {H} x {W}")
-    if lpips is not None and (H < 31 or W < 31):
-        raise ValueError(f"LPIPS (AlexNet) needs H, W >= 31, got {H} x {W}")
+    if lpips is not None and (H < lpips.min_size or W < lpips.min_size):
+        raise ValueError(f"LPIPS ({lpips.net_name}) needs H, W >= {lpips.min_size}, got {H} x {W}")
     up_to_scale = target_name in ("shading", "residual")
     p, g, m = _inputs(pred, gt, valid_mask)
     if lpips is not None and lpips._h is None:

@@ -6,8 +6,9 @@ torch lstsq, torch.quantile read back with float(), one .item() per metric; the 
 quantile for each metric it computes). LPIPS: evaluate_iid(..., lpips=...) against compute_iid_metric's "lpips" call
 restated on the GPU (the lstsq and quantile of the up-to-scale targets, the zeroing, torchvision's AlexNet and the
 restated head of tests/lpips_ref.py in float32, one .item()) under torch's default cuDNN TF32 setting, which the output
-records. Both on the fabricated weights of tests/lpips_ref.py. Prints one JSON line with the card's name and power
-limit.
+records. Both on the fabricated weights of tests/lpips_ref.py. The VGG16 and SqueezeNet 1.1 LPIPS the same way
+(keys iid_<target>_lpips_<net>_*), against torchvision's float32 module and the head of tests/lpips_nets_ref.py, on its
+fabricated weights. Prints one JSON line with the card's name and power limit.
 
     python tools/eval_time.py [--reps 20]
 """
@@ -25,7 +26,7 @@ import torch  # noqa: E402
 from bench import gpu_identity  # noqa: E402
 from marigold_b200.evaluation import evaluate_depth, evaluate_iid, evaluate_normals  # noqa: E402
 from marigold_b200.evaluation import LPIPS  # noqa: E402
-from tests import eval_ref, iid_eval_ref, lpips_ref  # noqa: E402
+from tests import eval_ref, iid_eval_ref, lpips_nets_ref, lpips_ref  # noqa: E402
 
 
 def _time(fn, reps):
@@ -82,6 +83,10 @@ def main():
            "cudnn_allow_tf32": torch.backends.cudnn.allow_tf32}
     weights = lpips_ref.fabricated_weights(0)
     lp, metric = LPIPS(*weights), lpips_ref.Lpips32(*weights)
+    nets = {}
+    for net_type in ("vgg", "squeeze"):
+        w = lpips_nets_ref.fabricated_weights(net_type, 0)
+        nets[net_type] = (LPIPS(*w, net_type=net_type), lpips_nets_ref.Net32(net_type, *w))
     g = torch.Generator(device="cuda").manual_seed(0)
     for H, W in [(480, 640), (1080, 1920)]:
         gt = torch.randn(3, H, W, device="cuda", generator=g)
@@ -116,6 +121,13 @@ def main():
                 f"iid_{target}_lpips_reference_path": _time(lambda: _ref_lpips(metric, ipred.clamp(0, 1), igt, target,
                                                                                imask), a.reps),
             })
+            for net_type, (nlp, nmetric) in nets.items():
+                res["cases"][f"{H}x{W}"].update({
+                    f"iid_{target}_lpips_{net_type}_device": _time(
+                        lambda: evaluate_iid(ipred.clamp(0, 1), igt, target, imask, lpips=nlp), a.reps),
+                    f"iid_{target}_lpips_{net_type}_reference_path": _time(
+                        lambda: _ref_lpips(nmetric, ipred.clamp(0, 1), igt, target, imask), a.reps),
+                })
     print(json.dumps(res))
 
 
