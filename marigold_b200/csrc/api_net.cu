@@ -535,6 +535,49 @@ static UNetStaging stage_unet(mgb_handle* h, Arena& a, int NB, int HW) {
   return {f32(size_t(NB) * HW * 4 * 4), f32(n), f32(n), f32(n)};
 }
 
+static size_t weight_bytes(const mgb_handle* h) {
+  size_t n = 0;
+  for (const auto& w : h->weights) n += w.bytes();
+  return n;
+}
+
+// What any call that decodes needs beside the workspace and the weights, at least: the CUDA context of a process that has
+// loaded torch and this library (measured 0.90 GB on an H100 80GB HBM3), and per output pixel the smallest reserve a
+// pipeline call holds, one depth member's (pipeline.call_reserve_bytes(h, w, 1, 1): 4 (1 * 4 + 3) bytes).
+constexpr size_t kDecodeContextBytes = size_t(768) << 20;
+constexpr size_t kDecodeReservePerPixel = 28;
+
+// Whether a decode of lh x lw latents runs its first full-resolution resnet in place (Ctx::dec_low_memory): where one
+// member's decode on the default path cannot be admitted on this device, i.e. needs more than its memory less the
+// weights, kDecodeContextBytes and kDecodeReservePerPixel per pixel. No decode that the default path could run is
+// moved, since each needs at least that much beside its workspace; or as mgb_debug_vae_low_memory sets it. The
+// decision depends on the shape and the VAE attention's row blocking alone, and is kept for the last shape asked.
+static int decode_low_memory(mgb_handle* h, int lh, int lw, bool* on) {
+  if (h->vae_low_memory != 0) { *on = h->vae_low_memory > 0; return MGB_OK; }
+  mgb_handle::DecodeRule& k = h->decode_rule;
+  if (k.valid && k.lh == lh && k.lw == lw && k.attn_budget == h->vae_attn_budget && k.attn_rows == h->vae_attn_force_rows) {
+    *on = k.in_place;
+    return MGB_OK;
+  }
+  if (h->device_bytes == 0) {
+    size_t free_b = 0, total = 0;
+    CUDA_TRY(cudaMemGetInfo(&free_b, &total));
+    h->device_bytes = total;
+  }
+  Arena dry; dry.dry = true;
+  Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
+  c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
+  c.arena->start();
+  c.planned = true;
+  TRY(vae_decode_forward(h, c, nullptr, nullptr, 1, lh, lw, 0));
+  dry.finish();
+  const size_t need = arena_place(dry.rec, 0) + c.splitk_need;
+  const size_t pixels = size_t(64) * lh * lw;
+  *on = need + weight_bytes(h) + kDecodeContextBytes + kDecodeReservePerPixel * pixels > h->device_bytes;
+  k = {true, lh, lw, h->vae_attn_budget, h->vae_attn_force_rows, *on};
+  return MGB_OK;
+}
+
 // a0..a3 meaning per op:
 //   UNET:   a0 = rgb latent NCHW, a1 = target NCHW (in/out), a2 = noise NCHW or null, a3 = model_out NCHW or null
 //   ENCODE: a0 = rgb NCHW, a1 = latent out NCHW
@@ -544,7 +587,10 @@ static int run_graph(mgb_handle* h, Ctx& c, int op, const float* a0, float* a1, 
   c.arena->start();
   c.planned = op != OP_UNET;
   if (op == OP_ENCODE) return vae_encode_forward(h, c, a0, a1, NB, d0, d1);
-  if (op == OP_DECODE) return vae_decode_forward(h, c, a0, a1, NB, d0, d1, mode);
+  if (op == OP_DECODE) {
+    TRY(decode_low_memory(h, d0, d1, &c.dec_low_memory));
+    return vae_decode_forward(h, c, a0, a1, NB, d0, d1, mode);
+  }
   // UNET single step through NCHW <-> NHWC conversions
   const int HW = d0 * d1, Ct = h->cfg.unet_out_channels;
   const UNetStaging s = stage_unet(h, *c.arena, NB, HW);
@@ -961,6 +1007,14 @@ int mgb_debug_arena(mgb_handle* h, int32_t poison, int32_t placement) {
   if (!h || placement < 0 || placement > 1) { set_error("debug_arena: bad argument"); return MGB_ERR_INVALID; }
   h->arena_poison = poison != 0;
   h->arena_placement = placement;
+  return MGB_OK;
+}
+
+// The decoder's full-resolution stage of this handle: mode 1 runs its first resnet in place at every size, -1 never, 0
+// where the library's rule (decode_low_memory) asks for it. Outputs are the same bits either way.
+int mgb_debug_vae_low_memory(mgb_handle* h, int32_t mode) {
+  if (!h || mode < -1 || mode > 1) { set_error("debug_vae_low_memory: bad argument"); return MGB_ERR_INVALID; }
+  h->vae_low_memory = mode;
   return MGB_OK;
 }
 

@@ -63,6 +63,24 @@ int launch_upsample2x(const float* x, bf16* y, int NB, int H, int W, int C, int 
                     reinterpret_cast<uint2*>(y), NB, H, W, Ho, Wo, C / 4);
 }
 
+// A block's 256 threads cover 256 / Q rows of Q quads each; no division in the loop.
+__global__ void copy_rows_kernel(const float4* __restrict__ x, long long lqx, float4* __restrict__ y, long long M, int Q) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int q = threadIdx.x % Q, rows = blockDim.x / Q;
+  for (long long m = (long long)blockIdx.x * rows + threadIdx.x / Q; m < M; m += (long long)gridDim.x * rows)
+    y[m * Q + q] = __ldg(x + m * lqx + q);
+}
+int launch_copy_rows(const float* x, long long ldx, float* y, long long M, int C, cudaStream_t stream) {
+  const int Q = C / 4;
+  if ((C & 3) || (ldx & 3) || ldx < C || Q > 256 || 256 % Q) {
+    set_error("copy_rows: C=%d ldx=%lld", C, ldx);
+    return MGB_ERR_INVALID;
+  }
+  return launch_pdl("copy rows", copy_rows_kernel, grid_for(size_t(M) * Q, 256), 256, 0, stream,
+                    reinterpret_cast<const float4*>(x), ldx / 4, reinterpret_cast<float4*>(y), M, Q);
+}
+
 // UNet conv_in operand (reference marigold_depth_pipeline.py:456-458, marigold_iid_pipeline.py:538-540: rgb latent FIRST):
 // out bf16 [M, 64] = [rgb(4) | target(Ct) | zeros], Ct = 4 (depth / normals) or 4 n (IID with n targets), 4 + Ct <= 64
 __global__ void pack_latents_kernel(const float4* __restrict__ rgb, const float4* __restrict__ tgt,

@@ -227,9 +227,10 @@ static Tile matmul_tile(int M, int N, int K, int flags) {
   return linear_tile(M, W, flags);
 }
 
-// 3x3 conv on NHWC bf16; Hout x Wout output; kind per ops.cu
+// 3x3 conv on NHWC bf16; Hout x Wout output; kind per ops.cu. ldo: the output's row stride (0: W.cout); ld2: x2's
+// pixel stride (0: its channel count). Neither changes the tile, the split or any output value.
 static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const ConvW& W, int kind, const Epi& e,
-                   int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr) {
+                   int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr, int ldo = 0, int ld2 = 0) {
   int tw, th;
   conv_tile_shape(Hout, Wout, &tw, &th);
   const int m_tiles = NB * ((Wout + tw - 1) / tw) * ((Hout + th - 1) / th);
@@ -240,10 +241,11 @@ static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const Conv
   if (sp > 1) c.splitk_need = std::max(c.splitk_need, size_t(sp) * M * W.cout * sizeof(float));
   if (c.dry) return MGB_OK;
   GemmParams p;
-  TRY(fill_conv_params(&p, x, W.w, NB, Hout, Wout, W.cin_pad, W.cout, kind, bn, sp, st, Hsrc, Wsrc, x2, W.k_extra));
+  TRY(fill_conv_params(&p, x, W.w, NB, Hout, Wout, W.cin_pad, W.cout, kind, bn, sp, st, Hsrc, Wsrc, x2, W.k_extra,
+                       ld2));
   Epi e2 = e;
   e2.hw = Hout * Wout;
-  return gemm_common(c, p, bn, effective_splits(p), e2, W.cout);
+  return gemm_common(c, p, bn, effective_splits(p), e2, ldo > 0 ? ldo : W.cout);
 }
 
 #define LAUNCH(call)               \
@@ -332,6 +334,66 @@ static int resnet_forward(Ctx& c, const ResnetW& R, Act& x, Act* skip, Act& y, i
   } else {
     c.arena->release(mk);
   }
+  return MGB_OK;
+}
+
+// GroupNorm statistics of x [NB * HW, C] at a row stride of ldx floats into stats (launch_gn_stats), with
+// groupnorm()'s scratch and barrier counter
+static int groupnorm_stats(Ctx& c, const float* x, int C, int ldx, float2* stats, const NormW& n, int NB, int HW,
+                           float eps) {
+  void* part = aalloc<char>(c, groupnorm_part_bytes(NB, HW, C, c.groups));
+  const size_t coff = c.sync_off;
+  c.sync_off += size_t(NB);
+  if (c.sync_off > c.sync_need) c.sync_need = c.sync_off;
+  int rc = MGB_OK;
+  if (!c.dry) {
+    if (c.sync_off > c.sync_cap) { set_error("groupnorm: barrier counter slab exhausted"); return MGB_ERR_STATE; }
+    rc = launch_gn_stats(x, C, ldx, stats, n.g, n.b, NB, HW, c.groups, eps, part, c.sync_base + coff, c.stream);
+  }
+  c.arena->free(part);
+  return rc;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The ResnetBlock2D with a 1x1 shortcut over cin = 2 cout channels, in the memory of its input x alone plus one bf16
+// cin-channel map: three fp32 cout-channel maps where resnet_forward takes four (x, t1 and raw at its first GroupNorm).
+// Same operands, tiles and splits as resnet_forward, hence the same bits. Planned arena only; consumes x.
+// Each row of x (cin floats) is reused in place once GroupNorm has read it:
+//   bytes [0, 2 cin)       raw = bf16(x), the shortcut's operand, written by the apply launch over its own row;
+//   bytes [2 cin, 4 cin)   h = conv1's output, then y = conv2's. conv1 reads only t1, and conv2 reads t2 and raw, so
+//                          neither writes a byte that any CTA of its grid reads.
+// y is then copied out to a packed buffer of its own, which is where the next block reads it.
+// ---------------------------------------------------------------------------------------------
+static int resnet_shortcut_in_place(Ctx& c, const ResnetW& R, Act& x, Act& y, int NB, int H, int W) {
+  if (R.cin != 2 * R.cout || !R.has_sc || !c.planned) {
+    set_error("resnet in place: needs a planned arena and a 1x1 shortcut over cin = 2 cout (got %d -> %d)", R.cin, R.cout);
+    return MGB_ERR_STATE;
+  }
+  const int HW = H * W, cin = R.cin, cout = R.cout;
+  const size_t M = size_t(NB) * HW;
+  float2* st = aalloc<float2>(c, size_t(NB) * cin);
+  TRY(groupnorm_stats(c, x.p, cin, cin, st, R.n1, NB, HW, R.eps));
+  bf16* t1 = aalloc<bf16>(c, M * cin);
+  bf16* raw = reinterpret_cast<bf16*>(x.p);
+  LAUNCH(launch_gn_apply_rows(x.p, cin, st, t1, raw, 2 * cin, NB, HW, cin, 1, c.stream));
+  c.arena->free(st);
+  float* hy = x.p + cout;   // h, then y: the second half of each row of x
+  Epi e1;
+  e1.bias = (R.bias_off >= 0 && c.cur_bias) ? c.cur_bias + R.bias_off : R.c1.b;
+  e1.out_f32 = hy;
+  TRY(conv3x3(c, t1, NB, H, W, R.c1, 0, e1, 0, 0, nullptr, cin));
+  c.arena->free(t1);
+  st = aalloc<float2>(c, size_t(NB) * cout);
+  TRY(groupnorm_stats(c, hy, cout, cin, st, R.n2, NB, HW, R.eps));
+  bf16* t2 = aalloc<bf16>(c, M * cout);
+  LAUNCH(launch_gn_apply_rows(hy, cin, st, t2, nullptr, 0, NB, HW, cout, 1, c.stream));
+  c.arena->free(st);
+  Epi e2; e2.bias = R.c2.b; e2.out_f32 = hy;
+  TRY(conv3x3(c, t2, NB, H, W, R.c2, 0, e2, 0, 0, raw, cin, 2 * cin));
+  c.arena->free(t2);
+  y = act_alloc(c, M, cout);
+  LAUNCH(launch_copy_rows(hy, cin, y.p, (long long)M, cout, c.stream));
+  c.arena->free(x.p);
   return MGB_OK;
 }
 
@@ -572,7 +634,9 @@ int unet_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* tgt, const flo
 // VAE forwards. Their arena is lifetime-planned (api_net.cu): every buffer is allocated where it is first written and
 // freed after its last read, so the memory live at once stays near the largest working set of one step. At full
 // resolution that is the decoder's first up-level resnet's GroupNorm: its 256-channel fp32 input and the two bf16
-// copies it writes.
+// copies it writes, 4 U (U = one fp32 128-channel map). With c.dec_low_memory that resnet runs in place
+// (resnet_shortcut_in_place), the two after it free their input and allocate their output as late as they can, and the
+// decoder's peak is 3 U: that resnet, and the up-conv before it (its bf16 operand and fp32 output).
 // ---------------------------------------------------------------------------------------------
 // mid block: resnet, attention, resnet; consumes h and leaves the result in it
 static int vae_mid_forward(Ctx& c, const ResnetW& r0, const VaeAttnW& A, const ResnetW& r1, Act& h, int NB, int H,
@@ -661,6 +725,19 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
   for (int i = 0; i < 4; ++i) {
     const int cout = ch[3 - i];
     buf[0] = buf[1] = Act();   // ping-pong trunk buffers, each allocated by the resnet that first writes it
+    if (c.dec_low_memory && i == 3) {
+      // Full resolution in 3 U: the first resnet in place, and every block's output a buffer of its own, allocated
+      // after the block's conv1 output is freed, with the block's input freed after its last read. (The ping-pong
+      // pair below holds both 128-channel trunk maps through every block: 3.5 U in the next two.)
+      for (int j = 0; j < L + 1; ++j) {
+        Act y;
+        if (j == 0) TRY(resnet_shortcut_in_place(c, V.dec_res[ri++], h, y, NB, H, W));
+        else TRY(resnet_forward(c, V.dec_res[ri++], h, nullptr, y, NB, H, W, true));
+        h = y; cur = cout;
+      }
+      buf[0] = h;     // freed after dec_norm_out below
+      continue;
+    }
     for (int j = 0; j < L + 1; ++j) {
       TRY(resnet_forward(c, V.dec_res[ri++], h, nullptr, buf[j & 1], NB, H, W, j == 0));
       h = buf[j & 1]; cur = cout;

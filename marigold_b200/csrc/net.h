@@ -134,6 +134,7 @@ struct Ctx {
   int attn_rows = 0;
   bool planned = false;    // the arena is lifetime-planned (the VAE forwards): buffers are freed after their last read
   bool poison = false;     // fill every buffer the arena hands out with 0xFF bytes (NaN in fp32 and bf16) first
+  bool dec_low_memory = false;   // the decoder's first full-resolution resnet runs in place (net.cu)
   float* splitk_ws = nullptr;
   size_t splitk_cap = 0;   // bytes available
   size_t splitk_need = 0;  // bytes needed (dry run)
@@ -196,6 +197,17 @@ struct mgb_handle {
   std::vector<mgb::ArenaBuf> arena_plan;
   int arena_placement = 0;
   bool arena_poison = false;
+  // The decoder's full-resolution stage in low memory (Ctx::dec_low_memory): 0 where one member's default decode does
+  // not fit the device beside the weights (decode_low_memory, api_net.cu), 1 always, -1 never (mgb_debug_vae_low_memory)
+  int vae_low_memory = 0;
+  size_t device_bytes = 0;          // the device's memory, read once
+  struct DecodeRule {                // the rule's last decision (decode_low_memory)
+    bool valid = false;
+    int lh = 0, lw = 0;
+    size_t attn_budget = 0;
+    int attn_rows = 0;
+    bool in_place = false;
+  } decode_rule;
   // conditioning / schedule
   bool text_set = false;
   int n_steps = 0;

@@ -30,12 +30,16 @@ static __device__ __noinline__ void gn_barrier_timeout(unsigned seen, unsigned w
   __trap();
 }
 
-template <int KQ>
+// kStats: statistics only. The source is xa alone at a row stride of lda floats, and instead of the normalised
+// operand the kernel writes each channel's (scale, shift) = (rstd gamma, beta - mean rstd gamma) to stats [NB][Ca],
+// from the same registers phase 2 applies them from: gn_apply_rows applies them bit for bit as this kernel would.
+template <int KQ, bool kStats = false>
 __global__ void __launch_bounds__(kGnThreads, kGnCtasPerSm)
     gn_fused_kernel(const float* __restrict__ xa, int Ca, const float* __restrict__ xb, int Cb, bf16* __restrict__ y,
                     bf16* __restrict__ raw, const float* __restrict__ gamma, const float* __restrict__ beta, int HW, int G,
                     float eps, int silu, GnGeom g, float2* __restrict__ part /* [NB][chunks][G] */,
-                    unsigned* __restrict__ counter /* [NB], zero on entry */) {
+                    unsigned* __restrict__ counter /* [NB], zero on entry */, int lda = 0,
+                    float2* __restrict__ stats = nullptr) {
   constexpr int R = kGnLoads / KQ;
   extern __shared__ float2 s_ch[];   // phase 1: [Tp][C] per-channel (sum, sumsq); phase 2: mean[G] | rstd[G] as floats
   const int img = blockIdx.y, chunk = blockIdx.x, chunks = gridDim.x;
@@ -44,7 +48,8 @@ __global__ void __launch_bounds__(kGnThreads, kGnCtasPerSm)
   const bool active = tp < g.Tp;
   const int p0 = chunk * g.P, p1 = min(HW, p0 + g.P);
   const int Qa = Ca / 4, Qb = Cb / 4;
-  const float4* xai = reinterpret_cast<const float4*>(xa + (size_t)img * HW * Ca);
+  const int lqa = kStats ? lda / 4 : Qa;   // row stride of source a, in quads
+  const float4* xai = reinterpret_cast<const float4*>(xa + (size_t)img * HW * lqa * 4);
   const float4* xbi = xb ? reinterpret_cast<const float4*>(xb + (size_t)img * HW * Cb) : nullptr;
   pdl_wait();
 
@@ -52,7 +57,7 @@ __global__ void __launch_bounds__(kGnThreads, kGnCtasPerSm)
   // quad qd of the concatenated channel space lives in source a (qd < Qa) or b
   auto px = [&](int k, int p) -> const float4* {
     const int qd = tq + k * g.Tq;
-    return qd < Qa ? xai + (size_t)p * Qa + qd : xbi + (size_t)p * Qb + (qd - Qa);
+    return qd < Qa ? xai + (size_t)p * lqa + qd : xbi + (size_t)p * Qb + (qd - Qa);
   };
   float4 v[KQ][R];
   float sum[KQ][4], sq[KQ][4];
@@ -195,6 +200,15 @@ __global__ void __launch_bounds__(kGnThreads, kGnCtasPerSm)
       sh[k][j] = bev[j] - s_stat[gj] * rstd * gav[j];
     }
   }
+  if constexpr (kStats) {
+    if (chunk == 0 && tp == 0) {
+#pragma unroll
+      for (int k = 0; k < KQ; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) stats[(size_t)img * C + 4 * (tq + k * g.Tq) + j] = make_float2(sc[k][j], sh[k][j]);
+    }
+    return;
+  }
   uint2* yo = reinterpret_cast<uint2*>(y + (size_t)img * HW * C);
   uint2* ro = raw ? reinterpret_cast<uint2*>(raw + (size_t)img * HW * C) : nullptr;
   for (int pb = p0 + tp;;) {
@@ -277,7 +291,79 @@ int launch_gn_fused(const float* xa, int Ca, const float* xb, int Cb, bf16* y, b
   float2* pp = static_cast<float2*>(part);
   auto kern = g.Kq == 1 ? gn_fused_kernel<1> : g.Kq == 2 ? gn_fused_kernel<2> : gn_fused_kernel<4>;
   return launch_pdl("groupnorm", kern, grid, kGnThreads, smem, stream, xa, Ca, xb, Cb, y, raw_copy, gamma, beta, HW, G, eps,
-                    silu, g, pp, counters);
+                    silu, g, pp, counters, 0, nullptr);
+}
+
+// GroupNorm statistics of x [NB, HW, C] at a row stride of ldx floats (>= C): per image and channel the (scale, shift)
+// that launch_gn_fused applies, to stats [NB][C]. part and counters as launch_gn_fused's.
+int launch_gn_stats(const float* x, int C, int ldx, float2* stats, const float* gamma, const float* beta, int NB, int HW,
+                    int G, float eps, void* part, unsigned* counters, cudaStream_t stream) {
+  GnGeom g;
+  if ((C & 3) || (ldx & 3) || ldx < C || !stats || !gn_plan(NB, HW, C, G, &g)) {
+    set_error("groupnorm stats: unsupported NB=%d C=%d ldx=%d G=%d", NB, C, ldx, G);
+    return MGB_ERR_INVALID;
+  }
+  dim3 grid(g.chunks, NB);
+  const size_t smem = std::max(size_t(g.Tp) * C * sizeof(float2), size_t(2) * G * sizeof(float));
+  if (smem > 40 * 1024) { set_error("groupnorm stats: C=%d needs %zu B of shared memory", C, smem); return MGB_ERR_INVALID; }
+  float2* pp = static_cast<float2*>(part);
+  auto kern = g.Kq == 1 ? gn_fused_kernel<1, true> : g.Kq == 2 ? gn_fused_kernel<2, true> : gn_fused_kernel<4, true>;
+  return launch_pdl("groupnorm stats", kern, grid, kGnThreads, smem, stream, x, C, nullptr, 0, nullptr, nullptr, gamma,
+                    beta, HW, G, eps, 0, g, pp, counters, ldx, stats);
+}
+
+// The apply phase of GroupNorm over rows given their statistics (launch_gn_stats): one warp per pixel row of
+// C = 128 NQ channels. y [M, C] = bf16(act(x * scale + shift)) with the GroupNorm kernel's operations in its order, and,
+// when raw is set, raw = bf16(x) at a row stride of ldr elements. raw may lie over x itself: a row's raw copy is written
+// only over bytes of that same row (ldr = 2 ldx, the copy in the first half of the fp32 row), and only after the whole
+// warp has read the row (__syncwarp orders the warp's loads before its stores); no other warp touches the row. Hence
+// plain loads here, not the read-only path.
+template <int NQ>
+__global__ void __launch_bounds__(256) gn_apply_rows_kernel(const float* x, long long ldx, const float2* __restrict__ stats,
+                                                            bf16* __restrict__ y, bf16* raw, long long ldr, int HW, int C,
+                                                            int silu, long long M) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long m = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); m < M; m += warps) {
+    const float2* st = stats + (m / HW) * C;
+    const float4* xr = reinterpret_cast<const float4*>(x + m * ldx);
+    float4 t[NQ];
+#pragma unroll
+    for (int i = 0; i < NQ; ++i) t[i] = xr[lane + 32 * i];
+    uint2* yo = reinterpret_cast<uint2*>(y + m * C);
+#pragma unroll
+    for (int i = 0; i < NQ; ++i) {
+      const int c = 4 * (lane + 32 * i);
+      const float4 a = __ldg(reinterpret_cast<const float4*>(st + c)), b = __ldg(reinterpret_cast<const float4*>(st + c + 2));
+      float o0 = fmaf(t[i].x, a.x, a.y), o1 = fmaf(t[i].y, a.z, a.w), o2 = fmaf(t[i].z, b.x, b.y), o3 = fmaf(t[i].w, b.z, b.w);
+      if (silu) { o0 = silu_f(o0); o1 = silu_f(o1); o2 = silu_f(o2); o3 = silu_f(o3); }
+      yo[lane + 32 * i] = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));
+    }
+    if (raw) {
+      __syncwarp();
+      uint2* ro = reinterpret_cast<uint2*>(raw + m * ldr);
+#pragma unroll
+      for (int i = 0; i < NQ; ++i)
+        ro[lane + 32 * i] = make_uint2(pack_bf16x2(t[i].x, t[i].y), pack_bf16x2(t[i].z, t[i].w));
+    }
+    __syncwarp();
+  }
+}
+
+int launch_gn_apply_rows(const float* x, long long ldx, const float2* stats, bf16* y, bf16* raw, long long ldr, int NB,
+                         int HW, int C, int silu, cudaStream_t stream) {
+  const bool in_place = raw && reinterpret_cast<const void*>(raw) == reinterpret_cast<const void*>(x);
+  if ((C != 128 && C != 256 && C != 512) || ldx < C || (ldx & 3) || (raw && (ldr < C || (ldr & 3))) ||
+      (raw && !in_place && ldr != C) || (in_place && ldr != 2 * ldx)) {
+    set_error("groupnorm apply rows: unsupported C=%d ldx=%lld ldr=%lld", C, ldx, ldr);
+    return MGB_ERR_INVALID;
+  }
+  const long long M = (long long)NB * HW;
+  const int blocks = int(std::min<long long>((M + 7) / 8, 64LL * kNumSMs));
+  auto kern = C == 128 ? gn_apply_rows_kernel<1> : C == 256 ? gn_apply_rows_kernel<2> : gn_apply_rows_kernel<4>;
+  return launch_pdl("groupnorm apply rows", kern, blocks, 256, 0, stream, x, ldx, stats, y, raw, ldr, HW, C, silu, M);
 }
 
 // Stand-alone GroupNorm (operator-level ABI): ws = groupnorm_ws_bytes() of scratch (counters zeroed here).

@@ -5,8 +5,11 @@ power limit, read in the same run. Then 24 MP (6048 x 4032): depth with E = 1 an
 normals, and a 2-target IID model (each its numbers, or the error with the bytes it needed); the largest 4:3 and 3:2
 photos select_batch_size accepts for one depth member on this card; mgb_workspace_bytes at the batch caps and the
 native sizes. Then a 1920 x 1080 decode with the VAE attention in one block against its default row blocks, alternated.
+48 MP (8064 x 6048), where the decoder runs its first full-resolution resnet in place: depth with E = 1 and 1 step.
 
-    python tools/native_res.py [--out DIR]      (prints one JSON line; with --out also writes DIR/native_res.json)
+    python tools/native_res.py [--out DIR] [--only-48mp]
+        (prints one JSON line; with --out also writes DIR/native_res.json; --only-48mp: the card, the 48 MP run and the
+        largest photos accepted)
 """
 import argparse
 import ctypes as C
@@ -165,9 +168,15 @@ def attention_ab(eng, reps=5):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
+    ap.add_argument("--only-48mp", action="store_true")
     a = ap.parse_args()
     res = {"card": gpu_identity(torch.cuda.current_device()), "runs": []}
     eng = make_engine()
+    if a.only_48mp:
+        res["mp48"] = try_run(eng, "depth", 6048, 8064, 1, 1)
+        res["largest_accepted"] = {"4:3": largest_accepted(eng, (4, 3)), "3:2": largest_accepted(eng, (3, 2))}
+        eng.close()
+        return _emit(res, a.out)
     for (H, W) in ((3000, 4000), (3024, 4032)):
         for E in (1, 10):
             for steps in (1, 4):
@@ -176,6 +185,7 @@ def main():
     res["runs"].append(run(eng, "normals", 3000, 4000, 1, 1))
     res["mp24"] = try_run(eng, "depth", 4032, 6048, 1, 1)
     res["mp24_runs"] = [try_run(eng, "depth", 4032, 6048, 10, 4), try_run(eng, "normals", 4032, 6048, 1, 1)]
+    res["mp48"] = try_run(eng, "depth", 6048, 8064, 1, 1)
     res["workspace_bytes"] = {f"{B}x{H}x{W}": eng.workspace_bytes(B, H, W) for B, H, W in
                               ((16, 768, 768), (8, 1024, 1024), (1, 3024, 4032), (2, 3024, 4032), (1, 4032, 6048))}
     res["largest_accepted"] = {"4:3": largest_accepted(eng, (4, 3)), "3:2": largest_accepted(eng, (3, 2))}
@@ -186,11 +196,15 @@ def main():
     res["runs"].append(run(eng, "iid", 3000, 4000, 1, 1))
     res["mp24_runs"].append(try_run(eng, "iid", 4032, 6048, 1, 1))
     eng.close()
+    _emit(res, a.out)
+
+
+def _emit(res, out):
     line = json.dumps(res)
     print(line, flush=True)
-    if a.out:
-        Path(a.out).mkdir(parents=True, exist_ok=True)
-        (Path(a.out) / "native_res.json").write_text(line + "\n")
+    if out:
+        Path(out).mkdir(parents=True, exist_ok=True)
+        (Path(out) / "native_res.json").write_text(line + "\n")
 
 
 if __name__ == "__main__":
