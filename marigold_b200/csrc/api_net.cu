@@ -547,10 +547,10 @@ static size_t weight_bytes(const mgb_handle* h) {
 constexpr size_t kDecodeContextBytes = size_t(768) << 20;
 constexpr size_t kDecodeReservePerPixel = 28;
 
-// Whether a decode of lh x lw latents runs its first full-resolution resnet in place (Ctx::dec_low_memory): where one
-// member's decode on the default path cannot be admitted on this device, i.e. needs more than its memory less the
-// weights, kDecodeContextBytes and kDecodeReservePerPixel per pixel. No decode that the default path could run is
-// moved, since each needs at least that much beside its workspace; or as mgb_debug_vae_low_memory sets it. The
+// Whether a decode of lh x lw latents runs its full-resolution 256-channel stage in low memory (Ctx::dec_low_memory):
+// where one member's decode on the default path cannot be admitted on this device, i.e. needs more than its memory
+// less the weights, kDecodeContextBytes and kDecodeReservePerPixel per pixel. No decode that the default path could
+// run is moved, since each needs at least that much beside its workspace; or as mgb_debug_vae_low_memory sets it. The
 // decision depends on the shape and the VAE attention's row blocking alone, and is kept for the last shape asked.
 static int decode_low_memory(mgb_handle* h, int lh, int lw, bool* on) {
   if (h->vae_low_memory != 0) { *on = h->vae_low_memory > 0; return MGB_OK; }
@@ -618,6 +618,7 @@ static int workspace_need(mgb_handle* h, int op, int NB, int d0, int d1, Workspa
   Arena dry; dry.dry = true;
   Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
   c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
+  c.band_up_tiles = h->vae_band_up_tiles; c.band_conv1_tiles = h->vae_band_conv1_tiles;
   TRY(run_graph(h, c, op, nullptr, nullptr, nullptr, nullptr, 0, NB, d0, d1, 0));
   dry.finish();
   const size_t arena = op == OP_UNET ? dry.peak : arena_place(dry.rec, h->arena_placement);
@@ -664,6 +665,7 @@ static Ctx make_ctx(mgb_handle* h, void* stream) {
   c.splitk_ws = h->splitk_ws; c.splitk_cap = h->splitk_ws.bytes();
   c.groups = h->cfg.norm_groups;
   c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
+  c.band_up_tiles = h->vae_band_up_tiles; c.band_conv1_tiles = h->vae_band_conv1_tiles;
   c.sync_base = h->sync_slab;
   c.sync_cap = h->sync_slab.bytes() / sizeof(unsigned);
   return c;
@@ -1010,11 +1012,21 @@ int mgb_debug_arena(mgb_handle* h, int32_t poison, int32_t placement) {
   return MGB_OK;
 }
 
-// The decoder's full-resolution stage of this handle: mode 1 runs its first resnet in place at every size, -1 never, 0
-// where the library's rule (decode_low_memory) asks for it. Outputs are the same bits either way.
+// The decoder's full-resolution stage of this handle: mode 1 runs it in low memory (the banded up-conv into two halves
+// and the first resnet on them) at every size, -1 never, 0 where the library's rule (decode_low_memory) asks for it.
+// Outputs are the same bits either way.
 int mgb_debug_vae_low_memory(mgb_handle* h, int32_t mode) {
   if (!h || mode < -1 || mode > 1) { set_error("debug_vae_low_memory: bad argument"); return MGB_ERR_INVALID; }
   h->vae_low_memory = mode;
+  return MGB_OK;
+}
+
+// Tile rows per band of the low-memory decoder's banded up-conv and conv1 on this handle (<= 0: the library's choice,
+// about an eighth of the image). Outputs are the same bits at every band height.
+int mgb_debug_vae_bands(mgb_handle* h, int32_t up_tiles, int32_t conv1_tiles) {
+  if (!h) { set_error("debug_vae_bands: bad argument"); return MGB_ERR_INVALID; }
+  h->vae_band_up_tiles = std::max(0, int(up_tiles));
+  h->vae_band_conv1_tiles = std::max(0, int(conv1_tiles));
   return MGB_OK;
 }
 

@@ -180,8 +180,55 @@ int mgb_debug_groupnorm_rows(const float* x, int32_t C, int64_t ldx, void* y, vo
     return MGB_ERR_CUDA;
   }
   float2* st = reinterpret_cast<float2*>(stats);
-  TRY(launch_gn_stats(x, C, int(ldx), st, gamma, beta, NB, HW, G, eps, ws, counters, s));
-  return launch_gn_apply_rows(x, ldx, st, reinterpret_cast<bf16*>(y), reinterpret_cast<bf16*>(raw), ldr, NB, HW, C, silu, s);
+  TRY(launch_gn_stats(x, C, int(ldx), nullptr, 0, st, gamma, beta, NB, HW, G, eps, ws, counters, s));
+  return launch_gn_apply_rows(x, ldx, nullptr, 0, st, reinterpret_cast<bf16*>(y), reinterpret_cast<bf16*>(raw), ldr, NB,
+                              HW, C, silu, s);
+}
+
+// GroupNorm in two launches over the concat [a | b] of two packed fp32 maps of Ch channels each, in their own memory as
+// the decoder's low-memory resnet runs it: raw = bf16([a | b]) [NB * HW, 2 Ch] over a, y [NB * HW, 2 Ch] over b.
+// ws: mgb_op_groupnorm_ws_bytes(NB, HW, 2 Ch, G); stats: NB * 2 Ch float2.
+int mgb_debug_groupnorm_halves(float* a, float* b, int32_t Ch, const float* gamma, const float* beta, float* ws,
+                               void* stats, int32_t NB, int32_t HW, int32_t G, float eps, int32_t silu, void* stream) {
+  if (!a || !b || !ws || !stats || Ch <= 0) { set_error("debug_groupnorm_halves: bad argument"); return MGB_ERR_INVALID; }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const size_t pb = (groupnorm_part_bytes(NB, HW, 2 * Ch, G) + 255) & ~size_t(255);
+  unsigned* counters = reinterpret_cast<unsigned*>(reinterpret_cast<char*>(ws) + pb);
+  if (cudaMemsetAsync(counters, 0, size_t(NB) * sizeof(unsigned), s) != cudaSuccess) {
+    set_error("debug_groupnorm_halves: counter memset failed");
+    return MGB_ERR_CUDA;
+  }
+  float2* st = reinterpret_cast<float2*>(stats);
+  TRY(launch_gn_stats(a, Ch, Ch, b, Ch, st, gamma, beta, NB, HW, G, eps, ws, counters, s));
+  return launch_gn_apply_rows(a, Ch, b, Ch, st, reinterpret_cast<bf16*>(b), reinterpret_cast<bf16*>(a), 2 * Ch, NB, HW,
+                              2 * Ch, silu, s);
+}
+
+// One band of the decoder's banded 3x3 pad-1 convs (net.cu, conv3x3_band): tile rows [ty0, ty0 + tiles) of one
+// H x W image, with the tile the network gives the whole conv over NB_tile such images. x: bf16 [src_rows, W, Cin],
+// image rows [src_y0, src_y0 + src_rows); output pixel (y, x) to fp32 row (y - out_y0) W + x at a row stride of ldo,
+// columns >= split_col to out_hi (or null: all to out). geom (or null) receives {tile_h, tiles_y}; x == null only
+// fills it.
+int mgb_debug_conv2d_band(const void* x, int32_t src_y0, int32_t src_rows, const void* w, const float* bias, float* out,
+                          float* out_hi, int32_t split_col, int32_t ldo, int32_t out_y0, int32_t NB_tile, int32_t H,
+                          int32_t W, int32_t Cin, int32_t Cout, int32_t ty0, int32_t tiles, int32_t* geom, void* stream) {
+  if (NB_tile <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) { set_error("debug_conv2d_band: bad argument"); return MGB_ERR_INVALID; }
+  int tw, th, bn, sp, st;
+  conv_tile_shape(H, W, &tw, &th);
+  const int tiles_y = (H + th - 1) / th;
+  choose_tile(NB_tile * ((W + tw - 1) / tw) * tiles_y, Cout, 9 * Cin / 64, 0, true, &bn, &sp, &st);
+  if (geom) { geom[0] = th; geom[1] = tiles_y; }
+  if (!x) return MGB_OK;
+  if (!w || !out || ldo <= 0 || sp != 1) { set_error("debug_conv2d_band: bad argument or a split-K tile"); return MGB_ERR_INVALID; }
+  GemmParams p;
+  TRY(fill_conv_params(&p, reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(w), 1, H, W, Cin, Cout, 0, bn,
+                       1, st, src_rows, W));
+  TRY(set_conv_band(&p, ty0, tiles, src_y0, out_y0));
+  fill_epi(&p.epi, bias, nullptr, out, nullptr, ldo, 0, 1.0f, nullptr, nullptr, nullptr, nullptr);
+  p.epi.out_f32_hi = out_hi;
+  p.epi.split_col = out_hi ? split_col : 0;
+  p.epi.hw = H * W;
+  return run_gemm(p, bn, nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int mgb_op_layernorm(const float* x, void* y, const float* gamma, const float* beta, int32_t M, int32_t C, float eps,

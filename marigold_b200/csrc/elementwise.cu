@@ -63,6 +63,44 @@ int launch_upsample2x(const float* x, bf16* y, int NB, int H, int W, int C, int 
                     reinterpret_cast<uint2*>(y), NB, H, W, Ho, Wo, C / 4);
 }
 
+__global__ void cast_bf16_kernel(const float4* __restrict__ x, uint2* __restrict__ y, size_t n4) {
+  pdl_launch_dependents();
+  pdl_wait();
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+    const float4 v = __ldg(x + i);
+    y[i] = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
+  }
+}
+int launch_cast_bf16(const float* x, bf16* y, size_t n, cudaStream_t stream) {
+  if (n % 4) { set_error("cast_bf16: n = %zu is not a multiple of 4", n); return MGB_ERR_INVALID; }
+  return launch_pdl("cast bf16", cast_bf16_kernel, grid_for(n / 4, 256), 256, 0, stream,
+                    reinterpret_cast<const float4*>(x), reinterpret_cast<uint2*>(y), n / 4);
+}
+
+// One thread per output 16-byte group (8 channels): rows [r0, r1) of the 2x image, each a copy of its source group.
+__global__ void upsample2x_rows_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int W, int Q, int r0,
+                                       size_t total) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int Wo = 2 * W;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int q = int(i % Q);
+    const size_t r = i / Q;
+    const int w = int(r % Wo);
+    const int h = r0 + int(r / Wo);
+    y[i] = __ldg(x + ((size_t)(h >> 1) * W + (w >> 1)) * Q + q);
+  }
+}
+int launch_upsample2x_rows(const bf16* x, bf16* y, int H, int W, int C, int r0, int r1, cudaStream_t stream) {
+  if (C % 8 || r0 < 0 || r1 <= r0 || r1 > 2 * H) {
+    set_error("upsample2x rows: C = %d (a multiple of 8), rows [%d, %d) of %d", C, r0, r1, 2 * H);
+    return MGB_ERR_INVALID;
+  }
+  const size_t n = size_t(r1 - r0) * 2 * W * (C / 8);
+  return launch_pdl("upsample2x rows", upsample2x_rows_kernel, grid_for(n, 256), 256, 0, stream,
+                    reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), W, C / 8, r0, n);
+}
+
 // A block's 256 threads cover 256 / Q rows of Q quads each; no division in the loop.
 __global__ void copy_rows_kernel(const float4* __restrict__ x, long long lqx, float4* __restrict__ y, long long M, int Q) {
   pdl_launch_dependents();

@@ -149,7 +149,7 @@ struct TileGeom {
   int mode;
   long long m_base;
   int M;
-  int img, ty, tx, H, W, tile_w_shift, tile_w_mask, tile_h;
+  int img, ty, tx, H, W, tile_w_shift, tile_w_mask, tile_h, out_y0;   // ty: the image's tile row
 };
 
 __device__ __forceinline__ bool tile_row_index(const TileGeom& g, int row, long long* m) {
@@ -159,18 +159,18 @@ __device__ __forceinline__ bool tile_row_index(const TileGeom& g, int row, long 
   }
   const int hh = row >> g.tile_w_shift, ww = row & g.tile_w_mask;
   const int h = g.ty * g.tile_h + hh, w = (g.tx << g.tile_w_shift) + ww;
-  *m = ((long long)g.img * g.H + h) * g.W + w;
+  *m = ((long long)g.img * g.H + h - g.out_y0) * g.W + w;
   return (h < g.H) && (w < g.W);
 }
 
 // Unaligned / ragged tail: rare, kept out of line.
 static __device__ __noinline__ void store_tail(float4 x, int nv, const float* residual, float* out_f32, bf16* out_bf16,
-                                        long long o) {
+                                        long long o, long long o32) {
   const float xs[4] = {x.x, x.y, x.z, x.w};
   for (int k = 0; k < 4 && k < nv; ++k) {
     float a = xs[k];
     if (residual) a += __ldg(residual + o + k);
-    if (out_f32) out_f32[o + k] = a;
+    if (out_f32) out_f32[o32 + k] = a;
     if (out_bf16) out_bf16[o + k] = __float2bfloat16(a);
   }
 }
@@ -178,11 +178,13 @@ static __device__ __noinline__ void store_tail(float4 x, int nv, const float* re
 // -------------------------------------------------------------------------------------------------
 // The kernel
 // -------------------------------------------------------------------------------------------------
+// kBand: the instantiation that reads GemmParams' row-band fields (ty0, src_y0, out_y0) and the split output
+// (GemmEpilogue::out_f32_hi); the others take them as absent, so that the network's other GEMMs pay nothing for them.
 // MINB = CTAs per SM the kernel is compiled for. 1: the register file of an SM for one CTA (accumulators of up to
 // 128 x 256), deep operand ring, one output tile per SM at a time. 2: <= 113 registers per thread and <= 113 KB of
 // shared memory, so TWO CTAs share an SM and the epilogue of one tile runs under the K loop of the other. Used for
 // multi-wave grids with block_n <= 128 (GEGLU feed-forward, QKV, VAE convs).
-template <int BLOCK_N, int MINB>
+template <int BLOCK_N, int MINB, bool kBand>
 __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   pdl_launch_dependents();
   const long long t_entry = clock64();
@@ -266,7 +268,8 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
           if (++stage == ustages) { stage = 0; phase ^= 1; }
         }
       } else {
-        const int cblocks = p.cblocks, x0 = tx * p.tile_w, y0 = ty * p.tile_h;
+        const int cblocks = p.cblocks, x0 = tx * p.tile_w;
+        const int y0 = ((kBand ? p.ty0 : 0) + ty) * p.tile_h, ya = y0 - (kBand ? p.src_y0 : 0);
         int tap = kb0 / cblocks, cb = kb0 - tap * cblocks;
         int kc = kb0 * BLOCK_K;
         for (int kb = kb0; kb < kb1; ++kb, kc += BLOCK_K) {
@@ -277,7 +280,7 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
             tma_load_2d_a(sb0 + stage * kBBytes, &p.tmap_b, fb, kc, ncol);
           }
           if (kb < p.num_kb1) {
-            tma_load_5d_a(sa0 + stage * kABytes, &p.tmap_a, fb, cb * BLOCK_K, x0 + p.tap_dx[tap], y0 + p.tap_dy[tap],
+            tma_load_5d_a(sa0 + stage * kABytes, &p.tmap_a, fb, cb * BLOCK_K, x0 + p.tap_dx[tap], ya + p.tap_dy[tap],
                           p.tap_p[tap], img);
             if (++cb == cblocks) { cb = 0; ++tap; }
           } else {
@@ -345,8 +348,9 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
   __syncwarp();
   TileGeom tg;
   tg.mode = p.mode; tg.m_base = (long long)m_tile * BLOCK_M; tg.M = p.M;
-  tg.img = img; tg.ty = ty; tg.tx = tx; tg.H = p.H; tg.W = p.W;
+  tg.img = img; tg.ty = (kBand ? p.ty0 : 0) + ty; tg.tx = tx; tg.H = p.H; tg.W = p.W;
   tg.tile_w_shift = p.tile_w_shift; tg.tile_w_mask = p.tile_w - 1; tg.tile_h = p.tile_h;
+  tg.out_y0 = kBand ? p.out_y0 : 0;
   const GemmEpilogue& e = p.epi;
   const int n0 = n_tile * BLOCK_N;
 
@@ -424,6 +428,10 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
       // warp-uniform: the whole 32-column chunk is inside the matrix
       const int chunk_nv = n_out - (col - c4);
       if (chunk_nv <= 0) break;
+      // split output: the whole chunk lies on one side of split_col (both multiples of 32)
+      const bool hi = kBand && !raw && e.out_f32_hi != nullptr && col - c4 >= e.split_col;
+      float* const o32 = hi ? e.out_f32_hi : out_f32;
+      const int ocol = hi ? col - e.split_col : col;
       const float* s_chunk = s_rd + j * 32;
       const bool vec = ld_vec && nv >= 4;
       if (!geglu && !silu && !relu && ld_vec && chunk_nv >= 32) {
@@ -447,7 +455,7 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
           }
           if ((vmask >> it) & 1u) {
             const long long o = off[it] + col;
-            if (out_f32) *reinterpret_cast<float4*>(out_f32 + o) = v;
+            if (o32) *reinterpret_cast<float4*>(o32 + off[it] + ocol) = v;
             if (out_bf16)
               *reinterpret_cast<uint2*>(out_bf16 + o) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
           }
@@ -477,11 +485,11 @@ __global__ void __launch_bounds__(kGemmThreads, MINB) gemm_tc_kernel(const __gri
               const float4 rr = __ldg(reinterpret_cast<const float4*>(residual + o));
               x.x += rr.x; x.y += rr.y; x.z += rr.z; x.w += rr.w;
             }
-            if (out_f32) *reinterpret_cast<float4*>(out_f32 + o) = x;
+            if (o32) *reinterpret_cast<float4*>(o32 + off[it] + ocol) = x;
             if (out_bf16)
               *reinterpret_cast<uint2*>(out_bf16 + o) = make_uint2(pack_bf16x2(x.x, x.y), pack_bf16x2(x.z, x.w));
           } else {
-            store_tail(x, nv, residual, out_f32, out_bf16, o);
+            store_tail(x, nv, residual, o32, out_bf16, o, off[it] + ocol);
           }
         }
       }
@@ -544,12 +552,12 @@ __global__ void __launch_bounds__(kSkThreads) splitk_epilogue_kernel(const GemmP
 static long long* g_gemm_dbg = nullptr;
 void set_gemm_debug_buffer(long long* dev_ptr) { g_gemm_dbg = dev_ptr; }
 
-template <int BN, int MINB>
+template <int BN, int MINB, bool kBand = false>
 static int launch_one(const GemmParams& p_in, int splits, cudaStream_t stream) {
   GemmParams p = p_in;
   p.dbg = g_gemm_dbg;
   const size_t smem = gemm_smem_bytes(BN, p.stages);
-  constexpr auto kernel = gemm_tc_kernel<BN, MINB>;
+  constexpr auto kernel = gemm_tc_kernel<BN, MINB, kBand>;
   TRY(raise_smem_limit_once<kernel>("gemm_tc", 227 * 1024));
   int m_tiles;
   if (p.mode == 0) {
@@ -562,6 +570,17 @@ static int launch_one(const GemmParams& p_in, int splits, cudaStream_t stream) {
 }
 
 int launch_gemm_tc(const GemmParams& p, int block_n, int splits, int ctas_per_sm, cudaStream_t stream) {
+  if (p.epi.out_f32_hi || p.ty0 || p.src_y0 || p.out_y0) {
+    switch (block_n * 4 + ctas_per_sm) {
+      case 64 * 4 + 2: return launch_one<64, 2, true>(p, splits, stream);
+      case 128 * 4 + 2: return launch_one<128, 2, true>(p, splits, stream);
+      case 64 * 4 + 1: return launch_one<64, 1, true>(p, splits, stream);
+      case 128 * 4 + 1: return launch_one<128, 1, true>(p, splits, stream);
+      case 160 * 4 + 1: return launch_one<160, 1, true>(p, splits, stream);
+      case 256 * 4 + 1: return launch_one<256, 1, true>(p, splits, stream);
+      default: set_error("gemm_tc: no row-band kernel for block_n %d", block_n); return MGB_ERR_INVALID;
+    }
+  }
   if (ctas_per_sm == 2) {
     switch (block_n) {
       case 64: return launch_one<64, 2>(p, splits, stream);

@@ -51,6 +51,10 @@ struct GemmEpilogue {
   const float* sched_z;   // EPI_SCHED: fresh noise     [M, ldo] or nullptr
   const float* sched_k;   // EPI_SCHED: device pointer to {kx, kv, kz}
   float* aux_out;         // EPI_SCHED: optional raw model output (acc + bias) [M, ldo], or nullptr
+  // Split fp32 output (or nullptr): columns [split_col, N) go to out_f32_hi [M, ldo] at column - split_col, the others to
+  // out_f32. split_col a multiple of 32; no residual, bf16 output, special epilogue or split-K with it.
+  float* out_f32_hi;
+  int split_col;
 };
 
 constexpr int kMaxTaps = 25;   // conv kind 5 (5 x 5)
@@ -78,6 +82,10 @@ struct GemmParams {
   float* partial;      // split-K: fp32 [splits, M, N] raw accumulators (epilogue deferred)
   long long* dbg;      // optional per-CTA phase timestamps [ctas][8] (tools/gemm_phases.py), else nullptr
   GemmEpilogue epi;
+  // Row bands (mode 1, no split-K, NB = 1): the launch runs tile rows [ty0, ty0 + tiles_y) of the image; tmap_a holds
+  // image rows from src_y0 on (its row 0 is image row src_y0; rows it does not hold read as zero, so it must hold
+  // every row of the band and its halo that lies in the image), and output pixel (y, x) goes to row (y - out_y0) W + x.
+  int ty0, src_y0, out_y0;
 };
 
 // Launch. block_n in {16, 32, 64, 128, 160, 256}; ctas_per_sm 1 or 2 (2: p.stages must keep gemm_smem_bytes <= 113 KB,
@@ -128,10 +136,13 @@ int launch_gn_fused(const float* xa, int Ca, const float* xb, int Cb, bf16* y, b
 // (scale, shift) float2 [NB][C] from launch_gn_fused's statistics; launch_gn_apply_rows applies them as launch_gn_fused
 // does, y bf16 [NB * HW, C] from x at a row stride of ldx floats, and raw = bf16(x) at a row stride of ldr elements
 // (raw == x: in place, the copy over the first half of each fp32 row, ldr = 2 ldx). C in {128, 256, 512}.
-int launch_gn_stats(const float* x, int C, int ldx, float2* stats, const float* gamma, const float* beta, int NB, int HW,
-                    int G, float eps, void* part, unsigned* counters, cudaStream_t stream);
-int launch_gn_apply_rows(const float* x, long long ldx, const float2* stats, bf16* y, bf16* raw, long long ldr, int NB,
-                         int HW, int C, int silu, cudaStream_t stream);
+// Two sources (xb != nullptr): the channel concat [x | xb] as launch_gn_fused reads it, x's Ca channels at a row
+// stride of ldx floats and xb's C - Ca packed; y may lie over xb (2 (C - Ca) = C) and raw over x (ldr = 2 ldx).
+int launch_gn_stats(const float* x, int Ca, int ldx, const float* xb, int Cb, float2* stats, const float* gamma,
+                    const float* beta, int NB, int HW, int G, float eps, void* part, unsigned* counters,
+                    cudaStream_t stream);
+int launch_gn_apply_rows(const float* x, long long ldx, const float* xb, int Ca, const float2* stats, bf16* y, bf16* raw,
+                         long long ldr, int NB, int HW, int C, int silu, cudaStream_t stream);
 // y [M, C] = the first C floats of each row of x at a row stride of ldx floats (elementwise.cu)
 int launch_copy_rows(const float* x, long long ldx, float* y, long long M, int C, cudaStream_t stream);
 // LayerNorm over the channel dim: x_f32 [M, C] -> y_bf16 [M, C]
@@ -149,6 +160,11 @@ int launch_xattn2_fold(const float* wq, const float* wo, const float* bo, const 
 int launch_space_to_depth(const float* x, bf16* y, int NB, int H, int W, int C, cudaStream_t stream);
 // nearest upsampling: x fp32 [NB, H, W, C] -> y bf16 [NB, Ho, Wo, C], Ho in {2H - 1, 2H}, Wo in {2W - 1, 2W}
 int launch_upsample2x(const float* x, bf16* y, int NB, int H, int W, int C, int Ho, int Wo, cudaStream_t stream);
+// y bf16 [n] = bf16(x fp32 [n]), n a multiple of 4
+int launch_cast_bf16(const float* x, bf16* y, size_t n, cudaStream_t stream);
+// Rows [r0, r1) of the nearest 2x upsampling of one image x bf16 [H, W, C] (2H x 2W output): y bf16 [r1 - r0, 2W, C].
+// The same bits as launch_upsample2x on the fp32 source that x rounds.
+int launch_upsample2x_rows(const bf16* x, bf16* y, int H, int W, int C, int r0, int r1, cudaStream_t stream);
 // UNet conv_in operand: [rgb(4) | target(Ct) | zeros] bf16 NHWC-64 from the fp32 NHWC latents (Ct = 4, or 4 n for IID)
 int launch_pack_latents(const float* rgb, const float* tgt, bf16* out, int M, int Ct, cudaStream_t stream);
 // NCHW fp32 <-> NHWC fp32 (small tensors at the ABI)

@@ -158,6 +158,8 @@ struct Epi {
   const float* sched_z = nullptr;
   const float* sched_k = nullptr;
   float* aux_out = nullptr;
+  float* out_f32_hi = nullptr;   // columns [split_col, N) of an fp32 output (GemmEpilogue::out_f32_hi)
+  int split_col = 0;
 };
 
 // Debug only (tools/marginal_cost.py): MGB_SKIP=gn,ln,attn,xattn,gemm drops a kernel family from the graph so
@@ -171,6 +173,7 @@ static void set_epi(GemmParams& p, const Epi& e, int ldo) {
   p.epi.bias = e.bias; p.epi.residual = e.residual; p.epi.out_f32 = e.out_f32; p.epi.out_bf16 = e.out_bf16;
   p.epi.ldo = ldo; p.epi.flags = e.flags; p.epi.hw = e.hw; p.epi.scale = e.scale;
   p.epi.sched_x = e.sched_x; p.epi.sched_z = e.sched_z; p.epi.sched_k = e.sched_k; p.epi.aux_out = e.aux_out;
+  p.epi.out_f32_hi = e.out_f32_hi; p.epi.split_col = e.split_col;
 }
 
 static int gemm_common(Ctx& c, GemmParams& p, int bn, int splits, const Epi& e, int ldo) {
@@ -227,16 +230,26 @@ static Tile matmul_tile(int M, int N, int K, int flags) {
   return linear_tile(M, W, flags);
 }
 
+// the tile of a conv3x3 over NB images of Hout x Wout (choose_tile's), and the image's tile rows
+static Tile conv_tile(int NB, int Hout, int Wout, const ConvW& W, int flags, int* tile_h = nullptr,
+                      int* tiles_y = nullptr) {
+  int tw, th;
+  conv_tile_shape(Hout, Wout, &tw, &th);
+  const int m_tiles = NB * ((Wout + tw - 1) / tw) * ((Hout + th - 1) / th);
+  Tile t;
+  choose_tile(m_tiles, W.cout, (9 * W.cin_pad + W.k_extra) / 64, flags, true, &t.bn, &t.sp, &t.st);
+  if (tile_h) *tile_h = th;
+  if (tiles_y) *tiles_y = (Hout + th - 1) / th;
+  return t;
+}
+
 // 3x3 conv on NHWC bf16; Hout x Wout output; kind per ops.cu. ldo: the output's row stride (0: W.cout); ld2: x2's
 // pixel stride (0: its channel count). Neither changes the tile, the split or any output value.
 static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const ConvW& W, int kind, const Epi& e,
                    int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr, int ldo = 0, int ld2 = 0) {
-  int tw, th;
-  conv_tile_shape(Hout, Wout, &tw, &th);
-  const int m_tiles = NB * ((Wout + tw - 1) / tw) * ((Hout + th - 1) / th);
-  int bn, sp, st;
   if ((x2 != nullptr) != (W.k_extra > 0)) { set_error("conv3x3: second operand / weight layout mismatch"); return MGB_ERR_STATE; }
-  choose_tile(m_tiles, W.cout, (9 * W.cin_pad + W.k_extra) / 64, e.flags, true, &bn, &sp, &st);
+  const Tile t = conv_tile(NB, Hout, Wout, W, e.flags);
+  const int bn = t.bn, sp = t.sp, st = t.st;
   const size_t M = size_t(NB) * Hout * Wout;
   if (sp > 1) c.splitk_need = std::max(c.splitk_need, size_t(sp) * M * W.cout * sizeof(float));
   if (c.dry) return MGB_OK;
@@ -246,6 +259,23 @@ static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const Conv
   Epi e2 = e;
   e2.hw = Hout * Wout;
   return gemm_common(c, p, bn, effective_splits(p), e2, ldo > 0 ? ldo : W.cout);
+}
+
+// Tile rows [ty0, ty0 + tiles) of one H x W image of a pad-1 3x3 conv run with tile t, the tile of the whole conv
+// (conv_tile over all its images): every output pixel comes out bit for bit as the whole conv computes it, since a
+// tile's arithmetic depends on the tile and never on where the tile is. x holds the operand's image rows
+// [src_y0, src_y0 + src_rows), which must include every row of the band and its one-row halo that lies in the image;
+// the output's row 0 is image row out_y0.
+static int conv3x3_band(Ctx& c, const bf16* x, int src_y0, int src_rows, int H, int W, const ConvW& Wt, const Tile& t,
+                        const Epi& e, int ldo, int ty0, int tiles, int out_y0) {
+  if (t.sp != 1 || Wt.k_extra) { set_error("conv band: the conv splits K or has a second operand"); return MGB_ERR_STATE; }
+  if (c.dry) return MGB_OK;
+  GemmParams p;
+  TRY(fill_conv_params(&p, x, Wt.w, 1, H, W, Wt.cin_pad, Wt.cout, 0, t.bn, 1, t.st, src_rows, W));
+  TRY(set_conv_band(&p, ty0, tiles, src_y0, out_y0));
+  Epi e2 = e;
+  e2.hw = H * W;
+  return gemm_common(c, p, t.bn, 1, e2, ldo);
 }
 
 #define LAUNCH(call)               \
@@ -337,63 +367,132 @@ static int resnet_forward(Ctx& c, const ResnetW& R, Act& x, Act* skip, Act& y, i
   return MGB_OK;
 }
 
-// GroupNorm statistics of x [NB * HW, C] at a row stride of ldx floats into stats (launch_gn_stats), with
-// groupnorm()'s scratch and barrier counter
-static int groupnorm_stats(Ctx& c, const float* x, int C, int ldx, float2* stats, const NormW& n, int NB, int HW,
-                           float eps) {
-  void* part = aalloc<char>(c, groupnorm_part_bytes(NB, HW, C, c.groups));
+// GroupNorm statistics of [x | xb] (launch_gn_stats: x's Ca channels at a row stride of ldx floats, xb's Cb packed, or
+// x alone) into stats, with groupnorm()'s scratch and barrier counter
+static int groupnorm_stats(Ctx& c, const float* x, int Ca, int ldx, const float* xb, int Cb, float2* stats,
+                           const NormW& n, int NB, int HW, float eps) {
+  void* part = aalloc<char>(c, groupnorm_part_bytes(NB, HW, Ca + Cb, c.groups));
   const size_t coff = c.sync_off;
   c.sync_off += size_t(NB);
   if (c.sync_off > c.sync_need) c.sync_need = c.sync_off;
   int rc = MGB_OK;
   if (!c.dry) {
     if (c.sync_off > c.sync_cap) { set_error("groupnorm: barrier counter slab exhausted"); return MGB_ERR_STATE; }
-    rc = launch_gn_stats(x, C, ldx, stats, n.g, n.b, NB, HW, c.groups, eps, part, c.sync_base + coff, c.stream);
+    rc = launch_gn_stats(x, Ca, ldx, xb, Cb, stats, n.g, n.b, NB, HW, c.groups, eps, part, c.sync_base + coff, c.stream);
   }
   c.arena->free(part);
   return rc;
 }
 
+// Tile rows per band of the decoder's banded full-resolution convs: about an eighth of the image, or as a test forces.
+static int band_tiles(int tiles_y, int force) {
+  return force > 0 ? std::min(force, tiles_y) : std::max(1, (tiles_y + 7) / 8);
+}
+
 // ---------------------------------------------------------------------------------------------
-// The ResnetBlock2D with a 1x1 shortcut over cin = 2 cout channels, in the memory of its input x alone plus one bf16
-// cin-channel map: three fp32 cout-channel maps where resnet_forward takes four (x, t1 and raw at its first GroupNorm).
-// Same operands, tiles and splits as resnet_forward, hence the same bits. Planned arena only; consumes x.
-// Each row of x (cin floats) is reused in place once GroupNorm has read it:
-//   bytes [0, 2 cin)       raw = bf16(x), the shortcut's operand, written by the apply launch over its own row;
-//   bytes [2 cin, 4 cin)   h = conv1's output, then y = conv2's. conv1 reads only t1, and conv2 reads t2 and raw, so
-//                          neither writes a byte that any CTA of its grid reads.
-// y is then copied out to a packed buffer of its own, which is where the next block reads it.
+// The decoder's last up-conv (Upsample2D: nearest 2x, then a 3x3 conv, cin = cout = 2 * 128) in low memory. h, the
+// half-resolution fp32 input, is rounded to bf16 once (a quarter of U; the same bits as upsample2x, a copy plus one
+// rounding) and freed with its ping-pong partner. The 2x operand then exists one band of tile rows (plus its halo rows)
+// at a time, and the conv runs that band's tiles through a map that starts at the band's first halo row. The epilogue
+// splits the output: channels [0, 128) to a, [128, 256) to b, each a packed fp32 128-channel map of its own.
+// Peak: a + b + the bf16 input + one band, 2.25 U plus a band. Same tile, split and K order as the whole conv.
 // ---------------------------------------------------------------------------------------------
-static int resnet_shortcut_in_place(Ctx& c, const ResnetW& R, Act& x, Act& y, int NB, int H, int W) {
-  if (R.cin != 2 * R.cout || !R.has_sc || !c.planned) {
-    set_error("resnet in place: needs a planned arena and a 1x1 shortcut over cin = 2 cout (got %d -> %d)", R.cin, R.cout);
+static int up_conv_low_memory(Ctx& c, const ConvW& Wt, Act& h, Act& partner, Act& a, Act& b, int NB, int H, int W) {
+  const int cin = Wt.cin_pad, half = Wt.cout / 2;
+  if (cin != Wt.cout || half % 32 || !c.planned) {
+    set_error("up-conv in low memory: needs a planned arena and cin = cout, a multiple of 64 (got %d -> %d)", cin, Wt.cout);
+    return MGB_ERR_STATE;
+  }
+  const int Hh = H / 2, Wh = W / 2, HW = H * W;
+  bf16* xh = aalloc<bf16>(c, size_t(NB) * Hh * Wh * cin);
+  LAUNCH(launch_cast_bf16(h.p, xh, size_t(NB) * Hh * Wh * cin, c.stream));
+  c.arena->free(h.p);
+  c.arena->free(partner.p);
+  h = partner = Act();
+  a = act_alloc(c, size_t(NB) * HW, half);
+  b = act_alloc(c, size_t(NB) * HW, half);
+  int th, tiles_y;
+  const Tile t = conv_tile(NB, H, W, Wt, 0, &th, &tiles_y);
+  const int bt = band_tiles(tiles_y, c.band_up_tiles);
+  bf16* band = aalloc<bf16>(c, size_t(std::min(H, bt * th + 2)) * W * cin);
+  Epi e; e.bias = Wt.b; e.split_col = half;
+  for (int n = 0; n < NB; ++n) {
+    e.out_f32 = a.p + size_t(n) * HW * half;
+    e.out_f32_hi = b.p + size_t(n) * HW * half;
+    for (int ty0 = 0; ty0 < tiles_y; ty0 += bt) {
+      const int tiles = std::min(bt, tiles_y - ty0);
+      const int lo = std::max(0, ty0 * th - 1), hi = std::min(H, (ty0 + tiles) * th + 1);
+      LAUNCH(launch_upsample2x_rows(xh + size_t(n) * Hh * Wh * cin, band, Hh, Wh, cin, lo, hi, c.stream));
+      TRY(conv3x3_band(c, band, lo, hi - lo, H, W, Wt, t, e, half, ty0, tiles, 0));
+    }
+  }
+  c.arena->free(band);
+  c.arena->free(xh);
+  return MGB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The ResnetBlock2D with a 1x1 shortcut over cin = 2 cout channels after up_conv_low_memory, on its input as the two
+// packed fp32 halves a = channels [0, cout) and b = [cout, cin), in 2.5 U. Same operands, tiles, splits and K order as
+// resnet_forward, hence the same bits. Planned arena only; consumes a, and y is b.
+//   GroupNorm 1  statistics over [a | b], then the row apply: each warp reads both halves of its row, then writes the
+//                shortcut's operand raw = bf16([a | b]) (2 cin bytes) over a's row and conv1's operand t1 over b's.
+//   conv1        in bands of tile rows, each into one of two staging bands; band k's output is copied over b's rows
+//                of band k only after band k + 1's conv is enqueued, the last conv that reads t1 rows of band k.
+//   GroupNorm 2  over h (b) into t2; conv2 reads t2 and raw (a) and writes y over b.
+// Peak: a + b + t2.
+// ---------------------------------------------------------------------------------------------
+static int resnet_shortcut_halves(Ctx& c, const ResnetW& R, Act& a, Act& b, Act& y, int NB, int H, int W) {
+  if (R.cin != 2 * R.cout || !R.has_sc || !c.planned || a.C != R.cout || b.C != R.cout) {
+    set_error("resnet on halves: needs a planned arena and a 1x1 shortcut over cin = 2 cout (got %d -> %d)", R.cin, R.cout);
     return MGB_ERR_STATE;
   }
   const int HW = H * W, cin = R.cin, cout = R.cout;
   const size_t M = size_t(NB) * HW;
   float2* st = aalloc<float2>(c, size_t(NB) * cin);
-  TRY(groupnorm_stats(c, x.p, cin, cin, st, R.n1, NB, HW, R.eps));
-  bf16* t1 = aalloc<bf16>(c, M * cin);
-  bf16* raw = reinterpret_cast<bf16*>(x.p);
-  LAUNCH(launch_gn_apply_rows(x.p, cin, st, t1, raw, 2 * cin, NB, HW, cin, 1, c.stream));
+  TRY(groupnorm_stats(c, a.p, cout, cout, b.p, cout, st, R.n1, NB, HW, R.eps));
+  bf16* raw = reinterpret_cast<bf16*>(a.p);
+  bf16* t1 = reinterpret_cast<bf16*>(b.p);
+  LAUNCH(launch_gn_apply_rows(a.p, cout, b.p, cout, st, t1, raw, 2 * cout, NB, HW, cin, 1, c.stream));
   c.arena->free(st);
-  float* hy = x.p + cout;   // h, then y: the second half of each row of x
+  int th, tiles_y;
+  const Tile t = conv_tile(NB, H, W, R.c1, 0, &th, &tiles_y);
+  const int bt = band_tiles(tiles_y, c.band_conv1_tiles);
+  const size_t band_px = size_t(std::min(H, bt * th)) * W;
+  float* stage[2] = {aalloc<float>(c, band_px * cout), aalloc<float>(c, band_px * cout)};
   Epi e1;
   e1.bias = (R.bias_off >= 0 && c.cur_bias) ? c.cur_bias + R.bias_off : R.c1.b;
-  e1.out_f32 = hy;
-  TRY(conv3x3(c, t1, NB, H, W, R.c1, 0, e1, 0, 0, nullptr, cin));
-  c.arena->free(t1);
+  for (int n = 0; n < NB; ++n) {
+    const bf16* x = t1 + size_t(n) * HW * cin;
+    float* hn = b.p + size_t(n) * HW * cout;
+    int prev = -1;   // first tile row of the band whose output waits in its staging band
+    for (int ty0 = 0;; ty0 += bt) {
+      if (ty0 < tiles_y) {
+        e1.out_f32 = stage[(ty0 / bt) & 1];
+        TRY(conv3x3_band(c, x, 0, H, H, W, R.c1, t, e1, cout, ty0, std::min(bt, tiles_y - ty0), ty0 * th));
+      }
+      if (prev >= 0) {
+        const int r0 = prev * th, r1 = std::min(H, (prev + bt) * th);
+        LAUNCH(launch_copy_rows(stage[(prev / bt) & 1], cout, hn + size_t(r0) * W * cout, (long long)(r1 - r0) * W,
+                                cout, c.stream));
+      }
+      if (ty0 >= tiles_y) break;
+      prev = ty0;
+    }
+  }
+  c.arena->free(stage[1]);
+  c.arena->free(stage[0]);
   st = aalloc<float2>(c, size_t(NB) * cout);
-  TRY(groupnorm_stats(c, hy, cout, cin, st, R.n2, NB, HW, R.eps));
+  TRY(groupnorm_stats(c, b.p, cout, cout, nullptr, 0, st, R.n2, NB, HW, R.eps));
   bf16* t2 = aalloc<bf16>(c, M * cout);
-  LAUNCH(launch_gn_apply_rows(hy, cin, st, t2, nullptr, 0, NB, HW, cout, 1, c.stream));
+  LAUNCH(launch_gn_apply_rows(b.p, cout, nullptr, 0, st, t2, nullptr, 0, NB, HW, cout, 1, c.stream));
   c.arena->free(st);
-  Epi e2; e2.bias = R.c2.b; e2.out_f32 = hy;
-  TRY(conv3x3(c, t2, NB, H, W, R.c2, 0, e2, 0, 0, raw, cin, 2 * cin));
+  Epi e2; e2.bias = R.c2.b; e2.out_f32 = b.p;
+  TRY(conv3x3(c, t2, NB, H, W, R.c2, 0, e2, 0, 0, raw));
   c.arena->free(t2);
-  y = act_alloc(c, M, cout);
-  LAUNCH(launch_copy_rows(hy, cin, y.p, (long long)M, cout, c.stream));
-  c.arena->free(x.p);
+  c.arena->free(a.p);
+  y = b;
+  a = b = Act();
   return MGB_OK;
 }
 
@@ -634,9 +733,11 @@ int unet_forward(mgb_handle* hd, Ctx& c, const float* rgb, float* tgt, const flo
 // VAE forwards. Their arena is lifetime-planned (api_net.cu): every buffer is allocated where it is first written and
 // freed after its last read, so the memory live at once stays near the largest working set of one step. At full
 // resolution that is the decoder's first up-level resnet's GroupNorm: its 256-channel fp32 input and the two bf16
-// copies it writes, 4 U (U = one fp32 128-channel map). With c.dec_low_memory that resnet runs in place
-// (resnet_shortcut_in_place), the two after it free their input and allocate their output as late as they can, and the
-// decoder's peak is 3 U: that resnet, and the up-conv before it (its bf16 operand and fp32 output).
+// copies it writes, 4 U (U = one fp32 128-channel map). With c.dec_low_memory the last up-conv runs in bands into two
+// 128-channel halves (up_conv_low_memory), that resnet runs on the halves in their own memory
+// (resnet_shortcut_halves), the two after it free their input and allocate their output as late as they can, and the
+// decoder's peak is 2.5 U (plus GroupNorm scratch): that resnet's second GroupNorm and conv2 (both halves and t2), and
+// each 128-channel resnet (input, output and one operand). The encoder's peak is 2.5 U too.
 // ---------------------------------------------------------------------------------------------
 // mid block: resnet, attention, resnet; consumes h and leaves the result in it
 static int vae_mid_forward(Ctx& c, const ResnetW& r0, const VaeAttnW& A, const ResnetW& r1, Act& h, int NB, int H,
@@ -721,17 +822,17 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
   c.arena->free(z);
   TRY(vae_mid_forward(c, V.dec_res[0], V.dec_attn, V.dec_res[1], h, NB, H, W));
   size_t ri = 2;
-  Act buf[2];
+  Act buf[2], half_a, half_b;   // half_a, half_b: the last up-conv's output in low memory (up_conv_low_memory)
   for (int i = 0; i < 4; ++i) {
     const int cout = ch[3 - i];
     buf[0] = buf[1] = Act();   // ping-pong trunk buffers, each allocated by the resnet that first writes it
     if (c.dec_low_memory && i == 3) {
-      // Full resolution in 3 U: the first resnet in place, and every block's output a buffer of its own, allocated
-      // after the block's conv1 output is freed, with the block's input freed after its last read. (The ping-pong
-      // pair below holds both 128-channel trunk maps through every block: 3.5 U in the next two.)
+      // Full resolution in 2.5 U: the first resnet on the up-conv's two halves, and every block's output a buffer of
+      // its own, allocated after the block's conv1 output is freed, with the block's input freed after its last read.
+      // (The ping-pong pair below holds both 128-channel trunk maps through every block: 3.5 U in the next two.)
       for (int j = 0; j < L + 1; ++j) {
         Act y;
-        if (j == 0) TRY(resnet_shortcut_in_place(c, V.dec_res[ri++], h, y, NB, H, W));
+        if (j == 0) TRY(resnet_shortcut_halves(c, V.dec_res[ri++], half_a, half_b, y, NB, H, W));
         else TRY(resnet_forward(c, V.dec_res[ri++], h, nullptr, y, NB, H, W, true));
         h = y; cur = cout;
       }
@@ -741,6 +842,13 @@ int vae_decode_forward(mgb_handle* hd, Ctx& c, const float* latent, float* out, 
     for (int j = 0; j < L + 1; ++j) {
       TRY(resnet_forward(c, V.dec_res[ri++], h, nullptr, buf[j & 1], NB, H, W, j == 0));
       h = buf[j & 1]; cur = cout;
+    }
+    if (c.dec_low_memory && i == 2) {
+      Act& partner = buf[0].p == h.p ? buf[1] : buf[0];
+      H *= 2; W *= 2; M = size_t(NB) * H * W;
+      TRY(up_conv_low_memory(c, V.dec_up[i], h, partner, half_a, half_b, NB, H, W));
+      buf[0] = buf[1] = Act();
+      continue;
     }
     if (i < 3) {
       bf16* up = aalloc<bf16>(c, M * 4 * cur);

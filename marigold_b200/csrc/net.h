@@ -134,7 +134,8 @@ struct Ctx {
   int attn_rows = 0;
   bool planned = false;    // the arena is lifetime-planned (the VAE forwards): buffers are freed after their last read
   bool poison = false;     // fill every buffer the arena hands out with 0xFF bytes (NaN in fp32 and bf16) first
-  bool dec_low_memory = false;   // the decoder's first full-resolution resnet runs in place (net.cu)
+  bool dec_low_memory = false;   // the decoder's full-resolution 256-channel stage runs in 2.5 U (net.cu)
+  int band_up_tiles = 0, band_conv1_tiles = 0;   // its bands' tile rows (0: the library's choice; mgb_handle's)
   float* splitk_ws = nullptr;
   size_t splitk_cap = 0;   // bytes available
   size_t splitk_need = 0;  // bytes needed (dry run)
@@ -208,6 +209,9 @@ struct mgb_handle {
     int attn_rows = 0;
     bool in_place = false;
   } decode_rule;
+  // Tile rows per band of the low-memory decoder's banded up-conv and conv1 (Ctx::band_up_tiles): 0 the library's
+  // choice, else forced (mgb_debug_vae_bands)
+  int vae_band_up_tiles = 0, vae_band_conv1_tiles = 0;
   // conditioning / schedule
   bool text_set = false;
   int n_steps = 0;

@@ -30,7 +30,7 @@ static __device__ __noinline__ void gn_barrier_timeout(unsigned seen, unsigned w
   __trap();
 }
 
-// kStats: statistics only. The source is xa alone at a row stride of lda floats, and instead of the normalised
+// kStats: statistics only. Source a is read at a row stride of lda floats, and instead of the normalised
 // operand the kernel writes each channel's (scale, shift) = (rstd gamma, beta - mean rstd gamma) to stats [NB][Ca],
 // from the same registers phase 2 applies them from: gn_apply_rows applies them bit for bit as this kernel would.
 template <int KQ, bool kStats = false>
@@ -294,13 +294,17 @@ int launch_gn_fused(const float* xa, int Ca, const float* xb, int Cb, bf16* y, b
                     silu, g, pp, counters, 0, nullptr);
 }
 
-// GroupNorm statistics of x [NB, HW, C] at a row stride of ldx floats (>= C): per image and channel the (scale, shift)
-// that launch_gn_fused applies, to stats [NB][C]. part and counters as launch_gn_fused's.
-int launch_gn_stats(const float* x, int C, int ldx, float2* stats, const float* gamma, const float* beta, int NB, int HW,
-                    int G, float eps, void* part, unsigned* counters, cudaStream_t stream) {
+// GroupNorm statistics of x [NB, HW, Ca] at a row stride of ldx floats (>= Ca), concatenated with xb [NB, HW, Cb]
+// packed when xb is set: per image and channel the (scale, shift) that launch_gn_fused applies to [x | xb], to stats
+// [NB][Ca + Cb]. part and counters as launch_gn_fused's.
+int launch_gn_stats(const float* x, int Ca, int ldx, const float* xb, int Cb, float2* stats, const float* gamma,
+                    const float* beta, int NB, int HW, int G, float eps, void* part, unsigned* counters,
+                    cudaStream_t stream) {
   GnGeom g;
-  if ((C & 3) || (ldx & 3) || ldx < C || !stats || !gn_plan(NB, HW, C, G, &g)) {
-    set_error("groupnorm stats: unsupported NB=%d C=%d ldx=%d G=%d", NB, C, ldx, G);
+  if (!xb) Cb = 0;
+  const int C = Ca + Cb;
+  if ((Ca & 3) || (Cb & 3) || (ldx & 3) || ldx < Ca || !stats || !gn_plan(NB, HW, C, G, &g)) {
+    set_error("groupnorm stats: unsupported NB=%d C=%d+%d ldx=%d G=%d", NB, Ca, Cb, ldx, G);
     return MGB_ERR_INVALID;
   }
   dim3 grid(g.chunks, NB);
@@ -308,30 +312,34 @@ int launch_gn_stats(const float* x, int C, int ldx, float2* stats, const float* 
   if (smem > 40 * 1024) { set_error("groupnorm stats: C=%d needs %zu B of shared memory", C, smem); return MGB_ERR_INVALID; }
   float2* pp = static_cast<float2*>(part);
   auto kern = g.Kq == 1 ? gn_fused_kernel<1, true> : g.Kq == 2 ? gn_fused_kernel<2, true> : gn_fused_kernel<4, true>;
-  return launch_pdl("groupnorm stats", kern, grid, kGnThreads, smem, stream, x, C, nullptr, 0, nullptr, nullptr, gamma,
+  return launch_pdl("groupnorm stats", kern, grid, kGnThreads, smem, stream, x, Ca, xb, Cb, nullptr, nullptr, gamma,
                     beta, HW, G, eps, 0, g, pp, counters, ldx, stats);
 }
 
 // The apply phase of GroupNorm over rows given their statistics (launch_gn_stats): one warp per pixel row of
 // C = 128 NQ channels. y [M, C] = bf16(act(x * scale + shift)) with the GroupNorm kernel's operations in its order, and,
-// when raw is set, raw = bf16(x) at a row stride of ldr elements. raw may lie over x itself: a row's raw copy is written
-// only over bytes of that same row (ldr = 2 ldx, the copy in the first half of the fp32 row), and only after the whole
-// warp has read the row (__syncwarp orders the warp's loads before its stores); no other warp touches the row. Hence
-// plain loads here, not the read-only path.
+// when raw is set, raw = bf16(x) at a row stride of ldr elements. With xb the row is the concat [x | xb], the first
+// 128 QA channels from x and the rest from xb packed. raw may lie over x and y over xb: a row's outputs are written only
+// over bytes of that same row (ldr = 2 ldx, the copy in the first half of the fp32 row; y's 2 C bytes over xb's row of
+// C / 2 floats), and only after the whole warp has read the row (__syncwarp orders the warp's loads before its stores);
+// no other warp touches the row. Hence plain loads here, not the read-only path.
 template <int NQ>
-__global__ void __launch_bounds__(256) gn_apply_rows_kernel(const float* x, long long ldx, const float2* __restrict__ stats,
-                                                            bf16* __restrict__ y, bf16* raw, long long ldr, int HW, int C,
-                                                            int silu, long long M) {
+__global__ void __launch_bounds__(256) gn_apply_rows_kernel(const float* x, long long ldx, const float* xb, int QA,
+                                                            const float2* __restrict__ stats, bf16* y, bf16* raw,
+                                                            long long ldr, int HW, int C, int silu, long long M) {
   pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31;
   const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  const int Cb = C - 128 * QA;
   for (long long m = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); m < M; m += warps) {
     const float2* st = stats + (m / HW) * C;
     const float4* xr = reinterpret_cast<const float4*>(x + m * ldx);
+    const float4* xbr = xb ? reinterpret_cast<const float4*>(xb + m * Cb) : nullptr;
     float4 t[NQ];
 #pragma unroll
-    for (int i = 0; i < NQ; ++i) t[i] = xr[lane + 32 * i];
+    for (int i = 0; i < NQ; ++i) t[i] = (xb && i >= QA) ? xbr[lane + 32 * (i - QA)] : xr[lane + 32 * i];
+    if (xb) __syncwarp();   // y over xb
     uint2* yo = reinterpret_cast<uint2*>(y + m * C);
 #pragma unroll
     for (int i = 0; i < NQ; ++i) {
@@ -352,18 +360,22 @@ __global__ void __launch_bounds__(256) gn_apply_rows_kernel(const float* x, long
   }
 }
 
-int launch_gn_apply_rows(const float* x, long long ldx, const float2* stats, bf16* y, bf16* raw, long long ldr, int NB,
-                         int HW, int C, int silu, cudaStream_t stream) {
+int launch_gn_apply_rows(const float* x, long long ldx, const float* xb, int Ca, const float2* stats, bf16* y, bf16* raw,
+                         long long ldr, int NB, int HW, int C, int silu, cudaStream_t stream) {
+  if (!xb) Ca = C;
   const bool in_place = raw && reinterpret_cast<const void*>(raw) == reinterpret_cast<const void*>(x);
-  if ((C != 128 && C != 256 && C != 512) || ldx < C || (ldx & 3) || (raw && (ldr < C || (ldr & 3))) ||
-      (raw && !in_place && ldr != C) || (in_place && ldr != 2 * ldx)) {
-    set_error("groupnorm apply rows: unsupported C=%d ldx=%lld ldr=%lld", C, ldx, ldr);
+  const bool y_over_b = xb && reinterpret_cast<const void*>(y) == reinterpret_cast<const void*>(xb);
+  if ((C != 128 && C != 256 && C != 512) || ldx < Ca || (ldx & 3) || (raw && (ldr < C || (ldr & 3))) ||
+      (raw && !in_place && ldr != C) || (in_place && ldr != 2 * ldx) || Ca <= 0 || Ca % 128 || Ca > C ||
+      (xb && Ca == C) || (y_over_b && 2 * (C - Ca) != C)) {
+    set_error("groupnorm apply rows: unsupported C=%d Ca=%d ldx=%lld ldr=%lld", C, Ca, ldx, ldr);
     return MGB_ERR_INVALID;
   }
   const long long M = (long long)NB * HW;
   const int blocks = int(std::min<long long>((M + 7) / 8, 64LL * kNumSMs));
   auto kern = C == 128 ? gn_apply_rows_kernel<1> : C == 256 ? gn_apply_rows_kernel<2> : gn_apply_rows_kernel<4>;
-  return launch_pdl("groupnorm apply rows", kern, blocks, 256, 0, stream, x, ldx, stats, y, raw, ldr, HW, C, silu, M);
+  return launch_pdl("groupnorm apply rows", kern, blocks, 256, 0, stream, x, ldx, xb, Ca / 128, stats, y, raw, ldr, HW,
+                    C, silu, M);
 }
 
 // Stand-alone GroupNorm (operator-level ABI): ws = groupnorm_ws_bytes() of scratch (counters zeroed here).

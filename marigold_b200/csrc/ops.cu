@@ -157,6 +157,17 @@ int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Ho
 
 int effective_splits(const GemmParams& p) { return (p.num_kb + p.kb_per_split - 1) / p.kb_per_split; }
 
+int set_conv_band(GemmParams* p, int ty0, int tiles, int src_y0, int out_y0) {
+  if (p->mode != 1 || p->M != p->H * p->W || effective_splits(*p) != 1 || ty0 < 0 || tiles < 1 ||
+      ty0 + tiles > p->tiles_y || src_y0 < 0 || out_y0 < 0 || p->num_kb1 < p->num_kb) {
+    set_error("conv band: needs one image, no split-K and no second operand; tile rows [%d, %d) of %d", ty0, ty0 + tiles,
+              p->tiles_y);
+    return MGB_ERR_INVALID;
+  }
+  p->ty0 = ty0; p->tiles_y = tiles; p->src_y0 = src_y0; p->out_y0 = out_y0;
+  return MGB_OK;
+}
+
 int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) {
   const int splits = effective_splits(p);
   // The special epilogues exist only in the 16-wide instantiation, where one lane holds a whole output row: any other
@@ -170,6 +181,13 @@ int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream) 
                 "out_f32, and sched_x + sched_k or hw", p.epi.flags, block_n, p.N);
       return MGB_ERR_INVALID;
     }
+  }
+  if (p.epi.out_f32_hi &&
+      (special || block_n <= 16 || splits > 1 || (p.epi.split_col & 31) || p.epi.split_col <= 0 || p.epi.residual ||
+       p.epi.out_bf16 || !p.epi.out_f32 || (p.epi.flags & EPI_GEGLU))) {
+    set_error("split output: needs out_f32, split_col a positive multiple of 32 (got %d), block_n > 16 (got %d), no "
+              "split-K, residual, bf16 output or special epilogue", p.epi.split_col, block_n);
+    return MGB_ERR_INVALID;
   }
   if ((p.epi.flags & EPI_GEGLU) && (block_n % 64 != 0)) {
     set_error("GEGLU epilogue needs block_n %% 64 == 0 (got %d)", block_n);

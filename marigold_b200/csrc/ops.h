@@ -16,6 +16,9 @@ int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Ho
                      int kind, int block_n, int splits, int stages, int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr,
                      int Cin2 = 0, int ld2 = 0);
 int effective_splits(const GemmParams& p);
+// Makes a filled conv (one image, no split-K, no second operand) run tile rows [ty0, ty0 + tiles) of its image with
+// tmap_a's row 0 at image row src_y0 and the output's row 0 at image row out_y0 (GemmParams::ty0).
+int set_conv_band(GemmParams* p, int ty0, int tiles, int src_y0, int out_y0);
 // Launch (plus the deferred epilogue when split-K is active). p.epi must be filled by the caller. Rejects, before any
 // launch, a special epilogue with block_n != 16, N > 16 (N != 3 for depth / normals) or missing epilogue inputs.
 int run_gemm(GemmParams& p, int block_n, float* splitk_ws, cudaStream_t stream);

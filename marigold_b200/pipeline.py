@@ -156,15 +156,33 @@ def call_reserve_bytes(h: int, w: int, ensemble_size: int, channels: int) -> int
     return 4 * h * w * (channels * (2 * ensemble_size + 2) + 3)
 
 
+def _on_free_memory(engine, free_bytes: Optional[int], select):
+    """select(free_bytes), with the device's free memory measured when free_bytes is None. Memory that torch's caching
+    allocator keeps for tensors already freed does not count as free there, and the engine's workspace cannot use it:
+    the workspace comes from the driver. So where select refuses on that measure, the cache is handed back to the
+    driver and select runs once more on a new measure. A call that fits without it leaves the cache alone."""
+    if free_bytes is not None:
+        return select(free_bytes)
+    try:
+        return select(torch.cuda.mem_get_info(engine.device)[0])
+    except ValueError:
+        torch.cuda.empty_cache()
+        return select(torch.cuda.mem_get_info(engine.device)[0])
+
+
 def select_batch_size(engine, n_members: int, h: int, w: int, batch_size: int = 0,
                       free_bytes: Optional[int] = None, reserve_bytes: int = 0) -> int:
     """Members per batch for n_members at h x w. batch_size > 0 is taken as given; 0 takes find_batch_size's value,
     lowered to the largest batch whose workspace (engine.workspace_bytes) fits the memory available to the engine: free
-    device memory (`free_bytes`, or the device's) plus the workspace the engine holds, which it gives back before it
-    grows, less `reserve_bytes` that the call needs for its own tensors (call_reserve_bytes). A batch that cannot fit,
-    explicit or of one member, raises ValueError before any inference work is spent."""
-    if free_bytes is None:
-        free_bytes = torch.cuda.mem_get_info(engine.device)[0]
+    device memory (`free_bytes`, or the device's, with torch's cache handed back where needed: _on_free_memory) plus
+    the workspace the engine holds, which it gives back before it grows, less `reserve_bytes` that the call needs for
+    its own tensors (call_reserve_bytes). A batch that cannot fit, explicit or of one member, raises ValueError before
+    any inference work is spent."""
+    return _on_free_memory(engine, free_bytes,
+                           lambda free: _select_batch_size(engine, n_members, h, w, batch_size, free, reserve_bytes))
+
+
+def _select_batch_size(engine, n_members, h, w, batch_size, free_bytes, reserve_bytes):
     avail = int(free_bytes) + engine.held_bytes() - int(reserve_bytes)
     explicit = batch_size > 0
     bs = min(batch_size, max(n_members, 1)) if explicit else find_batch_size(n_members, max(h, w), torch.float32)
@@ -216,10 +234,14 @@ def select_list_batch_size(engine, n_jobs: int, h: int, w: int, ensemble_size: i
     (one rank's share under world_size ranks), beside the call_reserve_bytes of every image one round of batches can
     hold open (parallel.open_images). The reserve grows with the batch, so the two are lowered together: the result is
     the largest batch that fits beside its own reserve. Raises ValueError like select_batch_size."""
+    return _on_free_memory(engine, free_bytes, lambda free: _select_list_batch_size(
+        engine, n_jobs, h, w, ensemble_size, channels, n_images, world_size, batch_size, free))
+
+
+def _select_list_batch_size(engine, n_jobs, h, w, ensemble_size, channels, n_images, world_size, batch_size,
+                            free_bytes):
     from . import parallel
 
-    if free_bytes is None:
-        free_bytes = torch.cuda.mem_get_info(engine.device)[0]
     per_image = call_reserve_bytes(h, w, ensemble_size, channels)
     explicit = batch_size > 0
     bs = min(batch_size, max(n_jobs, 1)) if explicit else find_batch_size(n_jobs, max(h, w), torch.float32)

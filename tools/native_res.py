@@ -5,11 +5,12 @@ power limit, read in the same run. Then 24 MP (6048 x 4032): depth with E = 1 an
 normals, and a 2-target IID model (each its numbers, or the error with the bytes it needed); the largest 4:3 and 3:2
 photos select_batch_size accepts for one depth member on this card; mgb_workspace_bytes at the batch caps and the
 native sizes. Then a 1920 x 1080 decode with the VAE attention in one block against its default row blocks, alternated.
-48 MP (8064 x 6048), where the decoder runs its first full-resolution resnet in place: depth with E = 1 and 1 step.
+48 MP (8064 x 6048) and 60 MP (9504 x 6336), where the decoder runs its full-resolution 256-channel stage in low
+memory: depth with E = 1 and 1 step.
 
-    python tools/native_res.py [--out DIR] [--only-48mp]
-        (prints one JSON line; with --out also writes DIR/native_res.json; --only-48mp: the card, the 48 MP run and the
-        largest photos accepted)
+    python tools/native_res.py [--out DIR] [--only-48mp] [--only-60mp]
+        (prints one JSON line; with --out also writes DIR/native_res.json; --only-48mp / --only-60mp: the card, that
+        run and the largest photos accepted)
 """
 import argparse
 import ctypes as C
@@ -169,11 +170,15 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--only-48mp", action="store_true")
+    ap.add_argument("--only-60mp", action="store_true")
     a = ap.parse_args()
     res = {"card": gpu_identity(torch.cuda.current_device()), "runs": []}
     eng = make_engine()
-    if a.only_48mp:
-        res["mp48"] = try_run(eng, "depth", 6048, 8064, 1, 1)
+    if a.only_48mp or a.only_60mp:
+        if a.only_48mp:
+            res["mp48"] = try_run(eng, "depth", 6048, 8064, 1, 1)
+        if a.only_60mp:
+            res["mp60"] = try_run(eng, "depth", 6336, 9504, 1, 1)
         res["largest_accepted"] = {"4:3": largest_accepted(eng, (4, 3)), "3:2": largest_accepted(eng, (3, 2))}
         eng.close()
         return _emit(res, a.out)
@@ -186,6 +191,7 @@ def main():
     res["mp24"] = try_run(eng, "depth", 4032, 6048, 1, 1)
     res["mp24_runs"] = [try_run(eng, "depth", 4032, 6048, 10, 4), try_run(eng, "normals", 4032, 6048, 1, 1)]
     res["mp48"] = try_run(eng, "depth", 6048, 8064, 1, 1)
+    res["mp60"] = try_run(eng, "depth", 6336, 9504, 1, 1)
     res["workspace_bytes"] = {f"{B}x{H}x{W}": eng.workspace_bytes(B, H, W) for B, H, W in
                               ((16, 768, 768), (8, 1024, 1024), (1, 3024, 4032), (2, 3024, 4032), (1, 4032, 6048))}
     res["largest_accepted"] = {"4:3": largest_accepted(eng, (4, 3)), "3:2": largest_accepted(eng, (3, 2))}
