@@ -120,6 +120,23 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent_dev, float* target_
 int mgb_decode(mgb_handle* h, const float* latent_dev, int32_t B, int32_t lh, int32_t lw, int32_t mode,
                float* out_dev, void* stream);
 
+/* ---- one image on several GPUs: the attentions' query rows split over the ranks --------------- */
+/* Exchange of one attention's output: buf_dev holds world chunks of chunk_bytes; on entry chunk `rank` holds this rank's
+ * rows. On return (in stream order) every chunk must hold its rank's rows: an in-place all-gather. Runs on `stream`, the
+ * call's stream. Returns 0, or a non-zero status that fails the call. */
+typedef int32_t (*mgb_exchange_fn)(void* ctx, void* buf_dev, size_t chunk_bytes, int32_t rank, int32_t world,
+                                   void* stream);
+/* Row-split mode of this handle. With fn installed, every attention of mgb_encode, mgb_unet_step, mgb_denoise(_range) and
+ * mgb_decode computes only this rank's share of its query rows, then calls fn once with the attention's output (16 calls
+ * per UNet step, one per encode, one per decode): of T rows, chunk = ceil(ceil(T / 128) / world) * 128 rows per rank,
+ * rank r's rows [r chunk, (r + 1) chunk) within [0, T) (a rank may have none; it still calls fn). Every other layer runs
+ * whole on every rank, so when every rank runs the same call with the same inputs, every rank's outputs are
+ * bit-identical to the same call without the split. fn is called even at world 1. While installed, the calls take
+ * B = 1 only (MGB_ERR_INVALID before any launch otherwise), and denoising runs each step eagerly: no CUDA graph is
+ * captured or replayed. fn = NULL clears the mode; the handle then runs, sizes and lays out its work exactly as one that
+ * never had it. MGB_ERR_INVALID for world < 1 or rank outside [0, world). */
+int mgb_set_row_split(mgb_handle* h, int32_t rank, int32_t world, mgb_exchange_fn fn, void* ctx);
+
 /* ---- ensembling (marigold/util/ensemble.py) ------------------------------------------------- */
 /* cost_fn of ensemble_depth (ensemble.py:138-152) at one point, in ONE host sync:
  * depth_dev [E,HW] fp32; param_host = [s_0..s_{E-1}, t_0..t_{E-1}] (or only s when !shift);
@@ -312,6 +329,12 @@ int mgb_op_conv2d_ex(const void* x_bf16_dev, const void* x2_bf16_dev, const void
  * growth) and is therefore not re-entrant across threads. The network path carves the workspace out of its arena. */
 int mgb_op_flash_attn64(const void* qkv_bf16_dev, void* out_bf16_dev, int32_t NB, int32_t T, int32_t C, float scale,
                         void* stream);
+/* The same on the 128-row query blocks [q_block_begin, q_block_end) of every (image, head) only: the rows of out_bf16_dev
+ * outside them are not written. The KV split and its workspace are chosen for the whole (NB, T, C) problem, so each row
+ * written is bit-identical to mgb_op_flash_attn64's. An empty range launches nothing; a range outside
+ * [0, ceil(T / 128)] returns MGB_ERR_INVALID. */
+int mgb_op_flash_attn64_ex(const void* qkv_bf16_dev, void* out_bf16_dev, int32_t NB, int32_t T, int32_t C, float scale,
+                           int32_t q_block_begin, int32_t q_block_end, void* stream);
 /* GroupNorm (+SiLU) -> bf16, one launch with a grid-wide barrier, run-to-run deterministic (replaces torch.nn.GroupNorm
  * + F.silu under diffusers' ResnetBlock2D / Transformer2DModel, reached from marigold_depth_pipeline.py:461-463).
  * ws_dev: mgb_op_groupnorm_ws_bytes(NB, HW, C, G) bytes of scratch (0 = unsupported shape). */

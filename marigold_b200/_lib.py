@@ -39,6 +39,9 @@ EPI_RELU = 256
 
 _vp, _i32, _i64, _f32, _f64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_double
 
+# mgb_exchange_fn(ctx, buf_dev, chunk_bytes, rank, world, stream) -> status
+EXCHANGE_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p)
+
 # name -> (restype, argtypes); every symbol include/marigold_b200.h declares
 SIGNATURES = {
     "mgb_create": (_i32, [C.POINTER(mgb_config), C.POINTER(_vp)]),
@@ -54,6 +57,7 @@ SIGNATURES = {
     "mgb_denoise": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "mgb_denoise_range": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "mgb_decode": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "mgb_set_row_split": (_i32, [_vp, _i32, _i32, _vp, _vp]),   # fn: an EXCHANGE_FN cast to void*
     "mgb_ens_depth_cost": (_i32, [_vp, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _f64, C.POINTER(_f64), _vp]),
     "mgb_ens_depth_cost_fd": (_i32, [_vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _f64, _vp, _vp]),
     "mgb_ens_max_members": (_i32, []),
@@ -90,6 +94,7 @@ SIGNATURES = {
     "mgb_op_conv2d_ex": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32,
                                  _i32, _f32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "mgb_op_flash_attn64": (_i32, [_vp, _vp, _i32, _i32, _i32, _f32, _vp]),
+    "mgb_op_flash_attn64_ex": (_i32, [_vp, _vp, _i32, _i32, _i32, _f32, _i32, _i32, _vp]),
     "mgb_op_groupnorm_ws_bytes": (C.c_size_t, [_i32, _i32, _i32, _i32]),
     "mgb_op_xattn2": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32, _vp]),
     "mgb_op_groupnorm": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _i32, _vp]),

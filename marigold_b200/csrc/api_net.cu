@@ -609,6 +609,15 @@ static int run_graph(mgb_handle* h, Ctx& c, int op, const float* a0, float* a1, 
 
 struct WorkspaceNeed { size_t arena = 0, splitk = 0, sync = 0; };   // bytes
 
+// The handle's row split (mgb_set_row_split) into a forward's context, or none
+static void set_split(const mgb_handle* h, Ctx& c) {
+  const mgb_handle::RowSplit& r = h->row_split;
+  c.split_world = r.fn ? r.world : 0;
+  c.split_rank = r.rank;
+  c.exchange_fn = r.fn;
+  c.exchange_ctx = r.ctx;
+}
+
 // Dry-runs one graph: its arena peak, split-K workspace and GroupNorm barrier counters. The VAE forwards' arena is
 // planned: their buffers, placed by lifetime (arena_place with the handle's placement), go to *bufs and the arena
 // peak is the plan's. The UNet step keeps the bump allocator's stack layout, which its captured graph holds; *bufs
@@ -619,6 +628,7 @@ static int workspace_need(mgb_handle* h, int op, int NB, int d0, int d1, Workspa
   Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
   c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
   c.band_up_tiles = h->vae_band_up_tiles; c.band_conv1_tiles = h->vae_band_conv1_tiles;
+  set_split(h, c);
   TRY(run_graph(h, c, op, nullptr, nullptr, nullptr, nullptr, 0, NB, d0, d1, 0));
   dry.finish();
   const size_t arena = op == OP_UNET ? dry.peak : arena_place(dry.rec, h->arena_placement);
@@ -668,7 +678,18 @@ static Ctx make_ctx(mgb_handle* h, void* stream) {
   c.band_up_tiles = h->vae_band_up_tiles; c.band_conv1_tiles = h->vae_band_conv1_tiles;
   c.sync_base = h->sync_slab;
   c.sync_cap = h->sync_slab.bytes() / sizeof(unsigned);
+  set_split(h, c);
   return c;
+}
+
+// A row-split handle runs one image per call
+static int check_split_batch(const mgb_handle* h, const char* what, int B) {
+  if (h->row_split.fn && B != 1) {
+    set_error("%s: the handle splits attention rows over %d ranks, which takes one image per call (got %d)", what,
+              h->row_split.world, B);
+    return MGB_ERR_INVALID;
+  }
+  return MGB_OK;
 }
 
 // Sizes the workspace for one graph, then runs it once on `stream` (run_graph's arguments).
@@ -693,6 +714,7 @@ int mgb_encode(mgb_handle* h, const float* rgb, int32_t B, int32_t H, int32_t W,
     return MGB_ERR_INVALID;
   }
   TRY(check_pixels("mgb_encode", B, H, W));
+  TRY(check_split_batch(h, "mgb_encode", B));
   return run_once(h, stream, OP_ENCODE, rgb, latent, nullptr, nullptr, 0, B, H, W, 0);
 }
 
@@ -705,6 +727,7 @@ int mgb_unet_step(mgb_handle* h, const float* rgb_latent, float* target, const f
   }
   if (step_index < 0 || step_index >= h->n_steps) { set_error("step_index %d outside schedule of %d", step_index, h->n_steps); return MGB_ERR_INVALID; }
   if (h->kz_host[step_index] != 0.f && !noise) { set_error("step %d needs noise (kz != 0)", step_index); return MGB_ERR_INVALID; }
+  TRY(check_split_batch(h, "mgb_unet_step", B));
   return run_once(h, stream, OP_UNET, rgb_latent, target, noise, model_out, step_index, B, lh, lw, 0);
 }
 
@@ -721,6 +744,7 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
   }
   for (int i = first_step; i < first_step + num_steps; ++i)
     if (h->kz_host[i] != 0.f && !step_noise) { set_error("schedule step %d injects noise but step_noise is NULL", i); return MGB_ERR_INVALID; }
+  TRY(check_split_batch(h, "mgb_denoise", B));
   TRY(ensure_workspace(h, OP_UNET, B, lh, lw));
   Ctx c = make_ctx(h, stream);
   const int HW = lh * lw, Ct = h->cfg.unet_out_channels;
@@ -731,7 +755,10 @@ int mgb_denoise_range(mgb_handle* h, const float* rgb_latent, float* target, con
   TRY(launch_nchw_to_nhwc(target, s.tgt, B, Ct, HW, 1.f, c.stream));
   const bool any_noise = step_noise != nullptr;
   if (!any_noise) CUDA_TRY(cudaMemsetAsync(s.nz, 0, n * 4, c.stream));   // kz * 0 must stay finite
-  static const bool graphs = getenv("MGB_NO_GRAPH") == nullptr;
+  static const bool graphs_env = getenv("MGB_NO_GRAPH") == nullptr;
+  // a row-split step calls the exchange function from the host between kernels: it runs eagerly, and leaves the
+  // graph of the unsplit shape as it is (unless ensure_workspace grew a buffer the graph holds, which drops it)
+  const bool graphs = graphs_env && !h->row_split.fn;
   mgb_handle::StepGraph& G = h->step_graph;
   for (int i = first_step; i < first_step + num_steps; ++i) {
     if (h->kz_host[i] != 0.f) TRY(launch_nchw_to_nhwc(step_noise + size_t(i) * n, s.nz, B, Ct, HW, 1.f, c.stream));
@@ -795,6 +822,7 @@ int mgb_decode(mgb_handle* h, const float* latent, int32_t B, int32_t lh, int32_
     return MGB_ERR_INVALID;
   }
   TRY(check_pixels("mgb_decode", B, 8 * lh, 8 * lw));
+  TRY(check_split_batch(h, "mgb_decode", B));
   return run_once(h, stream, OP_DECODE, latent, out, nullptr, nullptr, 0, B, lh, lw, mode);
 }
 
@@ -933,6 +961,17 @@ FieldRef find_field(const mgb_handle* h, const std::string& name) {
 }  // namespace
 
 extern "C" {
+
+int mgb_set_row_split(mgb_handle* h, int32_t rank, int32_t world, mgb_exchange_fn fn, void* ctx) {
+  if (!h) { set_error("set_row_split: null handle"); return MGB_ERR_INVALID; }
+  if (!fn) { h->row_split = mgb_handle::RowSplit(); return MGB_OK; }
+  if (world < 1 || rank < 0 || rank >= world) {
+    set_error("set_row_split: rank %d of world %d", rank, world);
+    return MGB_ERR_INVALID;
+  }
+  h->row_split = {rank, world, fn, ctx};
+  return MGB_OK;
+}
 
 /* debug hooks (not in the public header) */
 

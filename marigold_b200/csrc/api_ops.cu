@@ -128,7 +128,9 @@ int mgb_op_conv2d(const void* x, const void* w, const float* bias, const float* 
                           1.0f, nullptr, nullptr, nullptr, nullptr, block_n, splits, stages, splitk_ws, stream);
 }
 
-int mgb_op_flash_attn64(const void* qkv, void* out, int32_t NB, int32_t T, int32_t C, float scale, void* stream) {
+int mgb_op_flash_attn64_ex(const void* qkv, void* out, int32_t NB, int32_t T, int32_t C, float scale,
+                           int32_t q_block_begin, int32_t q_block_end, void* stream) {
+  if (q_block_end < 0) { set_error("op_flash_attn64_ex: q_block_end %d < 0", q_block_end); return MGB_ERR_INVALID; }
   // split-KV workspace of the operator-level entry point: a process-wide buffer grown on demand (the network
   // path carves it out of its arena instead). Never destroyed, so it is not freed during static destruction,
   // after the CUDA runtime may have unloaded.
@@ -139,7 +141,12 @@ int mgb_op_flash_attn64(const void* qkv, void* out, int32_t NB, int32_t T, int32
     if (int rc = ws.grow(need)) return rc;
   }
   return launch_flash_attn64(reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(out), NB, T, C, scale,
-                             need ? ws.get() : nullptr, need ? ws.bytes() : 0, reinterpret_cast<cudaStream_t>(stream));
+                             need ? ws.get() : nullptr, need ? ws.bytes() : 0, reinterpret_cast<cudaStream_t>(stream),
+                             q_block_begin, q_block_end);
+}
+
+int mgb_op_flash_attn64(const void* qkv, void* out, int32_t NB, int32_t T, int32_t C, float scale, void* stream) {
+  return mgb_op_flash_attn64_ex(qkv, out, NB, T, C, scale, 0, T > 0 ? (T + 127) / 128 : 0, stream);
 }
 
 size_t mgb_op_groupnorm_ws_bytes(int32_t NB, int32_t HW, int32_t C, int32_t G) { return groupnorm_ws_bytes(NB, HW, C, G); }

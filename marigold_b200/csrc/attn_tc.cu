@@ -17,6 +17,7 @@
 //   warp 8     TMA producer: Q tile (128 x 64) once, K / V tiles (64 x 64) through 3-stage rings
 // Two CTAs per SM (~66 KB of shared memory and <= 113 registers per thread each): the softmax of one warpgroup
 // overlaps the MMAs of the others.
+#include <algorithm>
 #include <cstdlib>
 #include "common.cuh"
 #include "kernels.h"
@@ -34,6 +35,7 @@ struct AttnParams {
   CUtensorMap tmap_kv;  // 3D {3C, T, NB}, box {64, 64, 1}
   bf16* out;
   int T, C;
+  int qb0;              // first 128-row query block of this launch (blockIdx.x 0); a row's arithmetic never depends on it
   float scale_log2;
   // split-KV (balances the last wave of CTAs): blockIdx.z = img * splits + split; split s covers KV blocks
   // [s * nkv / splits, (s+1) * ...). With splits > 1 the CTA writes un-normalised fp32 O plus (m, l) per row;
@@ -58,7 +60,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) flash_attn64_kernel(const __g
   uint64_t* v_empty = bars + 10;             // [3]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 128, head = blockIdx.y, img = blockIdx.z / p.splits, split = blockIdx.z % p.splits;
+  const int q0 = (blockIdx.x + p.qb0) * 128, head = blockIdx.y, img = blockIdx.z / p.splits, split = blockIdx.z % p.splits;
   const int nkv_all = (p.T + 63) / 64;
   const int jb0 = split * nkv_all / p.splits;                 // first KV block of this CTA
   const int nkv = (split + 1) * nkv_all / p.splits - jb0;     // its number of KV blocks (>= 1: host keeps splits <= nkv_all)
@@ -218,16 +220,19 @@ __global__ void __launch_bounds__(kAttnThreads, 2) flash_attn64_kernel(const __g
 }
 
 // Merge the split-KV partials: out[row, :] = sum_s w_s O_s / sum_s w_s l_s, w_s = 2^(m_s - max m). One thread per
-// (row, 8 columns).
+// (row, 8 columns), over the query rows [t0, t0 + nt) of every (image, head).
 __global__ void __launch_bounds__(256) attn_combine_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml,
-                                                           bf16* __restrict__ out, int splits, int NB, int heads, int T, int C) {
+                                                           bf16* __restrict__ out, int splits, int NB, int heads, int T, int C,
+                                                           int t0, int nt) {
   pdl_launch_dependents();
   pdl_wait();
   const size_t rows = size_t(NB) * heads * T;
   const size_t gid = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  const size_t r = gid >> 3;
+  const size_t rr = gid >> 3;
   const int c8 = int(gid & 7) * 8;
-  if (r >= rows) return;
+  if (rr >= size_t(NB) * heads * nt) return;
+  // row of the partials, (image, head) major, then the query
+  const size_t r = nt == T ? rr : rr / nt * T + t0 + rr % nt;
   float m = -INFINITY;
   for (int s = 0; s < splits; ++s) m = fmaxf(m, __ldg(part_ml + (size_t(s) * rows + r) * 2));
   float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, l = 0.f;
@@ -270,11 +275,14 @@ size_t flash_attn64_ws_bytes(int NB, int T, int C) {
 }
 
 int launch_flash_attn64(const bf16* qkv, bf16* out, int NB, int T, int C, float scale, float* ws, size_t ws_bytes,
-                        cudaStream_t stream) {
-  if (C % 64 != 0 || T <= 0) {
-    set_error("flash_attn64: C %% 64 != 0 or bad T");
+                        cudaStream_t stream, int qb_begin, int qb_end) {
+  const int nqb = (T + 127) / 128;
+  if (qb_end < 0) qb_end = nqb;
+  if (C % 64 != 0 || T <= 0 || qb_begin < 0 || qb_begin > qb_end || qb_end > nqb) {
+    set_error("flash_attn64: C %% 64 != 0, bad T or query blocks [%d, %d) outside [0, %d)", qb_begin, qb_end, nqb);
     return MGB_ERR_INVALID;
   }
+  if (qb_begin == qb_end) return MGB_OK;
   AttnParams p;
   const uint64_t dims[3] = {uint64_t(3 * C), uint64_t(T), uint64_t(NB)};
   const uint64_t strides[2] = {uint64_t(3 * C) * 2, uint64_t(T) * 3 * C * 2};
@@ -283,7 +291,7 @@ int launch_flash_attn64(const bf16* qkv, bf16* out, int NB, int T, int C, float 
   if (rc) return rc;
   rc = make_tmap_3d(&p.tmap_kv, qkv, dims, strides, box_kv);
   if (rc) return rc;
-  p.out = out; p.T = T; p.C = C;
+  p.out = out; p.T = T; p.C = C; p.qb0 = qb_begin;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.splits = 1; p.part_o = nullptr; p.part_ml = nullptr;
   {
@@ -296,12 +304,13 @@ int launch_flash_attn64(const bf16* qkv, bf16* out, int NB, int T, int C, float 
   }
   const size_t smem = 1024 + kQBytes + 2 * kKvStages * kKvBytes + 256;
   TRY(raise_smem_limit_once<flash_attn64_kernel>("flash_attn64", int(smem)));
-  dim3 grid((T + 127) / 128, C / 64, NB * p.splits);
+  dim3 grid(qb_end - qb_begin, C / 64, NB * p.splits);
   TRY(launch_pdl("flash_attn64", flash_attn64_kernel, grid, kAttnThreads, smem, stream, p));
   if (p.splits == 1) return MGB_OK;
-  const size_t threads = size_t(NB) * (C / 64) * T * 8;
+  const int t0 = qb_begin * 128, nt = std::min(T, qb_end * 128) - t0;
+  const size_t threads = size_t(NB) * (C / 64) * nt * 8;
   return launch_pdl("attn_combine", attn_combine_kernel, dim3(unsigned((threads + 255) / 256)), 256, 0, stream,
-                    (const float*)p.part_o, (const float*)p.part_ml, out, p.splits, NB, C / 64, T, C);
+                    (const float*)p.part_o, (const float*)p.part_ml, out, p.splits, NB, C / 64, T, C, t0, nt);
 }
 
 }  // namespace mgb

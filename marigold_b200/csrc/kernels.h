@@ -111,8 +111,11 @@ int make_tmap_5d(CUtensorMap* out, const void* base, const uint64_t dims[5], con
 //   qkv: bf16 [NB * T, 3 * C] (Q | K | V blocks, head h at columns h*64..), out: bf16 [NB * T, C]
 // ---------------------------------------------------------------------------------------------
 // ws (optional): split-KV workspace of flash_attn64_ws_bytes(); without it the kernel runs unsplit.
+// [qb_begin, qb_end): the 128-row query blocks computed (qb_end < 0: through the last); only those rows of out are
+// written. The KV split and the workspace layout are the whole (NB, T, C) problem's, so every row comes out bit for bit
+// as the whole launch computes it.
 int launch_flash_attn64(const bf16* qkv, bf16* out, int NB, int T, int C, float scale, float* ws, size_t ws_bytes,
-                        cudaStream_t stream);
+                        cudaStream_t stream, int qb_begin = 0, int qb_end = -1);
 int flash_attn64_splits(int NB, int T, int C);
 size_t flash_attn64_ws_bytes(int NB, int T, int C);
 

@@ -497,6 +497,31 @@ static int resnet_shortcut_halves(Ctx& c, const ResnetW& R, Act& a, Act& b, Act&
 }
 
 // ---------------------------------------------------------------------------------------------
+// Row split (Ctx::split_world > 0, one image): an attention's output o holds world chunks of row_split_chunk(T) rows;
+// this rank computes the rows of its chunk, and the exchange function fills the others in place (an all-gather).
+// ---------------------------------------------------------------------------------------------
+static size_t attn_out_rows(const Ctx& c, size_t M, int T) {
+  return c.split_world > 0 ? std::max(M, size_t(c.split_world) * row_split_chunk(T, c.split_world)) : M;
+}
+static void split_rows(const Ctx& c, int T, int* begin, int* end) {
+  if (c.split_world <= 0) { *begin = 0; *end = T; return; }
+  const int chunk = row_split_chunk(T, c.split_world);
+  *begin = std::min(T, c.split_rank * chunk);
+  *end = std::min(T, *begin + chunk);
+}
+static int exchange_rows(Ctx& c, bf16* o, int T, int C) {
+  if (c.split_world <= 0 || c.dry) return MGB_OK;
+  const size_t chunk_bytes = size_t(row_split_chunk(T, c.split_world)) * C * sizeof(bf16);
+  const int st = c.exchange_fn(c.exchange_ctx, o, chunk_bytes, c.split_rank, c.split_world, c.stream);
+  if (st != 0) {
+    set_error("row split: the exchange function returned %d (rank %d of %d, %zu bytes per rank)", st, c.split_rank,
+              c.split_world, chunk_bytes);
+    return MGB_ERR_STATE;
+  }
+  return MGB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Transformer2DModel (1 BasicTransformerBlock, linear projections). x fp32 [M, C] -> y fp32 [M, C]
 // ---------------------------------------------------------------------------------------------
 static int xfmr_forward(Ctx& c, const XfmrW& X, Act& x, Act& y, int NB, int T) {
@@ -507,7 +532,7 @@ static int xfmr_forward(Ctx& c, const XfmrW& X, Act& x, Act& y, int NB, int T) {
   float* hs0 = aalloc<float>(c, M * C);
   float* hs1 = aalloc<float>(c, M * C);
   bf16* qkv = aalloc<bf16>(c, M * 3 * C);
-  bf16* o = aalloc<bf16>(c, M * C);
+  bf16* o = aalloc<bf16>(c, attn_out_rows(c, M, T) * C);
   bf16* ffm = aalloc<bf16>(c, M * 4 * C);
   bf16* hsb = aalloc<bf16>(c, M * C);
   const size_t attn_ws_bytes = flash_attn64_ws_bytes(NB, T, C);
@@ -519,7 +544,14 @@ static int xfmr_forward(Ctx& c, const XfmrW& X, Act& x, Act& y, int NB, int T) {
   const bool no_ln = skip_family("ln"), no_attn = skip_family("attn"), no_x = skip_family("xattn");
   if (!no_ln) LAUNCH(launch_layernorm(hs0, a, X.ln1.g, X.ln1.b, int(M), C, 1e-5f, c.stream));
   { Epi e; e.out_bf16 = qkv; TRY(linear(c, a, int(M), X.qkv, e)); }
-  if (!no_attn) LAUNCH(launch_flash_attn64(qkv, o, NB, T, C, 0.125f, attn_ws, attn_ws_bytes, c.stream));
+  {
+    int r0, r1;
+    split_rows(c, T, &r0, &r1);
+    // a rank without rows (r0 = r1 = T) launches an empty range, not the partial last block another rank owns
+    const int qb0 = r0 / 128, qb1 = r1 > r0 ? (r1 + 127) / 128 : qb0;
+    if (!no_attn) LAUNCH(launch_flash_attn64(qkv, o, NB, T, C, 0.125f, attn_ws, attn_ws_bytes, c.stream, qb0, qb1));
+    TRY(exchange_rows(c, o, T, C));
+  }
   { Epi e; e.bias = X.o1.b; e.residual = hs0; e.out_f32 = hs1; TRY(linear(c, o, int(M), X.o1, e)); }
   // cross attention against the empty-prompt context, collapsed (norm.cu: xattn2_fused_kernel): LN2, to_q, the 2-key
   // softmax, to_out + residual and LN3 are one launch; hsb = bf16 trunk after attn2, a = LN3 of it for the feed-forward
@@ -559,7 +591,9 @@ int vae_attn_rows(int T, int C, size_t budget, int force_rows) {
   return std::min(T, std::max(budget_rows, wave_rows));
 }
 
-int vae_attn_core(Ctx& c, const bf16* q, const bf16* k, const bf16* v, bf16* o, int NB, int T, int C) {
+int vae_attn_core(Ctx& c, const bf16* q, const bf16* k, const bf16* v, bf16* o, int NB, int T, int C, int row_begin,
+                  int row_end) {
+  if (row_end < 0) row_end = T;
   const int Tp = (T + 63) / 64 * 64;
   const int R = vae_attn_rows(T, C, c.attn_budget, c.attn_rows);
   const Tile tile_s = matmul_tile(T, T, C, EPI_SCALE), tile_pv = matmul_tile(T, C, Tp, 0);
@@ -570,12 +604,12 @@ int vae_attn_core(Ctx& c, const bf16* q, const bf16* k, const bf16* v, bf16* o, 
   const float scale = 1.0f / sqrtf(float(C));
   for (int n = 0; n < NB; ++n) {
     const size_t off = size_t(n) * T * C;
-    for (int r0 = 0; r0 < T; r0 += R) {
-      const int rows = std::min(R, T - r0);
+    for (int r0 = row_begin; r0 < row_end; r0 += R) {
+      const int rows = std::min(R, row_end - r0);
       const size_t qo = off + size_t(r0) * C;
       { Epi e; e.out_f32 = s; e.flags = EPI_SCALE; e.scale = scale; TRY(matmul_nt(c, q + qo, k + off, rows, T, C, e, Tp, tile_s)); }
       LAUNCH(launch_softmax_rows(s, pr, rows, T, Tp, c.stream));
-      if (r0 == 0) LAUNCH(launch_transpose_bf16(v + off, vt, T, C, Tp, c.stream));
+      if (r0 == row_begin) LAUNCH(launch_transpose_bf16(v + off, vt, T, C, Tp, c.stream));
       { Epi e; e.out_bf16 = o + qo; TRY(matmul_nt(c, pr, vt, rows, C, Tp, e, 0, tile_pv)); }
     }
   }
@@ -591,12 +625,15 @@ static int vae_attn_forward(Ctx& c, const VaeAttnW& A, Act& x, Act& y, int NB, i
   bf16* q = aalloc<bf16>(c, M * C);
   bf16* k = aalloc<bf16>(c, M * C);
   bf16* v = aalloc<bf16>(c, M * C);
-  bf16* o = aalloc<bf16>(c, M * C);
+  bf16* o = aalloc<bf16>(c, attn_out_rows(c, M, T) * C);
   TRY(groupnorm(c, x, nullptr, a, nullptr, A.gn, NB, T, 1e-6f, 0));
   { Epi e; e.bias = A.q.b; e.out_bf16 = q; TRY(linear(c, a, int(M), A.q, e)); }
   { Epi e; e.bias = A.k.b; e.out_bf16 = k; TRY(linear(c, a, int(M), A.k, e)); }
   { Epi e; e.bias = A.v.b; e.out_bf16 = v; TRY(linear(c, a, int(M), A.v, e)); }
-  TRY(vae_attn_core(c, q, k, v, o, NB, T, C));
+  int r0, r1;
+  split_rows(c, T, &r0, &r1);
+  TRY(vae_attn_core(c, q, k, v, o, NB, T, C, r0, r1));
+  TRY(exchange_rows(c, o, T, C));
   { Epi e; e.bias = A.o.b; e.residual = x.p; e.out_f32 = y.p; TRY(linear(c, o, int(M), A.o, e)); }
   c.arena->release(mk);
   return MGB_OK;

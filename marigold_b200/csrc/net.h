@@ -144,12 +144,24 @@ struct Ctx {
   // grid-barrier counters of the GroupNorm launches of one forward (one per image and launch; zeroed once per forward)
   unsigned* sync_base = nullptr;
   size_t sync_off = 0, sync_cap = 0, sync_need = 0;
+  // row split (mgb_set_row_split): split_world > 0 runs this rank's share of every attention's query rows, then
+  // exchange(); 0 runs them whole
+  int split_rank = 0, split_world = 0;
+  mgb_exchange_fn exchange_fn = nullptr;
+  void* exchange_ctx = nullptr;
 };
+
+// Query rows per rank of a T-row attention split over `world` ranks: whole 128-row blocks, ceil(ceil(T / 128) / world)
+// of them. Rank r owns rows [r chunk, (r + 1) chunk) within [0, T).
+inline int row_split_chunk(int T, int world) { return ((T + 127) / 128 + world - 1) / world * 128; }
 
 // The VAE mid-block attention between its projections: o = softmax(q k^T / sqrt(C)) v per image, on bf16 q, k, v, o
 // [NB * T, C], in blocks of vae_attn_rows(T, C, c.attn_budget, c.attn_rows) query rows. Its scratch (V^T, one block's
 // fp32 scores and bf16 probabilities) comes from the arena and is released on return.
-int vae_attn_core(Ctx& c, const bf16* q, const bf16* k, const bf16* v, bf16* o, int NB, int T, int C);
+// Query rows [row_begin, row_end) only (row_end < 0: through T), in the blocks and tiles of the whole T-row problem,
+// so each row is bit-identical to the whole call's; row_begin a multiple of 128 (or of the block rows).
+int vae_attn_core(Ctx& c, const bf16* q, const bf16* k, const bf16* v, bf16* o, int NB, int T, int C,
+                  int row_begin = 0, int row_end = -1);
 
 struct UNetW {
   ConvW conv_in, conv_out;
@@ -212,6 +224,12 @@ struct mgb_handle {
   // Tile rows per band of the low-memory decoder's banded up-conv and conv1 (Ctx::band_up_tiles): 0 the library's
   // choice, else forced (mgb_debug_vae_bands)
   int vae_band_up_tiles = 0, vae_band_conv1_tiles = 0;
+  // row split (mgb_set_row_split): installed while fn != null
+  struct RowSplit {
+    int rank = 0, world = 0;
+    mgb_exchange_fn fn = nullptr;
+    void* ctx = nullptr;
+  } row_split;
   // conditioning / schedule
   bool text_set = false;
   int n_steps = 0;

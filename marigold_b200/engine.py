@@ -49,6 +49,14 @@ class EngineConfig:
 _DT = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 
 
+class _DeviceBytes:
+    """n bytes of device memory at `addr`, for torch.as_tensor to view without a copy."""
+
+    def __init__(self, addr: int, n: int):
+        self.__cuda_array_interface__ = {"shape": (int(n),), "typestr": "|u1", "data": (int(addr), False),
+                                         "strides": None, "version": 2}
+
+
 class Engine:
     def __init__(self, cfg: EngineConfig = EngineConfig(), device: Optional[torch.device] = None):
         if not torch.cuda.is_available():
@@ -62,6 +70,8 @@ class Engine:
             check(self.lib.mgb_create(C.byref(ccfg), C.byref(self._h)), "mgb_create")
         self._finalized = False
         self.n_steps = 0
+        self._exchange_cb = None         # the installed row-split callback, referenced while the library may call it
+        self._exchange_error = None
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -109,6 +119,44 @@ class Engine:
                   "mgb_set_schedule")
         self.n_steps = n
 
+    # ---- one image on several GPUs ------------------------------------------------------------------
+    def set_row_split(self, rank: int = 0, world: int = 1, exchange=None) -> None:
+        """Split every attention's query rows over `world` ranks (mgb_set_row_split); exchange=None clears it.
+        exchange(buf, rank, world) receives one attention's output as a uint8 CUDA tensor of `world` equal chunks, chunk
+        `rank` holding this rank's rows, and must fill the other chunks in place (an all-gather, parallel.exchange_rows).
+        It runs with the library call's stream as torch's current stream. While the split is installed the hot-path
+        calls take one image at a time."""
+        if exchange is None:
+            check(self.lib.mgb_set_row_split(self._h, 0, 1, None, None), "mgb_set_row_split")
+            self._exchange_cb = None
+            return
+
+        def call(ctx, buf, chunk_bytes, r, g, stream):
+            try:
+                view = torch.as_tensor(_DeviceBytes(buf, chunk_bytes * g), device=self.device)
+                s = torch.cuda.ExternalStream(stream, device=self.device) if stream else \
+                    torch.cuda.default_stream(self.device)
+                with torch.cuda.stream(s):
+                    exchange(view, r, g)
+                return 0
+            except Exception as e:  # noqa: BLE001 -- a Python error must not unwind through the library
+                self._exchange_error = e
+                return -1
+
+        cb = _lib.EXCHANGE_FN(call)
+        check(self.lib.mgb_set_row_split(self._h, rank, world, C.cast(cb, C.c_void_p), None), "mgb_set_row_split")
+        self._exchange_cb = cb
+
+    def _check(self, status: int, what: str) -> None:
+        """check(), with the exchange function's own exception as the cause of a failure it caused."""
+        err, self._exchange_error = self._exchange_error, None
+        if status != 0 and err is not None:
+            try:
+                check(status, what)
+            except _lib.MgbError as e:
+                raise _lib.MgbError(f"{e}: {err!r}") from err
+        check(status, what)
+
     # ---- hot path -------------------------------------------------------------------------------
     def _f32(self, t: torch.Tensor) -> torch.Tensor:
         return t.to(self.device, torch.float32).contiguous()
@@ -118,7 +166,7 @@ class Engine:
         B, _, H, W = rgb.shape
         out = torch.empty(B, 4, H // 8, W // 8, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            check(self.lib.mgb_encode(self._h, ptr(rgb), B, H, W, ptr(out), stream_ptr()), "mgb_encode")
+            self._check(self.lib.mgb_encode(self._h, ptr(rgb), B, H, W, ptr(out), stream_ptr()), "mgb_encode")
         return out
 
     def unet_step(self, rgb_latent, target, step_index: int, noise=None, want_model_out=False):
@@ -129,8 +177,8 @@ class Engine:
         mo = torch.empty_like(target) if want_model_out else None
         nz = self._f32(noise) if noise is not None else None
         with torch.cuda.device(self.device):
-            check(self.lib.mgb_unet_step(self._h, ptr(rgb_latent), ptr(target), ptr(nz), ptr(mo), step_index, B, lh, lw,
-                                         stream_ptr()), "mgb_unet_step")
+            self._check(self.lib.mgb_unet_step(self._h, ptr(rgb_latent), ptr(target), ptr(nz), ptr(mo), step_index, B, lh,
+                                               lw, stream_ptr()), "mgb_unet_step")
         return mo
 
     def denoise(self, rgb_latent, target, step_noise=None) -> torch.Tensor:
@@ -139,8 +187,8 @@ class Engine:
         B, _, lh, lw = target.shape
         sn = self._f32(step_noise) if step_noise is not None else None
         with torch.cuda.device(self.device):
-            check(self.lib.mgb_denoise(self._h, ptr(rgb_latent), ptr(target), ptr(sn), B, lh, lw, stream_ptr()),
-                  "mgb_denoise")
+            self._check(self.lib.mgb_denoise(self._h, ptr(rgb_latent), ptr(target), ptr(sn), B, lh, lw, stream_ptr()),
+                        "mgb_denoise")
         return target
 
     def denoise_range_(self, rgb_latent, target, first_step: int, num_steps: int, step_noise=None) -> None:
@@ -149,8 +197,8 @@ class Engine:
         assert rgb_latent.is_cuda and rgb_latent.dtype == torch.float32 and rgb_latent.is_contiguous()
         B, _, lh, lw = target.shape
         with torch.cuda.device(self.device):
-            check(self.lib.mgb_denoise_range(self._h, ptr(rgb_latent), ptr(target), ptr(step_noise), first_step,
-                                             num_steps, B, lh, lw, stream_ptr()), "mgb_denoise_range")
+            self._check(self.lib.mgb_denoise_range(self._h, ptr(rgb_latent), ptr(target), ptr(step_noise), first_step,
+                                                   num_steps, B, lh, lw, stream_ptr()), "mgb_denoise_range")
 
     def decode(self, latent, mode: int) -> torch.Tensor:
         """mode: 0 depth head [B,1,H,W], 1 normals head, 2 raw RGB, 3 (clip + 1) / 2 (one IID target); latent [B,4,h,w]."""
@@ -160,7 +208,7 @@ class Engine:
         ch = 1 if mode == 0 else 3
         out = torch.empty(B, ch, lh * 8, lw * 8, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            check(self.lib.mgb_decode(self._h, ptr(latent), B, lh, lw, mode, ptr(out), stream_ptr()), "mgb_decode")
+            self._check(self.lib.mgb_decode(self._h, ptr(latent), B, lh, lw, mode, ptr(out), stream_ptr()), "mgb_decode")
         return out
 
     def workspace_bytes(self, B, H, W) -> int:

@@ -73,6 +73,17 @@ def flash_attn64(qkv, NB, T, C, scale):
     return out
 
 
+def flash_attn64_blocks(qkv, NB, T, C, scale, q_block_begin, q_block_end, out=None):
+    """flash_attn64 on the 128-row query blocks [q_block_begin, q_block_end) of every (image, head): those rows of `out`
+    (allocated when None) are written, bit for bit as the whole launch writes them, and no other."""
+    lib = _lib.load()
+    if out is None:
+        out = torch.empty(NB * T, C, dtype=torch.bfloat16, device=qkv.device)
+    check(lib.mgb_op_flash_attn64_ex(ptr(qkv), ptr(out), NB, T, C, float(scale), q_block_begin, q_block_end,
+                                     stream_ptr()), "mgb_op_flash_attn64_ex")
+    return out
+
+
 def groupnorm(x, gamma, beta, NB, HW, C, G, eps, silu):
     lib = _lib.load()
     y = torch.empty(NB, HW, C, dtype=torch.bfloat16, device=x.device)

@@ -5,10 +5,16 @@ The reference is single-process (SURVEY.md §2.2); the only place members meet i
 r, r+G, r+2G, ...; every rank encodes its image locally (cheaper than a broadcast) and reads ITS rows
 of the pre-drawn noise tensor; one all-gather of the decoded per-member maps (NCCL over NVLink on
 GPUs, gloo on CPU in the tests) precedes the ensemble, which then runs replicated and deterministic.
-There is no collective inside the denoising loop.
+There is no collective inside the denoising loop of a sharded call.
+
+A size group of ONE job (one image with ensemble_size 1) would leave every rank but one idle, so at native resolution it
+runs row-split instead (row_split_rule): every rank runs the whole job, and every attention computes only its rank's
+share of the query rows, joined by one in-place all-gather per attention (mgb_set_row_split). Every rank ends with the
+same maps, bit-identical to the one-GPU call.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import List, Optional
 
 import torch
@@ -116,3 +122,75 @@ def barrier_max_ms(ms: float, device: Optional[torch.device] = None) -> float:
     t = torch.tensor([ms], dtype=torch.float64, device=device if device is not None else "cpu")
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return float(t.item())
+
+
+# ---- one job on every rank: the attentions' query rows split over the ranks ------------------------------------------
+# Smallest level-0 latent (h / 8 * w / 8 tokens) that runs row-split: 768 x 768. From tools/row_split.py on one H100
+# 80GB HBM3 (700 W power limit, 1980 MHz maximum SM clock; DESIGN.md section 7): the smallest of the measured sizes
+# (768², 1920x1080, 12, 24 and 48 MP) at which one rank's share of a UNet step at G = 2 beats the captured one-GPU step
+# by more than the all-gather time a model gives (bytes received over NVLink's 450 GB/s per direction, not measured). At
+# 768² that was 7.25 ms + 0.06 ms (model) against 8.09 ms. Smaller sizes were not measured, and the model leaves out
+# the latency of the step's 16 collectives, of the order of that margin.
+ROW_SPLIT_MIN_TOKENS = 9_216
+
+
+def row_split_chunk(T: int, world_size: int) -> int:
+    """Query rows per rank of a T-row attention: whole 128-row blocks (csrc/net.h row_split_chunk)."""
+    return -(-(-(-T // 128)) // world_size) * 128
+
+
+def row_split_rows(T: int, rank: int, world_size: int) -> range:
+    """The query rows rank `rank` computes: [r chunk, (r + 1) chunk) within [0, T), possibly empty."""
+    chunk = row_split_chunk(T, world_size)
+    return range(min(T, rank * chunk), min(T, (rank + 1) * chunk))
+
+
+def row_split_rule(n_jobs: int, h: int, w: int, world_size: int, min_tokens: Optional[int] = None) -> bool:
+    """Whether a size group of n_jobs (image, member) jobs at h x w pixels runs row-split on world_size ranks: one job,
+    several ranks, and a level-0 latent of at least min_tokens (ROW_SPLIT_MIN_TOKENS) tokens."""
+    if min_tokens is None:
+        min_tokens = ROW_SPLIT_MIN_TOKENS
+    return world_size > 1 and n_jobs == 1 and (h // 8) * (w // 8) >= min_tokens
+
+
+def exchange_rows(buf: torch.Tensor, rank: int, world_size: int, group=None) -> None:
+    """The row split's exchange: buf holds world_size equal chunks, chunk `rank` this rank's; fills the others in place.
+    NCCL all-gathers in place on the device; gloo goes through a host copy. Runs on torch's current stream."""
+    n = buf.numel() // world_size
+    if dist.get_backend(group) == "nccl":
+        dist.all_gather_into_tensor(buf, buf[rank * n:(rank + 1) * n], group=group)
+        return
+    host = buf.cpu()
+    out = torch.empty_like(host)
+    dist.all_gather_into_tensor(out, host[rank * n:(rank + 1) * n].clone(), group=group)
+    buf.copy_(out)
+
+
+@contextlib.contextmanager
+def row_split(engine, on: bool = True):
+    """Installs the row split on engine for this rank while the block runs, and clears it after."""
+    if not on:
+        yield
+        return
+    rank, G = world()
+    engine.set_row_split(rank, G, exchange_rows)
+    try:
+        yield
+    finally:
+        engine.set_row_split()
+
+
+def broadcast_from_first(tensors, device: Optional[torch.device] = None):
+    """Rank 0's tensors on every rank (None entries stay None): a row-split job must run on the same noise everywhere."""
+    rank, G = world()
+    if G == 1:
+        return list(tensors)
+    out = []
+    for t in tensors:
+        if t is None:
+            out.append(None)
+            continue
+        c = t.to(_collective_device(device)).contiguous()
+        dist.broadcast(c, src=0)
+        out.append(c.to(t.device))
+    return out

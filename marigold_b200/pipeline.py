@@ -340,22 +340,54 @@ class _MarigoldBase:
         assert rgb_norm.min() >= -1.0 and rgb_norm.max() <= 1.0
         return rgb_norm, input_size
 
-    def _member_batch_size(self, input_image, processing_res, ensemble_size, batch_size):
-        """select_batch_size for this call, from the input's shape alone: an input that cannot run is refused before
-        anything is allocated on the device or launched."""
+    def _call_size(self, input_image, processing_res):
+        """(h, w) the call processes, from the input's shape alone; None for an input _preprocess rejects."""
         if Image is not None and isinstance(input_image, Image.Image):
             w0, h0 = input_image.size
         elif isinstance(input_image, torch.Tensor) and input_image.dim() == 4:
             h0, w0 = input_image.shape[-2:]
         else:
+            return None
+        return _processing_size(h0, w0, processing_res)
+
+    def _member_batch_size(self, input_image, processing_res, ensemble_size, batch_size):
+        """select_batch_size for this call, from the input's shape alone: an input that cannot run is refused before
+        anything is allocated on the device or launched."""
+        size = self._call_size(input_image, processing_res)
+        if size is None:
             return batch_size                                # _preprocess rejects it
         from . import parallel
 
         rank, G = parallel.world()
         n = len(parallel.member_indices(ensemble_size, rank, G))
-        h, w = _processing_size(h0, w0, processing_res)
+        h, w = size
         return select_batch_size(self.engine, n, h, w, batch_size,
                                  reserve_bytes=call_reserve_bytes(h, w, ensemble_size, self.member_channels))
+
+    def _member_batch(self, input_image, processing_res, ensemble_size, batch_size):
+        """(member batch, row split) for this call: whether the ranks agreed to run its one member row-split
+        (parallel.row_split_rule), with its batch of 1, or _member_batch_size's batch and False. The caller passes the
+        decision on to _infer_members."""
+        from . import parallel
+
+        rank, G = parallel.world()
+        size = self._call_size(input_image, processing_res)
+        if size is None or not parallel.row_split_rule(ensemble_size, size[0], size[1], G):
+            return self._member_batch_size(input_image, processing_res, ensemble_size, batch_size), False
+        h, w = size
+        # every rank runs the one member: the ranks agree on the split and on its admission (each rank's depends on its
+        # own free memory) in one all-reduce, so that no rank enters an exchange alone
+        err = None
+        try:
+            with parallel.row_split(self.engine):
+                bs = select_batch_size(self.engine, 1, h, w, batch_size,
+                                       reserve_bytes=call_reserve_bytes(h, w, ensemble_size, self.member_channels))
+        except ValueError as e:
+            bs, err = 0, e
+        split, admitted = parallel.agree_batch_sizes([1, min(bs, 1)], self.device)
+        if not admitted:
+            raise err if err is not None else ValueError(f"another rank cannot admit one member at {h} x {w}")
+        return 1, split == 1
 
     def _draw_noise(self, shape, generator, noise):
         if noise is not None:
@@ -371,52 +403,60 @@ class _MarigoldBase:
         return self.engine.encode(rgb_in)
 
     def _infer_members(self, rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise, step_noise,
-                       decode_mode):
+                       decode_mode, row_split=False):
         """The body of the reference's batch loop (depth_pipeline.py:281-290) + single_infer (:397-477).
         Under torch.distributed (one process per GPU) the members are sharded round-robin and joined by
-        one all-gather of the decoded maps (parallel.py); the result is identical on every rank."""
+        one all-gather of the decoded maps (parallel.py); the result is identical on every rank. With row_split
+        (the ranks' agreed decision, _member_batch) the one member runs on every rank, on rank 0's noise."""
         from . import parallel
 
         rank, G = parallel.world()
-        mine = parallel.member_indices(ensemble_size, rank, G)
+        split = row_split
+        assert not split or ensemble_size == 1, "a row-split call runs one member"
+        mine = [0] if split else parallel.member_indices(ensemble_size, rank, G)
         _bs = batch_size if batch_size > 0 else select_batch_size(self.engine, len(mine), *rgb_norm.shape[-2:])
         self._set_schedule(denoising_steps)
-        rgb_latent1 = self.encode_rgb(rgb_norm)                      # [1,4,h,w]
-        lh, lw = rgb_latent1.shape[-2:]
-        is_lcm = isinstance(self.scheduler, LCMScheduler)
-        need_sn = is_lcm and denoising_steps > 1
-        ct = self.engine.cfg.unet_out_channels               # 4, or 4 n for an n-target IID model
-        if G > 1:
-            # every rank draws (or receives) the FULL noise tensors and takes its rows, so member k's noise
-            # does not depend on the partitioning (SURVEY.md F9)
-            noise = self._draw_noise((ensemble_size, ct, lh, lw), generator, noise)
-            if need_sn and step_noise is None:
-                dev = generator.device if generator is not None else self.device
-                step_noise = torch.randn((denoising_steps - 1, ensemble_size, ct, lh, lw), device=dev, dtype=self.dtype,
-                                         generator=generator)
-        preds = []
-        for s in range(0, len(mine), _bs):
-            ids = mine[s:s + _bs]
-            nb = len(ids)
-            if G > 1 or noise is not None:
-                z0 = noise[ids].to(self.device, torch.float32).contiguous()
-            else:
-                z0 = self._draw_noise((nb, ct, lh, lw), generator, None)
-            sn = None
-            if need_sn:
-                if step_noise is not None:
-                    sn = step_noise[:, ids].to(self.device, torch.float32).contiguous()
-                else:
-                    # one randn per step, in step order after z0: the draw sequence of scheduler.step(generator=...)
-                    # inside the reference loop (depth_pipeline.py:466-468), so a seeded generator gives the same stream
+        with parallel.row_split(self.engine, split):
+            rgb_latent1 = self.encode_rgb(rgb_norm)                      # [1,4,h,w]
+            lh, lw = rgb_latent1.shape[-2:]
+            is_lcm = isinstance(self.scheduler, LCMScheduler)
+            need_sn = is_lcm and denoising_steps > 1
+            ct = self.engine.cfg.unet_out_channels               # 4, or 4 n for an n-target IID model
+            if G > 1:
+                # every rank draws (or receives) the FULL noise tensors and takes its rows, so member k's noise
+                # does not depend on the partitioning (SURVEY.md F9)
+                noise = self._draw_noise((ensemble_size, ct, lh, lw), generator, noise)
+                if need_sn and step_noise is None:
                     dev = generator.device if generator is not None else self.device
-                    sn = torch.stack([torch.randn((nb, ct, lh, lw), device=dev, dtype=self.dtype, generator=generator)
-                                      for _ in range(denoising_steps - 1)]).to(self.device)
-            target = self.engine.denoise(rgb_latent1.expand(nb, -1, -1, -1).contiguous(), z0, sn)
-            preds.append(self._decode(target, decode_mode))
+                    step_noise = torch.randn((denoising_steps - 1, ensemble_size, ct, lh, lw), device=dev,
+                                             dtype=self.dtype, generator=generator)
+            if split:
+                noise, step_noise = parallel.broadcast_from_first([noise, step_noise], self.device)
+            preds = []
+            for s in range(0, len(mine), _bs):
+                ids = mine[s:s + _bs]
+                nb = len(ids)
+                if G > 1 or noise is not None:
+                    z0 = noise[ids].to(self.device, torch.float32).contiguous()
+                else:
+                    z0 = self._draw_noise((nb, ct, lh, lw), generator, None)
+                sn = None
+                if need_sn:
+                    if step_noise is not None:
+                        sn = step_noise[:, ids].to(self.device, torch.float32).contiguous()
+                    else:
+                        # one randn per step, in step order after z0: the draw sequence of scheduler.step(generator=...)
+                        # inside the reference loop (depth_pipeline.py:466-468), so a seeded generator gives the same
+                        # stream
+                        dev = generator.device if generator is not None else self.device
+                        sn = torch.stack([torch.randn((nb, ct, lh, lw), device=dev, dtype=self.dtype,
+                                                      generator=generator)
+                                          for _ in range(denoising_steps - 1)]).to(self.device)
+                target = self.engine.denoise(rgb_latent1.expand(nb, -1, -1, -1).contiguous(), z0, sn)
+                preds.append(self._decode(target, decode_mode))
         ch = 1 if decode_mode == 0 else (3 * (ct // 4) if decode_mode == _lib_decode_iid else 3)
         local = torch.concat(preds, dim=0) if preds else torch.empty((0, ch, lh * 8, lw * 8), device=self.device)
-        return parallel.gather_members(local, ensemble_size)
+        return local if split else parallel.gather_members(local, ensemble_size)
 
     def _decode(self, target, decode_mode):
         """The decode of one denoised member batch [NB, ct, lh, lw] -> [NB, member_channels, 8 lh, 8 lw]."""
@@ -492,14 +532,22 @@ class _MarigoldBase:
                 got = f"{len(per_image)} entries" if isinstance(per_image, (list, tuple)) else type(per_image).__name__
                 raise ValueError(f"{name} must be None or a list of one entry per image ({N}); got {got}")
         groups = size_groups([_processing_size(h0, w0, processing_res) for h0, w0 in hw0])
-        sizes = []
+        sizes, splits, refused = [], [], {}
         for (h, w), idx in groups:
             n_jobs = len(idx) * E
+            # a group of one job runs row-split on every rank (parallel.row_split_rule); its admission is agreed with
+            # the batch sizes below, before any rank runs it
+            split = parallel.row_split_rule(n_jobs, h, w, G)
             try:
-                sizes.append(select_list_batch_size(self.engine, parallel.slots_per_rank(n_jobs, G), h, w, E,
-                                                    self.member_channels, len(idx), G, batch_size))
+                with parallel.row_split(self.engine, split):
+                    sizes.append(select_list_batch_size(self.engine, 1 if split else parallel.slots_per_rank(n_jobs, G),
+                                                        h, w, E, self.member_channels, len(idx), G, batch_size))
             except ValueError as e:
-                raise ValueError(f"image {idx[0]}: {e}") from None
+                if not split:
+                    raise ValueError(f"image {idx[0]}: {e}") from None
+                refused[len(sizes)] = e
+                sizes.append(0)
+            splits.append(int(split))
             lh, lw = h // 8, w // 8
             for i in idx:
                 if noise is not None and noise[i] is not None:
@@ -511,7 +559,12 @@ class _MarigoldBase:
                         f"{(denoising_steps - 1, E, ct, lh, lw)}"
         if N == 0:
             return
-        sizes = parallel.agree_batch_sizes(sizes, self.device)
+        agreed = parallel.agree_batch_sizes(sizes + splits, self.device)
+        sizes, splits = agreed[:len(groups)], agreed[len(groups):]
+        for k, bs in enumerate(sizes):
+            if bs == 0:
+                why = refused.get(k, f"another rank cannot admit one member at {groups[k][0][0]} x {groups[k][0][1]}")
+                raise ValueError(f"image {groups[k][1][0]}: {why}")
         self._set_schedule(denoising_steps)
 
         def draw(i):
@@ -550,46 +603,51 @@ class _MarigoldBase:
                 next_draw += 1
             return drawn.pop(i)
 
-        for ((h, w), idx), bs in zip(groups, sizes):
+        for ((h, w), idx), bs, split in zip(groups, sizes, splits):
             lh, lw = h // 8, w // 8
             n_jobs = len(idx) * E
             lat, z, sn, maps, done = {}, {}, {}, {}, {}
-            for rnd in range(parallel.num_rounds(n_jobs, bs, G)):
-                jobs, mine = parallel.round_jobs(n_jobs, bs, rnd, rank, G)
-                for k in jobs:                       # open the images this round reaches
-                    i = idx[k // E]
-                    if i not in maps:
-                        z[i], sn[i] = noise_of(i)
-                        maps[i] = torch.empty((E, self.member_channels, 8 * lh, 8 * lw), device=self.device)
-                        done[i] = 0
-                if mine:
-                    runs = _image_runs(mine, idx, E)
-                    for i, _ in runs:
-                        if i not in lat:
-                            rgb_norm, _ = self._preprocess(images[i], processing_res, resample)
-                            lat[i] = self.encode_rgb(rgb_norm)
-                            del rgb_norm
-                    rgb_latent = torch.cat([lat[i].expand(len(ms), -1, -1, -1) for i, ms in runs]).contiguous()
-                    z0 = torch.cat([z[i][ms] for i, ms in runs]).contiguous()
-                    s = torch.cat([sn[i][:, ms] for i, ms in runs], dim=1).contiguous() if need_sn else None
-                    local = self._decode(self.engine.denoise(rgb_latent, z0, s), decode_mode)
-                    del rgb_latent, z0, s
-                else:
-                    local = torch.empty((0, self.member_channels, 8 * lh, 8 * lw), device=self.device)
-                pred = parallel.gather_round(local, bs, len(jobs))
-                del local
-                r0 = 0
-                for i, ms in _image_runs(jobs, idx, E):
-                    maps[i][ms[0]:ms[-1] + 1] = pred[r0:r0 + len(ms)]
-                    r0 += len(ms)
-                    done[i] += len(ms)
-                    if done[i] == E:
-                        member_maps = maps.pop(i)
-                        for held in (lat, z, sn, done):
-                            held.pop(i, None)
-                        finish(i, member_maps, hw0[i])
-                        del member_maps
-                del pred
+            with parallel.row_split(self.engine, split == 1):
+                for rnd in range(parallel.num_rounds(n_jobs, bs, G)):
+                    jobs, mine = parallel.round_jobs(n_jobs, bs, rnd, rank, G)
+                    if split:
+                        mine = jobs                      # every rank runs the one job
+                    for k in jobs:                       # open the images this round reaches
+                        i = idx[k // E]
+                        if i not in maps:
+                            z[i], sn[i] = noise_of(i)
+                            if split:
+                                z[i], sn[i] = parallel.broadcast_from_first([z[i], sn[i]], self.device)
+                            maps[i] = torch.empty((E, self.member_channels, 8 * lh, 8 * lw), device=self.device)
+                            done[i] = 0
+                    if mine:
+                        runs = _image_runs(mine, idx, E)
+                        for i, _ in runs:
+                            if i not in lat:
+                                rgb_norm, _ = self._preprocess(images[i], processing_res, resample)
+                                lat[i] = self.encode_rgb(rgb_norm)
+                                del rgb_norm
+                        rgb_latent = torch.cat([lat[i].expand(len(ms), -1, -1, -1) for i, ms in runs]).contiguous()
+                        z0 = torch.cat([z[i][ms] for i, ms in runs]).contiguous()
+                        s = torch.cat([sn[i][:, ms] for i, ms in runs], dim=1).contiguous() if need_sn else None
+                        local = self._decode(self.engine.denoise(rgb_latent, z0, s), decode_mode)
+                        del rgb_latent, z0, s
+                    else:
+                        local = torch.empty((0, self.member_channels, 8 * lh, 8 * lw), device=self.device)
+                    pred = local if split else parallel.gather_round(local, bs, len(jobs))
+                    del local
+                    r0 = 0
+                    for i, ms in _image_runs(jobs, idx, E):
+                        maps[i][ms[0]:ms[-1] + 1] = pred[r0:r0 + len(ms)]
+                        r0 += len(ms)
+                        done[i] += len(ms)
+                        if done[i] == E:
+                            member_maps = maps.pop(i)
+                            for held in (lat, z, sn, done):
+                                held.pop(i, None)
+                            finish(i, member_maps, hw0[i])
+                            del member_maps
+                    del pred
 
 
 class MarigoldDepthPipeline(_MarigoldBase):
@@ -643,11 +701,11 @@ class MarigoldDepthPipeline(_MarigoldBase):
         _check_ensemble_size(self.engine, ensemble_size)          # fail before any inference work is spent
         self._check_inference_step(denoising_steps)
         resample = get_tv_resample_method(resample_method)
-        batch_size = self._member_batch_size(input_image, processing_res, ensemble_size, batch_size)
+        batch_size, row_split = self._member_batch(input_image, processing_res, ensemble_size, batch_size)
         rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
 
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
-                                           step_noise, _lib_decode_depth)
+                                           step_noise, _lib_decode_depth, row_split)
         return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
                             ensemble_kwargs, color_map=color_map)
 
@@ -716,10 +774,10 @@ class MarigoldNormalsPipeline(_MarigoldBase):
         assert ensemble_size >= 1
         self._check_inference_step(denoising_steps)
         resample = get_tv_resample_method(resample_method)
-        batch_size = self._member_batch_size(input_image, processing_res, ensemble_size, batch_size)
+        batch_size, row_split = self._member_batch(input_image, processing_res, ensemble_size, batch_size)
         rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
-                                           None, _lib_decode_normals)
+                                           None, _lib_decode_normals, row_split)
         return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
                             ensemble_kwargs)
 
@@ -794,10 +852,10 @@ class MarigoldIIDPipeline(_MarigoldBase):
         assert ensemble_size >= 1
         self._check_inference_step(denoising_steps)
         resample = get_tv_resample_method(resample_method)
-        batch_size = self._member_batch_size(input_image, processing_res, ensemble_size, batch_size)
+        batch_size, row_split = self._member_batch(input_image, processing_res, ensemble_size, batch_size)
         rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
         target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
-                                           None, _lib_decode_iid)
+                                           None, _lib_decode_iid, row_split)
         return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
                             ensemble_kwargs)
 
