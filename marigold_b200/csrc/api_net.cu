@@ -556,7 +556,7 @@ static int decode_low_memory(mgb_handle* h, int lh, int lw, bool* on) {
   if (h->vae_low_memory != 0) { *on = h->vae_low_memory > 0; return MGB_OK; }
   mgb_handle::DecodeRule& k = h->decode_rule;
   if (k.valid && k.lh == lh && k.lw == lw && k.attn_budget == h->vae_attn_budget && k.attn_rows == h->vae_attn_force_rows) {
-    *on = k.in_place;
+    *on = k.low_memory;
     return MGB_OK;
   }
   if (h->device_bytes == 0) {

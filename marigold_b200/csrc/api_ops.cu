@@ -102,25 +102,6 @@ int mgb_op_conv2d_ex(const void* x, const void* x2, const void* w, const float* 
   return run_gemm(p, block_n, splitk_ws, reinterpret_cast<cudaStream_t>(stream));
 }
 
-// The 3x3 pad-1 conv as the decoder's in-place resnet runs it: fp32 output at a row stride of ldo floats, and the 1x1
-// shortcut's operand x2 (or null) at a pixel stride of ld2 elements; the network's tile, no split-K.
-int mgb_debug_conv2d_strided(const void* x, const void* x2, int32_t ld2, const void* w, const float* bias, float* out_f32,
-                             int32_t ldo, int32_t NB, int32_t Hout, int32_t Wout, int32_t Cin, int32_t Cin2, int32_t Cout,
-                             void* stream) {
-  if (!x || !w || !out_f32 || (x2 && Cin2 <= 0) || ldo < Cout) { set_error("debug_conv2d_strided: bad argument"); return MGB_ERR_INVALID; }
-  if (!x2) Cin2 = 0;
-  int tw, th, bn, sp, st;
-  conv_tile_shape(Hout, Wout, &tw, &th);
-  const int m_tiles = NB * ((Wout + tw - 1) / tw) * ((Hout + th - 1) / th);
-  choose_tile(m_tiles, Cout, (9 * Cin + Cin2) / 64, 0, false, &bn, &sp, &st);
-  GemmParams p;
-  TRY(fill_conv_params(&p, reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(w), NB, Hout, Wout, Cin, Cout,
-                       0, bn, 1, st, 0, 0, reinterpret_cast<const bf16*>(x2), Cin2, ld2));
-  fill_epi(&p.epi, bias, nullptr, out_f32, nullptr, ldo, 0, 1.0f, nullptr, nullptr, nullptr, nullptr);
-  p.epi.hw = Hout * Wout;
-  return run_gemm(p, bn, nullptr, reinterpret_cast<cudaStream_t>(stream));
-}
-
 int mgb_op_conv2d(const void* x, const void* w, const float* bias, const float* residual, float* out_f32,
                   void* out_bf16, int32_t NB, int32_t Hout, int32_t Wout, int32_t Cin, int32_t Cout, int32_t kind,
                   int32_t flags, int32_t block_n, int32_t splits, int32_t stages, float* splitk_ws, void* stream) {
@@ -172,26 +153,6 @@ int mgb_op_groupnorm_ex(const float* xa, int32_t Ca, const float* xb, int32_t Cb
                          G, eps, silu, ws, counters, s);
 }
 
-// GroupNorm in two launches as the decoder's in-place resnet runs it (launch_gn_stats, launch_gn_apply_rows): x rows at
-// a stride of ldx floats, y bf16 [NB * HW, C], raw (or null) = bf16(x) at a row stride of ldr elements, in place when
-// raw == x. ws: mgb_op_groupnorm_ws_bytes(NB, HW, C, G); stats: NB * C float2.
-int mgb_debug_groupnorm_rows(const float* x, int32_t C, int64_t ldx, void* y, void* raw, int64_t ldr, const float* gamma,
-                             const float* beta, float* ws, void* stats, int32_t NB, int32_t HW, int32_t G, float eps,
-                             int32_t silu, void* stream) {
-  if (!x || !y || !ws || !stats || ldx > (1 << 20)) { set_error("debug_groupnorm_rows: bad argument"); return MGB_ERR_INVALID; }
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const size_t pb = (groupnorm_part_bytes(NB, HW, C, G) + 255) & ~size_t(255);
-  unsigned* counters = reinterpret_cast<unsigned*>(reinterpret_cast<char*>(ws) + pb);
-  if (cudaMemsetAsync(counters, 0, size_t(NB) * sizeof(unsigned), s) != cudaSuccess) {
-    set_error("debug_groupnorm_rows: counter memset failed");
-    return MGB_ERR_CUDA;
-  }
-  float2* st = reinterpret_cast<float2*>(stats);
-  TRY(launch_gn_stats(x, C, int(ldx), nullptr, 0, st, gamma, beta, NB, HW, G, eps, ws, counters, s));
-  return launch_gn_apply_rows(x, ldx, nullptr, 0, st, reinterpret_cast<bf16*>(y), reinterpret_cast<bf16*>(raw), ldr, NB,
-                              HW, C, silu, s);
-}
-
 // GroupNorm in two launches over the concat [a | b] of two packed fp32 maps of Ch channels each, in their own memory as
 // the decoder's low-memory resnet runs it: raw = bf16([a | b]) [NB * HW, 2 Ch] over a, y [NB * HW, 2 Ch] over b.
 // ws: mgb_op_groupnorm_ws_bytes(NB, HW, 2 Ch, G); stats: NB * 2 Ch float2.
@@ -206,9 +167,9 @@ int mgb_debug_groupnorm_halves(float* a, float* b, int32_t Ch, const float* gamm
     return MGB_ERR_CUDA;
   }
   float2* st = reinterpret_cast<float2*>(stats);
-  TRY(launch_gn_stats(a, Ch, Ch, b, Ch, st, gamma, beta, NB, HW, G, eps, ws, counters, s));
-  return launch_gn_apply_rows(a, Ch, b, Ch, st, reinterpret_cast<bf16*>(b), reinterpret_cast<bf16*>(a), 2 * Ch, NB, HW,
-                              2 * Ch, silu, s);
+  TRY(launch_gn_stats(a, Ch, b, Ch, st, gamma, beta, NB, HW, G, eps, ws, counters, s));
+  return launch_gn_apply_rows(a, b, Ch, st, reinterpret_cast<bf16*>(b), reinterpret_cast<bf16*>(a), NB, HW, 2 * Ch, silu,
+                              s);
 }
 
 // One band of the decoder's banded 3x3 pad-1 convs (net.cu, conv3x3_band): tile rows [ty0, ty0 + tiles) of one

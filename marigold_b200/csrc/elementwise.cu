@@ -101,22 +101,17 @@ int launch_upsample2x_rows(const bf16* x, bf16* y, int H, int W, int C, int r0, 
                     reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), W, C / 8, r0, n);
 }
 
-// A block's 256 threads cover 256 / Q rows of Q quads each; no division in the loop.
-__global__ void copy_rows_kernel(const float4* __restrict__ x, long long lqx, float4* __restrict__ y, long long M, int Q) {
+__global__ void copy_rows_kernel(const float4* __restrict__ x, float4* __restrict__ y, size_t n4) {
   pdl_launch_dependents();
   pdl_wait();
-  const int q = threadIdx.x % Q, rows = blockDim.x / Q;
-  for (long long m = (long long)blockIdx.x * rows + threadIdx.x / Q; m < M; m += (long long)gridDim.x * rows)
-    y[m * Q + q] = __ldg(x + m * lqx + q);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x)
+    y[i] = __ldg(x + i);
 }
-int launch_copy_rows(const float* x, long long ldx, float* y, long long M, int C, cudaStream_t stream) {
-  const int Q = C / 4;
-  if ((C & 3) || (ldx & 3) || ldx < C || Q > 256 || 256 % Q) {
-    set_error("copy_rows: C=%d ldx=%lld", C, ldx);
-    return MGB_ERR_INVALID;
-  }
-  return launch_pdl("copy rows", copy_rows_kernel, grid_for(size_t(M) * Q, 256), 256, 0, stream,
-                    reinterpret_cast<const float4*>(x), ldx / 4, reinterpret_cast<float4*>(y), M, Q);
+int launch_copy_rows(const float* x, float* y, long long M, int C, cudaStream_t stream) {
+  if (C & 3) { set_error("copy_rows: C = %d is not a multiple of 4", C); return MGB_ERR_INVALID; }
+  const size_t n4 = size_t(M) * (C / 4);
+  return launch_pdl("copy rows", copy_rows_kernel, grid_for(n4, 256), 256, 0, stream, reinterpret_cast<const float4*>(x),
+                    reinterpret_cast<float4*>(y), n4);
 }
 
 // UNet conv_in operand (reference marigold_depth_pipeline.py:456-458, marigold_iid_pipeline.py:538-540: rgb latent FIRST):

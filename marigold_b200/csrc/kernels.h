@@ -135,19 +135,18 @@ size_t groupnorm_part_bytes(int NB, int HW, int C, int G);
 int launch_gn_fused(const float* xa, int Ca, const float* xb, int Cb, bf16* y, bf16* raw_copy, const float* gamma,
                     const float* beta, int NB, int HW, int G, float eps, int silu, void* part, unsigned* counters,
                     cudaStream_t stream);
-// GroupNorm in two launches over rows at a stride (norm.cu): launch_gn_stats writes each image's per-channel
-// (scale, shift) float2 [NB][C] from launch_gn_fused's statistics; launch_gn_apply_rows applies them as launch_gn_fused
-// does, y bf16 [NB * HW, C] from x at a row stride of ldx floats, and raw = bf16(x) at a row stride of ldr elements
-// (raw == x: in place, the copy over the first half of each fp32 row, ldr = 2 ldx). C in {128, 256, 512}.
-// Two sources (xb != nullptr): the channel concat [x | xb] as launch_gn_fused reads it, x's Ca channels at a row
-// stride of ldx floats and xb's C - Ca packed; y may lie over xb (2 (C - Ca) = C) and raw over x (ldr = 2 ldx).
-int launch_gn_stats(const float* x, int Ca, int ldx, const float* xb, int Cb, float2* stats, const float* gamma,
+// GroupNorm in two launches (norm.cu): launch_gn_stats writes each image's per-channel (scale, shift) float2 [NB][C]
+// from launch_gn_fused's statistics; launch_gn_apply_rows applies them as launch_gn_fused does, y bf16 [NB * HW, C]
+// from x [NB * HW, C]. C in {128, 256, 512}.
+// Two sources (xb != nullptr): the channel concat [x | xb] as launch_gn_fused reads it; launch_gn_apply_rows takes two
+// halves of C / 2 channels and writes y over xb and raw = bf16([x | xb]) over x.
+int launch_gn_stats(const float* x, int Ca, const float* xb, int Cb, float2* stats, const float* gamma,
                     const float* beta, int NB, int HW, int G, float eps, void* part, unsigned* counters,
                     cudaStream_t stream);
-int launch_gn_apply_rows(const float* x, long long ldx, const float* xb, int Ca, const float2* stats, bf16* y, bf16* raw,
-                         long long ldr, int NB, int HW, int C, int silu, cudaStream_t stream);
-// y [M, C] = the first C floats of each row of x at a row stride of ldx floats (elementwise.cu)
-int launch_copy_rows(const float* x, long long ldx, float* y, long long M, int C, cudaStream_t stream);
+int launch_gn_apply_rows(const float* x, const float* xb, int Ca, const float2* stats, bf16* y, bf16* raw, int NB,
+                         int HW, int C, int silu, cudaStream_t stream);
+// y [M, C] = x [M, C] (elementwise.cu)
+int launch_copy_rows(const float* x, float* y, long long M, int C, cudaStream_t stream);
 // LayerNorm over the channel dim: x_f32 [M, C] -> y_bf16 [M, C]
 int launch_layernorm(const float* x, bf16* y, const float* gamma, const float* beta, int M, int C, float eps,
                      cudaStream_t stream);

@@ -243,10 +243,9 @@ static Tile conv_tile(int NB, int Hout, int Wout, const ConvW& W, int flags, int
   return t;
 }
 
-// 3x3 conv on NHWC bf16; Hout x Wout output; kind per ops.cu. ldo: the output's row stride (0: W.cout); ld2: x2's
-// pixel stride (0: its channel count). Neither changes the tile, the split or any output value.
+// 3x3 conv on NHWC bf16; Hout x Wout output; kind per ops.cu
 static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const ConvW& W, int kind, const Epi& e,
-                   int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr, int ldo = 0, int ld2 = 0) {
+                   int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr) {
   if ((x2 != nullptr) != (W.k_extra > 0)) { set_error("conv3x3: second operand / weight layout mismatch"); return MGB_ERR_STATE; }
   const Tile t = conv_tile(NB, Hout, Wout, W, e.flags);
   const int bn = t.bn, sp = t.sp, st = t.st;
@@ -254,11 +253,10 @@ static int conv3x3(Ctx& c, const bf16* x, int NB, int Hout, int Wout, const Conv
   if (sp > 1) c.splitk_need = std::max(c.splitk_need, size_t(sp) * M * W.cout * sizeof(float));
   if (c.dry) return MGB_OK;
   GemmParams p;
-  TRY(fill_conv_params(&p, x, W.w, NB, Hout, Wout, W.cin_pad, W.cout, kind, bn, sp, st, Hsrc, Wsrc, x2, W.k_extra,
-                       ld2));
+  TRY(fill_conv_params(&p, x, W.w, NB, Hout, Wout, W.cin_pad, W.cout, kind, bn, sp, st, Hsrc, Wsrc, x2, W.k_extra));
   Epi e2 = e;
   e2.hw = Hout * Wout;
-  return gemm_common(c, p, bn, effective_splits(p), e2, ldo > 0 ? ldo : W.cout);
+  return gemm_common(c, p, bn, effective_splits(p), e2, W.cout);
 }
 
 // Tile rows [ty0, ty0 + tiles) of one H x W image of a pad-1 3x3 conv run with tile t, the tile of the whole conv
@@ -367,9 +365,9 @@ static int resnet_forward(Ctx& c, const ResnetW& R, Act& x, Act* skip, Act& y, i
   return MGB_OK;
 }
 
-// GroupNorm statistics of [x | xb] (launch_gn_stats: x's Ca channels at a row stride of ldx floats, xb's Cb packed, or
-// x alone) into stats, with groupnorm()'s scratch and barrier counter
-static int groupnorm_stats(Ctx& c, const float* x, int Ca, int ldx, const float* xb, int Cb, float2* stats,
+// GroupNorm statistics of [x | xb] (launch_gn_stats; or x alone) into stats, with groupnorm()'s scratch and barrier
+// counter
+static int groupnorm_stats(Ctx& c, const float* x, int Ca, const float* xb, int Cb, float2* stats,
                            const NormW& n, int NB, int HW, float eps) {
   void* part = aalloc<char>(c, groupnorm_part_bytes(NB, HW, Ca + Cb, c.groups));
   const size_t coff = c.sync_off;
@@ -378,7 +376,7 @@ static int groupnorm_stats(Ctx& c, const float* x, int Ca, int ldx, const float*
   int rc = MGB_OK;
   if (!c.dry) {
     if (c.sync_off > c.sync_cap) { set_error("groupnorm: barrier counter slab exhausted"); return MGB_ERR_STATE; }
-    rc = launch_gn_stats(x, Ca, ldx, xb, Cb, stats, n.g, n.b, NB, HW, c.groups, eps, part, c.sync_base + coff, c.stream);
+    rc = launch_gn_stats(x, Ca, xb, Cb, stats, n.g, n.b, NB, HW, c.groups, eps, part, c.sync_base + coff, c.stream);
   }
   c.arena->free(part);
   return rc;
@@ -450,10 +448,10 @@ static int resnet_shortcut_halves(Ctx& c, const ResnetW& R, Act& a, Act& b, Act&
   const int HW = H * W, cin = R.cin, cout = R.cout;
   const size_t M = size_t(NB) * HW;
   float2* st = aalloc<float2>(c, size_t(NB) * cin);
-  TRY(groupnorm_stats(c, a.p, cout, cout, b.p, cout, st, R.n1, NB, HW, R.eps));
+  TRY(groupnorm_stats(c, a.p, cout, b.p, cout, st, R.n1, NB, HW, R.eps));
   bf16* raw = reinterpret_cast<bf16*>(a.p);
   bf16* t1 = reinterpret_cast<bf16*>(b.p);
-  LAUNCH(launch_gn_apply_rows(a.p, cout, b.p, cout, st, t1, raw, 2 * cout, NB, HW, cin, 1, c.stream));
+  LAUNCH(launch_gn_apply_rows(a.p, b.p, cout, st, t1, raw, NB, HW, cin, 1, c.stream));
   c.arena->free(st);
   int th, tiles_y;
   const Tile t = conv_tile(NB, H, W, R.c1, 0, &th, &tiles_y);
@@ -473,8 +471,8 @@ static int resnet_shortcut_halves(Ctx& c, const ResnetW& R, Act& a, Act& b, Act&
       }
       if (prev >= 0) {
         const int r0 = prev * th, r1 = std::min(H, (prev + bt) * th);
-        LAUNCH(launch_copy_rows(stage[(prev / bt) & 1], cout, hn + size_t(r0) * W * cout, (long long)(r1 - r0) * W,
-                                cout, c.stream));
+        LAUNCH(launch_copy_rows(stage[(prev / bt) & 1], hn + size_t(r0) * W * cout, (long long)(r1 - r0) * W, cout,
+                                c.stream));
       }
       if (ty0 >= tiles_y) break;
       prev = ty0;
@@ -483,9 +481,9 @@ static int resnet_shortcut_halves(Ctx& c, const ResnetW& R, Act& a, Act& b, Act&
   c.arena->free(stage[1]);
   c.arena->free(stage[0]);
   st = aalloc<float2>(c, size_t(NB) * cout);
-  TRY(groupnorm_stats(c, b.p, cout, cout, nullptr, 0, st, R.n2, NB, HW, R.eps));
+  TRY(groupnorm_stats(c, b.p, cout, nullptr, 0, st, R.n2, NB, HW, R.eps));
   bf16* t2 = aalloc<bf16>(c, M * cout);
-  LAUNCH(launch_gn_apply_rows(b.p, cout, nullptr, 0, st, t2, nullptr, 0, NB, HW, cout, 1, c.stream));
+  LAUNCH(launch_gn_apply_rows(b.p, nullptr, 0, st, t2, nullptr, NB, HW, cout, 1, c.stream));
   c.arena->free(st);
   Epi e2; e2.bias = R.c2.b; e2.out_f32 = b.p;
   TRY(conv3x3(c, t2, NB, H, W, R.c2, 0, e2, 0, 0, raw));

@@ -219,7 +219,7 @@ struct mgb_handle {
     int lh = 0, lw = 0;
     size_t attn_budget = 0;
     int attn_rows = 0;
-    bool in_place = false;
+    bool low_memory = false;
   } decode_rule;
   // Tile rows per band of the low-memory decoder's banded up-conv and conv1 (Ctx::band_up_tiles): 0 the library's
   // choice, else forced (mgb_debug_vae_bands)

@@ -30,16 +30,15 @@ static __device__ __noinline__ void gn_barrier_timeout(unsigned seen, unsigned w
   __trap();
 }
 
-// kStats: statistics only. Source a is read at a row stride of lda floats, and instead of the normalised
-// operand the kernel writes each channel's (scale, shift) = (rstd gamma, beta - mean rstd gamma) to stats [NB][Ca],
-// from the same registers phase 2 applies them from: gn_apply_rows applies them bit for bit as this kernel would.
+// kStats: statistics only. Instead of the normalised operand the kernel writes each channel's
+// (scale, shift) = (rstd gamma, beta - mean rstd gamma) to stats [NB][Ca], from the same registers phase 2 applies
+// them from: gn_apply_rows applies them bit for bit as this kernel would.
 template <int KQ, bool kStats = false>
 __global__ void __launch_bounds__(kGnThreads, kGnCtasPerSm)
     gn_fused_kernel(const float* __restrict__ xa, int Ca, const float* __restrict__ xb, int Cb, bf16* __restrict__ y,
                     bf16* __restrict__ raw, const float* __restrict__ gamma, const float* __restrict__ beta, int HW, int G,
                     float eps, int silu, GnGeom g, float2* __restrict__ part /* [NB][chunks][G] */,
-                    unsigned* __restrict__ counter /* [NB], zero on entry */, int lda = 0,
-                    float2* __restrict__ stats = nullptr) {
+                    unsigned* __restrict__ counter /* [NB], zero on entry */, float2* __restrict__ stats = nullptr) {
   constexpr int R = kGnLoads / KQ;
   extern __shared__ float2 s_ch[];   // phase 1: [Tp][C] per-channel (sum, sumsq); phase 2: mean[G] | rstd[G] as floats
   const int img = blockIdx.y, chunk = blockIdx.x, chunks = gridDim.x;
@@ -48,8 +47,7 @@ __global__ void __launch_bounds__(kGnThreads, kGnCtasPerSm)
   const bool active = tp < g.Tp;
   const int p0 = chunk * g.P, p1 = min(HW, p0 + g.P);
   const int Qa = Ca / 4, Qb = Cb / 4;
-  const int lqa = kStats ? lda / 4 : Qa;   // row stride of source a, in quads
-  const float4* xai = reinterpret_cast<const float4*>(xa + (size_t)img * HW * lqa * 4);
+  const float4* xai = reinterpret_cast<const float4*>(xa + (size_t)img * HW * Qa * 4);
   const float4* xbi = xb ? reinterpret_cast<const float4*>(xb + (size_t)img * HW * Cb) : nullptr;
   pdl_wait();
 
@@ -57,7 +55,7 @@ __global__ void __launch_bounds__(kGnThreads, kGnCtasPerSm)
   // quad qd of the concatenated channel space lives in source a (qd < Qa) or b
   auto px = [&](int k, int p) -> const float4* {
     const int qd = tq + k * g.Tq;
-    return qd < Qa ? xai + (size_t)p * lqa + qd : xbi + (size_t)p * Qb + (qd - Qa);
+    return qd < Qa ? xai + (size_t)p * Qa + qd : xbi + (size_t)p * Qb + (qd - Qa);
   };
   float4 v[KQ][R];
   float sum[KQ][4], sq[KQ][4];
@@ -291,20 +289,20 @@ int launch_gn_fused(const float* xa, int Ca, const float* xb, int Cb, bf16* y, b
   float2* pp = static_cast<float2*>(part);
   auto kern = g.Kq == 1 ? gn_fused_kernel<1> : g.Kq == 2 ? gn_fused_kernel<2> : gn_fused_kernel<4>;
   return launch_pdl("groupnorm", kern, grid, kGnThreads, smem, stream, xa, Ca, xb, Cb, y, raw_copy, gamma, beta, HW, G, eps,
-                    silu, g, pp, counters, 0, nullptr);
+                    silu, g, pp, counters, nullptr);
 }
 
-// GroupNorm statistics of x [NB, HW, Ca] at a row stride of ldx floats (>= Ca), concatenated with xb [NB, HW, Cb]
-// packed when xb is set: per image and channel the (scale, shift) that launch_gn_fused applies to [x | xb], to stats
-// [NB][Ca + Cb]. part and counters as launch_gn_fused's.
-int launch_gn_stats(const float* x, int Ca, int ldx, const float* xb, int Cb, float2* stats, const float* gamma,
+// GroupNorm statistics of x [NB, HW, Ca], concatenated with xb [NB, HW, Cb] when xb is set: per image and channel the
+// (scale, shift) that launch_gn_fused applies to [x | xb], to stats [NB][Ca + Cb]. part and counters as
+// launch_gn_fused's.
+int launch_gn_stats(const float* x, int Ca, const float* xb, int Cb, float2* stats, const float* gamma,
                     const float* beta, int NB, int HW, int G, float eps, void* part, unsigned* counters,
                     cudaStream_t stream) {
   GnGeom g;
   if (!xb) Cb = 0;
   const int C = Ca + Cb;
-  if ((Ca & 3) || (Cb & 3) || (ldx & 3) || ldx < Ca || !stats || !gn_plan(NB, HW, C, G, &g)) {
-    set_error("groupnorm stats: unsupported NB=%d C=%d+%d ldx=%d G=%d", NB, Ca, Cb, ldx, G);
+  if ((Ca & 3) || (Cb & 3) || !stats || !gn_plan(NB, HW, C, G, &g)) {
+    set_error("groupnorm stats: unsupported NB=%d C=%d+%d G=%d", NB, Ca, Cb, G);
     return MGB_ERR_INVALID;
   }
   dim3 grid(g.chunks, NB);
@@ -313,28 +311,27 @@ int launch_gn_stats(const float* x, int Ca, int ldx, const float* xb, int Cb, fl
   float2* pp = static_cast<float2*>(part);
   auto kern = g.Kq == 1 ? gn_fused_kernel<1, true> : g.Kq == 2 ? gn_fused_kernel<2, true> : gn_fused_kernel<4, true>;
   return launch_pdl("groupnorm stats", kern, grid, kGnThreads, smem, stream, x, Ca, xb, Cb, nullptr, nullptr, gamma,
-                    beta, HW, G, eps, 0, g, pp, counters, ldx, stats);
+                    beta, HW, G, eps, 0, g, pp, counters, stats);
 }
 
 // The apply phase of GroupNorm over rows given their statistics (launch_gn_stats): one warp per pixel row of
-// C = 128 NQ channels. y [M, C] = bf16(act(x * scale + shift)) with the GroupNorm kernel's operations in its order, and,
-// when raw is set, raw = bf16(x) at a row stride of ldr elements. With xb the row is the concat [x | xb], the first
-// 128 QA channels from x and the rest from xb packed. raw may lie over x and y over xb: a row's outputs are written only
-// over bytes of that same row (ldr = 2 ldx, the copy in the first half of the fp32 row; y's 2 C bytes over xb's row of
-// C / 2 floats), and only after the whole warp has read the row (__syncwarp orders the warp's loads before its stores);
-// no other warp touches the row. Hence plain loads here, not the read-only path.
+// C = 128 NQ channels: y [M, C] = bf16(act(x * scale + shift)) with the GroupNorm kernel's operations in its order.
+// With xb the row is the concat [x | xb] of two halves of 128 QA channels, raw [M, C] = bf16([x | xb]) is written over
+// x and y over xb: a row's outputs are written only over bytes of that same row (2 C bytes each, over x's and xb's rows
+// of C / 2 floats), and only after the whole warp has read the row (__syncwarp orders the warp's loads before its
+// stores); no other warp touches the row. Hence plain loads here, not the read-only path.
 template <int NQ>
-__global__ void __launch_bounds__(256) gn_apply_rows_kernel(const float* x, long long ldx, const float* xb, int QA,
-                                                            const float2* __restrict__ stats, bf16* y, bf16* raw,
-                                                            long long ldr, int HW, int C, int silu, long long M) {
+__global__ void __launch_bounds__(256) gn_apply_rows_kernel(const float* x, const float* xb, int QA,
+                                                            const float2* __restrict__ stats, bf16* y, bf16* raw, int HW,
+                                                            int C, int silu, long long M) {
   pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31;
   const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
-  const int Cb = C - 128 * QA;
+  const int Ca = 128 * QA, Cb = C - Ca;
   for (long long m = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); m < M; m += warps) {
     const float2* st = stats + (m / HW) * C;
-    const float4* xr = reinterpret_cast<const float4*>(x + m * ldx);
+    const float4* xr = reinterpret_cast<const float4*>(x + m * Ca);
     const float4* xbr = xb ? reinterpret_cast<const float4*>(xb + m * Cb) : nullptr;
     float4 t[NQ];
 #pragma unroll
@@ -351,7 +348,8 @@ __global__ void __launch_bounds__(256) gn_apply_rows_kernel(const float* x, long
     }
     if (raw) {
       __syncwarp();
-      uint2* ro = reinterpret_cast<uint2*>(raw + m * ldr);
+      // over x's row (2 Ca = C); written as y's offset m * C it takes up to 6 more registers
+      uint2* ro = reinterpret_cast<uint2*>(raw + m * (2 * Ca));
 #pragma unroll
       for (int i = 0; i < NQ; ++i)
         ro[lane + 32 * i] = make_uint2(pack_bf16x2(t[i].x, t[i].y), pack_bf16x2(t[i].z, t[i].w));
@@ -360,22 +358,21 @@ __global__ void __launch_bounds__(256) gn_apply_rows_kernel(const float* x, long
   }
 }
 
-int launch_gn_apply_rows(const float* x, long long ldx, const float* xb, int Ca, const float2* stats, bf16* y, bf16* raw,
-                         long long ldr, int NB, int HW, int C, int silu, cudaStream_t stream) {
+int launch_gn_apply_rows(const float* x, const float* xb, int Ca, const float2* stats, bf16* y, bf16* raw, int NB,
+                         int HW, int C, int silu, cudaStream_t stream) {
   if (!xb) Ca = C;
-  const bool in_place = raw && reinterpret_cast<const void*>(raw) == reinterpret_cast<const void*>(x);
-  const bool y_over_b = xb && reinterpret_cast<const void*>(y) == reinterpret_cast<const void*>(xb);
-  if ((C != 128 && C != 256 && C != 512) || ldx < Ca || (ldx & 3) || (raw && (ldr < C || (ldr & 3))) ||
-      (raw && !in_place && ldr != C) || (in_place && ldr != 2 * ldx) || Ca <= 0 || Ca % 128 || Ca > C ||
-      (xb && Ca == C) || (y_over_b && 2 * (C - Ca) != C)) {
-    set_error("groupnorm apply rows: unsupported C=%d Ca=%d ldx=%lld ldr=%lld", C, Ca, ldx, ldr);
+  // x alone, or the halves: raw over x and y over xb
+  const bool halves = xb && reinterpret_cast<const void*>(raw) == reinterpret_cast<const void*>(x) &&
+                      reinterpret_cast<const void*>(y) == reinterpret_cast<const void*>(xb) && 2 * Ca == C;
+  if ((C != 128 && C != 256 && C != 512) || Ca % 128 || (xb ? !halves : raw != nullptr)) {
+    set_error("groupnorm apply rows: unsupported C=%d Ca=%d", C, Ca);
     return MGB_ERR_INVALID;
   }
   const long long M = (long long)NB * HW;
   const int blocks = int(std::min<long long>((M + 7) / 8, 64LL * kNumSMs));
   auto kern = C == 128 ? gn_apply_rows_kernel<1> : C == 256 ? gn_apply_rows_kernel<2> : gn_apply_rows_kernel<4>;
-  return launch_pdl("groupnorm apply rows", kern, blocks, 256, 0, stream, x, ldx, xb, Ca / 128, stats, y, raw, ldr, HW,
-                    C, silu, M);
+  return launch_pdl("groupnorm apply rows", kern, blocks, 256, 0, stream, x, xb, Ca / 128, stats, y, raw, HW, C, silu,
+                    M);
 }
 
 // Stand-alone GroupNorm (operator-level ABI): ws = groupnorm_ws_bytes() of scratch (counters zeroed here).

@@ -50,8 +50,7 @@ int fill_linear_params(GemmParams* p, const bf16* a, const bf16* w, int M, int N
 }
 
 int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Hout, int Wout, int Cin, int Cout,
-                     int kind, int block_n, int splits, int stages, int Hsrc, int Wsrc, const bf16* x2, int Cin2,
-                     int ld2) {
+                     int kind, int block_n, int splits, int stages, int Hsrc, int Wsrc, const bf16* x2, int Cin2) {
   // x2 (optional): bf16 NHWC [NB, Hout, Wout, Cin2], the operand of a 1x1 convolution over the same output pixels whose
   // weight columns follow the taps in w ([Cout, ntaps * Cin + Cin2]): K concatenation (stride-1 kinds only)
   // Hsrc x Wsrc: spatial extent of the tensor the taps address (the image for stride 1; one parity plane for
@@ -126,10 +125,6 @@ int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Ho
     set_error("conv2d: second operand needs Cin2 %% 64 == 0 and a stride-1 kind (got %d, kind %d)", Cin2, kind);
     return MGB_ERR_INVALID;
   }
-  if (x2 != nullptr && ld2 != 0 && (ld2 < Cin2 || ld2 % 8 != 0)) {
-    set_error("conv2d: second operand's pixel stride %d must be a multiple of 8 of at least Cin2 = %d", ld2, Cin2);
-    return MGB_ERR_INVALID;
-  }
   p->num_kb = p->num_kb1 + (x2 ? Cin2 / 64 : 0);
   if (splits < 1) splits = 1;
   splits = std::min(splits, p->num_kb);
@@ -143,7 +138,7 @@ int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Ho
   int rc = make_tmap_5d(&p->tmap_a, x, dims, strides, box);
   if (rc) return rc;
   if (x2) {
-    const uint64_t C22 = uint64_t(ld2 ? ld2 : Cin2) * 2;
+    const uint64_t C22 = uint64_t(Cin2) * 2;
     const uint64_t dims2[5] = {uint64_t(Cin2), uint64_t(Wout), uint64_t(Hout), 1, uint64_t(NB)};
     const uint64_t strides2[4] = {C22, C22 * Wout, C22 * Wout * Hout, C22 * Wout * Hout};
     const uint32_t box2[5] = {64, uint32_t(p->tile_w), uint32_t(p->tile_h), 1, 1};

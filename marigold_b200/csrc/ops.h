@@ -11,10 +11,10 @@ void conv_tile_shape(int Hout, int Wout, int* tile_w, int* tile_h);
 int fill_linear_params(GemmParams* p, const bf16* a, const bf16* w, int M, int N, int K, int block_n, int splits,
                        int stages, const bf16* a2 = nullptr, int K2 = 0);
 // x NHWC bf16 ([NB, Hout, Wout, Cin] for kind 0/1, [NB, 4, Hout, Wout, Cin] parity planes for kind 2/3);
-// w [Cout, taps * Cin] bf16 tap-major. ld2: x2's pixel stride in elements (0: Cin2).
+// w [Cout, taps * Cin] bf16 tap-major.
 int fill_conv_params(GemmParams* p, const bf16* x, const bf16* w, int NB, int Hout, int Wout, int Cin, int Cout,
                      int kind, int block_n, int splits, int stages, int Hsrc = 0, int Wsrc = 0, const bf16* x2 = nullptr,
-                     int Cin2 = 0, int ld2 = 0);
+                     int Cin2 = 0);
 int effective_splits(const GemmParams& p);
 // Makes a filled conv (one image, no split-K, no second operand) run tile rows [ty0, ty0 + tiles) of its image with
 // tmap_a's row 0 at image row src_y0 and the output's row 0 at image row out_y0 (GemmParams::ty0).

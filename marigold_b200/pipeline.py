@@ -152,7 +152,8 @@ def call_reserve_bytes(h: int, w: int, ensemble_size: int, channels: int) -> int
     """Device memory a pipeline call holds beside the engine's workspace at h x w: the decoded members and their
     concatenation (ensemble_size fp32 maps of `channels` each), the ensembled prediction and its uncertainty, and the
     normalised fp32 input. At 24 MP it is 2.4 GB for depth and 6.7 GB for normals with 10 members. The engine's choice of
-    the in-place decoder stage counts the smallest of these, one depth member's 28 bytes per pixel (csrc/api_net.cu)."""
+    the low-memory decoder stage counts the smallest of these, one depth member's 28 bytes per pixel
+    (csrc/api_net.cu)."""
     return 4 * h * w * (channels * (2 * ensemble_size + 2) + 3)
 
 

@@ -1,20 +1,16 @@
-"""45-48-megapixel photos (`-m gpu`): the decoder's first full-resolution resnet in place (net.cu,
-resnet_shortcut_in_place), which takes the decoder's planned peak from 4 U to 3 U (U = one fp32 128-channel map at full
-resolution, 512 bytes per pixel; 25.0 GB at 8064 x 6048).
+"""45-48-megapixel photos (`-m gpu`): the library's rule runs the decoder's full-resolution stage in low memory
+(net.cu, up_conv_low_memory and resnet_shortcut_halves) where one member's default decode does not fit (U = one fp32
+128-channel map at full resolution, 512 bytes per pixel; 25.0 GB at 8064 x 6048).
 
-  * the plans: at 8064 x 6048 the decoder's peak is 3 U (plus the GroupNorm scratch), no two buffers live at once share
-    a byte, and the plan is its own lifetimes' placement on every call; at 6048 x 4032 and 768 x 768 the library's
-    rule keeps the default path, so plans and workspace bytes are those of a handle that never runs in place;
-  * the same bits: decodes forced in place equal the default path's for the depth, normals and raw-3 modes, one and two
-    members, at 1920 x 1080 and 1000 x 744, also with a poisoned arena and the reversed placement; the two-launch
-    GroupNorm over strided rows (in place for the shortcut's copy) equals the fused GroupNorm's operand and copy;
-  * float64 at the new scale: that GroupNorm over [48.8M, 256] in place and over the [48.8M, 128] second halves of its
-    rows, on rows that include the first and last ones and those holding elements 2^30 .. 2^33;
+  * the plans: at 8064 x 6048 the decoder's peak is 2.5 U (plus the GroupNorm scratch), no two buffers live at once
+    share a byte, the plan is its own lifetimes' placement on every call, and the library's rule gives the forced plan;
+    at 6048 x 4032 and 768 x 768 the rule keeps the default path, so plans and workspace bytes are those of a handle
+    that never runs in low memory;
   * the pipelines at processing_res=0 on an 8064 x 6048 photo: depth with E = 1 and with E = 2 and uncertainty, normals
     with E = 1, a 2-target IID model with E = 1; select_batch_size takes one member at 7728 x 5152 (just past the
     default path's limit), 8192 x 5464 and 8256 x 5504;
-  * the two convs of the in-place resnet in its layout at 8064 x 6048 (strided output over a [48.8M, 256] buffer, the
-    shortcut's operand at a 1024-byte pixel stride) against float64 on rows holding elements 2^30 .. 2^33."""
+  * the two convs of that stage's resnet at 8064 x 6048 on packed operands (conv1; conv2 with the shortcut's
+    [48.8M, 256] bf16 operand) against float64 on rows holding elements 2^30 .. 2^33."""
 import ctypes as C
 import gc
 
@@ -24,41 +20,21 @@ import torch
 
 from tests import ops_ref as R
 from tests.helpers import engine_from_oracle, oracle_models, record
-from tests.test_native_res_24mp_gpu import (U_PER_PIXEL, _hook, _photo, _weight_bytes, arena_place, arena_plan,
-                                            group_stats64, groupnorm_rows_ref, no_overlap, set_arena)
+from tests.test_native_res_24mp_gpu import U_PER_PIXEL, _hook, _photo, _weight_bytes, arena_place, arena_plan, no_overlap
 
 pytestmark = pytest.mark.gpu
 
 H48, W48 = 6048, 8064
 P48 = H48 * W48            # 48 771 072 pixels
-SCRATCH = 1 << 20          # bytes of GroupNorm partials and statistics live beside the 3 U at the decoder's peak
+SCRATCH = 1 << 20          # bytes of GroupNorm partials and statistics live beside the 2.5 U at the decoder's peak
 
 
 def set_low_memory(eng, mode):
-    """1: the decoder's first full-resolution resnet in place at every size; -1: never; 0: the library's rule."""
+    """1: the decoder's full-resolution stage in low memory at every size; -1: never; 0: the library's rule."""
     from marigold_b200._lib import check
 
     f = _hook("mgb_debug_vae_low_memory", C.c_int32, [C.c_void_p, C.c_int32])
     check(f(eng._h, mode), "mgb_debug_vae_low_memory")
-
-
-def groupnorm_rows(x, C_, ldx, raw, ldr, gamma, beta, NB, HW, G, eps, silu):
-    """The two-launch GroupNorm (mgb_debug_groupnorm_rows) over rows of C_ channels at a stride of ldx floats of x."""
-    from marigold_b200 import _lib
-    from marigold_b200.ops import ptr, stream_ptr
-
-    lib = _lib.load()
-    x_p = C.c_void_p(x.data_ptr())                          # rows at a stride: x may be a column slice
-    raw_p = None if raw is None else C.c_void_p(raw.data_ptr())
-    f = _hook("mgb_debug_groupnorm_rows", C.c_int32,
-              [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-               C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_void_p])
-    y = torch.empty(NB * HW, C_, dtype=torch.bfloat16, device="cuda")
-    ws = torch.empty((int(lib.mgb_op_groupnorm_ws_bytes(NB, HW, C_, G)) + 3) // 4, device="cuda")
-    stats = torch.empty(NB * C_ * 2, device="cuda")
-    _lib.check(f(x_p, C_, ldx, ptr(y), raw_p, ldr, ptr(gamma), ptr(beta), ptr(ws), ptr(stats), NB, HW, G,
-                 float(eps), int(silu), stream_ptr()), "mgb_debug_groupnorm_rows")
-    return y
 
 
 def _rows(n_rows, width, seed, n_random=64):
@@ -110,111 +86,41 @@ def test_iid_at_48mp():
     eng.close()
 
 
-# ---- the two-launch GroupNorm ------------------------------------------------------------------------------------
-# Before the module's engine: the largest runs here need the card before it holds a workspace.
-def test_groupnorm_rows_past_2_33_elements():
-    """[48.8M, 256] with a mean of 100: the strided [48.8M, 128] second halves first, then the whole rows with the
-    shortcut's copy written over them, as the decoder runs them."""
-    G, eps = 32, 1e-6
-    g = torch.Generator(device="cuda").manual_seed(48)
-    x = torch.randn(P48, 256, device="cuda", generator=g).mul_(2).add_(100.0)
-    gamma, beta = torch.randn(256, device="cuda", generator=g), torch.randn(256, device="cuda", generator=g)
-    assert x.numel() > 2 ** 33
-    rows = _rows(P48, 256, seed=48).cuda()
-    # second halves: [48.8M, 128] at a row stride of 256 floats
-    mean, rstd = group_stats64(x[:, 128:], G, eps, chunk=1 << 18)
-    y = groupnorm_rows(x[:, 128:], 128, 256, None, 0, gamma[128:], beta[128:], 1, P48, G, eps, 1)
-    torch.cuda.synchronize()
-    ref, bound = groupnorm_rows_ref(x[rows, 128:], mean, rstd, gamma[128:], beta[128:], G)
-    R.assert_within(y[rows], ref, bound, "native_res_48mp/groupnorm_rows_c128_ld256/worst")
-    del y
-    # whole rows, in place
-    mean, rstd = group_stats64(x, G, eps, chunk=1 << 18)
-    xr = x[rows].clone()
-    y = groupnorm_rows(x, 256, 256, x, 512, gamma, beta, 1, P48, G, eps, 1)
-    torch.cuda.synchronize()
-    ref, bound = groupnorm_rows_ref(xr, mean, rstd, gamma, beta, G)
-    R.assert_within(y[rows], ref, bound, "native_res_48mp/groupnorm_rows_c256_in_place/worst")
-    raw = x.view(torch.bfloat16).view(P48, 512)[:, :256]
-    assert torch.equal(raw[rows], xr.to(torch.bfloat16))
-
-
-def conv_strided(x, x2, ld2, wp, bias, out_ptr, ldo, H, W, Cin, Cin2, Cout):
-    """The conv of the in-place resnet (mgb_debug_conv2d_strided): fp32 output at out_ptr with a row stride of ldo
-    floats, shortcut operand x2 (or None) at a pixel stride of ld2 elements."""
-    from marigold_b200 import _lib
-    from marigold_b200.ops import ptr, stream_ptr
-
-    f = _hook("mgb_debug_conv2d_strided", C.c_int32,
-              [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 7 + [C.c_void_p])
-    x2_p = None if x2 is None else C.c_void_p(x2.data_ptr())
-    _lib.check(f(ptr(x), x2_p, ld2, ptr(wp), ptr(bias), C.c_void_p(out_ptr), ldo, 1, H, W, Cin, Cin2, Cout,
-                 stream_ptr()), "mgb_debug_conv2d_strided")
-
-
+# Before the module's engine: conv2's operands and output take 62 GB of the card.
 @pytest.mark.parametrize("stage", ["conv1", "conv2_shortcut"])
-def test_in_place_convs_past_2_33_elements(stage):
-    """The two convs of the in-place resnet at 8064 x 6048 in its layout, over one [48.8M, 256] fp32 buffer: conv1
-    (256 -> 128) into the second half of each row; conv2 (128 + 256 -> 128) reading the shortcut's bf16 operand from the
-    first half of each row (1024-byte pixel stride) and writing the second half. Image rows holding elements 2^30 ..
-    2^33 of the buffer, as fp32 and as bf16, and the first and last rows, against float64 with tests/ops_ref.py's conv
-    bound."""
+def test_resnet_convs_past_2_33_elements(stage):
+    """The two convs of resnet_shortcut_halves at 8064 x 6048 on packed operands: conv1 (256 -> 128), and conv2
+    (128 + 256 -> 128) reading the shortcut's [48.8M, 256] bf16 operand. Image rows holding elements 2^30 .. 2^33 of
+    each operand and of the output, and the first and last rows, against float64 with tests/ops_ref.py's conv bound."""
     from marigold_b200 import ops
     from tests.test_native_res_24mp_gpu import conv_row_ref
 
     Cin, Cin2, Cout = (256, 0, 128) if stage == "conv1" else (128, 256, 128)
     K = 9 * Cin + Cin2
     g = torch.Generator(device="cuda").manual_seed(K)
-    buf = torch.empty(P48, 256, device="cuda")
-    raw = None
-    if Cin2:
-        raw = buf.view(torch.bfloat16).view(1, H48, W48, 512)[..., :256]
-        rv = raw.view(P48, 256)
-        for a in range(0, P48, 1 << 22):
-            rv[a:a + (1 << 22)] = torch.randn(min(1 << 22, P48 - a), 256, device="cuda", generator=g,
-                                              dtype=torch.bfloat16)
     x = torch.randn(1, H48, W48, Cin, device="cuda", generator=g, dtype=torch.bfloat16)
+    x2 = torch.randn(1, H48, W48, Cin2, device="cuda", generator=g, dtype=torch.bfloat16) if Cin2 else None
     wb = (torch.randn(Cout, Cin, 3, 3, device="cuda", generator=g) / K ** 0.5).to(torch.bfloat16)
     wsc = (torch.randn(Cout, Cin2, device="cuda", generator=g) / K ** 0.5).to(torch.bfloat16) if Cin2 else None
     b = torch.randn(Cout, device="cuda", generator=g)
     wp = ops.pack_conv_weight(wb)
     if Cin2:
         wp = torch.cat([wp, wsc], dim=1).contiguous()
-    conv_strided(x, raw, 512, wp, b, buf.data_ptr() + 128 * 4, 256, H48, W48, Cin, Cin2, Cout)
+    out = torch.empty(1, H48, W48, Cout, device="cuda")
+    ops.conv2d_ex(x, wp, b, 1, H48, W48, Cin, Cout, x2=x2, Cin2=Cin2, out=out)
     torch.cuda.synchronize()
-    out = buf.view(1, H48, W48, 256)[..., 128:]
     rows = set()
-    for width in (W48 * 256, W48 * 512):
-        rows |= set(_rows(H48, width, seed=K, n_random=0).tolist())
+    for c in (Cin, Cin2, Cout):
+        if c:
+            rows |= set(_rows(H48, W48 * c, seed=K, n_random=0).tolist())
     rows |= set(torch.randint(0, H48, (4,), generator=torch.Generator().manual_seed(K)).tolist())
     worst = 0.0
     for y in sorted(rows):
-        ref, bound = conv_row_ref(x, wb, y, b, raw, wsc)
+        ref, bound = conv_row_ref(x, wb, y, b, x2, wsc)
         r = R.within(out[0, y], ref, bound)
         assert not r["nan"] and r["worst"] <= 1.0, (y, r)
         worst = max(worst, r["worst"])
-    record(f"native_res_48mp/in_place_{stage}/worst", worst)
-
-
-@pytest.mark.parametrize("NB,HW", [(1, 1920 * 1080), (2, 1000 * 744), (1, 4099)])
-def test_groupnorm_rows_equal_fused(NB, HW):
-    """Bit for bit the fused GroupNorm's operand and raw copy (mgb_op_groupnorm_ex): in place over 256 channels, and
-    over 128 channels at a row stride of 256."""
-    from marigold_b200 import ops
-
-    G, eps = 32, 1e-6
-    g = torch.Generator(device="cuda").manual_seed(NB * HW)
-    x = torch.randn(NB * HW, 256, device="cuda", generator=g).mul_(3).add_(1.0)
-    gamma, beta = torch.randn(256, device="cuda", generator=g), torch.randn(256, device="cuda", generator=g)
-    half = x[:, 128:].contiguous()
-    y_ref, _ = ops.groupnorm_ex(half.view(NB, HW, 128), None, gamma[128:], beta[128:], NB, HW, G, eps, 1)
-    y = groupnorm_rows(x[:, 128:], 128, 256, None, 0, gamma[128:], beta[128:], NB, HW, G, eps, 1)
-    assert torch.equal(y, y_ref.view(NB * HW, 128))
-    y_ref, raw_ref = ops.groupnorm_ex(x.view(NB, HW, 256), None, gamma, beta, NB, HW, G, eps, 1, raw_copy=True)
-    y = groupnorm_rows(x, 256, 256, x, 512, gamma, beta, NB, HW, G, eps, 1)
-    torch.cuda.synchronize()
-    assert torch.equal(y, y_ref.view(NB * HW, 256))
-    assert torch.equal(x.view(torch.bfloat16).view(NB * HW, 512)[:, :256], raw_ref.view(NB * HW, 256))
+    record(f"native_res_48mp/resnet_{stage}/worst", worst)
 
 
 @pytest.fixture(scope="module")
@@ -240,10 +146,10 @@ def test_48mp_plan(engine):
     assert no_overlap(nbytes, t0, t1, off)
     peak = int((off + nbytes).max())
     record("native_res_48mp/plan_peak_over_U/decode", peak / U)
-    assert peak <= 3 * U + SCRATCH, peak / U
+    assert peak <= 2.5 * U + SCRATCH, peak / U
     assert arena_place(nbytes, t0, t1)[1].tolist() == off.tolist()
     assert arena_plan(engine, 2, 1, lh, lw)[3].tolist() == off.tolist()
-    # the library's rule chose the in-place resnet: the plan is the forced one
+    # the library's rule chose the low-memory stage: the plan is the forced one
     set_low_memory(engine, 1)
     try:
         assert [a.tolist() for a in arena_plan(engine, 2, 1, lh, lw)] == [a.tolist() for a in (nbytes, t0, t1, off)]
@@ -269,43 +175,6 @@ def test_plans_unchanged_where_the_default_fits(engine, NB, h, w):
     set_low_memory(engine, 0)
     assert plans[0] == plans[-1]
     assert need[0] == need[-1] > 0
-
-
-# ---- the same bits -----------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("NB", [1, 2])
-@pytest.mark.parametrize("h,w", [(1080, 1920), (744, 1000)])
-def test_in_place_decode_is_bit_identical(engine, NB, h, w):
-    lh, lw = h // 8, w // 8
-    lat = torch.randn(NB, 4, lh, lw, generator=torch.Generator().manual_seed(NB * h + w)).cuda()
-    try:
-        for mode in (0, 1, 2):            # depth, normals, raw 3-channel
-            set_low_memory(engine, -1)
-            ref = engine.decode(lat, mode)
-            set_low_memory(engine, 1)
-            out = engine.decode(lat, mode)
-            assert torch.isfinite(ref).all()
-            assert (out - ref).abs().max().item() == 0.0, mode
-            if mode == 2:
-                for poison, placement in ((True, 0), (True, 1)):
-                    set_arena(engine, poison, placement)
-                    assert torch.equal(engine.decode(lat, mode), ref), (poison, placement)
-                set_arena(engine)
-    finally:
-        set_arena(engine)
-        set_low_memory(engine, 0)
-    record(f"native_res_48mp/in_place_vs_default/{w}x{h}_nb{NB}/max_abs_diff", 0.0)
-
-
-def test_in_place_plan_at_24mp(engine):
-    """Forced at 6048 x 4032 the in-place plan is 3 U too, and overlaps nothing."""
-    set_low_memory(engine, 1)
-    try:
-        nbytes, t0, t1, off = arena_plan(engine, 2, 1, 504, 756)
-    finally:
-        set_low_memory(engine, 0)
-    U = 4032 * 6048 * U_PER_PIXEL
-    assert no_overlap(nbytes, t0, t1, off)
-    assert int((off + nbytes).max()) <= 3 * U + SCRATCH
 
 
 # ---- the pipelines at 48 MP --------------------------------------------------------------------------------------
