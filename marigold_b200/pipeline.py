@@ -2,12 +2,17 @@
 
     MarigoldDepthPipeline.__call__     marigold/marigold_depth_pipeline.py:155-338
     MarigoldNormalsPipeline.__call__   marigold/marigold_normals_pipeline.py:140-308
+    MarigoldIIDPipeline.__call__       marigold/marigold_iid_pipeline.py:164-585
 
 Same arguments, defaults, checks, warnings, output dataclasses and numpy post-processing; the objects
 the reference holds as `unet`, `vae`, `scheduler` are replaced by one `Engine` (libmarigold_b200) plus
 a host-side scheduler mirror. Two keyword-only additions exist because the reference draws noise from
 a generator shared across batches (depth_pipeline.py:430-435), which cannot be reproduced once members
 are sharded across GPUs:  noise=[E,4,h,w]  and  step_noise=[n-1,E,4,h,w] (LCM).
+
+Each __call__ only carries its signature: one body (_MarigoldBase._call) checks everything before any work, then runs
+one image through _infer_members or a list through _infer_list. Both loops take their member batch from one admission
+rule (_admit_group), their noise from one drawer (_draw_image_noise), and finish an image with the pipeline's _finish.
 
 Every pipeline also takes a list (or tuple) of images and returns a list of outputs in input order: the members of
 several images share network batches, and each image is finished (ensembled, resized, copied to the host) by the single
@@ -133,12 +138,6 @@ def colorize_depth_maps(depth, min_depth: float, max_depth: float, cmap: str = "
     return out
 
 
-def _check_ensemble_size(engine, ensemble_size: int) -> None:
-    mx = int(engine.lib.mgb_ens_max_members())
-    if ensemble_size > mx:
-        raise ValueError(f"ensemble_size={ensemble_size} exceeds the {mx} members the ensembling kernels accept")
-
-
 def find_batch_size(ensemble_size: int, input_res: int, dtype: torch.dtype) -> int:
     """reference batchsize.py:60-90 is a VRAM table for A100/3090/1080Ti; on an 80 GB H100 every supported
     configuration fits in batches of 16 members up to 768 px and 8 above, so that is the cap (it bounds the arena)."""
@@ -211,6 +210,23 @@ def _processing_size(h0: int, w0: int, processing_res: int):
     return int(h0), int(w0)
 
 
+def _input_hw(image, i=None):
+    """(H0, W0) of an input image, a PIL image or a 4-D tensor, from its shape alone, before any work. List element i
+    that the single call would reject raises its error, prefixed with "image {i}: "; a single image (i None) that
+    _preprocess rejects gives None, and _preprocess raises."""
+    if Image is not None and isinstance(image, Image.Image):
+        w0, h0 = image.size
+        return int(h0), int(w0)
+    if i is not None:
+        if not isinstance(image, torch.Tensor):
+            raise TypeError(f"image {i}: Unknown input type: {type(image) = }")
+        assert 4 == image.dim() and 1 == image.shape[0] and 3 == image.shape[1], \
+            f"image {i}: Wrong input shape {tuple(image.shape)}, expected [1, rgb, H, W]"
+    elif not isinstance(image, torch.Tensor) or image.dim() != 4:
+        return None
+    return int(image.shape[-2]), int(image.shape[-1])
+
+
 def size_groups(sizes):
     """[(size, [image indices])] in order of first appearance: the images of a list call that may share a batch."""
     groups = {}
@@ -234,7 +250,11 @@ def select_list_batch_size(engine, n_jobs: int, h: int, w: int, ensemble_size: i
     """Members per batch for a size group of a list call: select_batch_size over the group's n_jobs (image, member) jobs
     (one rank's share under world_size ranks), beside the call_reserve_bytes of every image one round of batches can
     hold open (parallel.open_images). The reserve grows with the batch, so the two are lowered together: the result is
-    the largest batch that fits beside its own reserve. Raises ValueError like select_batch_size."""
+    the largest batch that fits beside its own reserve. Raises ValueError like select_batch_size. The single call's
+    selection is the one-image case."""
+    if n_images == 1:                    # one image's reserve, whatever the batch
+        return select_batch_size(engine, n_jobs, h, w, batch_size, free_bytes,
+                                 call_reserve_bytes(h, w, ensemble_size, channels))
     return _on_free_memory(engine, free_bytes, lambda free: _select_list_batch_size(
         engine, n_jobs, h, w, ensemble_size, channels, n_images, world_size, batch_size, free))
 
@@ -270,9 +290,22 @@ def _image_runs(jobs, idx, ensemble_size):
     return runs
 
 
+_lib_decode_depth, _lib_decode_normals, _lib_decode_iid = 0, 1, 3   # mgb_decode_mode
+
+
 class _MarigoldBase:
     latent_scale_factor = 0.18215  # depth_pipeline.py:118
     member_channels = 1            # channels of one decoded member: 1 (depth), 3 (normals), 3 per target (IID)
+    decode_mode = _lib_decode_depth
+    # _check_inference_step: whether LCM runs (with a deprecation warning) or is refused, and the reference's DDIM
+    # warnings (timestep spacing, too many steps, zero SNR) in the depth and IID pipelines' words
+    lcm_supported = False
+    step_warnings = ('The loaded `DDIMScheduler` is configured with `timestep_spacing="{spacing}"`; the recommended '
+                     'setting is `"trailing"`.',
+                     "Setting too many denoising steps ({n_step}) may degrade the prediction; consider relying on the "
+                     "default values.",
+                     "The loaded `DDIMScheduler` is configured with `rescale_betas_zero_snr=False`; the recommended "
+                     "setting is True.")
 
     def __init__(self, engine: Engine, scheduler, empty_text_embed: torch.Tensor,
                  default_denoising_steps: Optional[int] = None, default_processing_resolution: Optional[int] = None):
@@ -298,6 +331,64 @@ class _MarigoldBase:
 
         return load_pipeline(cls, pretrained_model_name_or_path, variant=variant, torch_dtype=torch_dtype, device=device,
                              **kwargs)
+
+    @torch.no_grad()
+    def _call(self, input_image, denoising_steps, ensemble_size, processing_res, match_input_res, resample_method,
+              batch_size, generator, ensemble_kwargs, noise, step_noise, **finish_kw):
+        """The body of every pipeline's __call__ (depth_pipeline.py:155-338): one image, or a list of images with one
+        output per image in input order (_infer_list). Every check runs before any inference work is spent."""
+        if denoising_steps is None:
+            denoising_steps = self.default_denoising_steps
+        if processing_res is None:
+            processing_res = self.default_processing_resolution
+        assert processing_res >= 0
+        assert ensemble_size >= 1
+        mx = int(self.engine.lib.mgb_ens_max_members())
+        if ensemble_size > mx:
+            raise ValueError(f"ensemble_size={ensemble_size} exceeds the {mx} members the ensembling kernels accept")
+        self._check_inference_step(denoising_steps)
+        resample = get_tv_resample_method(resample_method)
+
+        def finish(member_maps, out_hw):
+            return self._finish(member_maps, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs,
+                                **finish_kw)
+
+        if isinstance(input_image, (list, tuple)):
+            outputs = [None] * len(input_image)
+
+            def finish_image(i, member_maps, out_hw):
+                outputs[i] = finish(member_maps, out_hw)
+
+            self._infer_list(input_image, ensemble_size, denoising_steps, processing_res, resample, batch_size,
+                             generator, noise, step_noise, self.decode_mode, finish_image)
+            return outputs
+        batch_size, row_split = self._member_batch(input_image, processing_res, ensemble_size, batch_size)
+        rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
+        target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
+                                           step_noise, self.decode_mode, row_split)
+        return finish(target_preds, tuple(input_size[-2:]))
+
+    def _check_inference_step(self, n_step: int) -> None:
+        """depth_pipeline.py:340-379, normals_pipeline.py:310-344, marigold_iid_pipeline.py:413-448: the same checks in
+        each pipeline's words (step_warnings); LCM is refused unless lcm_supported."""
+        assert n_step >= 1
+        spacing, too_many, zero_snr = self.step_warnings
+        if isinstance(self.scheduler, DDIMScheduler):
+            if "trailing" != self.scheduler.config.timestep_spacing:
+                logging.warning(spacing.format(spacing=self.scheduler.config.timestep_spacing))
+            elif n_step > 10:
+                logging.warning(too_many.format(n_step=n_step))
+            if not self.scheduler.config.rescale_betas_zero_snr:
+                logging.warning(zero_snr)
+        elif isinstance(self.scheduler, LCMScheduler):
+            if not self.lcm_supported:
+                raise RuntimeError("This pipeline implementation does not support the LCMScheduler. Please refer to "
+                                   "the project README.md for instructions about using LCM.")
+            logging.warning("DeprecationWarning: LCMScheduler will not be supported in the future.")
+            if n_step > 10:
+                logging.warning(too_many.format(n_step=n_step))
+        else:
+            raise RuntimeError(f"Unsupported scheduler type: {type(self.scheduler)}")
 
     def _set_schedule(self, n: int):
         self.scheduler.set_timesteps(n, device=self.device)
@@ -341,61 +432,44 @@ class _MarigoldBase:
         assert rgb_norm.min() >= -1.0 and rgb_norm.max() <= 1.0
         return rgb_norm, input_size
 
-    def _call_size(self, input_image, processing_res):
-        """(h, w) the call processes, from the input's shape alone; None for an input _preprocess rejects."""
-        if Image is not None and isinstance(input_image, Image.Image):
-            w0, h0 = input_image.size
-        elif isinstance(input_image, torch.Tensor) and input_image.dim() == 4:
-            h0, w0 = input_image.shape[-2:]
-        else:
-            return None
-        return _processing_size(h0, w0, processing_res)
-
-    def _member_batch_size(self, input_image, processing_res, ensemble_size, batch_size):
-        """select_batch_size for this call, from the input's shape alone: an input that cannot run is refused before
-        anything is allocated on the device or launched."""
-        size = self._call_size(input_image, processing_res)
-        if size is None:
-            return batch_size                                # _preprocess rejects it
+    def _admit_group(self, h, w, ensemble_size, n_images, n_mine, batch_size):
+        """(member batch, row split, refusal) of a size group of n_images images at h x w, n_mine of whose jobs are this
+        rank's: whether it runs row-split (parallel.row_split_rule), and select_list_batch_size's batch. A refused group
+        raises ValueError, except a row-split one, which gives batch 0 and the error: the ranks must agree on its
+        admission (each rank's depends on its own free memory) before any of them enters an exchange."""
         from . import parallel
 
-        rank, G = parallel.world()
-        n = len(parallel.member_indices(ensemble_size, rank, G))
-        h, w = size
-        return select_batch_size(self.engine, n, h, w, batch_size,
-                                 reserve_bytes=call_reserve_bytes(h, w, ensemble_size, self.member_channels))
+        G = parallel.world()[1]
+        split = parallel.row_split_rule(n_images * ensemble_size, h, w, G)
+        try:
+            with parallel.row_split(self.engine, split):
+                bs = select_list_batch_size(self.engine, 1 if split else n_mine, h, w, ensemble_size,
+                                            self.member_channels, n_images, G, batch_size)
+        except ValueError as e:
+            if not split:
+                raise
+            return 0, True, e
+        return bs, split, None
 
     def _member_batch(self, input_image, processing_res, ensemble_size, batch_size):
-        """(member batch, row split) for this call: whether the ranks agreed to run its one member row-split
-        (parallel.row_split_rule), with its batch of 1, or _member_batch_size's batch and False. The caller passes the
-        decision on to _infer_members."""
+        """(member batch, row split) of the single call, from the input's shape alone (_admit_group over this rank's
+        members), so that an input that cannot run is refused before any work. Only a row-split call agrees with the
+        other ranks, in one all-reduce. The caller passes the decision on to _infer_members."""
         from . import parallel
 
+        hw0 = _input_hw(input_image)
+        if hw0 is None:
+            return batch_size, False                         # _preprocess rejects it
+        h, w = _processing_size(*hw0, processing_res)
         rank, G = parallel.world()
-        size = self._call_size(input_image, processing_res)
-        if size is None or not parallel.row_split_rule(ensemble_size, size[0], size[1], G):
-            return self._member_batch_size(input_image, processing_res, ensemble_size, batch_size), False
-        h, w = size
-        # every rank runs the one member: the ranks agree on the split and on its admission (each rank's depends on its
-        # own free memory) in one all-reduce, so that no rank enters an exchange alone
-        err = None
-        try:
-            with parallel.row_split(self.engine):
-                bs = select_batch_size(self.engine, 1, h, w, batch_size,
-                                       reserve_bytes=call_reserve_bytes(h, w, ensemble_size, self.member_channels))
-        except ValueError as e:
-            bs, err = 0, e
+        bs, split, err = self._admit_group(h, w, ensemble_size, 1, len(parallel.member_indices(ensemble_size, rank, G)),
+                                           batch_size)
+        if not split:
+            return bs, False
         split, admitted = parallel.agree_batch_sizes([1, min(bs, 1)], self.device)
         if not admitted:
             raise err if err is not None else ValueError(f"another rank cannot admit one member at {h} x {w}")
         return 1, split == 1
-
-    def _draw_noise(self, shape, generator, noise):
-        if noise is not None:
-            assert tuple(noise.shape) == tuple(shape), f"noise shape {tuple(noise.shape)} != {tuple(shape)}"
-            return noise.to(self.device, torch.float32)
-        dev = generator.device if generator is not None else self.device
-        return torch.randn(shape, device=dev, dtype=self.dtype, generator=generator).to(self.device)
 
     @torch.no_grad()
     def encode_rgb(self, rgb_in: torch.Tensor) -> torch.Tensor:
@@ -420,44 +494,54 @@ class _MarigoldBase:
         with parallel.row_split(self.engine, split):
             rgb_latent1 = self.encode_rgb(rgb_norm)                      # [1,4,h,w]
             lh, lw = rgb_latent1.shape[-2:]
-            is_lcm = isinstance(self.scheduler, LCMScheduler)
-            need_sn = is_lcm and denoising_steps > 1
             ct = self.engine.cfg.unet_out_channels               # 4, or 4 n for an n-target IID model
-            if G > 1:
-                # every rank draws (or receives) the FULL noise tensors and takes its rows, so member k's noise
-                # does not depend on the partitioning (SURVEY.md F9)
-                noise = self._draw_noise((ensemble_size, ct, lh, lw), generator, noise)
-                if need_sn and step_noise is None:
-                    dev = generator.device if generator is not None else self.device
-                    step_noise = torch.randn((denoising_steps - 1, ensemble_size, ct, lh, lw), device=dev,
-                                             dtype=self.dtype, generator=generator)
+            # one rank draws in the batches it runs; G ranks each draw (or receive) the FULL noise tensors and take
+            # their rows, so member k's noise does not depend on the partitioning (SURVEY.md F9)
+            pieces = None if G > 1 else noise_draw_batches(ensemble_size, _bs, *rgb_norm.shape[-2:])
+            z, sn = self._draw_image_noise(generator, noise, step_noise, (ct, lh, lw), ensemble_size, denoising_steps,
+                                           pieces)
             if split:
-                noise, step_noise = parallel.broadcast_from_first([noise, step_noise], self.device)
+                z, sn = parallel.broadcast_from_first([z, sn], self.device)
             preds = []
             for s in range(0, len(mine), _bs):
                 ids = mine[s:s + _bs]
-                nb = len(ids)
-                if G > 1 or noise is not None:
-                    z0 = noise[ids].to(self.device, torch.float32).contiguous()
-                else:
-                    z0 = self._draw_noise((nb, ct, lh, lw), generator, None)
-                sn = None
-                if need_sn:
-                    if step_noise is not None:
-                        sn = step_noise[:, ids].to(self.device, torch.float32).contiguous()
-                    else:
-                        # one randn per step, in step order after z0: the draw sequence of scheduler.step(generator=...)
-                        # inside the reference loop (depth_pipeline.py:466-468), so a seeded generator gives the same
-                        # stream
-                        dev = generator.device if generator is not None else self.device
-                        sn = torch.stack([torch.randn((nb, ct, lh, lw), device=dev, dtype=self.dtype,
-                                                      generator=generator)
-                                          for _ in range(denoising_steps - 1)]).to(self.device)
-                target = self.engine.denoise(rgb_latent1.expand(nb, -1, -1, -1).contiguous(), z0, sn)
+                target = self.engine.denoise(rgb_latent1.expand(len(ids), -1, -1, -1).contiguous(), z[ids].contiguous(),
+                                             sn[:, ids].contiguous() if sn is not None else None)
                 preds.append(self._decode(target, decode_mode))
         ch = 1 if decode_mode == 0 else (3 * (ct // 4) if decode_mode == _lib_decode_iid else 3)
         local = torch.concat(preds, dim=0) if preds else torch.empty((0, ch, lh * 8, lw * 8), device=self.device)
         return local if split else parallel.gather_members(local, ensemble_size)
+
+    def _draw_image_noise(self, generator, noise, step_noise, shape, ensemble_size, denoising_steps, pieces):
+        """One image's z0 [E, *shape] and LCM step noise [n - 1, E, *shape] (None where no step draws noise), on the
+        device, drawn from generator in the single call's order: at world size 1 per piece of b members (pieces), z0
+        [b] then one [b] draw per step in step order, the draw sequence of scheduler.step(generator=...) inside the
+        reference loop (depth_pipeline.py:466-468); under G > 1 ranks (pieces None) z0 [E] then the step noise
+        [n - 1, E]. noise / step_noise, where given, replace their draws."""
+        need_sn = isinstance(self.scheduler, LCMScheduler) and denoising_steps > 1
+        dev = generator.device if generator is not None else self.device
+
+        def randn(*size):
+            return torch.randn(size + shape, device=dev, dtype=self.dtype, generator=generator)
+
+        if pieces is None:
+            if noise is not None:
+                want = (ensemble_size,) + shape
+                assert tuple(noise.shape) == want, f"noise shape {tuple(noise.shape)} != {want}"
+            else:
+                noise = randn(ensemble_size)
+            if need_sn and step_noise is None:
+                step_noise = randn(denoising_steps - 1, ensemble_size)
+        else:
+            zs, ss = [], []
+            for b in pieces:
+                if noise is None:
+                    zs.append(randn(b))
+                if need_sn and step_noise is None:
+                    ss.append(torch.stack([randn(b) for _ in range(denoising_steps - 1)]))
+            noise = torch.cat(zs) if zs else noise
+            step_noise = torch.cat(ss, dim=1) if ss else step_noise
+        return noise.to(self.device, torch.float32), (step_noise.to(self.device, torch.float32) if need_sn else None)
 
     def _decode(self, target, decode_mode):
         """The decode of one denoised member batch [NB, ct, lh, lw] -> [NB, member_channels, 8 lh, 8 lw]."""
@@ -467,40 +551,18 @@ class _MarigoldBase:
                               for i in range(target.shape[1] // 4)], dim=1)
         return self.engine.decode(target, decode_mode)
 
+    def _ensembled(self, target_preds, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs):
+        """The head of every _finish: (prediction, uncertainty or None) of one image's member maps, ensembled by the
+        pipeline's _ensemble when E > 1, and the prediction resized to out_hw when match_input_res."""
+        if ensemble_size > 1:
+            final_pred, pred_uncert = self._ensemble(target_preds, **(ensemble_kwargs or {}))
+        else:
+            final_pred, pred_uncert = target_preds, None
+        if match_input_res:
+            final_pred = _resize(final_pred, out_hw, resample)
+        return final_pred, pred_uncert
+
     # ---- lists of images -------------------------------------------------------------------------------------------
-    def _list_image_hw(self, i, image):
-        """(H, W) of list element i, checked as the single call checks its input, before any work."""
-        if Image is not None and isinstance(image, Image.Image):
-            w0, h0 = image.size
-            return int(h0), int(w0)
-        if not isinstance(image, torch.Tensor):
-            raise TypeError(f"image {i}: Unknown input type: {type(image) = }")
-        assert 4 == image.dim() and 1 == image.shape[0] and 3 == image.shape[1], \
-            f"image {i}: Wrong input shape {tuple(image.shape)}, expected [1, rgb, H, W]"
-        return int(image.shape[-2]), int(image.shape[-1])
-
-    def _call_list(self, images, denoising_steps, ensemble_size, processing_res, match_input_res, resample_method,
-                   batch_size, generator, ensemble_kwargs, noise, step_noise, decode_mode, **finish_kw):
-        """__call__ on a list of images: one output per image, in input order (see _infer_list)."""
-        if denoising_steps is None:
-            denoising_steps = self.default_denoising_steps
-        if processing_res is None:
-            processing_res = self.default_processing_resolution
-        assert processing_res >= 0
-        assert ensemble_size >= 1
-        _check_ensemble_size(self.engine, ensemble_size)
-        self._check_inference_step(denoising_steps)
-        resample = get_tv_resample_method(resample_method)
-        outputs = [None] * len(images)
-
-        def finish(i, member_maps, out_hw):
-            outputs[i] = self._finish(member_maps, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs,
-                                      **finish_kw)
-
-        self._infer_list(images, ensemble_size, denoising_steps, processing_res, resample, batch_size, generator, noise,
-                         step_noise, decode_mode, finish)
-        return outputs
-
     def _infer_list(self, images, ensemble_size, denoising_steps, processing_res, resample, batch_size, generator,
                     noise, step_noise, decode_mode, finish):
         """Every member of every image through shared member batches; finish(i, [E, C, H, W] member maps, (H0, W0)) is
@@ -511,12 +573,11 @@ class _MarigoldBase:
         agreed by MIN over ranks). An image is preprocessed and encoded alone, as in the single call, when its first
         member enters a batch. Under G ranks, round r runs every rank's r-th batch and one all-gather joins them.
 
-        Noise: image i draws from generator[i] (a list), or from the one shared generator in list order, exactly what
-        the single call with that generator draws: at world size 1 per noise_draw_batches piece of b members, z0
-        [b, ct, lh, lw] then the n - 1 LCM step-noise draws [b, ct, lh, lw]; under G > 1 z0 [E, ...] then step noise
-        [n - 1, E, ...]. noise[i] / step_noise[i] replace image i's draws. A member's maps depend only on its own inputs
-        and on its batch's size, so a member packed beside other images' members has the single call's bits wherever
-        the single call runs the same batch size (free memory can lower the single call's batch below b)."""
+        Noise: image i draws from generator[i] (a list), or from the one shared generator in list order, what the single
+        call with that generator draws where free memory does not lower its batch (_draw_image_noise in
+        noise_draw_batches pieces); noise[i] / step_noise[i] replace image i's draws. A member's maps depend only on its
+        own inputs and on its batch's size, so a member packed beside other images' members has the single call's bits
+        wherever the single call runs the same batch size."""
         from . import parallel
 
         N = len(images)
@@ -525,7 +586,7 @@ class _MarigoldBase:
         ct = self.engine.cfg.unet_out_channels
         need_sn = isinstance(self.scheduler, LCMScheduler) and denoising_steps > 1
         # ---- every check before any work
-        hw0 = [self._list_image_hw(i, im) for i, im in enumerate(images)]
+        hw0 = [_input_hw(im, i) for i, im in enumerate(images)]
         shared_gen = not isinstance(generator, (list, tuple))
         for name, per_image in (("generator", None if shared_gen else generator), ("noise", noise),
                                 ("step_noise", step_noise)):
@@ -535,19 +596,15 @@ class _MarigoldBase:
         groups = size_groups([_processing_size(h0, w0, processing_res) for h0, w0 in hw0])
         sizes, splits, refused = [], [], {}
         for (h, w), idx in groups:
-            n_jobs = len(idx) * E
-            # a group of one job runs row-split on every rank (parallel.row_split_rule); its admission is agreed with
-            # the batch sizes below, before any rank runs it
-            split = parallel.row_split_rule(n_jobs, h, w, G)
+            # a row-split group's admission is agreed with the batch sizes below, before any rank runs it
             try:
-                with parallel.row_split(self.engine, split):
-                    sizes.append(select_list_batch_size(self.engine, 1 if split else parallel.slots_per_rank(n_jobs, G),
-                                                        h, w, E, self.member_channels, len(idx), G, batch_size))
+                bs, split, err = self._admit_group(h, w, E, len(idx), parallel.slots_per_rank(len(idx) * E, G),
+                                                   batch_size)
             except ValueError as e:
-                if not split:
-                    raise ValueError(f"image {idx[0]}: {e}") from None
-                refused[len(sizes)] = e
-                sizes.append(0)
+                raise ValueError(f"image {idx[0]}: {e}") from None
+            if err is not None:
+                refused[len(sizes)] = err
+            sizes.append(bs)
             splits.append(int(split))
             lh, lw = h // 8, w // 8
             for i in idx:
@@ -569,29 +626,12 @@ class _MarigoldBase:
         self._set_schedule(denoising_steps)
 
         def draw(i):
-            """Image i's z0 [E, ...] and step noise [n - 1, E, ...] (or None), in the single call's draw order."""
-            gen = generator if shared_gen else generator[i]
-            z_i = noise[i] if noise is not None else None
-            s_i = step_noise[i] if (need_sn and step_noise is not None) else None
+            """Image i's z0 and step noise, drawn as the single call draws them with its generator."""
             h, w = _processing_size(*hw0[i], processing_res)
-            shape = (ct, h // 8, w // 8)
-            dev = gen.device if gen is not None else self.device
-            if G > 1:
-                z = self._draw_noise((E,) + shape, gen, z_i)
-                if need_sn and s_i is None:
-                    s_i = torch.randn((denoising_steps - 1, E) + shape, device=dev, dtype=self.dtype, generator=gen)
-            else:
-                zs, ss = [], []
-                for b in noise_draw_batches(E, batch_size, h, w):
-                    if z_i is None:
-                        zs.append(self._draw_noise((b,) + shape, gen, None))
-                    if need_sn and s_i is None:
-                        ss.append(torch.stack([torch.randn((b,) + shape, device=dev, dtype=self.dtype, generator=gen)
-                                               for _ in range(denoising_steps - 1)]))
-                z = z_i.to(self.device, torch.float32) if z_i is not None else torch.cat(zs)
-                if ss:
-                    s_i = torch.cat(ss, dim=1)
-            return z, (s_i.to(self.device, torch.float32) if need_sn else None)
+            return self._draw_image_noise(generator if shared_gen else generator[i],
+                                          noise[i] if noise is not None else None,
+                                          step_noise[i] if step_noise is not None else None, (ct, h // 8, w // 8), E,
+                                          denoising_steps, None if G > 1 else noise_draw_batches(E, batch_size, h, w))
 
         drawn, next_draw = {}, 0
 
@@ -652,6 +692,8 @@ class _MarigoldBase:
 
 
 class MarigoldDepthPipeline(_MarigoldBase):
+    lcm_supported = True
+
     def __init__(self, engine, scheduler, empty_text_embed, scale_invariant: Optional[bool] = True,
                  shift_invariant: Optional[bool] = True, default_denoising_steps: Optional[int] = None,
                  default_processing_resolution: Optional[int] = None):
@@ -659,29 +701,6 @@ class MarigoldDepthPipeline(_MarigoldBase):
         self.scale_invariant = scale_invariant
         self.shift_invariant = shift_invariant
 
-    def _check_inference_step(self, n_step: int) -> None:
-        """depth_pipeline.py:340-379"""
-        assert n_step >= 1
-        if isinstance(self.scheduler, DDIMScheduler):
-            if "trailing" != self.scheduler.config.timestep_spacing:
-                logging.warning(
-                    f'The loaded `DDIMScheduler` is configured with `timestep_spacing="'
-                    f'{self.scheduler.config.timestep_spacing}"`; the recommended setting is `"trailing"`.')
-            elif n_step > 10:
-                logging.warning(f"Setting too many denoising steps ({n_step}) may degrade the prediction; consider "
-                                f"relying on the default values.")
-            if not self.scheduler.config.rescale_betas_zero_snr:
-                logging.warning("The loaded `DDIMScheduler` is configured with `rescale_betas_zero_snr=False`; the "
-                                "recommended setting is True.")
-        elif isinstance(self.scheduler, LCMScheduler):
-            logging.warning("DeprecationWarning: LCMScheduler will not be supported in the future.")
-            if n_step > 10:
-                logging.warning(f"Setting too many denoising steps ({n_step}) may degrade the prediction; consider "
-                                f"relying on the default values.")
-        else:
-            raise RuntimeError(f"Unsupported scheduler type: {type(self.scheduler)}")
-
-    @torch.no_grad()
     def __call__(self, input_image, denoising_steps: Optional[int] = None, ensemble_size: int = 1,
                  processing_res: Optional[int] = None, match_input_res: bool = True,
                  resample_method: str = "bilinear", batch_size: int = 0,
@@ -689,37 +708,17 @@ class MarigoldDepthPipeline(_MarigoldBase):
                  show_progress_bar: bool = True, ensemble_kwargs: Dict = None, *,
                  noise: Optional[torch.Tensor] = None, step_noise: Optional[torch.Tensor] = None
                  ) -> MarigoldDepthOutput:
-        if isinstance(input_image, (list, tuple)):
-            return self._call_list(input_image, denoising_steps, ensemble_size, processing_res, match_input_res,
-                                   resample_method, batch_size, generator, ensemble_kwargs, noise, step_noise,
-                                   _lib_decode_depth, color_map=color_map)
-        if denoising_steps is None:
-            denoising_steps = self.default_denoising_steps
-        if processing_res is None:
-            processing_res = self.default_processing_resolution
-        assert processing_res >= 0
-        assert ensemble_size >= 1
-        _check_ensemble_size(self.engine, ensemble_size)          # fail before any inference work is spent
-        self._check_inference_step(denoising_steps)
-        resample = get_tv_resample_method(resample_method)
-        batch_size, row_split = self._member_batch(input_image, processing_res, ensemble_size, batch_size)
-        rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
+        return self._call(input_image, denoising_steps, ensemble_size, processing_res, match_input_res, resample_method,
+                          batch_size, generator, ensemble_kwargs, noise, step_noise, color_map=color_map)
 
-        target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
-                                           step_noise, _lib_decode_depth, row_split)
-        return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
-                            ensemble_kwargs, color_map=color_map)
+    def _ensemble(self, target_preds, **kwargs):
+        return ensemble_depth(target_preds, scale_invariant=self.scale_invariant, shift_invariant=self.shift_invariant,
+                              engine=self.engine, **kwargs)
 
     def _finish(self, target_preds, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs, color_map):
         """One image's [E, 1, h, w] member maps -> MarigoldDepthOutput (depth_pipeline.py:292-338)."""
-        if ensemble_size > 1:
-            final_pred, pred_uncert = ensemble_depth(target_preds, scale_invariant=self.scale_invariant,
-                                                     shift_invariant=self.shift_invariant, engine=self.engine,
-                                                     **(ensemble_kwargs or {}))
-        else:
-            final_pred, pred_uncert = target_preds, None
-        if match_input_res:
-            final_pred = _resize(final_pred, out_hw, resample)
+        final_pred, pred_uncert = self._ensembled(target_preds, out_hw, ensemble_size, resample, match_input_res,
+                                                  ensemble_kwargs)
         final_pred = final_pred.squeeze().cpu().numpy()
         if pred_uncert is not None:
             pred_uncert = pred_uncert.squeeze().cpu().numpy()
@@ -740,56 +739,26 @@ class MarigoldDepthPipeline(_MarigoldBase):
 
 class MarigoldNormalsPipeline(_MarigoldBase):
     member_channels = 3
+    decode_mode = _lib_decode_normals
+    step_warnings = ('The loaded `DDIMScheduler` is not configured with `timestep_spacing="trailing"`.',
+                     "Setting too many denoising steps ({n_step}) may degrade the prediction.",
+                     "The loaded `DDIMScheduler` is configured with `rescale_betas_zero_snr=False`.")
 
-    def _check_inference_step(self, n_step: int) -> None:
-        """normals_pipeline.py:310-344: LCM is refused."""
-        assert n_step >= 1
-        if isinstance(self.scheduler, DDIMScheduler):
-            if "trailing" != self.scheduler.config.timestep_spacing:
-                logging.warning("The loaded `DDIMScheduler` is not configured with `timestep_spacing=\"trailing\"`.")
-            elif n_step > 10:
-                logging.warning(f"Setting too many denoising steps ({n_step}) may degrade the prediction.")
-            if not self.scheduler.config.rescale_betas_zero_snr:
-                logging.warning("The loaded `DDIMScheduler` is configured with `rescale_betas_zero_snr=False`.")
-        elif isinstance(self.scheduler, LCMScheduler):
-            raise RuntimeError("This pipeline implementation does not support the LCMScheduler. Please refer to the "
-                               "project README.md for instructions about using LCM.")
-        else:
-            raise RuntimeError(f"Unsupported scheduler type: {type(self.scheduler)}")
-
-    @torch.no_grad()
     def __call__(self, input_image, denoising_steps: Optional[int] = None, ensemble_size: int = 1,
                  processing_res: Optional[int] = None, match_input_res: bool = True,
                  resample_method: str = "bilinear", batch_size: int = 0,
                  generator: Union[torch.Generator, None] = None, show_progress_bar: bool = True,
                  ensemble_kwargs: Dict = None, *, noise: Optional[torch.Tensor] = None) -> MarigoldNormalsOutput:
-        if isinstance(input_image, (list, tuple)):
-            return self._call_list(input_image, denoising_steps, ensemble_size, processing_res, match_input_res,
-                                   resample_method, batch_size, generator, ensemble_kwargs, noise, None,
-                                   _lib_decode_normals)
-        if denoising_steps is None:
-            denoising_steps = self.default_denoising_steps
-        if processing_res is None:
-            processing_res = self.default_processing_resolution
-        assert processing_res >= 0
-        assert ensemble_size >= 1
-        self._check_inference_step(denoising_steps)
-        resample = get_tv_resample_method(resample_method)
-        batch_size, row_split = self._member_batch(input_image, processing_res, ensemble_size, batch_size)
-        rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
-        target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
-                                           None, _lib_decode_normals, row_split)
-        return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
-                            ensemble_kwargs)
+        return self._call(input_image, denoising_steps, ensemble_size, processing_res, match_input_res, resample_method,
+                          batch_size, generator, ensemble_kwargs, noise, None)
+
+    def _ensemble(self, target_preds, **kwargs):
+        return ensemble_normals(target_preds, engine=self.engine, **kwargs)
 
     def _finish(self, target_preds, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs):
         """One image's [E, 3, h, w] member maps -> MarigoldNormalsOutput (normals_pipeline.py:278-308)."""
-        if ensemble_size > 1:
-            final_pred, pred_uncert = ensemble_normals(target_preds, engine=self.engine, **(ensemble_kwargs or {}))
-        else:
-            final_pred, pred_uncert = target_preds, None
-        if match_input_res:
-            final_pred = _resize(final_pred, out_hw, resample)
+        final_pred, pred_uncert = self._ensembled(target_preds, out_hw, ensemble_size, resample, match_input_res,
+                                                  ensemble_kwargs)
         final_pred = final_pred.squeeze().cpu().numpy()
         if pred_uncert is not None:
             pred_uncert = pred_uncert.squeeze().cpu().numpy()
@@ -804,6 +773,7 @@ class MarigoldIIDPipeline(_MarigoldBase):
     """Intrinsic image decomposition with an arbitrary number of 3-channel targets (reference
     marigold/marigold_iid_pipeline.py:164-585): ONE UNet whose conv_in takes 4 (n + 1) latent channels and whose
     conv_out produces 4 n; every target's 4-channel latent is decoded separately; E > 1 goes through `ensemble_iid`."""
+    decode_mode = _lib_decode_iid
 
     def __init__(self, engine, scheduler, empty_text_embed, target_properties: Optional[Dict] = None,
                  default_denoising_steps: Optional[int] = None, default_processing_resolution: Optional[int] = None):
@@ -816,66 +786,29 @@ class MarigoldIIDPipeline(_MarigoldBase):
             raise ValueError(f"the UNet predicts {engine.cfg.unet_out_channels} latent channels, but target_names "
                              f"{self.target_names} needs {4 * self.n_targets}")
 
-    def _check_inference_step(self, n_step: int) -> None:
-        """marigold_iid_pipeline.py:413-448: LCM is refused."""
-        assert n_step >= 1
-        if isinstance(self.scheduler, DDIMScheduler):
-            if "trailing" != self.scheduler.config.timestep_spacing:
-                logging.warning(f'The loaded `DDIMScheduler` is configured with `timestep_spacing="'
-                                f'{self.scheduler.config.timestep_spacing}"`; the recommended setting is `"trailing"`.')
-            elif n_step > 10:
-                logging.warning(f"Setting too many denoising steps ({n_step}) may degrade the prediction; consider "
-                                f"relying on the default values.")
-            if not self.scheduler.config.rescale_betas_zero_snr:
-                logging.warning("The loaded `DDIMScheduler` is configured with `rescale_betas_zero_snr=False`; the "
-                                "recommended setting is True.")
-        elif isinstance(self.scheduler, LCMScheduler):
-            raise RuntimeError("This pipeline implementation does not support the LCMScheduler. Please refer to the "
-                               "project README.md for instructions about using LCM.")
-        else:
-            raise RuntimeError(f"Unsupported scheduler type: {type(self.scheduler)}")
-
-    @torch.no_grad()
     def __call__(self, input_image, denoising_steps: Optional[int] = None, ensemble_size: int = 1,
                  processing_res: Optional[int] = None, match_input_res: bool = True,
                  resample_method: str = "bilinear", batch_size: int = 0,
                  generator: Union[torch.Generator, None] = None, show_progress_bar: bool = True,
                  ensemble_kwargs: Dict = None, *, noise: Optional[torch.Tensor] = None):
-        if isinstance(input_image, (list, tuple)):
-            return self._call_list(input_image, denoising_steps, ensemble_size, processing_res, match_input_res,
-                                   resample_method, batch_size, generator, ensemble_kwargs, noise, None,
-                                   _lib_decode_iid)
-        if denoising_steps is None:
-            denoising_steps = self.default_denoising_steps
-        if processing_res is None:
-            processing_res = self.default_processing_resolution
-        assert processing_res >= 0
-        assert ensemble_size >= 1
-        self._check_inference_step(denoising_steps)
-        resample = get_tv_resample_method(resample_method)
-        batch_size, row_split = self._member_batch(input_image, processing_res, ensemble_size, batch_size)
-        rgb_norm, input_size = self._preprocess(input_image, processing_res, resample)
-        target_preds = self._infer_members(rgb_norm, ensemble_size, denoising_steps, batch_size, generator, noise,
-                                           None, _lib_decode_iid, row_split)
-        return self._finish(target_preds, tuple(input_size[-2:]), ensemble_size, resample, match_input_res,
-                            ensemble_kwargs)
+        return self._call(input_image, denoising_steps, ensemble_size, processing_res, match_input_res, resample_method,
+                          batch_size, generator, ensemble_kwargs, noise, None)
+
+    def _ensemble(self, target_preds, **kwargs):
+        return ensemble_iid(target_preds, engine=self.engine, **kwargs)
 
     def _finish(self, target_preds, out_hw, ensemble_size, resample, match_input_res, ensemble_kwargs):
-        """One image's [E, 3 n, h, w] member maps -> MarigoldIIDOutput (marigold_iid_pipeline.py:367-411)."""
+        """One image's [E, 3 n, h, w] member maps -> MarigoldIIDOutput (marigold_iid_pipeline.py:367-411; the
+        uncertainty is not resized, :386-392)."""
         from .iid import MarigoldIIDOutput, fill_outputs
 
         assert target_preds.dim() == 4 and target_preds.shape[1] == 3 * self.n_targets      # :367-370
-        if ensemble_size > 1:
-            final_pred, pred_uncert = ensemble_iid(target_preds, engine=self.engine, **(ensemble_kwargs or {}))
-        else:
-            final_pred, pred_uncert = target_preds, None
-        if match_input_res:
-            final_pred = _resize(final_pred, out_hw, resample)      # (:386-392; uncertainty is NOT resized)
+        final_pred, pred_uncert = self._ensembled(target_preds, out_hw, ensemble_size, resample, match_input_res,
+                                                  ensemble_kwargs)
         output = MarigoldIIDOutput(target_names=self.target_names)
         fill_outputs(output, final_pred, pred_uncert, self.target_names, self.target_properties)
         assert output.is_complete
         return output
 
 
-_lib_decode_depth, _lib_decode_normals, _lib_decode_iid = 0, 1, 3   # mgb_decode_mode
 MarigoldPipeline = MarigoldDepthPipeline         # alias, reference marigold/__init__.py:41

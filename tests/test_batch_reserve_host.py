@@ -60,8 +60,8 @@ class _Eng(StubEngine):
 
 
 @pytest.mark.parametrize("cls,ch", [(MarigoldDepthPipeline, 1), (MarigoldNormalsPipeline, 3), (MarigoldIIDPipeline, 6)])
-def test_pipelines_reserve_their_members(cls, ch, monkeypatch):
-    """_member_batch_size passes call_reserve_bytes for the processing size, the task's channels and E."""
+def test_member_batch_reserves_the_call_members(cls, ch, monkeypatch):
+    """_member_batch passes call_reserve_bytes for the processing size, the task's channels and E."""
     import marigold_b200.pipeline as P
 
     seen = {}
@@ -74,5 +74,5 @@ def test_pipelines_reserve_their_members(cls, ch, monkeypatch):
     kw = {"target_properties": {"target_names": ["albedo", "shading"]}} if cls is MarigoldIIDPipeline else {}
     pipe = cls(_Eng(per_member=GB), None, None, **kw)
     img = torch.zeros(1, 3, 4032, 6048, dtype=torch.uint8)
-    assert pipe._member_batch_size(img, 0, 10, 0) == 1
+    assert pipe._member_batch(img, 0, 10, 0) == (1, False)
     assert seen == {"n": 10, "h": 4032, "w": 6048, "reserve": call_reserve_bytes(4032, 6048, 10, ch)}
