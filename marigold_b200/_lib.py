@@ -1,4 +1,5 @@
-"""ctypes binding of libmarigold_b200.so (the C ABI in include/marigold_b200.h).
+"""ctypes binding of libmarigold_b200.so (the C ABI in include/marigold_b200.h, and the debug entry points tests and
+tools use, in marigold_b200/csrc/debug.h).
 
 The product path has no CPU fallback: if the shared library is missing and cannot be built, or a
 call returns a non-zero status, this module raises.
@@ -108,6 +109,29 @@ SIGNATURES = {
     "mgb_op_pack_decoder_latent": (_i32, [_vp, _vp, _vp, _f32, _vp, _i32, _i32, _vp]),
 }
 
+_P32, _P64, _PU64 = C.POINTER(_i32), C.POINTER(_i64), C.POINTER(C.c_uint64)
+
+# name -> (restype, argtypes); every debug entry point marigold_b200/csrc/debug.h declares (tests and tools only)
+DEBUG_SIGNATURES = {
+    "mgb_debug_gemm_timing": (None, [_vp]),
+    "mgb_debug_live_device_bytes": (_i64, []),
+    "mgb_debug_groupnorm_halves": (_i32, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _i32, _vp]),
+    "mgb_debug_conv2d_band": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32,
+                                      _i32, _i32, _P32, _vp]),
+    "mgb_debug_lpips_features": (_i32, [_vp, _i32, _i32, _i32, _vp, _P32]),
+    "mgb_debug_lpips_net_features": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _P32]),
+    "mgb_debug_lpips_step": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _P32]),
+    "mgb_debug_read": (_i64, [_vp, C.c_char_p, _vp, _i64, _PU64]),
+    "mgb_debug_weight_buffers": (_i32, [_vp, _PU64, _P64, _i32]),
+    "mgb_debug_vae_attn_blocks": (_i32, [_vp, _i64, _i32, _i32, _i32, _P32, _P32]),
+    "mgb_debug_vae_attn_core": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32]),
+    "mgb_debug_arena": (_i32, [_vp, _i32, _i32]),
+    "mgb_debug_vae_low_memory": (_i32, [_vp, _i32]),
+    "mgb_debug_vae_bands": (_i32, [_vp, _i32, _i32]),
+    "mgb_debug_arena_place": (_i64, [_i64, _P64, _P64, _P64, _i32, _P64]),
+    "mgb_debug_arena_plan": (_i64, [_vp, _i32, _i32, _i32, _i32, _P64, _P64, _P64, _P64, _i64]),
+}
+
 
 def _stale() -> bool:
     try:
@@ -146,7 +170,7 @@ def load(build_if_missing: bool = True):
             warnings.warn(f"{_LIB_PATH.name} is older than its sources under csrc/; run `python -m marigold_b200.build`",
                           RuntimeWarning, stacklevel=2)
     lib = C.CDLL(str(_LIB_PATH), mode=os.RTLD_GLOBAL if hasattr(os, "RTLD_GLOBAL") else C.DEFAULT_MODE)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in {**SIGNATURES, **DEBUG_SIGNATURES}.items():
         try:
             fn = getattr(lib, name)
         except AttributeError as e:  # header and library out of sync

@@ -5,6 +5,7 @@
 #include <cstring>
 #include <vector>
 
+#include "debug.h"
 #include "device.h"
 #include "kernels.h"
 
@@ -188,9 +189,7 @@ int mgb_eval_iid_lpips(const float* pred, const float* gt, const uint8_t* mask, 
   return MGB_OK;
 }
 
-/* debug hook (not in the public header): copies the fp32 post-ReLU features of AlexNet layer `layer` (0..4) that the last
- * mgb_eval_iid_lpips call on ws left there, [2, h, w, C] (pred, then gt), to dst_dev; dims_out = {h, w, C}. dst_dev NULL:
- * only the dims. A device-to-device copy; nothing is launched. */
+/* debug hooks (declared in debug.h) */
 int mgb_debug_lpips_features(const void* ws, int32_t H, int32_t W, int32_t layer, float* dst_dev, int32_t dims_out[3]) {
   if (!ws || !dims_out || layer < 0 || layer >= kLpipsLayers || H < kLpipsMinSize || W < kLpipsMinSize) {
     set_error("mgb_debug_lpips_features: bad argument");
@@ -203,7 +202,6 @@ int mgb_debug_lpips_features(const void* ws, int32_t H, int32_t W, int32_t layer
   return MGB_OK;
 }
 
-/* debug hook (not in the public header): the same for the tapped layer `layer` (0 .. L - 1) of the handle's net. */
 int mgb_debug_lpips_net_features(const mgb_lpips* h, const void* ws, int32_t H, int32_t W, int32_t layer, float* dst_dev,
                                  int32_t dims_out[3]) {
   if (!h || !ws || !dims_out || layer < 0 || layer >= h->net->L || H < h->net->min_size || W < h->net->min_size) {
@@ -217,11 +215,7 @@ int mgb_debug_lpips_net_features(const mgb_lpips* h, const void* ws, int32_t H, 
   return MGB_OK;
 }
 
-/* debug hook (not in the public header): step `step` of the handle's net (-1: the prep operand). info_out = {op, input
- * step, output buffer's step, column, conv index (-1 for a pool), conv kind, tap (-1: none), h, w, ldo, nsteps}; with
- * dst_dev, copies the bf16 output buffer the step writes into, [2, h, w, ldo] (the prep operand of SqueezeNet: [2, 4, h,
- * w, 64]); MGB_ERR_INVALID when the step writes no bf16 output. */
-int mgb_debug_lpips_step(const mgb_lpips* h, const void* ws, int32_t H, int32_t W, int32_t step, bf16* dst_dev,
+int mgb_debug_lpips_step(const mgb_lpips* h, const void* ws, int32_t H, int32_t W, int32_t step, void* dst_dev,
                          int32_t info_out[11]) {
   if (!h || !ws || !info_out || step < -1 || step >= h->net->nsteps || H < h->net->min_size || W < h->net->min_size) {
     set_error("mgb_debug_lpips_step: bad argument");

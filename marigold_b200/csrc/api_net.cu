@@ -4,6 +4,7 @@
 #include <cstdlib>
 #include <cstring>
 
+#include "debug.h"
 #include "launch.h"
 #include "net.h"
 
@@ -547,15 +548,54 @@ static size_t weight_bytes(const mgb_handle* h) {
 constexpr size_t kDecodeContextBytes = size_t(768) << 20;
 constexpr size_t kDecodeReservePerPixel = 28;
 
+// The handle's row split (mgb_set_row_split) into a forward's context, or none
+static void set_split(const mgb_handle* h, Ctx& c) {
+  const mgb_handle::RowSplit& r = h->row_split;
+  c.split_world = r.fn ? r.world : 0;
+  c.split_rank = r.rank;
+  c.exchange_fn = r.fn;
+  c.exchange_ctx = r.ctx;
+}
+
+// The context of a real run on `stream`, in the handle's arena and workspaces
+static Ctx make_ctx(mgb_handle* h, void* stream) {
+  Ctx c;
+  c.stream = reinterpret_cast<cudaStream_t>(stream);
+  c.arena = &h->arena;
+  c.arena->base = h->arena_buf; c.arena->cap = h->arena_buf.bytes();
+  c.arena->dry = false; c.arena->status = MGB_OK; c.arena->plan = nullptr;
+  c.dry = false;
+  c.opt = h->opt;
+  c.splitk_ws = h->splitk_ws; c.splitk_cap = h->splitk_ws.bytes();
+  c.groups = h->cfg.norm_groups;
+  c.sync_base = h->sync_slab;
+  c.sync_cap = h->sync_slab.bytes() / sizeof(unsigned);
+  set_split(h, c);
+  return c;
+}
+
+// The context of a dry run: it launches nothing, records its allocations in *dry and sums its workspace needs
+static Ctx dry_ctx(const mgb_handle* h, Arena* dry) {
+  dry->dry = true;
+  Ctx c;
+  c.arena = dry;
+  c.dry = true;
+  c.opt = h->opt;
+  c.splitk_cap = ~size_t(0);
+  c.groups = h->cfg.norm_groups;
+  set_split(h, c);
+  return c;
+}
+
 // Whether a decode of lh x lw latents runs its full-resolution 256-channel stage in low memory (Ctx::dec_low_memory):
 // where one member's decode on the default path cannot be admitted on this device, i.e. needs more than its memory
 // less the weights, kDecodeContextBytes and kDecodeReservePerPixel per pixel. No decode that the default path could
 // run is moved, since each needs at least that much beside its workspace; or as mgb_debug_vae_low_memory sets it. The
 // decision depends on the shape and the VAE attention's row blocking alone, and is kept for the last shape asked.
 static int decode_low_memory(mgb_handle* h, int lh, int lw, bool* on) {
-  if (h->vae_low_memory != 0) { *on = h->vae_low_memory > 0; return MGB_OK; }
+  if (h->opt.low_memory != 0) { *on = h->opt.low_memory > 0; return MGB_OK; }
   mgb_handle::DecodeRule& k = h->decode_rule;
-  if (k.valid && k.lh == lh && k.lw == lw && k.attn_budget == h->vae_attn_budget && k.attn_rows == h->vae_attn_force_rows) {
+  if (k.valid && k.lh == lh && k.lw == lw && k.attn_budget == h->opt.attn_budget && k.attn_rows == h->opt.attn_rows) {
     *on = k.low_memory;
     return MGB_OK;
   }
@@ -564,9 +604,11 @@ static int decode_low_memory(mgb_handle* h, int lh, int lw, bool* on) {
     CUDA_TRY(cudaMemGetInfo(&free_b, &total));
     h->device_bytes = total;
   }
-  Arena dry; dry.dry = true;
-  Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
-  c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
+  Arena dry;
+  Ctx c = dry_ctx(h, &dry);
+  // the rule prices one member's whole decode on the default path: no rank's share of the rows, and no bands
+  c.split_world = 0;
+  c.opt.band_up_tiles = c.opt.band_conv1_tiles = 0;
   c.arena->start();
   c.planned = true;
   TRY(vae_decode_forward(h, c, nullptr, nullptr, 1, lh, lw, 0));
@@ -574,7 +616,7 @@ static int decode_low_memory(mgb_handle* h, int lh, int lw, bool* on) {
   const size_t need = arena_place(dry.rec, 0) + c.splitk_need;
   const size_t pixels = size_t(64) * lh * lw;
   *on = need + weight_bytes(h) + kDecodeContextBytes + kDecodeReservePerPixel * pixels > h->device_bytes;
-  k = {true, lh, lw, h->vae_attn_budget, h->vae_attn_force_rows, *on};
+  k = {true, lh, lw, h->opt.attn_budget, h->opt.attn_rows, *on};
   return MGB_OK;
 }
 
@@ -609,29 +651,17 @@ static int run_graph(mgb_handle* h, Ctx& c, int op, const float* a0, float* a1, 
 
 struct WorkspaceNeed { size_t arena = 0, splitk = 0, sync = 0; };   // bytes
 
-// The handle's row split (mgb_set_row_split) into a forward's context, or none
-static void set_split(const mgb_handle* h, Ctx& c) {
-  const mgb_handle::RowSplit& r = h->row_split;
-  c.split_world = r.fn ? r.world : 0;
-  c.split_rank = r.rank;
-  c.exchange_fn = r.fn;
-  c.exchange_ctx = r.ctx;
-}
-
 // Dry-runs one graph: its arena peak, split-K workspace and GroupNorm barrier counters. The VAE forwards' arena is
 // planned: their buffers, placed by lifetime (arena_place with the handle's placement), go to *bufs and the arena
 // peak is the plan's. The UNet step keeps the bump allocator's stack layout, which its captured graph holds; *bufs
 // then receives the buffers at their bump offsets.
 static int workspace_need(mgb_handle* h, int op, int NB, int d0, int d1, WorkspaceNeed* need,
                           std::vector<ArenaBuf>* bufs = nullptr) {
-  Arena dry; dry.dry = true;
-  Ctx c; c.arena = &dry; c.dry = true; c.groups = h->cfg.norm_groups; c.splitk_cap = ~size_t(0);
-  c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
-  c.band_up_tiles = h->vae_band_up_tiles; c.band_conv1_tiles = h->vae_band_conv1_tiles;
-  set_split(h, c);
+  Arena dry;
+  Ctx c = dry_ctx(h, &dry);
   TRY(run_graph(h, c, op, nullptr, nullptr, nullptr, nullptr, 0, NB, d0, d1, 0));
   dry.finish();
-  const size_t arena = op == OP_UNET ? dry.peak : arena_place(dry.rec, h->arena_placement);
+  const size_t arena = op == OP_UNET ? dry.peak : arena_place(dry.rec, h->opt.placement);
   *need = {arena, c.splitk_need, c.sync_need * sizeof(unsigned)};
   if (bufs) bufs->swap(dry.rec);
   return MGB_OK;
@@ -662,24 +692,6 @@ static int check_pixels(const char* what, int B, int H, int W) {
     return MGB_ERR_UNSUPPORTED;
   }
   return MGB_OK;
-}
-
-static Ctx make_ctx(mgb_handle* h, void* stream) {
-  Ctx c;
-  c.stream = reinterpret_cast<cudaStream_t>(stream);
-  c.arena = &h->arena;
-  c.arena->base = h->arena_buf; c.arena->cap = h->arena_buf.bytes();
-  c.arena->dry = false; c.arena->status = MGB_OK; c.arena->plan = nullptr;
-  c.dry = false;
-  c.poison = h->arena_poison;
-  c.splitk_ws = h->splitk_ws; c.splitk_cap = h->splitk_ws.bytes();
-  c.groups = h->cfg.norm_groups;
-  c.attn_budget = h->vae_attn_budget; c.attn_rows = h->vae_attn_force_rows;
-  c.band_up_tiles = h->vae_band_up_tiles; c.band_conv1_tiles = h->vae_band_conv1_tiles;
-  c.sync_base = h->sync_slab;
-  c.sync_cap = h->sync_slab.bytes() / sizeof(unsigned);
-  set_split(h, c);
-  return c;
 }
 
 // A row-split handle runs one image per call
@@ -973,10 +985,8 @@ int mgb_set_row_split(mgb_handle* h, int32_t rank, int32_t world, mgb_exchange_f
   return MGB_OK;
 }
 
-/* debug hooks (not in the public header) */
+/* debug hooks (declared in debug.h) */
 
-// Copies the device array behind one field (find_field's paths) into dst, when dst is not null, and returns its size in
-// bytes; *dev_addr receives its device address. It copies memory only: no kernel runs and no handle state changes.
 int64_t mgb_debug_read(mgb_handle* h, const char* field, void* dst, int64_t cap_bytes, uint64_t* dev_addr) {
   if (!h || !field) { set_error("debug_read: null argument"); return MGB_ERR_INVALID; }
   if (!h->finalized) { set_error("debug_read('%s') before finalize_weights", field); return MGB_ERR_STATE; }
@@ -994,7 +1004,6 @@ int64_t mgb_debug_read(mgb_handle* h, const char* field, void* dst, int64_t cap_
   return int64_t(r.bytes);
 }
 
-// Every device array the weights own (h->weights): addresses and sizes of the first `cap`; returns how many there are.
 int32_t mgb_debug_weight_buffers(mgb_handle* h, uint64_t* addr, int64_t* bytes, int32_t cap) {
   if (!h) { set_error("debug_weight_buffers: null handle"); return MGB_ERR_INVALID; }
   if (!h->finalized) { set_error("debug_weight_buffers before finalize_weights"); return MGB_ERR_STATE; }
@@ -1006,32 +1015,25 @@ int32_t mgb_debug_weight_buffers(mgb_handle* h, uint64_t* addr, int64_t* bytes, 
   return n;
 }
 
-// VAE mid-block attention row blocking of this handle: sets its workspace budget (budget_bytes <= 0: the library's,
-// kVaeAttnBudget) and forced rows per block (force_rows <= 0: none), then reports the rows per block (*rows) and the
-// blocks over all NB images (*blocks) that an (NB, T)-token attention of the VAE's width runs with.
 int mgb_debug_vae_attn_blocks(mgb_handle* h, int64_t budget_bytes, int32_t force_rows, int32_t NB, int32_t T,
                               int32_t* rows, int32_t* blocks) {
   if (!h || NB <= 0 || T <= 0) { set_error("debug_vae_attn_blocks: bad argument"); return MGB_ERR_INVALID; }
-  h->vae_attn_budget = budget_bytes > 0 ? size_t(budget_bytes) : kVaeAttnBudget;
-  h->vae_attn_force_rows = force_rows > 0 ? force_rows : 0;
-  const int R = vae_attn_rows(T, h->cfg.vae_block_channels[3], h->vae_attn_budget, h->vae_attn_force_rows);
+  h->opt.attn_budget = budget_bytes > 0 ? size_t(budget_bytes) : kVaeAttnBudget;
+  h->opt.attn_rows = force_rows > 0 ? force_rows : 0;
+  const int R = vae_attn_rows(T, h->cfg.vae_block_channels[3], h->opt.attn_budget, h->opt.attn_rows);
   if (rows) *rows = R;
   if (blocks) *blocks = NB * ((T + R - 1) / R);
   return MGB_OK;
 }
 
-// The VAE mid-block attention's core (vae_attn_core) alone, as vae_attn_forward runs it: bf16 q, k, v [NB * T, C] ->
-// bf16 o, C = the VAE's mid-block width, in this handle's arena and split-K workspace (grown to a dry pass's need) with
-// the row blocking mgb_debug_vae_attn_blocks set, on the default stream.
 int mgb_debug_vae_attn_core(mgb_handle* h, const void* q, const void* k, const void* v, void* o, int32_t NB,
                             int32_t T) {
   TRY(check_ready(h, false));
   if (!q || !k || !v || !o || NB <= 0 || T <= 0) { set_error("debug_vae_attn_core: bad argument"); return MGB_ERR_INVALID; }
   const int C = h->cfg.vae_block_channels[3];
   auto in = [](const void* p) { return reinterpret_cast<const bf16*>(p); };
-  Arena dry; dry.dry = true;
-  Ctx d; d.arena = &dry; d.dry = true; d.splitk_cap = ~size_t(0);
-  d.attn_budget = h->vae_attn_budget; d.attn_rows = h->vae_attn_force_rows;
+  Arena dry;
+  Ctx d = dry_ctx(h, &dry);
   TRY(vae_attn_core(d, in(q), in(k), in(v), reinterpret_cast<bf16*>(o), NB, T, C));
   TRY(grow_captured(h, h->arena_buf, dry.peak + (1 << 20)));
   TRY(grow_captured(h, h->splitk_ws, d.splitk_need));
@@ -1041,36 +1043,26 @@ int mgb_debug_vae_attn_core(mgb_handle* h, const void* q, const void* k, const v
   return h->arena.status;
 }
 
-// Debug switches of this handle's arena: poison != 0 fills every buffer a forward's arena hands out with 0xFF bytes
-// (NaN in fp32 and bf16) before the forward uses it; placement is arena_place's placement of the VAE forwards' plans
-// (0: the library's, 1: first fit in reverse allocation order). No result may depend on either.
 int mgb_debug_arena(mgb_handle* h, int32_t poison, int32_t placement) {
   if (!h || placement < 0 || placement > 1) { set_error("debug_arena: bad argument"); return MGB_ERR_INVALID; }
-  h->arena_poison = poison != 0;
-  h->arena_placement = placement;
+  h->opt.poison = poison != 0;
+  h->opt.placement = placement;
   return MGB_OK;
 }
 
-// The decoder's full-resolution stage of this handle: mode 1 runs it in low memory (the banded up-conv into two halves
-// and the first resnet on them) at every size, -1 never, 0 where the library's rule (decode_low_memory) asks for it.
-// Outputs are the same bits either way.
 int mgb_debug_vae_low_memory(mgb_handle* h, int32_t mode) {
   if (!h || mode < -1 || mode > 1) { set_error("debug_vae_low_memory: bad argument"); return MGB_ERR_INVALID; }
-  h->vae_low_memory = mode;
+  h->opt.low_memory = mode;
   return MGB_OK;
 }
 
-// Tile rows per band of the low-memory decoder's banded up-conv and conv1 on this handle (<= 0: the library's choice,
-// about an eighth of the image). Outputs are the same bits at every band height.
 int mgb_debug_vae_bands(mgb_handle* h, int32_t up_tiles, int32_t conv1_tiles) {
   if (!h) { set_error("debug_vae_bands: bad argument"); return MGB_ERR_INVALID; }
-  h->vae_band_up_tiles = std::max(0, int(up_tiles));
-  h->vae_band_conv1_tiles = std::max(0, int(conv1_tiles));
+  h->opt.band_up_tiles = std::max(0, int(up_tiles));
+  h->opt.band_conv1_tiles = std::max(0, int(conv1_tiles));
   return MGB_OK;
 }
 
-// arena_place on n buffers, a pure host function: sizes and lifetimes [t_alloc, t_free) in, offsets out. Returns the
-// peak, or a negative status.
 int64_t mgb_debug_arena_place(int64_t n, const int64_t* bytes, const int64_t* t_alloc, const int64_t* t_free,
                               int32_t placement, int64_t* off) {
   if (n < 0 || (n > 0 && (!bytes || !t_alloc || !t_free || !off)) || placement < 0 || placement > 1) {
@@ -1091,9 +1083,6 @@ int64_t mgb_debug_arena_place(int64_t n, const int64_t* bytes, const int64_t* t_
   return int64_t(peak);
 }
 
-// The arena of one forward at this shape (op 0: UNet step on a d0 x d1 latent, 1: encode of d0 x d1 pixels, 2: decode
-// of a d0 x d1 latent), as workspace_need lays it out: per buffer in allocation order its size, lifetime and offset,
-// for the first `cap` buffers. Returns the buffer count, or a negative status.
 int64_t mgb_debug_arena_plan(mgb_handle* h, int32_t op, int32_t B, int32_t d0, int32_t d1, int64_t* bytes,
                              int64_t* t_alloc, int64_t* t_free, int64_t* off, int64_t cap) {
   if (!h || op < OP_UNET || op > OP_DECODE || B <= 0 || d0 <= 0 || d1 <= 0) {

@@ -3,6 +3,7 @@
 #include <cstdio>
 #include <cstring>
 
+#include "debug.h"
 #include "device.h"
 #include "kernels.h"
 #include "launch.h"
@@ -29,9 +30,8 @@ const char* mgb_build_info(void) {
          "SWIZZLE_128B, mbarrier pipelines; no CPU fallback";
 }
 int64_t mgb_launch_count(void) { return launch_count(); }
-/* debug hook (not in the public header): per-CTA clock64 phase stamps of subsequent GEMM launches */
+/* debug hooks (declared in debug.h) */
 void mgb_debug_gemm_timing(void* dev_buffer) { set_gemm_debug_buffer(reinterpret_cast<long long*>(dev_buffer)); }
-/* debug hook (not in the public header): bytes of device and pinned host memory the library's buffers hold now */
 int64_t mgb_debug_live_device_bytes(void) { return g_live_bytes.load(); }
 
 static void fill_epi(GemmEpilogue* e, const float* bias, const float* residual, float* out_f32, void* out_bf16,
@@ -153,9 +153,7 @@ int mgb_op_groupnorm_ex(const float* xa, int32_t Ca, const float* xb, int32_t Cb
                          G, eps, silu, ws, counters, s);
 }
 
-// GroupNorm in two launches over the concat [a | b] of two packed fp32 maps of Ch channels each, in their own memory as
-// the decoder's low-memory resnet runs it: raw = bf16([a | b]) [NB * HW, 2 Ch] over a, y [NB * HW, 2 Ch] over b.
-// ws: mgb_op_groupnorm_ws_bytes(NB, HW, 2 Ch, G); stats: NB * 2 Ch float2.
+// debug hook (debug.h)
 int mgb_debug_groupnorm_halves(float* a, float* b, int32_t Ch, const float* gamma, const float* beta, float* ws,
                                void* stats, int32_t NB, int32_t HW, int32_t G, float eps, int32_t silu, void* stream) {
   if (!a || !b || !ws || !stats || Ch <= 0) { set_error("debug_groupnorm_halves: bad argument"); return MGB_ERR_INVALID; }
@@ -172,11 +170,7 @@ int mgb_debug_groupnorm_halves(float* a, float* b, int32_t Ch, const float* gamm
                               s);
 }
 
-// One band of the decoder's banded 3x3 pad-1 convs (net.cu, conv3x3_band): tile rows [ty0, ty0 + tiles) of one
-// H x W image, with the tile the network gives the whole conv over NB_tile such images. x: bf16 [src_rows, W, Cin],
-// image rows [src_y0, src_y0 + src_rows); output pixel (y, x) to fp32 row (y - out_y0) W + x at a row stride of ldo,
-// columns >= split_col to out_hi (or null: all to out). geom (or null) receives {tile_h, tiles_y}; x == null only
-// fills it.
+// debug hook (debug.h)
 int mgb_debug_conv2d_band(const void* x, int32_t src_y0, int32_t src_rows, const void* w, const float* bias, float* out,
                           float* out_hi, int32_t split_col, int32_t ldo, int32_t out_y0, int32_t NB_tile, int32_t H,
                           int32_t W, int32_t Cin, int32_t Cout, int32_t ty0, int32_t tiles, int32_t* geom, void* stream) {

@@ -135,7 +135,7 @@ static T* aalloc(Ctx& c, size_t n) {
   if (c.dry) return reinterpret_cast<T*>(p);
   if (!p) {
     c.dry = true;
-  } else if (c.poison && cudaMemsetAsync(p, 0xFF, n * sizeof(T), c.stream) != cudaSuccess) {
+  } else if (c.opt.poison && cudaMemsetAsync(p, 0xFF, n * sizeof(T), c.stream) != cudaSuccess) {
     set_error("arena poison memset failed");
     c.arena->status = MGB_ERR_CUDA;
     c.dry = true;
@@ -411,7 +411,7 @@ static int up_conv_low_memory(Ctx& c, const ConvW& Wt, Act& h, Act& partner, Act
   b = act_alloc(c, size_t(NB) * HW, half);
   int th, tiles_y;
   const Tile t = conv_tile(NB, H, W, Wt, 0, &th, &tiles_y);
-  const int bt = band_tiles(tiles_y, c.band_up_tiles);
+  const int bt = band_tiles(tiles_y, c.opt.band_up_tiles);
   bf16* band = aalloc<bf16>(c, size_t(std::min(H, bt * th + 2)) * W * cin);
   Epi e; e.bias = Wt.b; e.split_col = half;
   for (int n = 0; n < NB; ++n) {
@@ -455,7 +455,7 @@ static int resnet_shortcut_halves(Ctx& c, const ResnetW& R, Act& a, Act& b, Act&
   c.arena->free(st);
   int th, tiles_y;
   const Tile t = conv_tile(NB, H, W, R.c1, 0, &th, &tiles_y);
-  const int bt = band_tiles(tiles_y, c.band_conv1_tiles);
+  const int bt = band_tiles(tiles_y, c.opt.band_conv1_tiles);
   const size_t band_px = size_t(std::min(H, bt * th)) * W;
   float* stage[2] = {aalloc<float>(c, band_px * cout), aalloc<float>(c, band_px * cout)};
   Epi e1;
@@ -593,7 +593,7 @@ int vae_attn_core(Ctx& c, const bf16* q, const bf16* k, const bf16* v, bf16* o, 
                   int row_end) {
   if (row_end < 0) row_end = T;
   const int Tp = (T + 63) / 64 * 64;
-  const int R = vae_attn_rows(T, C, c.attn_budget, c.attn_rows);
+  const int R = vae_attn_rows(T, C, c.opt.attn_budget, c.opt.attn_rows);
   const Tile tile_s = matmul_tile(T, T, C, EPI_SCALE), tile_pv = matmul_tile(T, C, Tp, 0);
   const size_t mk = c.arena->mark();
   bf16* vt = aalloc<bf16>(c, size_t(C) * Tp);

@@ -126,16 +126,31 @@ constexpr size_t kVaeAttnBudget = size_t(2) << 30;
 // of the SMs. force_rows > 0 overrides the choice (tests).
 int vae_attn_rows(int T, int C, size_t budget, int force_rows);
 
+// A handle's settings of its forwards: the library's defaults unless a debug hook (debug.h) sets them. Each forward's
+// Ctx holds a copy.
+struct ForwardOptions {
+  // VAE mid-block attention row blocking: vae_attn_rows' budget and forced rows (mgb_debug_vae_attn_blocks)
+  size_t attn_budget = kVaeAttnBudget;
+  int attn_rows = 0;
+  // fill every buffer the arena hands out with 0xFF bytes (NaN in fp32 and bf16) first; arena_place's placement of the
+  // VAE forwards' plans (mgb_debug_arena)
+  bool poison = false;
+  int placement = 0;
+  // The decoder's full-resolution stage in low memory (Ctx::dec_low_memory): 0 where one member's default decode does
+  // not fit the device beside the weights (decode_low_memory, api_net.cu), 1 always, -1 never (mgb_debug_vae_low_memory)
+  int low_memory = 0;
+  // Tile rows per band of the low-memory decoder's banded up-conv and conv1: 0 the library's choice, else forced
+  // (mgb_debug_vae_bands)
+  int band_up_tiles = 0, band_conv1_tiles = 0;
+};
+
 struct Ctx {
   cudaStream_t stream = nullptr;
   Arena* arena = nullptr;
   bool dry = false;
-  size_t attn_budget = kVaeAttnBudget;  // vae_attn_rows' budget and forced rows (mgb_handle's, see there)
-  int attn_rows = 0;
+  ForwardOptions opt;      // the handle's
   bool planned = false;    // the arena is lifetime-planned (the VAE forwards): buffers are freed after their last read
-  bool poison = false;     // fill every buffer the arena hands out with 0xFF bytes (NaN in fp32 and bf16) first
   bool dec_low_memory = false;   // the decoder's full-resolution 256-channel stage runs in 2.5 U (net.cu)
-  int band_up_tiles = 0, band_conv1_tiles = 0;   // its bands' tile rows (0: the library's choice; mgb_handle's)
   float* splitk_ws = nullptr;
   size_t splitk_cap = 0;   // bytes available
   size_t splitk_need = 0;  // bytes needed (dry run)
@@ -156,7 +171,7 @@ struct Ctx {
 inline int row_split_chunk(int T, int world) { return ((T + 127) / 128 + world - 1) / world * 128; }
 
 // The VAE mid-block attention between its projections: o = softmax(q k^T / sqrt(C)) v per image, on bf16 q, k, v, o
-// [NB * T, C], in blocks of vae_attn_rows(T, C, c.attn_budget, c.attn_rows) query rows. Its scratch (V^T, one block's
+// [NB * T, C], in blocks of vae_attn_rows(T, C, c.opt.attn_budget, c.opt.attn_rows) query rows. Its scratch (V^T, one block's
 // fp32 scores and bf16 probabilities) comes from the arena and is released on return.
 // Query rows [row_begin, row_end) only (row_end < 0: through T), in the blocks and tiles of the whole T-row problem,
 // so each row is bit-identical to the whole call's; row_begin a multiple of 128 (or of the block rows).
@@ -202,17 +217,9 @@ struct mgb_handle {
   mgb::Arena arena;                 // view of arena_buf, refreshed by each call that runs a graph
   mgb::DevBuf<float> splitk_ws;
   mgb::DevBuf<unsigned> sync_slab;  // GroupNorm grid-barrier counters of one forward
-  // VAE mid-block attention row blocking: the library's budget unless a test overrides it (mgb_debug_vae_attn_blocks)
-  size_t vae_attn_budget = mgb::kVaeAttnBudget;
-  int vae_attn_force_rows = 0;
+  mgb::ForwardOptions opt;
   // The VAE forwards' arena plan: placed by the dry run that sizes each call's workspace, replayed by its real run.
-  // arena_placement and arena_poison are arena_place's placement and Ctx::poison (mgb_debug_arena).
   std::vector<mgb::ArenaBuf> arena_plan;
-  int arena_placement = 0;
-  bool arena_poison = false;
-  // The decoder's full-resolution stage in low memory (Ctx::dec_low_memory): 0 where one member's default decode does
-  // not fit the device beside the weights (decode_low_memory, api_net.cu), 1 always, -1 never (mgb_debug_vae_low_memory)
-  int vae_low_memory = 0;
   size_t device_bytes = 0;          // the device's memory, read once
   struct DecodeRule {                // the rule's last decision (decode_low_memory)
     bool valid = false;
@@ -221,9 +228,6 @@ struct mgb_handle {
     int attn_rows = 0;
     bool low_memory = false;
   } decode_rule;
-  // Tile rows per band of the low-memory decoder's banded up-conv and conv1 (Ctx::band_up_tiles): 0 the library's
-  // choice, else forced (mgb_debug_vae_bands)
-  int vae_band_up_tiles = 0, vae_band_conv1_tiles = 0;
   // row split (mgb_set_row_split): installed while fn != null
   struct RowSplit {
     int rank = 0, world = 0;

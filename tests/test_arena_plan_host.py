@@ -21,13 +21,7 @@ PEAK_SLACK = 1.15
 def place():
     from marigold_b200 import _lib
 
-    lib = C.CDLL(str(_lib.lib_path())) if _lib.lib_path().exists() else None
-    if lib is None:
-        _lib.load()          # builds (nvcc cross-compiles without a GPU)
-        lib = C.CDLL(str(_lib.lib_path()))
-    f = lib.mgb_debug_arena_place
-    f.restype = C.c_int64
-    f.argtypes = [C.c_int64] + [C.POINTER(C.c_int64)] * 3 + [C.c_int32, C.POINTER(C.c_int64)]
+    f = _lib.load().mgb_debug_arena_place   # builds when missing (nvcc cross-compiles without a GPU)
 
     def run(nbytes, t0, t1, placement=0):
         arrs = [np.ascontiguousarray(a, dtype=np.int64) for a in (nbytes, t0, t1)]

@@ -23,7 +23,7 @@ import pytest
 import torch
 
 from tests import net_ref as N
-from tests.helpers import engine_from_oracle, oracle_models, record, rel_err
+from tests.helpers import engine_from_oracle, oracle_models, record, rel_err, weight_bytes
 
 pytestmark = pytest.mark.gpu
 
@@ -220,15 +220,6 @@ def test_iid_3_targets_nb6():
 
 
 # ---- memory -------------------------------------------------------------------------------------------------------------
-def _weight_bytes(eng):
-    import ctypes as C
-
-    f = eng.lib.mgb_debug_weight_buffers
-    f.restype, f.argtypes = C.c_int32, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_int64), C.c_int32]
-    n = f(eng._h, None, None, 0)
-    size = (C.c_int64 * n)()
-    assert f(eng._h, None, size, n) == n
-    return sum(size)
 
 
 # 80 GB card; 6 GiB are left for the CUDA context, the caller's tensors (inputs, outputs, the ensemble) and fragmentation
@@ -243,7 +234,7 @@ def test_workspace_fits_at_the_batch_caps(sd2):
     fails = []
     iid3 = _iid_engine()
     for name, e in (("depth", sd2[0]), ("iid3", iid3)):
-        wb = _weight_bytes(e)
+        wb = weight_bytes(e)
         record(f"batch/workspace/{name}/weights_gib", wb / GIB)
         for H, W in ((768, 768), (432, 768), (768, 432), (1024, 1024), (576, 1024), (1024, 576)):
             B = find_batch_size(64, max(H, W), torch.float32)

@@ -5,7 +5,7 @@ import torch
 
 from marigold_b200.pipeline import (MarigoldDepthPipeline, MarigoldIIDPipeline, MarigoldNormalsPipeline,
                                     call_reserve_bytes, find_batch_size, select_batch_size)
-from tests.test_native_res_host import GB, StubEngine
+from tests.helpers import GB, StubEngine
 
 
 def test_zero_reserve_is_the_default():

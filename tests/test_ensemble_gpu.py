@@ -12,27 +12,10 @@ import pytest
 import torch
 
 from tests.golden.cases import DEPTH_CASES, NORMALS_CASES, depth_input, normals_input
+from tests.helpers import _ref_cost
 
 pytestmark = pytest.mark.gpu
 GOLD = np.load(__file__.rsplit("/", 1)[0] + "/golden/ensemble_golden.npz")
-
-
-def _ref_cost(d, p, shift, reduction, reg):
-    """reference cost_fn (ensemble.py:138-152) restated with torch CPU ops."""
-    E = d.shape[0]
-    if shift:
-        s, t = np.split(p, 2)
-        a = d * torch.from_numpy(s).float().view(E, 1, 1, 1) + torch.from_numpy(t).float().view(E, 1, 1, 1)
-    else:
-        a = d * torch.from_numpy(p).float().view(E, 1, 1, 1)
-    c = 0.0
-    for i in range(E):
-        for j in range(i + 1, E):
-            c += ((a[i] - a[j]) ** 2).mean().sqrt().item()
-    if reg > 0:
-        pr = a.median(0).values if reduction == "median" else a.mean(0)
-        c += (abs(0.0 - pr.min().item()) + abs(1.0 - pr.max().item())) * reg
-    return c
 
 
 @pytest.mark.parametrize("name", list(DEPTH_CASES))

@@ -6,7 +6,7 @@ import torch
 
 from tests import ensemble_ref as R
 from tests.golden.cases import (DEPTH_CASES, IID_CASES, NORMALS_CASES, depth_input, iid_input, normals_input)
-from tests.test_ensemble_gpu import _ref_cost
+from tests.helpers import _ref_cost
 
 _DIR = __file__.rsplit("/", 1)[0] + "/golden/"
 GOLD = np.load(_DIR + "ensemble_golden.npz")

@@ -1,11 +1,9 @@
 """One engine handle over its life: the device memory it owns is all released by close(), its cached CUDA graph of a
 UNet step follows the buffers it captured, and a call rejected for its arguments leaves the handle as it was."""
-import ctypes as C
-
 import pytest
 import torch
 
-from tests.helpers import engine_from_oracle, oracle_models
+from tests.helpers import engine_from_oracle, live_device_bytes, oracle_models
 
 pytestmark = pytest.mark.gpu
 
@@ -13,15 +11,6 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def models():
     return oracle_models("tiny")
-
-
-def _live_bytes() -> int:
-    """Device and pinned host bytes the library's buffers hold (a debug hook outside the public header)."""
-    from marigold_b200 import _lib
-
-    fn = _lib.load().mgb_debug_live_device_bytes
-    fn.restype, fn.argtypes = C.c_int64, []
-    return int(fn())
 
 
 def _ddim(eng, n):
@@ -47,7 +36,7 @@ def test_close_releases_every_buffer_the_handle_allocated(models):
 
     ends = []
     for cycle in range(2):
-        start = _live_bytes()
+        start = live_device_bytes()
         eng = engine_from_oracle(*models)
         for n in (4, 10, 4):
             _ddim(eng, n)
@@ -57,9 +46,9 @@ def test_close_releases_every_buffer_the_handle_allocated(models):
         depth = eng.decode(x, 0)
         ensemble_depth(torch.cat([depth, depth.flip(-1), depth.flip(-2)]), engine=eng)   # E = 3: the ensemble scratch
         torch.cuda.synchronize()
-        assert _live_bytes() > start
+        assert live_device_bytes() > start
         eng.close()
-        ends.append(_live_bytes())
+        ends.append(live_device_bytes())
         assert ends[-1] == start, f"cycle {cycle}: {ends[-1] - start} bytes still held after close()"
     assert ends[0] == ends[1]
 
@@ -69,9 +58,9 @@ def test_step_graph_is_rebuilt_when_a_captured_buffer_moves(models):
     _ddim(eng, 4)
     rgb, x = _latents()
     a = eng.denoise(rgb, x)
-    before = _live_bytes()
+    before = live_device_bytes()
     eng.encode(_image(2, 256, 5))                              # the arena is reallocated, larger
-    assert _live_bytes() > before
+    assert live_device_bytes() > before
     _ddim(eng, 10)
     _ddim(eng, 4)                                              # sched_k and the bias table are reallocated
     b = eng.denoise(rgb, x)

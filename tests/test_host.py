@@ -71,20 +71,34 @@ def test_lcm_coefficients_match_oracle_step(n):
     assert kz[-1] == 0 and (kz[:-1] > 0).all()
 
 
+def _declarations(header: Path) -> dict:
+    """name -> (return type, parameter count) of every mgb_* function a C header declares."""
+    src = re.sub(r"/\*.*?\*/", " ", header.read_text(), flags=re.S)
+    src = re.sub(r"//[^\n]*", " ", src)
+    decls = re.findall(r"^\s*((?:const\s+)?\w+\s*\**)\s*\b(mgb_\w+)\s*\(([^()]*)\)\s*;", src, flags=re.M)
+    return {name: (ret.strip(), 0 if " ".join(args.split()) in ("", "void") else args.count(",") + 1)
+            for ret, name, args in decls}
+
+
 def test_library_exports_every_declared_symbol():
     from marigold_b200 import _lib
 
-    header = (ROOT / "include" / "marigold_b200.h").read_text()
-    declared = set(re.findall(r"\b(mgb_[a-z0-9_]+)\s*\(", header))
-    declared -= {"mgb_status", "mgb_dtype", "mgb_decode_mode"}
-    assert declared, "no declarations parsed"
+    public = _declarations(ROOT / "include" / "marigold_b200.h")
+    debug = _declarations(ROOT / "marigold_b200" / "csrc" / "debug.h")
+    assert public and debug, "no declarations parsed"
     lib = ctypes.CDLL(str(_lib.lib_path())) if _lib.lib_path().exists() else None
     if lib is None:
         _lib.load()          # builds (nvcc cross-compiles without a GPU)
         lib = ctypes.CDLL(str(_lib.lib_path()))
-    missing = [s for s in sorted(declared) if not hasattr(lib, s)]
-    assert not missing, f"header declares symbols the library does not export: {missing}"
-    assert declared == set(_lib.SIGNATURES), "ctypes SIGNATURES out of sync with include/marigold_b200.h"
+    missing = [s for s in sorted({**public, **debug}) if not hasattr(lib, s)]
+    assert not missing, f"headers declare symbols the library does not export: {missing}"
+    assert set(public) == set(_lib.SIGNATURES), "ctypes SIGNATURES out of sync with include/marigold_b200.h"
+    assert set(debug) == set(_lib.DEBUG_SIGNATURES), "ctypes DEBUG_SIGNATURES out of sync with csrc/debug.h"
+    for decls, table in ((public, _lib.SIGNATURES), (debug, _lib.DEBUG_SIGNATURES)):
+        for name, (ret, nargs) in decls.items():
+            res, args = table[name]
+            assert len(args) == nargs, f"{name}: {nargs} parameters declared, {len(args)} bound"
+            assert (ret == "void") == (res is None), f"{name}: returns {ret}, bound to return {res}"
     loaded = _lib.load()
     assert b"sm_90a" in loaded.mgb_build_info()
 

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from tests import iid_eval_ref, lpips_ref, ops_ref
-from tests.golden.iid_eval_cases import iid_eval_input
+from tests.helpers import CONFIGS, _inputs, _launches, live_device_bytes
 
 pytestmark = pytest.mark.gpu
 pytest.importorskip("torchvision")
@@ -23,28 +23,6 @@ IID_LAUNCHES = {False: 2, True: 6}
 SCALAR_TOL_64, SCALAR_TOL_32 = 5e-6, 5e-4
 HEAD_TOL = 1e-6              # relative: the device head (double) against the float64 head on the device's own features
 FEATURE_SIZES = [(31, 31), (77, 131), (481, 642), (480, 640), (1080, 1920)]
-# (target, mask, transform, kind): see tests/golden/iid_eval_cases.py
-CONFIGS = [
-    ("albedo", "none", None, "noisy"),
-    ("material", "pixel", "srgb2linear", "noisy"),
-    ("shading", "split", "linear2srgb", "noisy"),
-    ("residual", "pixel", None, "q255"),
-    ("shading", "none", "srgb2linear", "q255"),
-    ("residual", "split", None, "nan"),
-    ("albedo", "split", "linear2srgb", "nan"),
-    ("shading", "single", None, "noisy"),
-    ("residual", "none", None, "dark"),
-    ("albedo", "empty", None, "noisy"),
-]
-
-
-def _inputs(H, W, target, mask, transform, kind, seed=0):
-    """CUDA (pred, gt, mask); the non-scale targets' predictions clipped to [0, 1], as LPIPS requires."""
-    cfg = dict(H=H, W=W, seed=1000 + seed + H + W, target=target, mask=mask, transform=transform, kind=kind)
-    pred, gt, m = iid_eval_input(cfg)
-    if target not in iid_eval_ref.UP_TO_SCALE:
-        pred = np.clip(pred, 0.0, 1.0)
-    return (torch.from_numpy(pred).cuda(), torch.from_numpy(gt).cuda(), torch.from_numpy(m).cuda() if m is not None else None)
 
 
 @pytest.fixture(scope="module")
@@ -81,9 +59,7 @@ def _debug_features(lp, H, W):
     """The five fp32 feature maps of the last call, NCHW float64 [2, C, h, w] (pred, gt)."""
     from marigold_b200 import _lib
 
-    lib = _lib.load()
-    fn = lib.mgb_debug_lpips_features
-    fn.restype, fn.argtypes = C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(C.c_int32)]
+    fn = _lib.load().mgb_debug_lpips_features
     dims = (C.c_int32 * 3)()
     out = []
     for l in range(5):
@@ -92,16 +68,6 @@ def _debug_features(lp, H, W):
         _lib.check(fn(_lib.ptr(lp._ws), H, W, l, _lib.ptr(t), dims), "mgb_debug_lpips_features")
         out.append(t.permute(0, 3, 1, 2).to(torch.float64))
     return out
-
-
-def _launches(fn):
-    from marigold_b200 import _lib
-
-    lib = _lib.load()
-    torch.cuda.synchronize()
-    l0 = lib.mgb_launch_count()
-    r = fn()
-    return r, lib.mgb_launch_count() - l0
 
 
 # ---- the new conv kinds and EPI_RELU ---------------------------------------------------------------------------------
@@ -311,12 +277,9 @@ LPIPS_LAUNCHES = {(31, 31): 14, (77, 131): 14, (480, 640): 12, (1080, 1920): 10}
 
 
 def test_handle_memory(weights):
-    from marigold_b200 import _lib
     from marigold_b200.evaluation import LPIPS
 
-    lib = _lib.load()
-    fn = lib.mgb_debug_live_device_bytes
-    fn.restype, fn.argtypes = C.c_int64, []
+    fn = live_device_bytes
     b0 = fn()
     h = LPIPS(*weights, device="cuda")
     bf16_bytes = 2 * (64 * 9 * 64 + 192 * 25 * 64 + 384 * 9 * 192 + 256 * 9 * 384 + 256 * 9 * 256)

@@ -12,7 +12,7 @@ import torch
 import torch.nn.functional as F
 
 from tests import lpips_nets_ref, lpips_ref, ops_ref
-from tests.test_lpips_gpu import CONFIGS, _inputs, _launches
+from tests.helpers import CONFIGS, _inputs, _launches, live_device_bytes
 
 pytestmark = pytest.mark.gpu
 pytest.importorskip("torchvision")
@@ -64,20 +64,11 @@ def _eval(pred, gt, target, mask, transform, lp):
     return evaluate_iid(pred, gt, target, mask, transform, lpips=lp)
 
 
-def _hook(name, args):
-    from marigold_b200 import _lib
-
-    fn = getattr(_lib.load(), name)
-    fn.restype, fn.argtypes = C.c_int32, args
-    return fn
-
-
 def _step(lp, H, W, s, copy=True):
     """(info dict, the bf16 output buffer of step s as float64 NHWC [2, h, w, ldo] or None)."""
     from marigold_b200 import _lib
 
-    fn = _hook("mgb_debug_lpips_step", [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
-                                        C.POINTER(C.c_int32)])
+    fn = _lib.load().mgb_debug_lpips_step
     info = (C.c_int32 * 11)()
     _lib.check(fn(lp._h, _lib.ptr(lp._ws), H, W, s, None, info), "mgb_debug_lpips_step")
     d = dict(zip(("op", "in", "buf", "col", "conv", "kind", "tap", "h", "w", "ldo", "nsteps"), list(info)))
@@ -93,8 +84,7 @@ def _step(lp, H, W, s, copy=True):
 def _features(lp, H, W, layer):
     from marigold_b200 import _lib
 
-    fn = _hook("mgb_debug_lpips_net_features", [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
-                                                C.POINTER(C.c_int32)])
+    fn = _lib.load().mgb_debug_lpips_net_features
     dims = (C.c_int32 * 3)()
     _lib.check(fn(lp._h, _lib.ptr(lp._ws), H, W, layer, None, dims), "mgb_debug_lpips_net_features")
     t = torch.empty(2, dims[0], dims[1], dims[2], device="cuda")
@@ -294,8 +284,7 @@ def test_handle_memory(net_type):
     from marigold_b200 import _lib
     from marigold_b200.evaluation import LPIPS, LPIPS_NETS
 
-    fn = _hook("mgb_debug_live_device_bytes", [])
-    fn.restype = C.c_int64
+    fn = live_device_bytes
     sd, lin = lpips_nets_ref.fabricated_weights(net_type, 0)
     b0 = fn()
     h = LPIPS(sd, lin, device="cuda", net_type=net_type)

@@ -10,10 +10,8 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from marigold_b200 import parallel
-from marigold_b200.pipeline import (MarigoldDepthPipeline, MarigoldNormalsPipeline, find_batch_size,
-                                    noise_draw_batches, select_list_batch_size, size_groups)
-from marigold_b200.schedulers import DDIMScheduler, LCMScheduler
-from tests.test_native_res_host import GB, StubEngine
+from marigold_b200.pipeline import find_batch_size, noise_draw_batches, select_list_batch_size, size_groups
+from tests.helpers import GB, StubEngine, _expected, _images, _pipe, _run
 
 
 def test_rounds_partition_the_jobs():
@@ -93,76 +91,6 @@ def test_list_batch_reserves_the_open_images(monkeypatch):
 
 
 # ---- the list driver on a stub engine ------------------------------------------------------------------------------
-
-class _Cfg:
-    unet_out_channels = 4
-
-
-class _Lib:
-    @staticmethod
-    def mgb_ens_max_members():
-        return 64
-
-
-class FakeEngine:
-    """encode: a per-image constant latent; denoise: rgb_latent + z0 (+ the step noise's sum); decode: the first channel,
-    8x nearest. Every member map is therefore a known function of its own image and noise. Records the batch shapes."""
-    cfg, lib, device = _Cfg(), _Lib(), torch.device("cpu")
-
-    def __init__(self):
-        self.log = []
-
-    def set_text_embedding(self, t):
-        pass
-
-    def set_schedule(self, *a):
-        pass
-
-    def workspace_bytes(self, B, H, W):
-        return GB
-
-    def held_bytes(self):
-        return 0
-
-    def encode(self, rgb):
-        self.log.append(("encode",))
-        return rgb.mean().reshape(1, 1, 1, 1).expand(1, 4, rgb.shape[-2] // 8, rgb.shape[-1] // 8).contiguous()
-
-    def denoise(self, rl, z, sn=None):
-        self.log.append(("denoise", tuple(z.shape)))
-        return rl + z + (sn.sum(0) if sn is not None else 0)
-
-    def decode(self, t, mode):
-        return t[:, :1].repeat_interleave(8, 2).repeat_interleave(8, 3)
-
-
-def _pipe(lcm=False, normals=False):
-    cls = MarigoldNormalsPipeline if normals else MarigoldDepthPipeline
-    pipe = cls(FakeEngine(), LCMScheduler() if lcm else DDIMScheduler(), None)
-    pipe._preprocess = lambda im, pr, rs: (im.float() / 255 * 2 - 1, im.shape)
-    return pipe
-
-
-def _images(sizes):
-    g = torch.Generator().manual_seed(3)
-    return [torch.randint(0, 256, (1, 3, h, w), generator=g, dtype=torch.uint8) for h, w in sizes]
-
-
-def _expected(img, z, sn):
-    lat = (img.float() / 255 * 2 - 1).mean()
-    t = lat + z + (sn.sum(0) if sn is not None else 0)
-    return t[:, :1].repeat_interleave(8, 2).repeat_interleave(8, 3)
-
-
-def _run(pipe, images, E, steps, bs, generator=None, noise=None, step_noise=None):
-    done, log = {}, pipe.engine.log
-
-    def finish(i, maps, hw):
-        log.append(("finish", i))
-        done[i] = maps.clone()
-
-    pipe._infer_list(images, E, steps, 0, "bilinear", bs, generator, noise, step_noise, 0, finish)
-    return done
 
 
 @pytest.fixture(autouse=True)

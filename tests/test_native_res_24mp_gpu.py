@@ -22,7 +22,6 @@
   * the pipelines at processing_res=0 on a 6048 x 4032 photo: depth with E = 2 and uncertainty, normals with E = 2, a
     2-target IID model with E = 1; 8192 x 8192 is still refused before any work."""
 import copy
-import ctypes as C
 import gc
 
 import numpy as np
@@ -30,59 +29,15 @@ import pytest
 import torch
 
 from tests import ops_ref as R
-from tests.helpers import engine_from_oracle, oracle_models, record, rel_err, synthetic_image
+from tests.helpers import (U_PER_PIXEL, VAE_C, _block_rows, _core_inputs, _core_ref, _photo, arena_place, arena_plan,
+                           attn_blocks, attn_core, conv_row_ref, engine_from_oracle, group_stats64, groupnorm_rows_ref,
+                           live_device_bytes, no_overlap, oracle_models, record, rel_err, set_arena, weight_bytes)
 
 pytestmark = pytest.mark.gpu
 
 H24, W24 = 4032, 6048
 P24 = H24 * W24
 T24 = P24 // 64            # latent tokens: 756 x 504 = 381 024
-U_PER_PIXEL = 512          # bytes of one fp32 128-channel map per output pixel
-
-
-def _hook(name, res, args):
-    from marigold_b200 import _lib
-
-    f = getattr(_lib.load(), name)        # debug hooks outside the public header
-    f.restype, f.argtypes = res, args
-    return f
-
-
-def set_arena(eng, poison=False, placement=0):
-    from marigold_b200._lib import check
-
-    f = _hook("mgb_debug_arena", C.c_int32, [C.c_void_p, C.c_int32, C.c_int32])
-    check(f(eng._h, int(poison), placement), "mgb_debug_arena")
-
-
-def arena_plan(eng, op, B, d0, d1):
-    """(bytes, t_alloc, t_free, offset) per buffer of one forward's arena (op 0 UNet step, 1 encode, 2 decode)."""
-    f = _hook("mgb_debug_arena_plan", C.c_int64, [C.c_void_p] + [C.c_int32] * 4 + [C.POINTER(C.c_int64)] * 4
-              + [C.c_int64])
-    n = f(eng._h, op, B, d0, d1, None, None, None, None, 0)
-    assert n > 0, n
-    arrs = [np.zeros(n, dtype=np.int64) for _ in range(4)]
-    p = [a.ctypes.data_as(C.POINTER(C.c_int64)) for a in arrs]
-    assert f(eng._h, op, B, d0, d1, *p, n) == n
-    return arrs
-
-
-def arena_place(nbytes, t0, t1, placement=0):
-    f = _hook("mgb_debug_arena_place", C.c_int64, [C.c_int64] + [C.POINTER(C.c_int64)] * 3
-              + [C.c_int32, C.POINTER(C.c_int64)])
-    off = np.zeros(len(nbytes), dtype=np.int64)
-    p = lambda a: a.ctypes.data_as(C.POINTER(C.c_int64))   # noqa: E731
-    peak = f(len(off), p(nbytes), p(t0), p(t1), placement, p(off))
-    assert peak >= 0
-    return peak, off
-
-
-def no_overlap(nbytes, t0, t1, off):
-    live = (t0[:, None] < t1[None, :]) & (t0[None, :] < t1[:, None])
-    mem = (off[:, None] < (off + nbytes)[None, :]) & (off[None, :] < (off + nbytes)[:, None]) & (nbytes[:, None] > 0)
-    both = live & mem & (nbytes[None, :] > 0)
-    np.fill_diagonal(both, False)
-    return not both.any()
 
 
 @pytest.fixture(scope="module")
@@ -103,10 +58,6 @@ def _give_back_memory():
     yield
     gc.collect()
     torch.cuda.empty_cache()
-
-
-def _photo(h, w, seed=3):
-    return synthetic_image(max(h, w), seed=seed)[..., :h, :w].contiguous()
 
 
 def test_iid_at_24mp():
@@ -152,43 +103,6 @@ def _rows(n_rows, widths, seed, n_random=64):
     return torch.tensor(sorted(r for r in rows if 0 <= r < n_rows), dtype=torch.long)
 
 
-def _block_rows(T, block, seed, every=1, n_random=128):
-    """Query rows of a row-blocked (or row-tiled) kernel: the first 32 and last 64, both sides of every `every`-th block
-    boundary, and n_random seeded rows."""
-    rows = set(range(32)) | set(range(T - 64, T))
-    for r0 in range(block, T, block * every):
-        rows |= {r0 - 1, r0}
-    g = torch.Generator().manual_seed(seed)
-    rows |= set(torch.randint(0, T, (n_random,), generator=g).tolist())
-    return torch.tensor(sorted(rows), dtype=torch.long)
-
-
-def group_stats64(x, G, eps, chunk=1 << 20):
-    """float64 mean and 1 / sqrt(var + eps) per group of x [HW, C] ([1, G, 1] each), two passes over row chunks."""
-    HW, C = x.shape
-    n = HW * (C // G)
-    s = torch.zeros(G, dtype=torch.float64, device=x.device)
-    for a in range(0, HW, chunk):
-        s += R.f64(x[a:a + chunk]).view(-1, G, C // G).sum(dim=(0, 2))
-    mean = (s / n).view(1, G, 1)
-    q = torch.zeros(G, dtype=torch.float64, device=x.device)
-    for a in range(0, HW, chunk):
-        q += ((R.f64(x[a:a + chunk]).view(-1, G, C // G) - mean) ** 2).sum(dim=(0, 2))
-    return mean, (1.0 / torch.sqrt(q / n + eps)).view(1, G, 1)
-
-
-def groupnorm_rows_ref(x_rows, mean, rstd, gamma, beta, G):
-    """float64 SiLU(GroupNorm) of rows [n, C] given the statistics, and the bound of tests/ops_cases.py's GroupNorm case."""
-    from tests.ops_cases import _norm_mag
-
-    n, C = x_rows.shape
-    x64 = R.f64(x_rows).view(n, G, C // G)
-    ga, be = R.f64(gamma).view(G, C // G), R.f64(beta).view(G, C // G)
-    ref = R.silu64(((x64 - mean) * rstd * ga + be).reshape(n, C))
-    mag = _norm_mag(x64, mean, rstd, ga, be).reshape(n, C)
-    return ref, R.bf16_bound(ref, mag * R.SILU_GAIN)
-
-
 @pytest.mark.parametrize("C", [256, 128])
 def test_groupnorm_past_2_32_elements(C):
     from marigold_b200 import ops
@@ -206,24 +120,6 @@ def test_groupnorm_past_2_32_elements(C):
     ref, bound = groupnorm_rows_ref(x[0, rows], mean, rstd, gamma, beta, G)
     R.assert_within(y[0, rows], ref, bound, f"native_res_24mp/groupnorm_c{C}/worst")
     assert torch.equal(raw[0, rows], x[0, rows].to(torch.bfloat16))
-
-
-def conv_row_ref(x, wb, y, b, x2=None, wsc=None):
-    """float64 output row y [W, Cout] of the 3x3 pad-1 conv of NHWC x [1, H, W, Cin] (bf16) with bias b, plus the 1x1
-    x2 [1, H, W, Cin2] @ wsc^T; and the bound of tests/ops_cases.py's conv case (K = 9 Cin + Cin2, fp32 output)."""
-    H, Cin = x.shape[1], x.shape[3]
-    lo, hi = max(0, y - 1), min(H, y + 2)
-    band = torch.zeros(1, Cin, 3, x.shape[2], dtype=torch.float64, device=x.device)
-    band[0, :, lo - (y - 1):hi - (y - 1)] = R.f64(x[0, lo:hi]).permute(2, 0, 1)
-    acc, absprod = R.conv64(band, wb, 1, (0, 1))
-    acc, absprod = acc[0, :, 0].t(), absprod[0, :, 0].t()
-    K = 9 * Cin
-    if x2 is not None:
-        a2, p2 = R.matmul64(x2[0, y], wsc)
-        acc, absprod = acc + a2, absprod + p2
-        K += x2.shape[3]
-    ref = acc + R.f64(b)
-    return ref, R.acc_bound(K, absprod) + 2 * R.R_F32_OUT * ref.abs() + R.TINY
 
 
 @pytest.mark.parametrize("Cin,Cin2,Cout", [(256, 0, 256), (128, 256, 128)], ids=["up_256", "conv2_shortcut"])
@@ -266,8 +162,6 @@ def test_softmax_rows_at_24mp(std):
 def test_vae_attn_core_at_24mp(engine, regime):
     """The VAE attention core in the decoder's row blocks at T = 381 024, within test_native_res_gpu.py's float64
     bound (its module docstring)."""
-    from tests.test_native_res_gpu import VAE_C, _core_inputs, _core_ref, attn_blocks, attn_core
-
     rows_per_block, blocks = attn_blocks(engine, 1, T24)
     assert rows_per_block < T24 and blocks == -(-T24 // rows_per_block)
     q, k, v = _core_inputs(1, T24, regime)
@@ -361,19 +255,10 @@ def test_24mp_plans(engine):
         assert arena_place(nbytes, t0, t1)[1].tolist() == off.tolist()
         assert arena_plan(engine, op, 1, d0, d1)[3].tolist() == off.tolist()
     need = engine.workspace_bytes(1, H24, W24)
-    weights = sum(_weight_bytes(engine))
+    weights = weight_bytes(engine)
     total = torch.cuda.get_device_properties(0).total_memory
     record("native_res_24mp/workspace_bytes", need)
     assert need + call_reserve_bytes(H24, W24, 10, 3) + weights < total, (need, weights, total)
-
-
-def _weight_bytes(eng):
-    f = _hook("mgb_debug_weight_buffers", C.c_int32, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_int64),
-                                                         C.c_int32])
-    n = f(eng._h, None, None, 0)
-    b = (C.c_int64 * n)()
-    f(eng._h, None, b, n)
-    return list(b)
 
 
 @pytest.mark.parametrize("NB,lh,lw", [(1, 96, 96), (2, 77, 131)])
@@ -423,7 +308,7 @@ def test_8192_is_still_refused_before_any_work(models, engine):
     from marigold_b200.pipeline import MarigoldDepthPipeline
     from marigold_b200.schedulers import DDIMScheduler
 
-    live = _hook("mgb_debug_live_device_bytes", C.c_int64, [])
+    live = live_device_bytes
     pipe = MarigoldDepthPipeline(engine, DDIMScheduler(), models[2], default_denoising_steps=1,
                                  default_processing_resolution=0)
     torch.cuda.synchronize()

@@ -11,7 +11,6 @@
     default path's limit), 8192 x 5464 and 8256 x 5504;
   * the two convs of that stage's resnet at 8064 x 6048 on packed operands (conv1; conv2 with the shortcut's
     [48.8M, 256] bf16 operand) against float64 on rows holding elements 2^30 .. 2^33."""
-import ctypes as C
 import gc
 
 import numpy as np
@@ -19,33 +18,14 @@ import pytest
 import torch
 
 from tests import ops_ref as R
-from tests.helpers import engine_from_oracle, oracle_models, record
-from tests.test_native_res_24mp_gpu import U_PER_PIXEL, _hook, _photo, _weight_bytes, arena_place, arena_plan, no_overlap
+from tests.helpers import (U_PER_PIXEL, _photo, _rows, arena_place, arena_plan, conv_row_ref, engine_from_oracle,
+                           no_overlap, oracle_models, record, set_low_memory, weight_bytes)
 
 pytestmark = pytest.mark.gpu
 
 H48, W48 = 6048, 8064
 P48 = H48 * W48            # 48 771 072 pixels
 SCRATCH = 1 << 20          # bytes of GroupNorm partials and statistics live beside the 2.5 U at the decoder's peak
-
-
-def set_low_memory(eng, mode):
-    """1: the decoder's full-resolution stage in low memory at every size; -1: never; 0: the library's rule."""
-    from marigold_b200._lib import check
-
-    f = _hook("mgb_debug_vae_low_memory", C.c_int32, [C.c_void_p, C.c_int32])
-    check(f(eng._h, mode), "mgb_debug_vae_low_memory")
-
-
-def _rows(n_rows, width, seed, n_random=64):
-    """The first and last 64 rows of a [n_rows, width] tensor, those holding elements 2^30 .. 2^33 and their neighbours,
-    and n_random seeded rows."""
-    rows = set(range(64)) | set(range(n_rows - 64, n_rows))
-    for e in (2 ** 30, 2 ** 31, 2 ** 32, 2 ** 33):
-        rows |= {e // width - 1, e // width, e // width + 1}
-    g = torch.Generator().manual_seed(seed)
-    rows |= set(torch.randint(0, n_rows, (n_random,), generator=g).tolist())
-    return torch.tensor(sorted(r for r in rows if 0 <= r < n_rows), dtype=torch.long)
 
 
 @pytest.fixture(autouse=True)
@@ -93,8 +73,6 @@ def test_resnet_convs_past_2_33_elements(stage):
     (128 + 256 -> 128) reading the shortcut's [48.8M, 256] bf16 operand. Image rows holding elements 2^30 .. 2^33 of
     each operand and of the output, and the first and last rows, against float64 with tests/ops_ref.py's conv bound."""
     from marigold_b200 import ops
-    from tests.test_native_res_24mp_gpu import conv_row_ref
-
     Cin, Cin2, Cout = (256, 0, 128) if stage == "conv1" else (128, 256, 128)
     K = 9 * Cin + Cin2
     g = torch.Generator(device="cuda").manual_seed(K)
@@ -162,7 +140,7 @@ def test_48mp_plan(engine):
     need = engine.workspace_bytes(1, H48, W48)
     record("native_res_48mp/workspace_bytes", need)
     total = torch.cuda.get_device_properties(0).total_memory
-    assert need + call_reserve_bytes(H48, W48, 2, 1) + sum(_weight_bytes(engine)) < total, (need, total)
+    assert need + call_reserve_bytes(H48, W48, 2, 1) + weight_bytes(engine) < total, (need, total)
 
 
 @pytest.mark.parametrize("NB,h,w", [(1, 4032, 6048), (1, 768, 768), (2, 768, 768)])
@@ -217,5 +195,5 @@ def test_select_batch_size_at_45mp(engine):
         fits = False
     record("native_res_48mp/workspace_bytes_8160x6144", need)
     record("native_res_48mp/fits_8160x6144", float(fits))
-    weights = sum(_weight_bytes(engine))
+    weights = weight_bytes(engine)
     print(f"8160 x 6144: workspace {need} B, weights {weights} B, fits: {fits}")

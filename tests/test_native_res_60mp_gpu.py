@@ -24,11 +24,10 @@ import pytest
 import torch
 
 from tests import ops_ref as R
-from tests.helpers import engine_from_oracle, oracle_models, record
-from tests.test_native_res_24mp_gpu import (U_PER_PIXEL, _block_rows, _hook, _photo, _weight_bytes, arena_place,
-                                            arena_plan, conv_row_ref, group_stats64, groupnorm_rows_ref, no_overlap,
-                                            set_arena)
-from tests.test_native_res_48mp_gpu import _rows, set_low_memory
+from tests.helpers import (U_PER_PIXEL, VAE_C, _block_rows, _core_inputs, _core_ref, _photo, _rows, arena_place,
+                           arena_plan, attn_blocks, attn_core, conv_row_ref, engine_from_oracle, group_stats64,
+                           groupnorm_rows_ref, no_overlap, oracle_models, record, set_arena, set_bands, set_low_memory,
+                           weight_bytes)
 
 pytestmark = pytest.mark.gpu
 
@@ -38,22 +37,12 @@ T60 = P60 // 64            # latent tokens: 1188 x 792 = 940 896
 SCRATCH = 1 << 20          # bytes of GroupNorm partials and statistics live beside the 2.5 U at the decoder's peak
 
 
-def set_bands(eng, up_tiles=0, conv1_tiles=0):
-    """Tile rows per band of the low-memory decoder's banded up-conv and conv1 (0: the library's choice)."""
-    from marigold_b200._lib import check
-
-    f = _hook("mgb_debug_vae_bands", C.c_int32, [C.c_void_p, C.c_int32, C.c_int32])
-    check(f(eng._h, up_tiles, conv1_tiles), "mgb_debug_vae_bands")
-
-
 def conv_band(x, src_y0, wp, bias, out, out_hi, split_col, ldo, out_y0, NB_tile, H, W, Cin, Cout, ty0, tiles):
     """One band of the decoder's banded conv (mgb_debug_conv2d_band); x None: only returns (tile_h, tiles_y)."""
     from marigold_b200 import _lib
     from marigold_b200.ops import ptr, stream_ptr
 
-    f = _hook("mgb_debug_conv2d_band", C.c_int32,
-              [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 10
-              + [C.POINTER(C.c_int32), C.c_void_p])
+    f = _lib.load().mgb_debug_conv2d_band
     geom = (C.c_int32 * 2)()
     xp = None if x is None else ptr(x)
     src_rows = 0 if x is None else x.shape[-3]
@@ -72,8 +61,7 @@ def groupnorm_halves(a, b, gamma, beta, NB, HW, G, eps, silu):
 
     lib = _lib.load()
     Ch = a.shape[-1]
-    f = _hook("mgb_debug_groupnorm_halves", C.c_int32,
-              [C.c_void_p] * 6 + [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_void_p])
+    f = lib.mgb_debug_groupnorm_halves
     ws = torch.empty((int(lib.mgb_op_groupnorm_ws_bytes(NB, HW, 2 * Ch, G)) + 3) // 4, device="cuda")
     stats = torch.empty(NB * 2 * Ch * 2, device="cuda")
     _lib.check(f(ptr(a), ptr(b), Ch, ptr(gamma), ptr(beta), ptr(ws), ptr(stats), NB, HW, G, float(eps), int(silu),
@@ -264,8 +252,6 @@ def test_vae_attn_core_at_60mp(regime):
     """The VAE attention core in the decoder's row blocks at T = 940 896 (the 60 MP latent), within
     test_native_res_gpu.py's float64 bound. Its blocks are the one-wave minimum of the P V GEMM, 4 224 rows: their
     scores (23.8 GB) pass kVaeAttnBudget but stay far below the decoder's full-resolution peak."""
-    from tests.test_native_res_gpu import VAE_C, _core_inputs, _core_ref, attn_blocks, attn_core
-
     eng = engine_from_oracle(*oracle_models("full"))
     try:
         rows_per_block, blocks = attn_blocks(eng, 1, T60)
@@ -403,7 +389,7 @@ def test_60mp_plan(engine):
     need = engine.workspace_bytes(1, H60, W60)
     record("native_res_60mp/workspace_bytes", need)
     print(f"9504 x 6336: decoder peak {peak / U:.3f} U, encoder {int((enc[3] + enc[0]).max()) / U:.3f} U, "
-          f"workspace {need} B, weights {sum(_weight_bytes(engine))} B")
+          f"workspace {need} B, weights {weight_bytes(engine)} B")
 
 
 @pytest.mark.parametrize("h,w", [(6048, 8064), (4032, 6048)])

@@ -38,30 +38,11 @@ import pytest
 import torch
 
 from tests import ops_ref
-from tests.helpers import engine_from_oracle, oracle_models, record, rel_err, synthetic_image
-from tests.ops_cases import check_rows, dominant_key
+from tests.helpers import (VAE_C, _core_inputs, _core_ref, _photo, attn_blocks, attn_core, engine_from_oracle,
+                           live_device_bytes, oracle_models, record, rel_err, synthetic_image)
+from tests.ops_cases import check_rows
 
 pytestmark = pytest.mark.gpu
-
-
-def _hook(name, res, args):
-    from marigold_b200 import _lib
-
-    f = getattr(_lib.load(), name)        # debug hooks outside the public header
-    f.restype, f.argtypes = res, args
-    return f
-
-
-def attn_blocks(eng, NB, T, budget=0, force_rows=0):
-    """(rows per block, blocks over the NB images) of an (NB, T) VAE attention; sets the handle's budget and forced rows
-    (0: the library's)."""
-    from marigold_b200._lib import check
-
-    f = _hook("mgb_debug_vae_attn_blocks", C.c_int32,
-              [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)])
-    r, b = C.c_int32(), C.c_int32()
-    check(f(eng._h, budget, force_rows, NB, T, C.byref(r), C.byref(b)), "mgb_debug_vae_attn_blocks")
-    return r.value, b.value
 
 
 @pytest.fixture(scope="module")
@@ -105,8 +86,6 @@ def test_row_blocks_are_bit_identical(engine, lh, lw, NB):
 
 
 # ---- pipelines at processing_res = 0 -----------------------------------------------------------------------------
-def _photo(h, w, seed=3):
-    return synthetic_image(max(h, w), seed=seed)[..., :h, :w].contiguous()
 
 
 def test_depth_and_normals_at_native_resolution(models, engine):
@@ -167,7 +146,7 @@ def test_too_large_for_one_member_is_refused_before_any_work(models, engine):
     from marigold_b200.pipeline import MarigoldDepthPipeline
     from marigold_b200.schedulers import DDIMScheduler
 
-    live = _hook("mgb_debug_live_device_bytes", C.c_int64, [])
+    live = live_device_bytes
     lib = engine.lib
     pipe = MarigoldDepthPipeline(engine, DDIMScheduler(), models[2], default_denoising_steps=1,
                                  default_processing_resolution=0)
@@ -316,7 +295,6 @@ def test_unet_step_at_native_resolution_matches_oracle(models):
 
 
 # ---- the VAE attention core at native token counts ---------------------------------------------------------------
-VAE_C = 512
 # 4000 x 3000 (T % 64 = 44), 4032 x 3024 (T % 64 = 48), two 1920 x 1080 images (blocks and per-image offsets) and
 # 77 x 131 latents (one block)
 CORE_SIZES = [(1, 187500), (1, 190512), (2, 32400), (1, 10087)]
@@ -330,60 +308,6 @@ def core_engine(models):
     eng = engine_from_oracle(*models)
     yield eng
     eng.close()
-
-
-def attn_core(eng, q, k, v, NB, T):
-    """mgb_debug_vae_attn_core: bf16 q, k, v [NB T, 512] -> bf16 o, with the handle's row blocking."""
-    from marigold_b200._lib import check
-
-    f = _hook("mgb_debug_vae_attn_core", C.c_int32, [C.c_void_p] * 5 + [C.c_int32, C.c_int32])
-    o = torch.empty_like(q)
-    check(f(eng._h, q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), NB, T), "mgb_debug_vae_attn_core")
-    torch.cuda.synchronize()
-    return o
-
-
-def _core_inputs(NB, T, regime):
-    g = torch.Generator(device="cuda").manual_seed(7 * T + NB)
-    std = 6.3 if regime == "logits80" else 1.0
-    q = torch.randn(NB, T, VAE_C, device="cuda", generator=g) * std
-    k = torch.randn(NB, T, VAE_C, device="cuda", generator=g) * std
-    v = torch.randn(NB, T, VAE_C, device="cuda", generator=g)
-    if regime in ("key_last", "key_mid"):
-        dominant_key(q, k, T - 1 if regime == "key_last" else T // 2 + 7, 14.0, VAE_C ** -0.5, VAE_C, seed=T)
-    return [t.reshape(NB * T, VAE_C).to(torch.bfloat16) for t in (q, k, v)]
-
-
-def _core_ref(q, k, v, NB, T, rows):
-    """float64 o, its bound (module docstring) and sum_j p_j |v_j| at `rows` of every image: [NB, len(rows), C]."""
-    R = ops_ref
-    Cc, Tp, scale = VAE_C, (T + 63) // 64 * 64, VAE_C ** -0.5
-    ref = torch.empty(NB, len(rows), Cc, dtype=torch.float64, device="cuda")
-    bound, pv_abs = torch.empty_like(ref), torch.empty_like(ref)
-    step = max(1, (1 << 26) // T)
-    for n in range(NB):
-        k64, v64 = R.f64(k[n * T:(n + 1) * T]), R.f64(v[n * T:(n + 1) * T])
-        ka, va = k64.abs(), v64.abs()
-        for i in range(0, len(rows), step):
-            qr = R.f64(q[n * T + rows[i:i + step]])
-            s = qr @ k64.t() * scale
-            ds = R.C_ACC * Cc * R.U_F32 * scale * (qr.abs() @ ka.t()) + R.R_F32_OUT * s.abs()
-            dist = s.max(dim=1, keepdim=True).values - s
-            del s
-            p = torch.exp(-dist)
-            p /= p.sum(dim=1, keepdim=True)
-            o = p @ v64
-            pds = p * ds
-            del ds
-            w = p * (R.softmax_rel(T, dist, p) + R.C_ACC * Tp * R.U_F32) + pds
-            del dist
-            pa = p @ va
-            sl = slice(i, i + step)
-            ref[n, sl], pv_abs[n, sl] = o, pa
-            bound[n, sl] = ((R.U_BF16 + 2 * R.R_F32_OUT) * o.abs() + R.C_P * R.U_BF16 * pa + w @ va
-                            + o.abs() * pds.sum(dim=1, keepdim=True) + R.TINY)
-            del p, pds, w
-    return ref, bound, pv_abs
 
 
 @pytest.mark.parametrize("regime", REGIMES)

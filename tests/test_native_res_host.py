@@ -5,24 +5,7 @@ import pytest
 import torch
 
 from marigold_b200.pipeline import MAX_PIXELS, _processing_size, find_batch_size, select_batch_size
-
-GB = 1 << 30
-
-
-class StubEngine:
-    """workspace_bytes: `per_member` bytes per member plus a fixed part; 0 past the supported maximum (like the
-    library). held_bytes: what the engine holds now."""
-
-    def __init__(self, per_member, fixed=GB, held=0):
-        self.per_member, self.fixed, self.held = per_member, fixed, held
-        self.asked = []
-
-    def workspace_bytes(self, B, H, W):
-        self.asked.append(B)
-        return 0 if B * H * W > MAX_PIXELS else self.fixed + B * self.per_member
-
-    def held_bytes(self):
-        return self.held
+from tests.helpers import GB, StubEngine
 
 
 @pytest.mark.parametrize("E,h,w", [(1, 768, 768), (10, 768, 576), (16, 768, 768), (10, 1024, 1024), (64, 1024, 768)])

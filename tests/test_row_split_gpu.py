@@ -16,7 +16,7 @@ import torch
 
 from marigold_b200 import ops, parallel
 from marigold_b200._lib import MgbError
-from tests.helpers import engine_from_oracle, oracle_models, synthetic_image
+from tests.helpers import arena_plan, attn_blocks, engine_from_oracle, oracle_models, synthetic_image
 
 pytestmark = pytest.mark.gpu
 
@@ -207,18 +207,6 @@ def test_virtual_ranks_are_the_unsplit_call(request, model, H, W):
     _check_virtual_ranks(eng, _workloads(eng, H, W, 1 if model == "depth" else 2))
 
 
-def _vae_attn_rows(eng, force_rows, T):
-    """mgb_debug_vae_attn_blocks: forces the VAE attention's rows per block (0: the library's), returns them."""
-    import ctypes as C
-
-    f = eng.lib.mgb_debug_vae_attn_blocks
-    f.restype = C.c_int32
-    f.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-    rows, blocks = C.c_int32(), C.c_int32()
-    assert f(eng._h, 0, force_rows, 1, T, C.byref(rows), C.byref(blocks)) == 0
-    return rows.value
-
-
 @pytest.mark.parametrize("force_rows", [128, 384])
 def test_virtual_ranks_with_vae_row_blocks(depth_eng, force_rows):
     """The VAE attention in row blocks that do not line up with the ranks' shares (large photos run it so): 4800 tokens
@@ -227,26 +215,15 @@ def test_virtual_ranks_with_vae_row_blocks(depth_eng, force_rows):
     w = {k: v for k, v in _workloads(eng, 480, 640, 1).items() if k in ("encode", "decode_depth")}
     default = {k: run().clone() for k, (run, _) in w.items()}
     try:
-        assert _vae_attn_rows(eng, force_rows, 60 * 80) == force_rows
+        assert attn_blocks(eng, 1, 60 * 80, force_rows=force_rows)[0] == force_rows
         for k, (run, _) in w.items():
             assert torch.equal(run(), default[k]), k                   # row blocks never change the bits
         _check_virtual_ranks(eng, w)
     finally:
-        _vae_attn_rows(eng, 0, 60 * 80)
+        attn_blocks(eng, 1, 60 * 80)
 
 
 # ---- unchanged paths and errors -----------------------------------------------------------------------------------
-
-def _plan(eng, op, d0, d1):
-    import ctypes as C
-
-    f = eng.lib.mgb_debug_arena_plan
-    f.restype = C.c_int64
-    f.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 4 + [C.c_int64]
-    n = f(eng._h, op, 1, d0, d1, None, None, None, None, 0)
-    arrs = [np.zeros(n, np.int64) for _ in range(4)]
-    assert f(eng._h, op, 1, d0, d1, *[a.ctypes.data for a in arrs], n) == n
-    return [a.tolist() for a in arrs]
 
 
 def test_cleared_split_leaves_plans_bytes_and_graphs(depth_eng):
@@ -254,12 +231,12 @@ def test_cleared_split_leaves_plans_bytes_and_graphs(depth_eng):
     fresh = engine_from_oracle(*oracle_models("tiny"))
     try:
         shapes = [(0, 60, 80), (1, 480, 640), (2, 60, 80), (0, 43, 59), (2, 43, 59)]
-        want = [_plan(fresh, *s) for s in shapes]
+        want = [[a.tolist() for a in arena_plan(fresh, op, 1, d0, d1)] for op, d0, d1 in shapes]
         want_ws = [fresh.workspace_bytes(1, 480, 640), fresh.workspace_bytes(4, 472, 344)]
         eng.set_row_split(1, 3, lambda buf, r, g: None)
         assert eng.workspace_bytes(1, 480, 640) > 0   # sized for this rank's share
         eng.set_row_split()
-        assert [_plan(eng, *s) for s in shapes] == want
+        assert [[a.tolist() for a in arena_plan(eng, op, 1, d0, d1)] for op, d0, d1 in shapes] == want
         assert [eng.workspace_bytes(1, 480, 640), eng.workspace_bytes(4, 472, 344)] == want_ws
         # a denoise launches what the captured step graph holds, as before, after a row-split call
         lat, z0 = torch.randn(1, 4, 60, 80, device="cuda"), torch.randn(1, 4, 60, 80, device="cuda")

@@ -10,8 +10,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from marigold_b200 import parallel
-from tests.test_multi_image_host import FakeEngine, _expected, _images, _pipe, _run
-from tests.test_native_res_host import GB
+from tests.helpers import GB, FakeEngine, _expected, _images, _pipe, _run
 
 
 def test_chunk_geometry():

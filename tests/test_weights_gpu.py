@@ -21,12 +21,6 @@ pytestmark = pytest.mark.gpu
 
 
 # ---- read-back ------------------------------------------------------------------------------------------------------
-def _fn(name, res, args):
-    from marigold_b200 import _lib
-
-    f = getattr(_lib.load(), name)        # debug hooks outside the public header
-    f.restype, f.argtypes = res, args
-    return f
 
 
 class Reader:
@@ -34,8 +28,7 @@ class Reader:
 
     def __init__(self, eng):
         self.eng, self.seen, self._last = eng, {}, (None, None)
-        self._rd = _fn("mgb_debug_read", C.c_int64, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64,
-                                                      C.POINTER(C.c_uint64)])
+        self._rd = eng.lib.mgb_debug_read
 
     def addr(self, field):
         a = C.c_uint64()
@@ -62,7 +55,7 @@ def _raise(status, field):
 
 
 def weight_buffers(eng):
-    f = _fn("mgb_debug_weight_buffers", C.c_int32, [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_int64), C.c_int32])
+    f = eng.lib.mgb_debug_weight_buffers
     n = f(eng._h, None, None, 0)
     assert n > 0
     addr, size = (C.c_uint64 * n)(), (C.c_int64 * n)()

@@ -11,8 +11,6 @@ import torch  # noqa: E402
 from marigold_b200 import _lib, ops  # noqa: E402
 
 lib = _lib.load()
-raw = C.CDLL(str(_lib.lib_path()))
-raw.mgb_debug_gemm_timing.argtypes = [C.c_void_p]
 
 
 def run(H, W, Cin, Cout, bn, stages, reps=20, flags=0):
@@ -30,10 +28,10 @@ def run(H, W, Cin, Cout, bn, stages, reps=20, flags=0):
     e1.record()
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 1e3 / reps
-    raw.mgb_debug_gemm_timing(C.c_void_p(dbg.data_ptr()))
+    lib.mgb_debug_gemm_timing(C.c_void_p(dbg.data_ptr()))
     fn()
     torch.cuda.synchronize()
-    raw.mgb_debug_gemm_timing(None)
+    lib.mgb_debug_gemm_timing(None)
     d = dbg.cpu().double()
     d = d[d[:, 0] > 0]
     ph = {"prologue": d[:, 1] - d[:, 0], "first": d[:, 2] - d[:, 1], "mainloop": d[:, 3] - d[:, 2],

@@ -12,8 +12,6 @@ from marigold_b200 import _lib  # noqa: E402
 from marigold_b200._lib import check, ptr, stream_ptr  # noqa: E402
 
 lib = _lib.load()
-raw = C.CDLL(str(_lib.lib_path()))
-raw.mgb_debug_gemm_timing.argtypes = [C.c_void_p]
 
 
 def run(M, N, K, bn, stages, out_dtype="f32", flags=0):
@@ -31,11 +29,11 @@ def run(M, N, K, bn, stages, out_dtype="f32", flags=0):
     for _ in range(3):
         fn()
     torch.cuda.synchronize()
-    raw.mgb_debug_gemm_timing(C.c_void_p(dbg.data_ptr()))
+    lib.mgb_debug_gemm_timing(C.c_void_p(dbg.data_ptr()))
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(); fn(); e1.record()
     torch.cuda.synchronize()
-    raw.mgb_debug_gemm_timing(None)
+    lib.mgb_debug_gemm_timing(None)
     d = dbg.cpu().double()
     ph = {"prologue": (d[:, 1] - d[:, 0]), "first_stage": (d[:, 2] - d[:, 1]), "mainloop": (d[:, 3] - d[:, 2]),
           "epilogue": (d[:, 4] - d[:, 3]), "teardown": (d[:, 5] - d[:, 4]), "total": (d[:, 5] - d[:, 0])}

@@ -13,7 +13,6 @@ memory: depth with E = 1 and 1 step.
         run and the largest photos accepted)
 """
 import argparse
-import ctypes as C
 import json
 import sys
 from pathlib import Path
@@ -25,16 +24,7 @@ from bench import gpu_identity  # noqa: E402
 from marigold_b200.ensemble import ensemble_depth, ensemble_iid, ensemble_normals  # noqa: E402
 from marigold_b200.pipeline import call_reserve_bytes, select_batch_size  # noqa: E402
 from marigold_b200.schedulers import DDIMScheduler  # noqa: E402
-from tests.helpers import synthetic_image  # noqa: E402
-
-
-def attn_blocks(eng, NB, T, budget=0):
-    f = eng.lib.mgb_debug_vae_attn_blocks        # debug hook outside the public header
-    f.restype = C.c_int32
-    f.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-    r, b = C.c_int32(), C.c_int32()
-    assert f(eng._h, budget, 0, NB, T, C.byref(r), C.byref(b)) == 0
-    return r.value, b.value
+from tests.helpers import attn_blocks, synthetic_image  # noqa: E402
 
 
 def make_engine(n_targets=1, seed=0):
